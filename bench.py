@@ -2,11 +2,11 @@
 """Headline benchmark: samples/sec of the data-parallel training step on the synthetic 2-task
 MLP Problem (BASELINE.json configs[1] at N=1, configs[2] at N>1; batch 4096 per rank).
 
-    python bench.py --gpus N --steps K --warmup W            # this repo's B200 path
+    python bench.py --gpus N --steps K --warmup W            # this repo's H100 path
     python bench.py --impl reference --gpus N --steps K ...  # reference algorithm on host CPU
     python bench.py --impl torch-gpu --gpus N ...            # stock PyTorch on the GPU: autocast +
                                                              # torch.optim (+ DDP at N>1), the
-                                                             # "kernel to beat" of SURVEY §8(d)
+                                                             # "kernel to beat"
     python bench.py --workload resnet18|resnet50x4 ...       # BASELINE configs[3] / configs[4]
 
 One JSON line on stdout (rank 0).  Everything else goes to stderr.
@@ -59,6 +59,9 @@ def parse_args():
     ap.add_argument("--graph", type=int, default=1, help="replay the step from a CUDA graph (1) or issue it eagerly (0)")
     ap.add_argument("--profile", default=None,
                     help="write a JSON summary (device time per kernel per step, torch.profiler over 5 steps) here")
+    ap.add_argument("--dump-outputs", default=None, metavar="DIR",
+                    help="b200 arm, rank 0: write what the last timed step returned (model outputs, losses) and a "
+                         "seeded sample of the updated fp32 master weights as DIR/<name>.npy")
     args = ap.parse_args()
     wl = WORKLOADS[args.workload]
     if args.algo is None:
@@ -293,7 +296,7 @@ class ClockSampler:
 
 
 # --------------------------------------------------------------------------------------------------
-# stock-PyTorch-GPU arm: what the reference does on a GPU (SURVEY §8d "kernel to beat")
+# stock-PyTorch-GPU arm: what the reference does on a GPU (the "kernel to beat")
 # --------------------------------------------------------------------------------------------------
 
 def run_torch_gpu(args, rank, local_rank, world, steps, warmup, with_e2e=True, profile_path=None):
@@ -429,8 +432,8 @@ def align_ranks(world, dev):
     """Device-side barrier enqueued right before a start event (world > 1): a 1-element NCCL
     all-reduce completes on every GPU when the LAST rank has enqueued it, so the start events of
     all ranks are recorded within microseconds of one another.  The host barrier before it lets
-    the ranks go up to a millisecond apart (8 GPUs: first timed step 1.86 ms against 1.02 for the
-    rest, all of it one rank waiting at the first exchange for a peer that started later)."""
+    the ranks go up to a millisecond apart, and the first timed step would then include one rank
+    waiting at the first exchange for a peer that started later."""
     if world > 1:
         import torch
         import torch.distributed as dist
@@ -466,13 +469,66 @@ def main_torch_gpu(args, rank, local_rank, world):
 
 
 # --------------------------------------------------------------------------------------------------
-# B200 arm
+# the project's own arm ("b200", its historical name; built for H100)
 # --------------------------------------------------------------------------------------------------
 
 BYTES_PER_PARAM = {  # algorithmic, fp32 master + state, bf16 gradient read, bf16 shadow written
     ("sgd", "bf16"): 2 + 4 + 4 + 4 + 4 + 2, ("sgd", "fp32"): 4 + 4 + 4 + 4 + 4,
     ("adam", "bf16"): 2 + 4 * 3 + 4 * 3 + 2, ("adam", "fp32"): 4 * 4 + 4 * 3,
     ("rmsprop", "bf16"): 2 + 4 * 3 + 4 * 3 + 2, ("rmsprop", "fp32"): 4 * 4 + 4 * 3}
+
+
+DUMP_BUDGET_BYTES = 64 << 20
+DUMP_MASTER_SAMPLE = 1 << 20          # elements of the fp32 master arena written by --dump-outputs
+
+
+def _seeded_rows(a, max_bytes, seed):
+    """``a`` itself if it fits ``max_bytes`` as float32, else a fixed seeded subset of its rows
+    (of its elements if one row does not fit) and the indices taken, as float64."""
+    import numpy as np
+    import torch
+    if a.numel() * 4 <= max_bytes:
+        return a, None
+    if a.dim() < 2 or a[0].numel() * 4 + 8 > max_bytes:
+        a = a.reshape(-1)
+    keep = max(1, max_bytes // (a[0].numel() * 4 + 8))
+    idx = np.sort(np.random.default_rng(seed).choice(a.shape[0], keep, replace=False))
+    return a[torch.from_numpy(idx).to(a.device)], idx.astype(np.float64)
+
+
+def snapshot_step_outputs(result, master):
+    """Host copies of what ``_pass_one_minibatch`` returned (outputs per task, total loss, loss per
+    task) and of a fixed, seeded sample of the fp32 master weights after the step, at most
+    ``DUMP_BUDGET_BYTES`` in all: an output too large for its share is written as a seeded sample
+    of its rows, with the row indices."""
+    output, total_loss, sub_loss = result[0], result[1], result[2]
+    arrays = {"total_loss": total_loss.detach().float().cpu().numpy()}
+    for name, v in sub_loss.items():
+        arrays["loss_%s" % name] = v.detach().float().cpu().numpy()
+    sample, idx = _seeded_rows(master.detach(), DUMP_MASTER_SAMPLE * (4 + 8), 0)
+    if idx is None:
+        arrays["master"] = sample.float().cpu().numpy()
+    else:
+        arrays["master_sample"] = sample.float().cpu().numpy()
+        arrays["master_sample_index"] = idx
+    used = sum(a.nbytes for a in arrays.values())
+    share = (DUMP_BUDGET_BYTES - used) // max(len(output), 1)
+    for i, o in enumerate(output):
+        sample, idx = _seeded_rows(o.detach(), share, 1 + i)
+        arrays["output_%d" % i] = sample.float().cpu().numpy()
+        if idx is not None:
+            arrays["output_%d_row_index" % i] = idx
+    total = sum(a.nbytes for a in arrays.values())
+    assert total <= DUMP_BUDGET_BYTES, "outputs to dump: %d bytes > %d" % (total, DUMP_BUDGET_BYTES)
+    return arrays
+
+
+def write_outputs(directory, arrays):
+    import numpy as np
+    os.makedirs(directory, exist_ok=True)
+    for name, a in arrays.items():
+        np.save(os.path.join(directory, name + ".npy"), a)
+    log("wrote %d arrays (%.1f MB) to %s" % (len(arrays), sum(a.nbytes for a in arrays.values()) / 1e6, directory))
 
 
 def gpu_numa_node(local_rank):
@@ -684,7 +740,7 @@ def main_b200(args, rank, local_rank, world):
     def step_resident(i):
         data, target = pool[i % POOL]
         worker.criterion.set_step_sink(log_ring.row(i), log_ring.nan_flag)
-        worker._pass_one_minibatch(i, t.Split.TRAIN, data, target)
+        return worker._pass_one_minibatch(i, t.Split.TRAIN, data, target)
 
     # ======================= leg 1: inputs resident in HBM =======================
     # spin-up: a GPU that sat idle (every GPU but the first on a fresh multi-GPU box) needs tens of
@@ -709,10 +765,18 @@ def main_b200(args, rank, local_rank, world):
         marks[0].record()
         host_t0 = time.perf_counter()
         for i in range(K):
-            step_resident(W + i)
+            last = step_resident(W + i)
             marks[i + 1].record()
         host_issue_ms = 1e3 * (time.perf_counter() - host_t0) / K     # CPU time to ISSUE a step
         barrier()
+    if args.dump_outputs:
+        # before any further step: replayed graphs return their static output buffers.  With the
+        # fused NVLS step each rank holds current master weights for its own shards only: make
+        # them whole on every rank first (collective)
+        worker.pipeline.sync_sharded_state()
+        if rank == 0:
+            write_outputs(args.dump_outputs, snapshot_step_outputs(last, arena.master))
+    del last
     launches = _native.launch_count() + graph_step.REPLAYED_LAUNCHES - launches0
     worker.pipeline.record_update_events = False
     total_ms = marks[0].elapsed_time(marks[K])
@@ -747,11 +811,7 @@ def main_b200(args, rank, local_rank, world):
     if os.path.exists(peaks_path):
         peak, peak_src = json.load(open(peaks_path))["hbm_gbs"], "measured (MEASURED_PEAKS.json hbm_gbs)"
     else:
-        peak, peak_src = 6650.0, "fallback (B200_PROFILING.md)"
-    traffic = None
-    tpath = os.path.join(REPO, "profiles", "k2_traffic.json")
-    if os.path.exists(tpath):
-        traffic = json.load(open(tpath)).get("%s_%s" % (args.algo, args.precision))
+        peak, peak_src = 3350.0, "H100 SXM data sheet (HBM3), not measured"
     nv_link = worker.pipeline.nvls
     kernel_name = "frl::update_kernel (fused grad-bucket + optimizer, K2)"
     nvlink = None
@@ -765,16 +825,16 @@ def main_b200(args, rank, local_rank, world):
         g_b = 2 if args.precision == "bf16" else 4
         link_bytes = upd_elems * g_b * (1.0 + 1.0 / world)          # per direction, per GPU
         nvlink = {"bytes_per_direction_per_launch": link_bytes / len(upd_ms),
-                  "achieved": link_bytes / (sum(upd_ms) / 1e3) / 1e9, "peak": 770.0, "unit": "GB/s",
-                  "peak_source": "measured peer copy per direction (B200_PROFILING.md); 900 nominal",
-                  "note": "NVLink 5 per-direction payload of the fused step: out = own gradient copy "
+                  "achieved": link_bytes / (sum(upd_ms) / 1e3) / 1e9, "peak": 450.0, "unit": "GB/s",
+                  "peak_source": "H100 SXM data sheet: NVLink 4, 900 GB/s bidirectional, not measured",
+                  "note": "NVLink per-direction payload of the fused step: out = own gradient copy "
                           "read by the switch + multicast of the shard's new weights, in = reduced shard "
                           "+ every shard's new weights; this, the barriers and the SMs left over by the "
                           "overlapped backward GEMMs bound K7, not HBM"}
     achieved = bpp * upd_elems / (sum(upd_ms) / 1e3) / 1e9 if upd_ms else None
     roofline = {"bound": "hbm", "kernel": kernel_name,
                 "achieved": achieved, "peak": peak, "unit": "GB/s",
-                "frac": (achieved / peak) if achieved else None, "traffic": traffic,
+                "frac": (achieved / peak) if achieved else None,
                 "peak_source": peak_src, "bytes_per_param": bpp, "timed_by": roofline_from,
                 "elems_per_launch": upd_elems / max(len(upd), 1),
                 "avg_launch_ms": (sum(upd_ms) / len(upd_ms)) if upd_ms else None,
@@ -783,7 +843,6 @@ def main_b200(args, rank, local_rank, world):
         roofline["share_of_step"] = roofline["update_ms_per_step"] / (total_ms / K)
     if nvlink is not None:
         roofline["nvlink"] = nvlink
-        roofline["traffic"] = None
         roofline["note"] = ("multi-GPU: the update is sharded 1/world per rank and overlapped with "
                             "backward; the single-GPU run carries the HBM roofline of the update kernel (K2)")
 
@@ -974,7 +1033,7 @@ def main_b200(args, rank, local_rank, world):
                                         "optimizer state" if precision == Precision.BF16 else "fp32",
                            "l2": "no flush needed: each step streams the %.1fM-element arena "
                                  "(%.2f GB of update traffic) and 4 rotating input batches, larger than the "
-                                 "126 MB L2" % (arena.numel / 1e6, arena.numel * BYTES_PER_PARAM[(args.algo, args.precision)] / 1e9),
+                                 "50 MB L2" % (arena.numel / 1e6, arena.numel * BYTES_PER_PARAM[(args.algo, args.precision)] / 1e9),
                            "grad_allreduce": grad_sync_desc},
                 "roofline": roofline, "cpu_baseline": cpu, "e2e": e2e, "gpu_launches": launches,
                 "torch_gpu_baseline": torch_base, "parity_check": parity,

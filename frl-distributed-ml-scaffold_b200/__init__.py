@@ -1,4 +1,4 @@
-"""frl_b200 — B200-native data-parallel training step behind the FRL Distributed ML Scaffold
+"""frl_b200 — H100-native data-parallel training step behind the FRL Distributed ML Scaffold
 plugin API (``Problem`` / ``Task`` / criteria / ``Solver.solve``).
 
 Import as ``frl_b200`` (see ``frl_b200.py`` at the repository root).  ``install_reference_alias``

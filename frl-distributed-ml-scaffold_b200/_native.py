@@ -91,7 +91,7 @@ _lib: Optional[C.CDLL] = None
 
 
 def build(verbose: bool = False) -> str:
-    """Compile the library in-tree with nvcc for sm_100a (cross-compiles without a GPU)."""
+    """Compile the library in-tree with nvcc for sm_90a (cross-compiles without a GPU)."""
     cmd = ["make", "-C", CSRC_DIR, "-j8"]
     res = subprocess.run(cmd, capture_output=True, text=True)
     if verbose or res.returncode != 0:
@@ -107,7 +107,7 @@ def lib() -> C.CDLL:
     if _lib is None:
         if not os.path.exists(LIB_PATH):
             raise NativeLibraryError(
-                f"{LIB_PATH} is missing: the sm_100a kernel library has not been built "
+                f"{LIB_PATH} is missing: the sm_90a kernel library has not been built "
                 "(run `python __graft_entry__.py build` or `make -C <pkg>/csrc`). "
                 "There is no fallback path.")
         handle = C.CDLL(LIB_PATH)

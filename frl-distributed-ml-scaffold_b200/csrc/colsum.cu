@@ -1,8 +1,8 @@
-// K6 — column sum of a row-major matrix: out[c] (+)= sum_r x[r, c]   (sm_100a).
+// K6 — column sum of a row-major matrix: out[c] (+)= sum_r x[r, c]   (sm_90a).
 //
 // This is the bias gradient of a linear layer (db = sum over the batch of dY).  Stock autograd
 // computes it with a generic reduction that re-reads dY at a fraction of HBM speed
-// (at::reduce_kernel: ~27 us for a 4096x4096 bf16 dY, 5 launches per step in the MLP config);
+// (at::reduce_kernel, 5 launches per step in the MLP config);
 // here it is one bandwidth-bound pass whose result lands directly in the gradient arena.
 //
 // Grid (column tiles, row splits).  A warp reads one row segment of 32 lanes x 8 columns with a

@@ -1,5 +1,5 @@
 // K4 — fused multitask criterion: per-task MSE / cross-entropy (optionally masked), weighted
-// sum, loss log and NaN flag in ONE forward launch and ONE backward launch (sm_100a).
+// sum, loss log and NaN flag in ONE forward launch and ONE backward launch (sm_90a).
 //
 // The reference evaluates T loss modules, T scalar multiplies and T-1 scalar adds as separate
 // PyTorch kernels, then synchronises the host 2+T times per minibatch to test for NaN and to
@@ -20,7 +20,7 @@ namespace frl {
 
 constexpr int kCThreads = 256;
 constexpr int kCWarps = kCThreads / 32;
-constexpr int kCMaxBlocksPerTask = 592;   // 148 SMs x 4
+constexpr int kCMaxBlocksPerTask = 528;   // 132 SMs x 4
 constexpr int kCVecPerLane = 8;           // 4-element vectors a lane holds per row chunk
 constexpr int kCRowChunk = 32 * 4 * kCVecPerLane;   // 1024 columns: one register-resident chunk
 

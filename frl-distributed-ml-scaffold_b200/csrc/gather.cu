@@ -1,4 +1,4 @@
-// K8 — row gather from a pinned (device-mapped) host dataset straight into HBM (sm_100a).
+// K8 — row gather from a pinned (device-mapped) host dataset straight into HBM (sm_90a).
 //
 // The reference assembles every minibatch on the host: per-sample __getitem__ + transform in
 // Python, default_collate, then a pageable H2D copy (reference solver_worker.py:462-469,
@@ -8,8 +8,8 @@
 // The batch is walked as a flat array of 16-byte units (unit u lives in batch row u / units_per_row),
 // so short rows (an 8 KB bf16 feature row) fill a CTA pass as well as long ones; every thread keeps
 // kGUnroll independent 16-byte reads in flight — 32 KB per CTA — which is what hides the ~2 us PCIe
-// round trip with only a handful of CTAs (55 GB/s x 2 us = 110 KB in flight for the whole GPU): the
-// fewer SMs this kernel occupies for the ~0.6 ms a batch takes, the less the training step's GEMMs
+// round trip with only a handful of CTAs (tens of GB/s x a few us = ~100 KB in flight for the whole GPU): the
+// fewer SMs this kernel occupies for the time a batch takes, the less the training step's GEMMs
 // running beside it lose.
 #include "frl_common.cuh"
 

@@ -6,9 +6,8 @@
 // (reference solver_worker.py:805-832, transform.py:25-38): here the only per-sample host work is a
 // memcpy of the raw row, done by native threads outside the GIL; the per-sample arithmetic runs on
 // the device afterwards (K5).  Why not let the GPU gather over PCIe (K8)?  It can, and that path
-// stays: but any CTA that sits on an SM for the ~1.3 ms a 67 MB batch needs on PCIe costs the
-// step's cluster-scheduled GEMMs far more than its share of SMs (measured: 4 CTAs -> GEMMs +35 %).
-// The DMA engines cost the SMs nothing.
+// stays: but any CTA that sits on an SM for the milliseconds a 67 MB batch needs on PCIe takes
+// that SM from the step's GEMMs for the whole transfer.  The DMA engines cost the SMs nothing.
 //
 // Jobs are FIFO; a job is split into chunks of rows that workers claim with an atomic counter.
 // Stores to the staging buffer are non-temporal (no read-for-ownership traffic, the CPU never

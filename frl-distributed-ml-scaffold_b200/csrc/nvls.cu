@@ -1,5 +1,5 @@
 // K7 — fused gradient all-reduce + optimizer update + weight broadcast over NVSwitch multicast
-// (NVLS), one kernel per gradient bucket (sm_100a, world_size > 1).
+// (NVLS), one kernel per gradient bucket (sm_90a, world_size > 1).
 //
 // The reference step is "DDP all-reduces every bucket, then torch.optim updates every replica"
 // (reference solver.py:287-289 + solver_worker.py:586-592): every GPU receives the full reduced
@@ -109,9 +109,8 @@ struct NvlsCommon {
 // thread first issues kNRemote of them back to back and only then walks the items, loading the
 // (short-latency) local master/state slices item by item.
 // How many remote loads a thread keeps in flight is a template parameter (FRL_B200_NVLS_INFLIGHT,
-// default 4).  Deeper pipelines (8, 16) were tried to let a small grid cover NVLink's
-// bandwidth-latency product; measured at world 2 (the case with the largest shard per rank) they
-// do not pay: 74 CTAs x depth 4 = 1.170 ms/step, 32 x 8 = 1.190, 74 x 16 = 1.198, 16 x 16 = 1.648.
+// default 4).  Deeper pipelines (8, 16) let a small grid cover more of NVLink's bandwidth-latency
+// product; which depth pays on H100 has not been measured.
 template <typename Rule, int NS, int kNRemote>
 __global__ void __launch_bounds__(kNThreads)
 nvls_update_bf16(float* __restrict__ p_, float* __restrict__ s0_, float* __restrict__ s1_,
@@ -240,7 +239,7 @@ static int launch_nvls(const Rule& rule, float* p, float* s0, float* s1, float* 
         const char* e = getenv("FRL_B200_NVLS_INFLIGHT");
         return e ? atoi(e) : 0;
     }();
-    const int depth = env_depth > 0 ? env_depth : 4;   // measured at world 2: 4 -> 1.170, 8 -> 1.190, 16 -> 1.198 ms/step
+    const int depth = env_depth > 0 ? env_depth : 4;
     // the grid must be identical on every rank: it depends on arguments only
 #define FRL_NV(NR)                                                                                    \
     do {                                                                                              \

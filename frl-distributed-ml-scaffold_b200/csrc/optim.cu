@@ -1,4 +1,4 @@
-// K2 — fused optimizer update over a flat bucket of the parameter arena (sm_100a).
+// K2 — fused optimizer update over a flat bucket of the parameter arena (sm_90a).
 //
 // One streaming pass: read the (already all-reduced) gradient bucket, the fp32 master weights
 // and the optimizer state; apply torch 2.11's update rule in fp32; write master, state and —
@@ -12,7 +12,7 @@
 // Layout: every thread owns 4 consecutive elements per item, so fp32 arrays move as fully
 // coalesced 16-byte accesses (bf16 as 8-byte).  Each thread issues the loads of UNROLL items
 // before the first use (UNROLL * (2 + NSTATE) independent 128-bit loads in flight), which is
-// what keeps ~100 KB per SM outstanding — the amount Little's law asks for at ~6.5 TB/s.
+// what keeps ~100 KB per SM outstanding — more than Little's law asks for at the H100's 3.35 TB/s.
 #include "frl_common.cuh"
 #include "optim_rules.cuh"
 

@@ -1,4 +1,4 @@
-// K5 — device-side batch preprocessing and dtype/scale copies (sm_100a).
+// K5 — device-side batch preprocessing and dtype/scale copies (sm_90a).
 //
 // The reference transforms every sample in Python on the host (reference transform.py:25-38,
 // multitask_problem.py:56-71) and ships fp32 over a pageable copy.  Here the raw bytes are
@@ -23,7 +23,7 @@ template <> __device__ __forceinline__ __nv_bfloat16 from_f32<__nv_bfloat16>(flo
 
 // One ITEM = 16 bytes of source per thread: 4 fp32 / 8 bf16 / 16 u8 elements, converted and stored
 // as one 8-, 16- or 2x16-byte vector.  Every thread issues the loads of kPUnroll items before the
-// first use (64 B in flight per thread, ~128 KB per SM at full occupancy: what ~6.5 TB/s asks for).
+// first use (64 B in flight per thread, ~128 KB per SM at full occupancy: more than 3.35 TB/s asks for).
 // The affine coefficients are resolved per ITEM, not per element: one channel covers the whole
 // item whenever `inner` is a multiple of the item width (images: H*W; flat fields: everything),
 // so the two integer divisions of the channel index are paid once per 16 source bytes and in

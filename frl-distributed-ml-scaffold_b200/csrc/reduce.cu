@@ -1,4 +1,4 @@
-// K3 — one-pass global gradient norm + clip coefficient (sm_100a).
+// K3 — one-pass global gradient norm + clip coefficient (sm_90a).
 //
 // Replaces torch.nn.utils.clip_grad_norm_ (reference solver_worker.py:588-591): a single read
 // of the model range of the gradient arena (4 B/param fp32, 2 B/param bf16).  Warp-shuffle
@@ -11,7 +11,7 @@ namespace frl {
 
 constexpr int kRThreads = 256;
 constexpr int kRUnroll = 4;
-constexpr int kMaxPartials = 148 * 8;   // upper bound on the grid
+constexpr int kMaxPartials = 132 * 8;   // upper bound on the grid (8 CTAs per H100 SM)
 
 struct ReduceScratch {
     float partial[kMaxPartials];

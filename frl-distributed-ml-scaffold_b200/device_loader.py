@@ -2,8 +2,8 @@
 
 The reference feeds the loop through ``DataLoader`` -> per-sample ``__getitem__`` -> Python
 ``MultifieldTransform`` -> ``default_collate`` -> pageable H2D copy (reference
-solver_worker.py:462-469, 805-832; transform.py:25-38): ~0.15 ms of host Python per sample, which
-starves a B200 at batch 4096.  A dataset that exposes
+solver_worker.py:462-469, 805-832; transform.py:25-38): host Python per sample, which starves an
+H100 at batch 4096.  A dataset that exposes
 
     pinned_fields     Dict[str, Tensor]   whole raw dataset, one pinned host tensor per field
     device_transform  DeviceBatchTransform
@@ -25,13 +25,12 @@ Three ways to move the rows (``FRL_B200_INPUT_PATH``):
                     sources that are not pinned (memory-mapped ``.bin`` files), and the only one
                     that can ship bf16 over PCIe (``FRL_B200_INPUT_WIRE=bf16``).
 
-Measured on B200 (round 1): every path reaches PCIe speed (51-55 GB/s, 1.2-1.3 ms for a 67 MB
-batch) when run alone.  Under the training step, CTAs that occupy SMs for that long slow the
-cluster-scheduled GEMMs: the TMA kernel's 128 KB of staging evicts a GEMM CTA per CTA (2.1 ms/step
-end to end), the LSU kernel's CTAs fit beside them (1.53 with 16 CTAs; 1.69 with 8, 1.80 with 32).
-The host path is the fastest on a quiet single-GPU node (1.47) and the most fragile: 3x the
-payload in host DRAM traffic and 16-24 busy threads — 3.8 ms/step with two ranks on a socket, 4.3
-with eight, and 1.7 to 5.5 on a shared host depending on the neighbours.
+Alone, every path is bound by PCIe.  Under the training step, CTAs that occupy SMs for the
+length of a batch transfer slow the GEMMs: the TMA kernel's 128 KB of staging takes an SM from
+the GEMMs per CTA, the LSU kernel's CTAs fit beside them.  The host path costs 3x the payload
+in host DRAM traffic and 16-24 busy threads, so its speed depends on how many ranks share a
+socket and on the neighbours' load.  Which path is fastest on H100 has not been measured; the
+default (``kernel``) is not tuned on H100.
 """
 from collections import deque
 from typing import Dict, Iterator, List, Optional, Tuple
@@ -69,7 +68,7 @@ def randperm_quiet(n: int, generator: torch.Generator) -> torch.Tensor:
     afterwards — with intra-op parallelism off for the call.  The draw itself is serial
     (Fisher-Yates on the generator); only the initial ``arange`` fill is parallel, and waking a
     64-128-thread OpenMP team that went to sleep during the previous epoch costs milliseconds
-    (measured on the GPU box: 0.6 ms with a warm team, 4.9 ms with a cold one, per epoch)."""
+    per epoch."""
     threads = torch.get_num_threads()
     if threads == 1:
         return torch.randperm(n, generator=generator)
@@ -95,15 +94,11 @@ def _local_world() -> int:
 
 
 def default_input_path() -> str:
-    """``kernel`` everywhere: it needs nothing from the host but PCIe reads.  ``host`` is faster by
-    ~5 % when ONE rank has the node's CPUs and DRAM to itself (1.47 vs 1.53 ms/step), but it costs
+    """``kernel`` everywhere (not tuned on H100): it needs nothing from the host but PCIe reads.
+    ``host`` can be faster when ONE rank has the node's CPUs and DRAM to itself, but it costs
     host DRAM 3x the PCIe payload (gather read + staging write + DMA read) and 16-24 busy threads:
-    two ranks on one socket already lose (3.8 ms/step), and on a shared host its speed follows the
-    neighbours' load (same box, same day: 1.70 and 5.5 ms/step through the public loop).
-    Measured, 67 MB fp32 batches, ms/step end to end: 1 x B200 host 1.47 | kernel (16 CTAs) 1.53 |
-    kernel (8) 1.69 | tma (2 CTAs) 2.08 | tma (8) 2.85; 2 x B200 (one socket) host 3.8;
-    4 x B200 host 2.47 | tma 2.03;
-    8 x B200 host 4.3 | tma 2.0 (the box's aggregate H2D rate, ~270 GB/s, is the floor there).
+    several ranks on one socket compete for it, and on a shared host its speed follows the
+    neighbours' load.
     The LSU kernel's CTAs (256 threads, no shared memory) fit beside the GEMM CTAs on an SM; the
     TMA kernel's 128 KB of staging does not, so each of its CTAs takes an SM from the GEMMs."""
     return "kernel"
@@ -226,7 +221,7 @@ class DeviceBatchLoader:
         ``RandomSampler`` takes its permutation seed on the first ``next``.  For the stock
         samplers the permutation stays a tensor: ``randperm(n).tolist()`` plus the per-batch list
         handling is O(n) Python work per epoch, ~60 ns per sample against ~360 ns per sample of
-        B200 step time."""
+        H100 step time."""
         sampler = self.sampler
         perm = None
         if (type(sampler) is torch.utils.data.RandomSampler and not sampler.replacement

@@ -1,6 +1,6 @@
 """Arena optimizers: ``torch.optim``-compatible front, one fused kernel launch per bucket behind.
 
-``create_fused_optimizer`` is the B200 counterpart of the reference's ``_create_optimizer``
+``create_fused_optimizer`` is the H100 counterpart of the reference's ``_create_optimizer``
 (reference solver.py:162-188): same three algorithms, same hyper-parameter mapping
 (``OptimOpts.momentum`` feeds SGD *and* RMSprop, ``epsilon``/``amsgrad`` feed Adam, weight decay
 is L2-coupled and applies to every parameter).  ``state_dict()`` / ``load_state_dict()`` speak
@@ -64,8 +64,8 @@ class FusedArenaOptimizer(torch.optim.Optimizer):
     def refresh_dynamic_scalars(self) -> None:
         """Upload the scalars if they changed: 16 bytes from a ring of pinned rows, so the copy is
         truly asynchronous (a pageable source makes the driver synchronise the stream first,
-        which serialises the host's work for step k+1 with the device's work for step k —
-        measured on Adam, whose bias corrections change every step: 2.4 vs 1.7 ms/step)."""
+        which serialises the host's work for step k+1 with the device's work for step k; Adam's
+        bias corrections change every step)."""
         if self._dyn is None:
             return
         vals = self._dyn_values()

@@ -2,7 +2,7 @@
 
 Stands where the reference wraps the model in ``DistributedDataParallel`` (reference
 solver.py:265-294) and later calls ``clip_grad_norm_`` / ``optimizer.step()`` (reference
-solver_worker.py:585-592).  Differences that matter on B200:
+solver_worker.py:585-592).  Differences that matter on H100:
 
 * ``nn.Linear`` gradients are written straight into the flat ``grad`` arena by ``arena_linear``;
   every other gradient (convolutions, normalisation layers: cuDNN allocates its own output) is
@@ -83,8 +83,8 @@ class GradBucketPipeline:
         self.on_cuda = arena.device.type == "cuda"
         # eager: update a bucket on the side stream as soon as it is complete (and reduced) while
         # backward is still running.  Needs no global norm, so clipping turns it off.  On one GPU
-        # the caller decides (measured on B200: the persistent cuBLAS GEMMs leave the update no
-        # SMs to overlap on, so a single tail launch is faster and cheaper to issue).
+        # the caller decides (the persistent cuBLAS GEMMs leave the update few SMs to overlap on,
+        # so a single tail launch is cheaper to issue).
         self.eager = eager_update and self.clip_norm == 0.0 and (self.distributed or self.on_cuda)
 
         cap = int(bucket_cap_mb * 1024 * 1024)
@@ -108,9 +108,9 @@ class GradBucketPipeline:
         # launch ranges define which rank owns which shard of the master weights and state.
         self._row_split: Dict[int, int] = {}            # slot.index -> rows in the first half
         min_bytes = int(os.environ.get("FRL_B200_TAIL_SPLIT_MIN_BYTES", str(4 << 20)))
-        # measured (MLP, 24 MiB buckets): 2 GPUs 1.167 -> 1.141 ms/step; 8 GPUs 1.019 -> 1.032 (p50):
-        # there a half-bucket exchange is mostly its two cross-GPU barriers, and one more launch
-        # costs more than the exposed half saves -> on by default at world 2 only
+        # at larger worlds a half-bucket exchange is mostly its two cross-GPU barriers, and one
+        # more launch can cost more than the exposed half saves -> on by default at world 2 only
+        # (not tuned on H100)
         want_split = os.environ.get("FRL_B200_TAIL_SPLIT", "1" if world_size == 2 else "0") != "0"
         if self.distributed and self.eager and ranges and want_split:
             lo, hi = ranges[-1]

@@ -1,8 +1,8 @@
 """CUDA-graph replay of the training step.
 
 The reference's minibatch is ~60 kernel launches issued from Python (forward, T loss modules,
-autograd, DDP hooks, optimizer); on a B200 the GPU finishes them in ~1.3 ms, about as long as
-one CPU core needs to issue them, and with per-bucket collectives the host becomes the
+autograd, DDP hooks, optimizer); on an H100 the GPU finishes them in about the time one CPU
+core needs to issue them, and with per-bucket collectives the host becomes the
 bottleneck.  Shapes are static from step to step, so after a few eager steps the whole
 sequence — input cast, model forward, fused criterion, backward with gradients landing in the
 arena, per-bucket NCCL all-reduce and fused update on the side stream — is captured once into a

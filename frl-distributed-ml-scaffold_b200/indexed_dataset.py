@@ -14,7 +14,7 @@ reference's writer stores ``magic = version = 0`` (dataset.py:618-619) and its r
 neither (dataset.py:567-568): both are preserved.  Like the reference's reader, this one assumes
 every frame has the shape of frame 0 (dataset.py:586-594).
 
-What is added for the B200 path: a fixed-shape indexed file IS a row-major ``[N, framesize]``
+What is added for the H100 path: a fixed-shape indexed file IS a row-major ``[N, framesize]``
 array, so ``MultifieldIndexedDataset.host_fields`` exposes the memory-mapped ``.bin`` files as
 zero-copy CPU tensors and the batched input path (``DeviceBatchLoader``, ``host`` mode) lets the
 native gather pool copy a minibatch's frames from the page cache straight into pinned staging —
@@ -118,7 +118,7 @@ class PosixIndexedDatasetReader(IndexedDatasetReader):
         del state["data"]
         return state
 
-    # ---- batched access (B200 path) -------------------------------------------------------------
+    # ---- batched access (H100 path) -------------------------------------------------------------
     def frames_tensor(self) -> torch.Tensor:
         """The whole ``.bin`` file as a zero-copy CPU tensor ``[N, *frame shape]`` over the page
         cache.  Requires every frame to have frame 0's shape and the file to hold N frames."""

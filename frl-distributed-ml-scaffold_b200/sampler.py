@@ -38,8 +38,8 @@ class ScaffoldSampler(torch.utils.data.distributed.DistributedSampler):
         self._node_idx = node_idx
         self._node_count = node_count
         # the global permutation of an epoch depends on the epoch NUMBER only, and every rank needs
-        # the whole of it: at 8 ranks x 4096 samples x 20 steps that is 655 360 draws = 18 ms of
-        # serial Fisher-Yates per rank per epoch.  The next epoch's permutation is therefore drawn
+        # the whole of it: at 8 ranks x 4096 samples x 20 steps that is 655 360 draws of serial
+        # Fisher-Yates per rank per epoch.  The next epoch's permutation is therefore drawn
         # on a helper thread while this epoch trains (same generator seed, same values).
         self._perm_ready: Dict[int, torch.Tensor] = {}
         self._perm_thread: Optional[threading.Thread] = None

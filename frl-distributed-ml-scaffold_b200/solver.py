@@ -262,7 +262,7 @@ class Solver:
         """Everything `_run_solver_worker` sets up, returned instead of run (bench/tests)."""
         run_opts, problem = args.run_opts, args.problem
         if args.run_device != Device.GPU:
-            raise RuntimeError("frl_b200 has no CPU path: a CUDA (sm_100a) device is required")
+            raise RuntimeError("frl_b200 has no CPU path: a CUDA (sm_90a) device is required")
         torch.cuda.set_device(args.local_rank)
         device = torch.device("cuda", args.local_rank)
         if args.world_size > 1 and os.environ.get("FRL_B200_NUMA_BIND", "1") != "0":
@@ -317,13 +317,11 @@ class Solver:
             from .symm import make_link
             # grid of the fused NVLS step: each rank streams 1/world of a bucket, and every CTA it
             # parks on an SM while backward runs costs the cluster-scheduled GEMMs a wave, so the
-            # grid shrinks with the world size.  Measured, ms/step with 24 MiB buckets:
-            #   8 x B200: 16 CTAs 1.12 | 32: 1.17 | 74: 1.25 | 148: 1.40
-            #   4 x B200:  8 CTAs 1.42 | 16: 1.16 | 37: 1.17 | 74: 1.25
-            #   2 x B200: 32 CTAs 1.48 | 74: 1.26 | 148: 1.31   (half of every bucket per rank)
-            default_blocks = 74 if args.world_size <= 2 else 16
+            # grid shrinks with the world size: half the H100's 132 SMs at 2 GPUs (half of every
+            # bucket per rank), 16 CTAs from 4 GPUs on.  Not yet tuned on a multi-GPU H100 box.
+            default_blocks = 66 if args.world_size <= 2 else 16
             # the launch for the bucket that becomes ready last runs alone (backward has ended), so it
-            # gets a wider grid: 4 x B200, 16 -> 64 CTAs for that launch only: 1.109 -> 1.074 ms/step
+            # gets a wider grid
             default_tail = 64 if args.world_size >= 4 else 0
             nvls_link = make_link(symm_alloc, arena.grad,
                                   arena.lp if arena.lp is not None else arena.master,
@@ -587,7 +585,7 @@ class Solver:
         n_visible = 0 if run_opts.cpuonly else _cuda_device_count_without_poisoning_fork()
         if n_visible == 0:
             raise RuntimeError(
-                "frl_b200 runs the training step on B200 GPUs only (cpuonly=%s, visible CUDA "
+                "frl_b200 runs the training step on H100 GPUs only (cpuonly=%s, visible CUDA "
                 "devices=%d); there is no CPU path" % (run_opts.cpuonly, n_visible))
         run_device = Device.GPU
         if run_opts.singleThreaded:

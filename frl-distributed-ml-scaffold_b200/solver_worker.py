@@ -174,7 +174,7 @@ class _MetricWorker:
     metrics.  The Problem's ``compute_batch_metrics`` hook returns host arrays, i.e. it ends in a
     device-to-host read; called from the training thread (as the reference does every
     ``metricAmortizationSchedule`` steps, solver_worker.py:286-312) that read drains the whole
-    launch pipeline — about one step of idle GPU per window at B200 step times.  Here the read
+    launch pipeline — about one step of idle GPU per window at H100 step times.  Here the read
     blocks only this thread; jobs run FIFO, so per-sample metrics keep their order."""
 
     def __init__(self, device: torch.device) -> None:
@@ -376,7 +376,7 @@ class SamplerState:
                         int(i), data_batches, starts, target, output, meta, sample_metric)))
         self._cur_samples += n_group
 
-    # -- device-side fold (SURVEY §8 f1) ----------------------------------------------------------
+    # -- device-side fold -----------------------------------------------------------------------
     # The Problem's hook returned per-sample metrics as DEVICE tensors: they go into
     # [n_samples] device columns, the random picks are row-gathered by host-known positions, the
     # worst-k set is kept as running device buffers merged per window with ``topk`` — no
@@ -439,7 +439,7 @@ class SamplerState:
         picks = sorted(j - base for j in self._random_indices if base <= j < base + n_group)
         if picks:
             # a few int64s from pageable memory: the driver stages them, the host does not wait
-            # for the device (a pinned allocation here would cost a ~0.5 ms system call)
+            # for the device (a pinned allocation here would cost a system call)
             idx = torch.tensor(picks, dtype=torch.int64, device=dev)
             self._dev_random.append(self._pick(idx, data_batches, starts, target, output, meta, sample_metric))
         # worst-k of this window, merged into the running set: all on the device
@@ -479,8 +479,8 @@ class SamplerState:
         def flush() -> List[torch.Tensor]:
             # everything is packed into ONE device buffer (a single concatenation launch) and moved
             # by ONE copy into ONE pinned staging block, then carved into aligned views: a pinned
-            # allocation per tensor is a ~0.3 ms system call, and even the 22 separate
-            # device-to-host copies of an MLP split cost the host 1 ms to issue
+            # allocation per tensor is a system call, and even the 22 separate
+            # device-to-host copies of an MLP split cost the host time to issue
             parts, offs, total = [], [], 0
             pad = None
             for t in requests:
@@ -546,9 +546,8 @@ class SamplerState:
         def own(t: torch.Tensor) -> torch.Tensor:
             # a pageable copy out of the staging block by plain memcpy.  ``clone()``/``copy_`` of a
             # CPU tensor above ATen's grain size (32 768 elements) is an OpenMP parallel region:
-            # waking a 128-thread pool that sleeps between epochs was measured at 4-6 ms PER CALL
-            # (13 calls = 58-76 ms per ResNet epoch); numpy's copy is single-threaded and takes
-            # 0.15 ms for a 600 KB image
+            # waking a 128-thread pool that sleeps between epochs costs milliseconds PER CALL;
+            # numpy's copy is single-threaded
             return torch.from_numpy(t.numpy().copy())
 
         cols = {k: v.numpy().copy() for k, v in cols_h.items()}
@@ -617,7 +616,7 @@ def _planned_order(sampler, accessor) -> List[int]:
     RNG: a stock ``RandomSampler`` draws one int64 seed and shuffles with a private generator, a
     ``ScaffoldSampler`` seeds a private generator with the epoch.  Materialising the order is
     O(len(dataset)) Python objects per split per epoch, comparable to the epoch's whole step
-    time on a B200."""
+    time on an H100."""
     if isinstance(accessor, NullAccessor):
         if (type(sampler) is torch.utils.data.RandomSampler and not sampler.replacement
                 and sampler.generator is None and sampler._num_samples is None):
@@ -636,7 +635,7 @@ def _pinned_block(nbytes: int) -> torch.Tensor:
     have = _PINNED_BLOCKS.get(0)
     if have is None or have.numel() < nbytes:
         # twice what is asked for: the payload varies from split to split with the number of random
-        # picks, and every regrowth is a cudaHostAlloc — 22 ms with eight ranks page-locking at once
+        # picks, and every regrowth is a cudaHostAlloc, slow with several ranks page-locking at once
         have = _PINNED_BLOCKS[0] = torch.empty(max(2 * nbytes, 4 << 20), dtype=torch.uint8, pin_memory=True)
     return have
 
@@ -721,8 +720,8 @@ class SolverWorker:
         if not getattr(self, "_gc_frozen", False) and os.environ.get("FRL_B200_GC_IN_LOOP", "0") == "0":
             # everything alive now (model, optimizer, arena, datasets, loaders) lives as long as the
             # run: move it to the permanent generation so the collections that follow every
-            # minibatch loop traverse only what an epoch created (measured: the collection at the
-            # loop's end took 3.5 ms for the MLP Problem and ~60 ms for the ResNet-18 one)
+            # minibatch loop traverse only what an epoch created (the collection at the loop's end
+            # is milliseconds, more for the ResNet Problems)
             import gc
             gc.collect()
             gc.freeze()
@@ -759,9 +758,9 @@ class SolverWorker:
             mark("setup done")
 
             # The cyclic garbage collector stays out of the minibatch loop: a generation-2 pass over
-            # a process holding a model, an optimizer and a loader takes 5-10 ms — a handful of B200
-            # steps — and fires wherever the allocation counter happens to trip (measured: the first
-            # batch of an epoch served 1 to 13 ms late).  A step leaves no reference cycles behind
+            # a process holding a model, an optimizer and a loader takes milliseconds — several
+            # steps — and fires wherever the allocation counter happens to trip (the first batch of
+            # an epoch is then served late).  A step leaves no reference cycles behind
             # (its autograd graph is dropped explicitly below); FRL_B200_GC_IN_LOOP=1 keeps the
             # collector on for Problems whose hooks do.
             with StepWatchdog(self.run_opts.minibatchTimeoutMs) as dog, sampler_state, _gc_paused():
@@ -1081,7 +1080,7 @@ class SolverWorker:
                 logger.warning(
                     "input path for split %s: per-sample DataLoader (__getitem__ + Python transform + "
                     "collate, as the reference) — the dataset does not expose `pinned_fields` + a "
-                    "`device_transform` (transform.DeviceBatchTransform), so the host, not the B200, "
+                    "`device_transform` (transform.DeviceBatchTransform), so the host, not the GPU, "
                     "sets the step rate at large batches", split.value)
             loaders[split] = torch.utils.data.DataLoader(
                 dataset, batch_size=batchSize, shuffle=sampler is None,

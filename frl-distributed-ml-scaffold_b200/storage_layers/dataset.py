@@ -1,7 +1,7 @@
 """Dataset protocol seen by the training loop (reference storage_layers/dataset.py:493-518).
 
 Only the protocol is on the hot path.  The reference's shared-memory frame cache and the
-.idx/.bin reader are storage-engine components (SURVEY §8 marks them out of scope / "next");
+.idx/.bin reader are storage-engine components (out of scope here);
 ``NullAccessor`` stands where the loop hands a cache accessor to the dataset
 (reference solver_worker.py:431-432) — for POSIX and synthetic datasets that call is a no-op
 in the reference too (reference posix_storage.py:76-80).

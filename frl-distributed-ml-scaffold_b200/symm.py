@@ -87,7 +87,7 @@ def make_link(alloc: SymmetricAllocator, grad: torch.Tensor, out: torch.Tensor,
     link.mc_grad, link.mc_out = hg.multicast_ptr, ho.multicast_ptr
     link.grad_esz, link.out_esz = grad.element_size(), out.element_size()
     link.handles = [hg, ho]
-    # barriers inside the update kernel (default: measured best with the small grids used) or as
+    # barriers inside the update kernel (default; not tuned on H100) or as
     # separate 1-CTA launches (wins when the grid is large and ranks arrive skewed)
     link.flags = 1 if os.environ.get("FRL_B200_NVLS_SPLIT_SYNC", "0") != "0" else 0
     if link.mc_grad == 0 or link.mc_out == 0:

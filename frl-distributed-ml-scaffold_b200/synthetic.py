@@ -1,6 +1,6 @@
 """Synthetic multitask Problems used by the parity tests and the benchmark.
 
-The reference ships no concrete ``Problem`` (SURVEY §4), so the configurations BASELINE.json
+The reference ships no concrete ``Problem``, so the configurations BASELINE.json
 names are defined here, written purely against the plugin API.  Every builder takes the API
 namespace as an argument: pass ``frl_b200`` to run on this package, or the reference imported
 as ``frldistml.scaffold`` (oracle only) to run the very same Problem on the reference Solver.
@@ -137,7 +137,7 @@ def _channel_affine_device_transform(scale, bias, target_fields):
 
 def _pinned_dataset_class(ns):
     """ArrayDataset whose fields also exist as pinned host tensors + a batched device transform
-    (the B200 input path); the per-sample path stays available and equivalent."""
+    (the H100 input path); the per-sample path stays available and equivalent."""
     import torch
     Base = _array_dataset_class(ns)
 
@@ -349,7 +349,7 @@ def synthetic_fields(n: int, in_dim: int, reg_dim: int, n_classes: int, seed: in
 def make_toy_problem(ns, save_dir: str, n_train: int = 512, n_test: int = 128,
                      criterion_kind: str = "parallel", pinned: bool = False,
                      indexed_dir: Optional[str] = None):
-    """Config 1 (SURVEY §8d): trunk 64->128->128, reg head 128->4 (w 0.5), cls head 128->10 (w 2)."""
+    """Config 1: trunk 64->128->128, reg head 128->4 (w 0.5), cls head 128->10 (w 2)."""
     Reg, Cls = _task_classes(ns)
     tasks = [Reg(128, 4, 0.5), Cls(128, 10, 2.0)]
     fields = [(ns.Split.TRAIN, synthetic_fields(n_train, 64, 4, 10, 0, True)),
@@ -415,7 +415,7 @@ def resnet_fields(n: int, image: int, heads, seed: int, uint8: bool = False) -> 
 def make_resnet_problem(ns, save_dir: str, config: str = "resnet18", image: int = 224,
                         n_train: int = 64, n_test: int = 0, pinned: bool = False,
                         uint8: bool = False):
-    """Configs 4/5 (SURVEY §8d): a torchvision ResNet trunk (its ``fc`` removed) behind
+    """Configs 4/5: a torchvision ResNet trunk (its ``fc`` removed) behind
     ``ListSelect`` and one ``nn.Linear`` head per task; x ~ N(0,1) of shape [3, image, image], or
     (``uint8``) raw 8-bit images normalised per channel by the transform (150 kB/sample over
     PCIe instead of 602 kB)."""

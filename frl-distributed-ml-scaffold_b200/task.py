@@ -1,7 +1,7 @@
 """One task of a multitask problem: head, loss, targets, metrics (reference task.py:34-80).
 
 The abstract surface is the reference's, member for member; the docstrings say when and where
-the B200 loop calls each member, which is what a Task author needs to know to stay on the fast
+the H100 loop calls each member, which is what a Task author needs to know to stay on the fast
 path.
 """
 from abc import abstractmethod

@@ -2,7 +2,7 @@
 
 ``MultifieldTransform`` is the reference contract: a raw record (dict of ndarrays) becomes
 ``(Sample(data, target), meta)`` and ``__call__`` flattens that to the triple the DataLoader
-collates.  ``DeviceBatchTransform`` is the B200 addition: the same arithmetic applied to a
+collates.  ``DeviceBatchTransform`` is the H100 addition: the same arithmetic applied to a
 whole batch after the raw bytes reached HBM, through the ``frl_preproc_affine`` kernel.
 """
 from abc import ABC, abstractmethod

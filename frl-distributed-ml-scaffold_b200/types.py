@@ -75,7 +75,7 @@ class LRSchedulerOpts(NamedTuple):
 
 
 class OptimOpts(NamedTuple):
-    """Optimizer options (reference types.py:85-93).  How the B200 step consumes them:
+    """Optimizer options (reference types.py:85-93).  How the H100 step consumes them:
 
     algo          which fused update rule K2/K7 applies (``frl_sgd_momentum`` / ``frl_adam`` /
                   ``frl_rmsprop``); anything else raises ``ValueError`` like the reference
@@ -102,7 +102,7 @@ class OptimOpts(NamedTuple):
 
 class RunOpts(NamedTuple):
     """Run options (reference types.py:102-121).  Field names, order and defaults are the
-    reference's; what each means on the B200 path:
+    reference's; what each means on the H100 path:
 
     batchSize                   minibatch PER RANK (weak scaling, as DDP in the reference)
     cpuonly                     must stay False: there is no CPU path, ``Solver.solve`` raises

@@ -1,5 +1,5 @@
 /*
- * frl_b200.h — C ABI of the B200 (sm_100a) data-parallel training-step kernels.
+ * frl_b200.h — C ABI of the H100 (sm_90a) data-parallel training-step kernels.
  *
  * The reference (facebookresearch/FRL-Distributed-ML-Scaffold) has no native boundary of its
  * own: its step arithmetic runs inside PyTorch.  Each entry point below replaces the PyTorch

@@ -31,7 +31,13 @@ from oracle.ref_shim import import_reference     # noqa: E402
 
 CONFIGS = {
     # name: (algo, lr, scheduler, nEpochs, clip, amsgrad, criterion_kind)
-    "toy_sgd": ("sgd", 0.01, "drop", 2, 0.0, False, "parallel"),
+    # lr 0.008, not 0.01: at 0.01 a trunk pre-activation of the second epoch is 7e-9 against terms
+    # summing to 0.79 in magnitude (1e-8 relative, below fp32 resolution), so its ReLU decision,
+    # and with it 32 first-layer weights, depends on the summation order of the GEMM.  The
+    # smallest one left (shared by every toy configuration: the first forward, trunk layer 2,
+    # sample 55, unit 8) is 8.9e-8 against 0.79, about one fp32 ulp of the sum: a future
+    # divergence confined to one trunk unit should be looked for there first
+    "toy_sgd": ("sgd", 0.008, "drop", 2, 0.0, False, "parallel"),
     "toy_adam_clip": ("adam", 0.003, "multistep", 3, 1.0, False, "parallel"),
     "toy_adam_amsgrad": ("adam", 0.003, "drop", 2, 0.0, True, "parallel"),
     "toy_rmsprop": ("rmsprop", 0.0005, "drop", 2, 0.0, False, "parallel"),

@@ -1,7 +1,7 @@
 """TEST INFRASTRUCTURE — CPU restatement of the reference's per-rank training loop.
 
 Plain PyTorch on the CPU, no import from the product package.  It restates, citing the
-reference line by line, exactly the part of the reference the B200 path replaces:
+reference line by line, exactly the part of the reference the H100 path replaces:
 
     _create_optimizer            solver.py:162-188      -> make_optimizer
     create_lr_scheduler + get_lr solver.py:191-218, lr_scheduler.py:29-33, 65-78 -> lr_at_epoch

@@ -1,12 +1,12 @@
 """Import the UNMODIFIED reference as the package ``frldistml.scaffold``.
 
-TEST INFRASTRUCTURE.  Source: ``/root/reference`` where it exists (the build container), else the
-archive ``oracle/build_ref.py`` packed into the git-ignored ``oracle/_ref/reference.zip`` (which
-travels to the GPU box); used by ``oracle/make_golden.py`` to generate the committed fixtures, by
-the ``-m reference`` tests that pin ``oracle/ref_loop.py`` against the live reference and by the
-CPU arm of ``bench.py``.
+TEST INFRASTRUCTURE.  Source: the reference checkout at ``REFERENCE_DIR`` where it exists, else
+the archive ``oracle/build_ref.py`` packed into the git-ignored ``oracle/_ref/reference.zip``;
+used by ``oracle/make_golden.py`` to generate the committed fixtures, by ``oracle/live_golden.py``
+(the reference side of the tests that compare against it, live where it is importable) and by
+the CPU arm of ``bench.py``.
 
-What the shim does (SURVEY §8c), without touching the reference tree:
+What the shim does, without touching the reference tree:
   * a temp dir with ``frldistml/__init__.py`` and a symlink ``frldistml/scaffold -> /root/reference``
     (the reference uses relative imports and its tests use that package name);
   * ``sys.modules`` stubs for two absent visualisation deps: ``plotly.graph_objs`` (types.py:20)

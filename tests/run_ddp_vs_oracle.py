@@ -3,7 +3,7 @@ or by hand:  torchrun --nproc-per-node 2 tests/run_ddp_vs_oracle.py).
 
 N ranks train the toy 2-task model with the real kernels + NCCL bucket all-reduce on their
 share of every batch; rank 0 then checks the weights against the single-process CPU oracle fed
-the concatenated batch (SURVEY §8c: mean of per-rank mean losses == global mean for MSE/CE with
+the concatenated batch (mean of per-rank mean losses == global mean for MSE/CE with
 equal per-rank batch)."""
 import os
 import sys

@@ -13,13 +13,14 @@ import torch  # noqa: E402
 import frl_b200  # noqa: E402,F401
 from frl_b200 import synthetic  # noqa: E402
 from frl_b200.local_solver import LocalSolver  # noqa: E402
+from oracle.make_golden import CONFIGS  # noqa: E402
 
 
 def main(save_dir: str) -> None:
     ns = synthetic.api_namespace("frl_b200")
     t = ns.types
     n_gpu = torch.cuda.device_count()
-    run_opts = t.RunOpts(optim=t.OptimOpts(algo=t.OptAlgorithm.SGD, lr=0.01), batchSize=64,
+    run_opts = t.RunOpts(optim=t.OptimOpts(algo=t.OptAlgorithm.SGD, lr=CONFIGS["toy_sgd"][1]), batchSize=64,
                          nEpochs=2, numThreads=0, numVisualizedSamples=4)
     torch.manual_seed(0)
     problem = synthetic.make_toy_problem(ns, save_dir)

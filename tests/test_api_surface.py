@@ -1,5 +1,5 @@
-"""The plugin API keeps the reference's names, signatures, defaults and error behaviour
-(SURVEY §8b); includes the reference's own unit tests for this path, restated."""
+"""The plugin API keeps the reference's names, signatures, defaults and error behaviour;
+includes the reference's own unit tests for this path, restated."""
 import inspect
 import json
 import os

@@ -10,7 +10,7 @@ agreed to 1e-6).  That is a property of ReLU in fp32 on any two devices (the ref
 GPU-vs-CPU comparison included), not of this path; the batch keeps the expected number of such
 units well below one for the fixed seed.
 
-Both sides build the model from the same seed and train on the same batches; the B200 side goes
+Both sides build the model from the same seed and train on the same batches; the H100 side goes
 through ``Solver.build_worker`` + ``SolverWorker._pass_one_minibatch`` — the call ``bench.py``
 times — with every switch of the benchmarked configuration: arena-born Linear gradients,
 fused Linear+ReLU units, fused criterion, fused update, CUDA-graph replay on and off.
@@ -117,7 +117,7 @@ _STOCK = {}
 
 def _stock_gpu_first_grads():
     """First-step gradients of the plain module in stock fp32 torch on cuda:0 (same seed, same
-    batch, TF32 off): the same GEMM library and rounding as the B200 path's contractions, so what
+    batch, TF32 off): the same GEMM library and rounding as the H100 path's contractions, so what
     separates the two is this repo's criterion / ReLU-backward / bias-gradient kernels only."""
     if "g" not in _STOCK:
         torch.backends.cuda.matmul.allow_tf32 = False
@@ -175,7 +175,7 @@ def test_mlp_config_matches_oracle_fp32(algo, graph, monkeypatch):
         assert a[2] <= 1e-5, ("vs stock torch on the same GPU", shape, a)
         assert b[0] <= 1e-5 and b[3] <= 5e-2, ("vs the CPU oracle", shape, b)
     # six steps of weights vs the CPU oracle: SGD moves by lr*g; Adam turns last-bit gradient
-    # differences into visible fractions of lr where v is tiny (DESIGN §6: final weights are
+    # differences into visible fractions of lr where v is tiny (final weights are
     # outside the 1e-5 claim)
     for a, b in zip(final, want_final):
         med = float((a - b).abs().flatten()[: 1 << 24].median())

@@ -37,9 +37,14 @@ pytestmark = pytest.mark.gpu
 SEED = 3
 
 CASES = {
-    # config, algo, lr, image, batch, n_train, epochs, param count (SURVEY §8)
+    # config, algo, lr, image, batch, n_train, epochs, param count
     "resnet18_sgd": ("resnet18", "sgd", 0.01, 64, 8, 16, 1, 11_689_512),
-    "resnet50x4_adam": ("resnet50x4", "adam", 1e-4, 64, 8, 16, 1, 25_790_618),
+    # Adam lr 2e-5: its first step moves every weight by about lr * sign(g), so the step-2 loss
+    # carries rounding noise in proportion to lr.  At lr 1e-4, on an H100 80GB HBM3 (700 W), the
+    # step-2 loss of the last task was 1.4391 with cuDNN autotuning and 1.4183 without it (1.45 %
+    # apart), against 1.4420 from the CPU oracle: the run-to-run spread alone exceeded the 1 %
+    # bound below
+    "resnet50x4_adam": ("resnet50x4", "adam", 2e-5, 64, 8, 16, 1, 25_790_618),
 }
 
 

@@ -1,4 +1,4 @@
-"""End-to-end parity of the B200 training step against the reference's CPU Solver.
+"""End-to-end parity of the H100 training step against the reference's CPU Solver.
 
 The golden files hold what the UNMODIFIED reference produced on the toy 2-task Problem
 (per-step losses of every split, learning rates, served sample order, first gradients, final
@@ -227,7 +227,7 @@ def test_device_batch_loader_path_matches_reference_solver(ns, golden_dir, monke
 
 
 def test_indexed_files_feed_the_loop_through_the_host_pool(ns, golden_dir, monkeypatch, tmp_path):
-    """SURVEY §8f row 4: the toy Problem's datasets written as .idx/.bin files (this repo's writer,
+    """The toy Problem's datasets written as .idx/.bin files (this repo's writer,
     byte-identical to the reference's) and served from the memory-mapped files — the host gather
     pool copies each minibatch's frames from the page cache into pinned staging, one DMA per field,
     transform on the device.  Same samples in the same order => the golden per-step losses."""
@@ -334,7 +334,7 @@ def test_fused_linear_relu_units_keep_reference_parity(ns, golden_dir, monkeypat
 
 @pytest.mark.parametrize("config", ["err_MSE_DESC", "score_ASC", "score_DESC"])
 def test_device_side_sampler_state_matches_reference_fixture(golden_dir, config):
-    """SURVEY §8 f1: the Problem's hook returns DEVICE tensors; per-sample metrics stay in HBM
+    """The Problem's hook returns DEVICE tensors; per-sample metrics stay in HBM
     columns, the worst-k set is a running device buffer merged with topk per window, everything is
     read back once at the end of the split.  Same fixtures as the host path: the reference's own
     SamplerState on the same scenario (oracle/make_sampler_state_golden.py)."""

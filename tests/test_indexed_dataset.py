@@ -1,4 +1,4 @@
-"""``.idx`` / ``.bin`` indexed datasets (SURVEY §8f row 4): the on-disk format that feeds the loop.
+"""``.idx`` / ``.bin`` indexed datasets: the on-disk format that feeds the loop.
 
 * golden files written by the UNMODIFIED reference's writer (oracle/make_indexed_golden.py) are
   read back frame by frame and compared with what the reference's own reader returned for them
@@ -6,7 +6,8 @@
 * the reference's own tests for this path (tests/test_indexed_dataset.py: header synthesised by
   hand with magic 0 / version 1, write->read round trip, reader survives pickling into another
   process) are restated against this repo's classes;
-* with /root/reference present, writer and reader are compared live on random frames;
+* writer and reader are compared with the reference's on random frames (live where the reference
+  is present, else its recorded side under tests/golden/live);
 * the batched path: ``host_fields`` (zero-copy [N, ...] tensors over the mapped .bin) gathered by
   the native host pool equals per-sample ``__getitem__`` + stacking.
 """
@@ -26,6 +27,7 @@ import torch
 import frl_b200  # noqa: F401
 from frl_b200 import _native
 from frl_b200 import indexed_dataset as idm
+from oracle.live_golden import plain, reference_side
 from oracle.make_indexed_golden import FILES, frames_of
 
 GOLD = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden", "indexed")
@@ -161,37 +163,60 @@ def test_malformed_index_files_are_rejected(tmp_path):
         r._init_from_index_data(bad)
 
 
-# ---- live comparison with the reference (build container only) -------------------------------------
+# ---- comparison with the reference ----------------------------------------------------------------
 
-@pytest.mark.reference
 def test_writer_and_reader_match_the_live_reference(tmp_path):
-    from oracle.ref_shim import import_reference
-    import_reference()
-    from frldistml.scaffold.storage import StoragePath
-    from frldistml.scaffold.storage_layers.dataset import IndexedDatasetWriter as RefWriter
-    from frldistml.scaffold.storage_layers.posix_storage import PosixIndexedDatasetReader as RefReader
     rs = np.random.RandomState(7)
+    cases = []
     for dt, shape, n in [("float32", (3, 4), 5), ("uint8", (2, 3, 5), 7), ("int64", (), 4),
                          ("float64", (128,), 3), ("int16", (1,), 1), ("int8", (4, 1, 2), 9),
                          ("int32", (17,), 33)]:
-        frames = [np.asarray(rs.randn(*shape) * 50).astype(dt) for _ in range(n)]
-        mine_i, mine_b, ref_i, ref_b = io.BytesIO(), io.BytesIO(), io.BytesIO(), io.BytesIO()
-        w, rw = idm.IndexedDatasetWriter(idxfile=mine_i, binfile=mine_b), RefWriter(idxfile=ref_i, binfile=ref_b)
+        cases.append((dt, shape, [np.asarray(rs.randn(*shape) * 50).astype(dt) for _ in range(n)]))
+    idx, binf = str(tmp_path / "x.idx"), str(tmp_path / "x.bin")
+
+    def as_bytes(t):
+        return t.numpy().tobytes()
+
+    def reference():
+        from oracle.ref_shim import import_reference
+        import_reference()
+        from frldistml.scaffold.storage import StoragePath
+        from frldistml.scaffold.storage_layers.dataset import IndexedDatasetWriter as RefWriter
+        from frldistml.scaffold.storage_layers.posix_storage import PosixIndexedDatasetReader as RefReader
+        out = []
+        for _, _, frames in cases:
+            ref_i, ref_b = io.BytesIO(), io.BytesIO()
+            rw = RefWriter(idxfile=ref_i, binfile=ref_b)
+            for f in frames:
+                rw.push_back(f)
+            rw.flush()
+            open(idx, "wb").write(ref_i.getvalue())
+            open(binf, "wb").write(ref_b.getvalue())
+            ref = RefReader(idxfile=StoragePath(idx), binfile=StoragePath(binf))
+            out.append({"idx": torch.frombuffer(bytearray(ref_i.getvalue()), dtype=torch.uint8),
+                        "bin": torch.frombuffer(bytearray(ref_b.getvalue()), dtype=torch.uint8),
+                        "len": len(ref), "framesize": int(ref.framesize), "dtype": str(np.dtype(ref.dtype)),
+                        "frames": [plain(np.asarray(ref[i])) for i in range(len(ref))],
+                        "frame_dtypes": [str(np.asarray(ref[i]).dtype) for i in range(len(ref))]})
+        return out
+
+    recorded, _ = reference_side("indexed_writer_reader", reference)
+    for (dt, shape, frames), ref in zip(cases, recorded):
+        mine_i, mine_b = io.BytesIO(), io.BytesIO()
+        w = idm.IndexedDatasetWriter(idxfile=mine_i, binfile=mine_b)
         for f in frames:
             w.push_back(f)
-            rw.push_back(f)
         w.flush()
-        rw.flush()
-        assert mine_i.getvalue() == ref_i.getvalue() and mine_b.getvalue() == ref_b.getvalue(), (dt, shape)
-        idx, binf = str(tmp_path / "x.idx"), str(tmp_path / "x.bin")
-        open(idx, "wb").write(ref_i.getvalue())
-        open(binf, "wb").write(ref_b.getvalue())
+        assert mine_i.getvalue() == as_bytes(ref["idx"]) and mine_b.getvalue() == as_bytes(ref["bin"]), (dt, shape)
+        open(idx, "wb").write(as_bytes(ref["idx"]))
+        open(binf, "wb").write(as_bytes(ref["bin"]))
         mine = idm.PosixIndexedDatasetReader(idxfile=idx, binfile=binf)
-        ref = RefReader(idxfile=StoragePath(idx), binfile=StoragePath(binf))
-        assert len(mine) == len(ref) and mine.framesize == ref.framesize and mine.dtype == ref.dtype
-        for i in range(n):
-            a, b = mine[i], ref[i]
-            assert a.dtype == b.dtype and a.shape == b.shape and np.array_equal(a, b)
+        assert len(mine) == ref["len"] and mine.framesize == ref["framesize"]
+        assert str(np.dtype(mine.dtype)) == ref["dtype"]
+        for i in range(len(frames)):
+            a, b = mine[i], ref["frames"][i]
+            assert str(a.dtype) == ref["frame_dtypes"][i] and tuple(a.shape) == tuple(b.shape)
+            assert torch.equal(plain(np.asarray(a)), b)
 
 
 # ---- batched access: mapped .bin -> native host pool ---------------------------------------------
@@ -231,13 +256,7 @@ def test_batched_access_refuses_ragged_files(tmp_path):
 
 # ---- Concat / Subset containers over indexed datasets (reference dataset.py:518-552) ---------------
 
-@pytest.mark.reference
 def test_concat_and_subset_containers_match_the_live_reference(tmp_path):
-    from oracle.ref_shim import import_reference
-    import_reference()
-    import frldistml.scaffold.storage_layers.dataset as ref_ds
-    from frldistml.scaffold.indexed_dataset import MultifieldIndexedDataset as RefMulti
-    from frldistml.scaffold.storage import StoragePath
     import frl_b200.storage_layers.dataset as my_ds
     rs = np.random.RandomState(9)
     sizes = [5, 1, 7]
@@ -256,23 +275,41 @@ def test_concat_and_subset_containers_match_the_live_reference(tmp_path):
             self.log.append((self.offset, field))
             return Recorder(self.log, self.offset, field)
 
+    picks = [12, 0, 5, 5, 3]
+
+    def observe(concat, subset):
+        log = []
+        seen = {"len": len(concat),
+                "raw": [{k: (plain(np.asarray(v)), str(np.asarray(v).dtype)) for k, v in concat.get_raw_item(i).items()}
+                        for i in range(len(concat))],
+                "items": [{k: plain(np.asarray(v)) for k, v in concat[i].items()} for i in range(len(concat))]}
+        concat.set_accessor(Recorder(log))
+        sub = subset(concat, picks)
+        seen.update(log=log, sub_len=len(sub),
+                    sub=[{k: plain(np.asarray(sub[j][k])) for k in ("a", "b")} for j in range(len(sub))])
+        return seen
+
+    def reference():
+        from oracle.ref_shim import import_reference
+        import_reference()
+        import frldistml.scaffold.storage_layers.dataset as ref_ds
+        from frldistml.scaffold.indexed_dataset import MultifieldIndexedDataset as RefMulti
+        from frldistml.scaffold.storage import StoragePath
+        ref_parts = [RefMulti(StoragePath(str(tmp_path / ("part%d" % k))), fields=["a", "b"], filenames=["a", "b"])
+                     for k in range(3)]
+        return observe(ref_ds.ConcatMultifieldDataset(ref_parts), ref_ds.SubsetMultifieldDataset)
+
+    ref, _ = reference_side("indexed_concat_subset", reference)
     mine_parts = [idm.MultifieldIndexedDataset(str(tmp_path / ("part%d" % k)), fields=["a", "b"], filenames=["a", "b"])
                   for k in range(3)]
-    ref_parts = [RefMulti(StoragePath(str(tmp_path / ("part%d" % k))), fields=["a", "b"], filenames=["a", "b"])
-                 for k in range(3)]
-    mine, ref = my_ds.ConcatMultifieldDataset(mine_parts), ref_ds.ConcatMultifieldDataset(ref_parts)
-    assert len(mine) == len(ref) == sum(sizes)
-    for i in range(len(ref)):
-        a, b = mine.get_raw_item(i), ref.get_raw_item(i)
-        assert list(a) == list(b) and all(np.array_equal(a[k], b[k]) and a[k].dtype == b[k].dtype for k in a)
-        c, d = mine[i], ref[i]
-        assert all(np.array_equal(c[k], d[k]) for k in c)
-    log_mine, log_ref = [], []
-    mine.set_accessor(Recorder(log_mine))
-    ref.set_accessor(Recorder(log_ref))
-    assert log_mine == log_ref == [(0, "a"), (0, "b"), (5, "a"), (5, "b"), (6, "a"), (6, "b")]
-    picks = [12, 0, 5, 5, 3]
-    sub_mine, sub_ref = my_ds.SubsetMultifieldDataset(mine, picks), ref_ds.SubsetMultifieldDataset(ref, picks)
-    assert len(sub_mine) == len(sub_ref) == 5
+    mine = observe(my_ds.ConcatMultifieldDataset(mine_parts), my_ds.SubsetMultifieldDataset)
+    assert mine["len"] == ref["len"] == sum(sizes)
+    for a, b in zip(mine["raw"], ref["raw"]):
+        assert list(a) == list(b) and all(torch.equal(a[k][0], b[k][0]) and a[k][1] == b[k][1] for k in a)
+    for c, d in zip(mine["items"], ref["items"]):
+        assert list(c) == list(d) and all(torch.equal(c[k], d[k]) for k in c)
+    assert [tuple(e) for e in mine["log"]] == [tuple(e) for e in ref["log"]] == \
+        [(0, "a"), (0, "b"), (5, "a"), (5, "b"), (6, "a"), (6, "b")]
+    assert mine["sub_len"] == ref["sub_len"] == 5
     for j in range(5):
-        assert all(np.array_equal(sub_mine[j][k], sub_ref[j][k]) for k in ("a", "b"))
+        assert all(torch.equal(mine["sub"][j][k], ref["sub"][j][k]) for k in ("a", "b"))

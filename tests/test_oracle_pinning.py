@@ -1,6 +1,6 @@
 """The oracle (oracle/ref_loop.py, optim_np.py, criteria_np.py) against the committed golden
-vectors recorded from the live reference, against the reference itself where it is present,
-and against torch's own ops."""
+vectors recorded from the live reference, against the reference itself (live where it is
+present, else its recorded side under tests/golden/live), and against torch's own ops."""
 import json
 import os
 import re
@@ -10,6 +10,7 @@ import pytest
 import torch
 
 from oracle import criteria_np, optim_np, ref_loop
+from oracle.live_golden import plain, reference_side, tensors_equal
 from oracle.make_golden import BATCH, CONFIGS, SEED, run_oracle
 
 
@@ -62,16 +63,20 @@ def test_sampler_restatement_matches_reference_lists(golden_dir):
             assert got == expect, key
 
 
-@pytest.mark.reference
 def test_ref_loop_equals_live_reference_bitwise():
-    from oracle.make_golden import run_live_reference
     name = "toy_sgd"
-    live = run_live_reference(name, CONFIGS[name])
+
+    def reference():
+        from oracle.make_golden import run_live_reference
+        run = run_live_reference(name, CONFIGS[name])
+        return plain({"rows": run["rows"], "param_00": run["param_00"]})
+
+    want, live = reference_side("ref_loop_" + name, reference)
     trace, _ = run_oracle(name, CONFIGS[name])
     rows = np.concatenate([trace.losses[k] for k in sorted(
         trace.losses, key=lambda ek: (ek[0], 0 if ek[1] == "training" else 1))])
-    assert np.array_equal(rows, live["rows"])
-    assert np.array_equal(trace.params[0], live["param_00"])
+    assert tensors_equal(plain(rows), want["rows"], live)
+    assert tensors_equal(plain(trace.params[0]), want["param_00"], live)
 
 
 # ---- numpy update rules vs torch.optim (what the reference actually calls) --------------------
@@ -154,19 +159,14 @@ def test_bf16_round_matches_torch():
 
 
 # ------------------------------------------------------------------------------------------------
-# SURVEY §8 a16 — SamplerState (retained minibatches -> per-sample metrics, random picks, worst-k)
+# SamplerState (retained minibatches -> per-sample metrics, random picks, worst-k)
 # against the live reference class on identical inputs
 # ------------------------------------------------------------------------------------------------
 
-@pytest.mark.reference
 @pytest.mark.parametrize("metric_name,ordering", [("err_MSE", "DESC"), ("score", "ASC"), ("score", "DESC")])
 def test_sampler_state_matches_live_reference(metric_name, ordering):
     import random
     from typing import NamedTuple
-    from oracle.ref_shim import import_reference
-    import_reference()
-    import frldistml.scaffold.solver_worker as ref_sw
-    from frldistml.scaffold.problem import Ordering as RefOrdering
     import frl_b200  # noqa: F401
     import frl_b200.solver_worker as my_sw
     from frl_b200.problem import Ordering as MyOrdering
@@ -204,50 +204,63 @@ def test_sampler_state_matches_live_reference(metric_name, ordering):
         sampler = list(range(total))
 
     dev = torch.device("cpu")
-    random.seed(5)
-    ref = ref_sw.SamplerState(make_problem(RefOrdering), FakeLoader, list(range(total)), dev, 6)
-    random.seed(5)
-    mine = my_sw.SamplerState(make_problem(MyOrdering), total, total, dev, 6)
-    for s in (ref, mine):
+
+    def feed(s):
         for k, b in enumerate(batches):
             if k % 2 == 0:                            # amortisation: fold every second minibatch
                 s.compute_metrics()
             s.append_sample(b["meta"], b["data"], outputs=b["outputs"], targets=b["targets"])
         s.compute_metrics()
-    mine.finish()
-
-    assert mine.n_samples == ref.n_samples == total
-    for k in ("err_MSE", "score"):
-        np.testing.assert_array_equal(np.asarray(mine.data_metric[k]), np.asarray(ref.data_metric[k]))
+        return s
 
     def ids(samples):
         return [int(s.meta["index"]) for s in samples]
 
-    assert ids(mine.random_samples) == ids(ref.random_samples) and len(ids(ref.random_samples)) == 6
-    assert sorted(ids(mine.worst_samples)) == sorted(ids(ref.worst_samples))
-    assert len(ref.worst_samples) == 6
-    by_id = {int(s.meta["index"]): s for s in ref.worst_samples + ref.random_samples}
-    for s in mine.worst_samples + mine.random_samples:
-        r = by_id[int(s.meta["index"])]
-        assert all(torch.equal(a, b) for a, b in zip(s.data, r.data))
-        assert all(torch.equal(a, b) for a, b in zip(s.output, r.output))
-        assert all(torch.equal(a[0], b[0]) for a, b in zip(s.target, r.target))
-        assert {k: float(v) for k, v in s.metric.items()} == {k: float(v) for k, v in r.metric.items()}
+    def summary(s):
+        return plain({"n_samples": s.n_samples,
+                      "data_metric": {k: np.asarray(s.data_metric[k]) for k in ("err_MSE", "score")},
+                      "random": ids(s.random_samples), "worst": ids(s.worst_samples),
+                      "samples": {int(x.meta["index"]): {"data": list(x.data), "output": list(x.output),
+                                                         "target": [t[0] for t in x.target],
+                                                         "metric": {k: float(v) for k, v in x.metric.items()}}
+                                  for x in s.worst_samples + s.random_samples}})
+
+    def reference():
+        from oracle.ref_shim import import_reference
+        import_reference()
+        import frldistml.scaffold.solver_worker as ref_sw
+        from frldistml.scaffold.problem import Ordering as RefOrdering
+        random.seed(5)
+        return summary(feed(ref_sw.SamplerState(make_problem(RefOrdering), FakeLoader, list(range(total)), dev, 6)))
+
+    ref, live = reference_side("sampler_state_%s_%s" % (metric_name, ordering), reference)
+    random.seed(5)
+    mine = feed(my_sw.SamplerState(make_problem(MyOrdering), total, total, dev, 6))
+    mine.finish()
+    mine = summary(mine)
+
+    assert mine["n_samples"] == ref["n_samples"] == total
+    for k in ("err_MSE", "score"):
+        assert tensors_equal(mine["data_metric"][k], ref["data_metric"][k], live), k
+
+    assert mine["random"] == ref["random"] and len(ref["random"]) == 6
+    assert sorted(mine["worst"]) == sorted(ref["worst"])
+    assert len(ref["worst"]) == 6
+    for i, s in mine["samples"].items():
+        r = ref["samples"][i]
+        assert all(torch.equal(a, b) for a, b in zip(s["data"], r["data"]))
+        assert all(torch.equal(a, b) for a, b in zip(s["output"], r["output"]))
+        assert all(torch.equal(a, b) for a, b in zip(s["target"], r["target"]))
+        assert s["metric"] == (r["metric"] if live else pytest.approx(r["metric"], rel=2e-6, abs=1e-7))
 
 
 # ------------------------------------------------------------------------------------------------
-# SURVEY §8 a8-a11 — the criterion classes' own composition (what runs for arbitrary user losses,
+# the criterion classes' own composition (what runs for arbitrary user losses,
 # and what the fused kernels are checked against on the GPU) against the live reference classes
 # ------------------------------------------------------------------------------------------------
 
-@pytest.mark.reference
 @pytest.mark.parametrize("kind", ["parallel", "uncertainty", "gradnorm", "masked"])
 def test_criterion_classes_match_live_reference(kind):
-    from oracle.ref_shim import import_reference
-    import_reference()
-    import frldistml.scaffold.criteria as ref_c
-    import frldistml.scaffold.model as ref_m
-    import frldistml.scaffold.types as ref_t
     import frl_b200  # noqa: F401
     import frl_b200.criteria as my_c
     import frl_b200.model as my_m
@@ -298,13 +311,22 @@ def test_criterion_classes_match_live_reference(kind):
             opt.step()
         return trace, [p.detach().clone() for p in params]
 
-    ref_trace, ref_params = run(ref_c, ref_m, ref_t)
+    def reference():
+        from oracle.ref_shim import import_reference
+        import_reference()
+        import frldistml.scaffold.criteria as ref_c
+        import frldistml.scaffold.model as ref_m
+        import frldistml.scaffold.types as ref_t
+        return plain(run(ref_c, ref_m, ref_t))
+
+    (ref_trace, ref_params), live = reference_side("criterion_" + kind, reference)
     my_trace, my_params = run(my_c, my_m, my_t)
+    assert len(my_trace) == len(ref_trace) and len(my_params) == len(ref_params)
     for (rt, rs, rg), (mt, ms, mg) in zip(ref_trace, my_trace):
-        assert torch.equal(mt, rt)
-        assert list(ms) == list(rs) and all(torch.equal(ms[k], rs[k]) for k in rs)
-        assert len(mg) == len(rg) and all(torch.equal(a, b) for a, b in zip(mg, rg))
-    assert all(torch.equal(a, b) for a, b in zip(my_params, ref_params))
+        assert tensors_equal(mt, rt, live)
+        assert list(ms) == list(rs) and all(tensors_equal(ms[k], rs[k], live) for k in rs)
+        assert len(mg) == len(rg) and all(tensors_equal(a, b, live) for a, b in zip(mg, rg))
+    assert all(tensors_equal(a, b, live) for a, b in zip(my_params, ref_params))
 
 
 # ------------------------------------------------------------------------------------------------
@@ -312,13 +334,7 @@ def test_criterion_classes_match_live_reference(kind):
 # weighted means over ranks, MSE -> RMSE renaming, invalid (negative) metrics passed through
 # ------------------------------------------------------------------------------------------------
 
-@pytest.mark.reference
 def test_rank_aggregation_matches_live_reference():
-    from oracle.ref_shim import import_reference
-    import_reference()
-    import frldistml.scaffold.solver as ref_solver
-    import frldistml.scaffold.solver_worker as ref_sw
-    import frldistml.scaffold.types as ref_t
     import frl_b200  # noqa: F401
     import frl_b200.solver as my_solver
     import frl_b200.solver_worker as my_sw
@@ -353,8 +369,16 @@ def test_rank_aggregation_matches_live_reference():
         out = solver_mod.Solver._aggregate_fractional_results(ro, P(), fracs)
         return {split.value: (dict(s.losses), dict(s.metrics)) for split, s in out.items()}
 
-    want = run(ref_solver, ref_sw, ref_t)
-    got = run(my_solver, my_sw, my_t)
+    def reference():
+        from oracle.ref_shim import import_reference
+        import_reference()
+        import frldistml.scaffold.solver as ref_solver
+        import frldistml.scaffold.solver_worker as ref_sw
+        import frldistml.scaffold.types as ref_t
+        return plain(run(ref_solver, ref_sw, ref_t))
+
+    want, _ = reference_side("rank_aggregation", reference)
+    got = plain(run(my_solver, my_sw, my_t))
     assert got == want
     assert set(want["training"][1]) == {"reg_RMSE", "cls_err", "pose_RMSE_deg"}
     assert want["testing"][1]["pose_RMSE_deg"] == -1.0          # invalid metric: not square-rooted
@@ -365,16 +389,9 @@ def test_rank_aggregation_matches_live_reference():
 # contents, and each side's loader reads the other's checkpoint
 # ------------------------------------------------------------------------------------------------
 
-@pytest.mark.reference
 def test_checkpoint_files_match_live_reference(tmp_path):
     import io
     from typing import NamedTuple
-    from oracle.ref_shim import import_reference
-    import_reference()
-    import frldistml.scaffold.solver as ref_solver
-    import frldistml.scaffold.solver_worker as ref_sw
-    import frldistml.scaffold.types as ref_t
-    from frldistml.scaffold.storage import StoragePath
     import frl_b200  # noqa: F401
     import frl_b200.solver as my_solver
     import frl_b200.solver_worker as my_sw
@@ -419,7 +436,22 @@ def test_checkpoint_files_match_live_reference(tmp_path):
     ref_dir, my_dir = tmp_path / "ref", tmp_path / "mine"
     ref_dir.mkdir()
     my_dir.mkdir()
-    write(ref_solver, ref_sw, ref_t, StoragePath(str(ref_dir)))
+
+    def reference():
+        from oracle.ref_shim import import_reference
+        import_reference()
+        import frldistml.scaffold.solver as ref_solver
+        import frldistml.scaffold.solver_worker as ref_sw
+        import frldistml.scaffold.types as ref_t
+        from frldistml.scaffold.storage import StoragePath
+        write(ref_solver, ref_sw, ref_t, StoragePath(str(ref_dir)))
+        return {n: torch.frombuffer(bytearray(open(os.path.join(ref_dir, n), "rb").read()), dtype=torch.uint8)
+                for n in sorted(os.listdir(ref_dir))}
+
+    ref_files, live = reference_side("checkpoint_files", reference)
+    if not live:
+        for n, data in ref_files.items():
+            open(os.path.join(ref_dir, n), "wb").write(data.numpy().tobytes())
     write(my_solver, my_sw, my_t, str(my_dir))
     names = sorted(os.listdir(ref_dir))
     assert sorted(os.listdir(my_dir)) == names == [".checkpoint.pth", ".checkpoint.pth.annotate_param",
@@ -427,7 +459,7 @@ def test_checkpoint_files_match_live_reference(tmp_path):
 
     def same(a, b):
         if torch.is_tensor(a):
-            return torch.is_tensor(b) and a.dtype == b.dtype and torch.equal(a, b)
+            return torch.is_tensor(b) and a.dtype == b.dtype and tensors_equal(a, b, live)
         if isinstance(a, dict):
             return isinstance(b, dict) and list(a) == list(b) and all(same(a[k], b[k]) for k in a)
         if isinstance(a, (list, tuple)):
@@ -441,23 +473,22 @@ def test_checkpoint_files_match_live_reference(tmp_path):
     whole_ref = torch.load(os.path.join(ref_dir, ".checkpoint.pth.model"), weights_only=False)
     whole_mine = torch.load(os.path.join(my_dir, ".checkpoint.pth.model"), weights_only=False)
     assert same(dict(whole_ref.state_dict()), dict(whole_mine.state_dict()))
-    # each loader reads the other side's file
-    with open(os.path.join(my_dir, ".checkpoint.pth"), "rb") as f:
-        got = ref_solver.Solver._load_checkpoint(f)
+    # each loader reads the other side's file (the reference's loader where it is present)
     with open(os.path.join(ref_dir, ".checkpoint.pth"), "rb") as f:
         back = my_solver.Solver._load_checkpoint(f)
+    got = back
+    if live:
+        import frldistml.scaffold.solver as ref_solver
+        with open(os.path.join(my_dir, ".checkpoint.pth"), "rb") as f:
+            got = ref_solver.Solver._load_checkpoint(f)
     assert got.epoch == back.epoch == 7
     assert same(dict(got.modelState), dict(back.modelState)) and same(got.optimizerState, back.optimizerState)
     torch.optim.SGD(whole_mine.parameters(), lr=0.1, momentum=0.9).load_state_dict(got.optimizerState)
 
 
-@pytest.mark.reference
 def test_initial_model_loading_matches_live_reference(tmp_path, capsys):
     """``initialModelPath`` (reference solver.py:122-159): strict load, and the partial load that
     copies what matches in name and shape and reports the rest — same weights, same messages."""
-    from oracle.ref_shim import import_reference
-    import_reference()
-    import frldistml.scaffold.solver as ref_solver
     import frl_b200  # noqa: F401
     import frl_b200.solver as my_solver
 
@@ -471,36 +502,42 @@ def test_initial_model_loading_matches_live_reference(tmp_path, capsys):
     state["0.weight"] = torch.nn.Parameter(state["0.weight"].clone())      # legacy serialised Parameter
     path = str(tmp_path / "init.pth")
     torch.save({"state_dict": state}, path)
-    results = []
-    for mod in (ref_solver, my_solver):
+
+    def load_with(mod):
         target = net(5)
         del_key = net(7)                       # different width: shape mismatches on every tensor but one
         mod._load_model_state(target, path, strict=False)
         mod._load_model_state(del_key, path, strict=False)
         out = capsys.readouterr().out
         lines = [l for l in out.splitlines() if l.startswith("Warning")]
-        results.append((dict(target.state_dict()), dict(del_key.state_dict()), lines))
         with pytest.raises(RuntimeError):
             mod._load_model_state(net(5), path, strict=True)               # unexpected key "extra.weight"
         capsys.readouterr()
-    (ra, rb, rl), (ma, mb, ml) = results
-    assert all(torch.equal(ra[k], ma[k]) for k in ra) and all(torch.equal(rb[k], mb[k]) for k in rb)
+        return plain((dict(target.state_dict()), dict(del_key.state_dict()), lines))
+
+    def reference():
+        from oracle.ref_shim import import_reference
+        import_reference()
+        import frldistml.scaffold.solver as ref_solver
+        return load_with(ref_solver)
+
+    (ra, rb, rl), live = reference_side("initial_model_loading", reference)
+    ma, mb, ml = load_with(my_solver)
+    assert list(ra) == list(ma) and list(rb) == list(mb)
+    assert all(tensors_equal(ra[k], ma[k], live) for k in ra) and all(tensors_equal(rb[k], mb[k], live) for k in rb)
     assert ml == rl and len(rl) >= 4
     assert torch.equal(ma["0.weight"], donor.state_dict()["0.weight"])
 
 
-@pytest.mark.reference
 def test_multitask_problem_plumbing_matches_live_reference():
     """The same synthetic MultiTaskProblem source instantiated against this package and against
-    the reference (SURVEY §8b: Problem/MultiTaskProblem/MultiTaskTransform/Task/MultiTaskModel):
+    the reference (Problem/MultiTaskProblem/MultiTaskTransform/Task/MultiTaskModel):
     per-sample items, model structure and initial weights, criterion composition, merged metric
     hooks and rankable metric must coincide."""
-    from oracle.ref_shim import import_reference
-    import_reference()
     import frl_b200  # noqa: F401
     from frl_b200 import synthetic
-    built = {}
-    for pkg in ("frldistml.scaffold", "frl_b200"):
+
+    def build(pkg):
         ns = synthetic.api_namespace(pkg)
         problem = synthetic.make_toy_problem(ns, "/tmp/unused")
         torch.manual_seed(21)
@@ -514,7 +551,7 @@ def test_multitask_problem_plumbing_matches_live_reference():
         metrics = problem.compute_batch_metrics(meta=meta, target=tgt, output=out, device=torch.device("cpu"))
         with torch.no_grad():
             y = model([torch.ones(2, 64)])
-        built[pkg] = dict(
+        return plain(dict(
             model_type=type(model).__name__, crit_type=type(crit).__name__,
             state={k: v.clone() for k, v in model.state_dict().items()},
             names=list(crit.loss_names), weights=[float(w) for w in crit.loss_weights],
@@ -523,15 +560,23 @@ def test_multitask_problem_plumbing_matches_live_reference():
             rank=(problem.get_rankable_metric()[0], problem.get_rankable_metric()[1].name),
             epoch=problem.summarize_epoch_metrics({k: np.asarray(v) for k, v in metrics.items()}),
             meta_fields=meta._fields, y=[t.clone() for t in y],
-            splits=[d.data_type.value for d in problem.datasets], lens=[len(d) for d in problem.datasets])
-    ref, mine = built["frldistml.scaffold"], built["frl_b200"]
+            splits=[d.data_type.value for d in problem.datasets], lens=[len(d) for d in problem.datasets]))
+
+    def reference():
+        from oracle.ref_shim import import_reference
+        import_reference()
+        return build("frldistml.scaffold")
+
+    ref, live = reference_side("multitask_problem_plumbing", reference)
+    mine = build("frl_b200")
     for k in ("model_type", "crit_type", "names", "weights", "loss_mods", "rank", "epoch", "meta_fields",
               "splits", "lens"):
         assert mine[k] == ref[k], k
     assert list(mine["state"]) == list(ref["state"])
-    assert all(torch.equal(mine["state"][k], ref["state"][k]) for k in ref["state"])
-    assert all(torch.equal(a, b) for a, b in zip(mine["y"], ref["y"]))
-    assert all(np.array_equal(mine["metrics"][k], ref["metrics"][k]) for k in ref["metrics"])
+    assert all(tensors_equal(mine["state"][k], ref["state"][k], live) for k in ref["state"])
+    assert len(mine["y"]) == len(ref["y"]) and all(tensors_equal(a, b, live) for a, b in zip(mine["y"], ref["y"]))
+    assert list(mine["metrics"]) == list(ref["metrics"])
+    assert all(tensors_equal(mine["metrics"][k], ref["metrics"][k], live) for k in ref["metrics"])
     for a, b in zip(mine["items"], ref["items"]):
         assert len(a) == len(b) == 3
         assert all(torch.equal(x, y) for x, y in zip(a[0], b[0]))                      # data list

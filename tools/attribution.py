@@ -2,8 +2,8 @@
 """Kernel-by-kernel attribution of the step-time difference between this repo's arm and the
 stock-PyTorch arm, from the per-kernel profiles `bench.py --profile` writes.
 
-    python tools/attribution.py profiles/r2j_profile_mlp_b200.json profiles/r2j_profile_mlp_torch.json
-    python tools/attribution.py profiles/r2p_profile_mlp_b200.json profiles/r2p_profile_mlp_b200_e2e.json   # resident vs e2e epoch
+    python tools/attribution.py mlp.json mlp_torch.json      # bench.py --profile mlp.json / --impl torch-gpu --profile mlp_torch.json
+    python tools/attribution.py mlp.json mlp_e2e.json        # resident vs e2e epoch
 """
 import json
 import sys

@@ -33,7 +33,7 @@ def main():
     opt._steps = 1
     gbytes = arena.numel * 2
     res = {}
-    for blocks in (16, 32, 64, 96, 148):
+    for blocks in (16, 32, 64, 96, 132):
         link = make_link(alloc, arena.grad, arena.lp, max_blocks=blocks)
         opt.nvls = link
         for _ in range(5):

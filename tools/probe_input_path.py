@@ -62,12 +62,12 @@ perms_dev = [p.to(dev) for p in perms]
 perms_pin = [p.pin_memory() for p in perms]
 
 report("cudaMemcpyAsync contiguous", timed(lambda r: dst.copy_(src[r * B:(r + 1) * B], non_blocking=True)))
-for blocks in (32, 64, 148, 296, 592, 1184):
+for blocks in (32, 66, 132, 264, 528, 1056):
     report("frl_gather_rows blocks=%d" % blocks,
            timed(lambda r: _native.gather_rows(src, perms_dev[r], dst, max_blocks=blocks)))
 ok = torch.equal(dst.cpu(), src[perms[5]])
 print("gather_rows correct:", ok)
-for blocks in (16, 37, 74, 148, 296):
+for blocks in (16, 33, 66, 132, 264):
     try:
         dst.zero_()
         report("frl_gather_rows_tma blocks=%d" % blocks,
@@ -84,8 +84,7 @@ for blocks in (1, 2, 3, 4, 8):
 for blocks in (2, 4, 8, 16):
     report("frl_gather_rows blocks=%d" % blocks,
            timed(lambda r: _native.gather_rows(src, perms_dev[r], dst, max_blocks=blocks)))
-# (cudaMemcpyBatchAsync with one descriptor per row was measured once and rejected: 7.4 GB/s,
-#  19 ms of host time per 4096-row submission; see profiles/r1b_probe_input_path_b.log)
+# (cudaMemcpyBatchAsync with one descriptor per row is left out: its host cost grows with the rows)
 stage = torch.empty(B, W).pin_memory()
 for th in (1, 4, 8, 16, 32):
     pool = _native.HostGatherPool(th)

@@ -2,7 +2,7 @@
 """In-process sweep of the fused NVLS step's launch knobs (grid size, barrier placement) on the
 bench workload, one torchrun launch:
 
-    torchrun --nproc-per-node N tools/sweep_nvls.py [--bucket-mb 48] [--blocks 32,74,148] [--steps 40]
+    torchrun --nproc-per-node N tools/sweep_nvls.py [--bucket-mb 48] [--blocks 32,66,132] [--steps 40]
 
 Prints one line per configuration (rank 0): ms/step as max over ranks of the CUDA-event time.
 """
@@ -21,7 +21,7 @@ import bench  # noqa: E402
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--bucket-mb", type=float, default=48.0)
-    ap.add_argument("--blocks", default="32,74,148")
+    ap.add_argument("--blocks", default="32,66,132")
     ap.add_argument("--steps", type=int, default=40)
     ap.add_argument("--warmup", type=int, default=8)
     ap.add_argument("--algo", default="sgd")
