@@ -12,7 +12,7 @@ __version__ = "0.1.0"
 
 _SUBMODULES = ("types", "criteria", "model", "lr_scheduler", "sampler", "transform", "task",
                "problem", "multitask_problem", "solver_worker", "solver", "local_solver",
-               "storage_layers", "storage_layers.dataset", "indexed_dataset")
+               "storage_layers", "storage_layers.dataset", "indexed_dataset", "text_dataset")
 
 
 def install_reference_alias(top: str = "frldistml", sub: str = "scaffold") -> None:

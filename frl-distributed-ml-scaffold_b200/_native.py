@@ -73,6 +73,7 @@ SIGNATURES = {
     "frl_gather_rows": (_i, [_vp, _i64, _vp, _vp, _i64, _i64, _i, _vp]),
     "frl_gather_rows_tma": (_i, [_vp, _i64, _vp, _vp, _i64, _i64, _i, _vp]),
     "frl_gather_window_rows": (_i, [_vp, _vp, _i, _vp, _vp, _i64, _i64, _vp]),
+    "frl_gather_lines": (_i, [_vp, _i64, _i64, _vp, _i64, _vp, _vp, _i64, _i64, _i, _i, _vp]),
     "frl_gather_pool_create": (_vp, [_i]),
     "frl_gather_pool_destroy": (None, [_vp]),
     "frl_gather_pool_threads": (_i, [_vp]),
@@ -355,6 +356,20 @@ def gather_rows_tma(src_pinned, idx_dev, dst, max_blocks: int = 0) -> None:
     _check(lib().frl_gather_rows_tma(_ptr(src_pinned), src_pinned.shape[0], _ptr(idx_dev), _ptr(dst),
                                      idx_dev.numel(), _row_bytes(src_pinned), max_blocks, _stream()),
            "frl_gather_rows_tma")
+
+
+def gather_lines(corpus_ptr: int, corpus_bytes: int, corpus_alloc_bytes: int, starts_dev, idx_dev, dst,
+                 pad: int = 0, max_blocks: int = 0) -> None:
+    """dst[r] = line idx[r] of a text corpus, cut or padded with ``pad`` to ``dst.shape[1]`` bytes.
+    ``corpus_ptr``: address of the pinned, device-mapped corpus (16-byte aligned, allocation of
+    ``corpus_alloc_bytes``); ``starts_dev``: device int64 line-start table [n_lines + 1];
+    ``dst``: contiguous device uint8 [len(idx), row_len], any alignment."""
+    assert starts_dev.dtype == torch.int64 and starts_dev.is_cuda and starts_dev.is_contiguous()
+    assert idx_dev.dtype == torch.int64 and dst.dtype == torch.uint8 and dst.dim() == 2
+    assert dst.is_contiguous() and dst.shape[0] == idx_dev.numel()
+    _check(lib().frl_gather_lines(corpus_ptr, corpus_bytes, corpus_alloc_bytes, _ptr(starts_dev),
+                                  starts_dev.numel() - 1, _ptr(idx_dev), _ptr(dst), dst.shape[0], dst.shape[1],
+                                  pad, max_blocks, _stream()), "frl_gather_lines")
 
 
 def gather_window_rows(batches, idx_dev, dst=None):

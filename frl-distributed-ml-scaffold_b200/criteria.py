@@ -47,7 +47,7 @@ class MaskedLoss(L._Loss):
         if output.is_cuda:
             plan = _plan_for([self], [output], [(target, mask)])
             if plan is not None:
-                return _FusedLosses.apply(plan, None, output)[1]
+                return _FusedLosses.apply(plan, None, *_kernel_outputs(plan, [output]))[1]
         # generic composition (any inner loss): same arithmetic as the reference
         if mask.sum() == 0:
             return self.loss_layer.forward(output - output, target - target)
@@ -85,13 +85,14 @@ def _classify(module: nn.Module) -> Optional[_TaskPlan]:
 
 class _Plan:
     """Per-call launch description: task plans + the tensors of this minibatch."""
-    __slots__ = ("tasks", "targets", "masks", "weights", "n", "sink", "nan_flag")
+    __slots__ = ("tasks", "targets", "masks", "weights", "n", "sink", "nan_flag", "per_position")
 
-    def __init__(self, tasks, targets, masks, weights):
+    def __init__(self, tasks, targets, masks, weights, per_position):
         self.tasks = tasks
         self.targets = targets
         self.masks = masks
         self.weights = weights
+        self.per_position = per_position
         self.n = len(tasks)
         self.sink = None
         self.nan_flag = None
@@ -107,7 +108,7 @@ def _plan_for(modules: Sequence[nn.Module], outputs: Sequence[torch.Tensor],
     n = len(modules)
     if n == 0 or n > _native.MAX_TASKS or len(outputs) < n or len(targets) < n:
         return None
-    tasks, tgts, masks = [], [], []
+    tasks, tgts, masks, per_position = [], [], [], []
     for i, mod in enumerate(modules):
         tp = _classify(mod)
         out = outputs[i]
@@ -128,6 +129,12 @@ def _plan_for(modules: Sequence[nn.Module], outputs: Sequence[torch.Tensor],
             if mask is not None:
                 if mask.dim() > out.dim() or tuple(out.shape[:mask.dim()]) != tuple(mask.shape):
                     return None
+        elif out.dim() > 2 and mask is None:
+            # per-position classes, torch's [N, C, d1, ...] layout with targets [N, d1, ...]: the
+            # kernels see the rows of out.movedim(1, -1) as [N * d1 * ..., C]
+            if tgt.dtype != torch.int64 or tgt.shape != out.shape[:1] + out.shape[2:]:
+                return None
+            tgt = tgt.reshape(-1)
         else:
             if out.dim() != 2 or tgt.dtype != torch.int64 or tgt.shape != out.shape[:1]:
                 return None
@@ -138,8 +145,15 @@ def _plan_for(modules: Sequence[nn.Module], outputs: Sequence[torch.Tensor],
         tasks.append(tp)
         tgts.append(tgt)
         masks.append(mask)
+        per_position.append(tp.kind == _native.LOSS_CE and out.dim() > 2)
     w = [1.0] * n if weights is None else [float(x) for x in weights]
-    return _Plan(tasks, tgts, masks, w)
+    return _Plan(tasks, tgts, masks, w, per_position)
+
+
+def _kernel_outputs(plan: _Plan, outputs: Sequence[torch.Tensor]) -> List[torch.Tensor]:
+    """The task outputs as the kernels read them: per-position CE outputs as [rows, C]."""
+    return [o.movedim(1, -1).reshape(-1, o.shape[1]) if flat else o
+            for o, flat in zip(outputs[:plan.n], plan.per_position)]
 
 
 _scratch: Dict[Tuple[int, int], torch.Tensor] = {}
@@ -248,7 +262,7 @@ def fused_task_losses(modules, outputs, targets, weights=None, sink=None, nan_fl
         return None
     plan.sink = sink
     plan.nan_flag = nan_flag
-    return _FusedLosses.apply(plan, None, *outputs[:plan.n])
+    return _FusedLosses.apply(plan, None, *_kernel_outputs(plan, outputs))
 
 
 # =============================================================================================

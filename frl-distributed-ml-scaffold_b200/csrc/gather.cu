@@ -199,6 +199,138 @@ gather_window_rows_kernel(const WindowTable tab, const int64_t* __restrict__ idx
         for (int64_t u = threadIdx.x; u < row_bytes; u += kGThreads) to[u] = from[u];
     }
 }
+
+
+// ---- K8t — padded text lines --------------------------------------------------------------------
+// Row r of the batch is line idx[r] of a newline-separated corpus in mapped host memory, cut or
+// padded to row_len bytes.  Lines start at arbitrary byte offsets and row_len is usually odd, so
+// neither side is 16-byte aligned.  The batch is split into contiguous runs of whole rows, one per
+// warp; a row is walked as a sequence of 16-byte units: unit t (t = 0..M) is the aligned source
+// unit A + t of the corpus, and the output unit t - 1 (an ALIGNED 16-byte unit of dst) is the
+// byte window [sh, sh + 16) of source units A + t - 1 and A + t.  Every lane loads one source
+// unit and takes its left neighbour from the lane before it (from the previous group / pass for
+// lane 0), so each source unit crosses PCIe once.  Units that hold no byte of the line are not
+// read at all: the line's bytes cover at most the row, padding comes from the register file.
+constexpr int kLUnroll = 8;
+
+struct LineRow {
+    int64_t a;       // first source unit of the window (may be -1 for a line starting at byte < 16)
+    int64_t u_lo;    // source units [u_lo, u_hi] hold the line's bytes (u_hi < u_lo: none)
+    int64_t u_hi;
+    int64_t len;     // bytes of the line that go into the row
+    int d_off;       // dst row start & 15
+    int sh;          // byte shift of the source window against the aligned dst units
+    int m;           // aligned dst units the row touches
+};
+
+__device__ __forceinline__ LineRow line_row(const int64_t* __restrict__ starts, int64_t n_lines,
+                                           const int64_t* __restrict__ idx, int64_t row, int64_t row_len,
+                                           int64_t corpus_bytes, uintptr_t dst) {
+    int64_t i = __ldg(idx + row);
+    if (i < 0 || i >= n_lines) i = 0;                               // never read outside the dataset
+    const int64_t lo = __ldg(starts + i);
+    int64_t len = __ldg(starts + i + 1) - 1 - lo;                   // the reference's slice [lo, end - 1)
+    len = len < 0 ? 0 : (len > row_len ? row_len : len);
+    if (lo < 0 || lo >= corpus_bytes) len = 0;
+    else if (len > corpus_bytes - lo) len = corpus_bytes - lo;
+    LineRow p;
+    p.d_off = static_cast<int>((dst + static_cast<uintptr_t>(row * row_len)) & 15u);
+    const int64_t delta = (len > 0 ? lo : 0) - p.d_off;
+    p.a = delta >> 4;                                               // floor division
+    p.sh = static_cast<int>(delta & 15);
+    p.len = len;
+    p.u_lo = len > 0 ? lo >> 4 : 1;
+    p.u_hi = len > 0 ? (lo + len - 1) >> 4 : 0;
+    p.m = static_cast<int>((p.d_off + row_len + 15) >> 4);
+    return p;
+}
+
+// bytes [k, k + 4) of the 32-byte little-endian sequence w0..w7
+__device__ __forceinline__ uint32_t window_word(const uint32_t (&w)[8], int k) {
+    const int q = k >> 2;
+    const uint32_t x = q == 0 ? w[0] : q == 1 ? w[1] : q == 2 ? w[2] : q == 3 ? w[3] : q == 4 ? w[4]
+                     : q == 5 ? w[5] : q == 6 ? w[6] : w[7];
+    const uint32_t y = q == 0 ? w[1] : q == 1 ? w[2] : q == 2 ? w[3] : q == 3 ? w[4] : q == 4 ? w[5]
+                     : q == 5 ? w[6] : w[7];
+    const uint32_t b = static_cast<uint32_t>(k & 3);
+    return __byte_perm(x, y, 0x3210u + b * 0x1111u);                // prmt: bytes b..b+3 of y:x
+}
+
+template <typename IDX>
+__global__ void __launch_bounds__(kGThreads, 1)
+gather_lines_kernel(const uint8_t* __restrict__ corpus, int64_t corpus_bytes, const int64_t* __restrict__ starts,
+                    int64_t n_lines, const int64_t* __restrict__ idx, uint8_t* __restrict__ dst, int64_t n_rows,
+                    int64_t row_len, uint32_t pad) {
+    const int lane = threadIdx.x & 31;
+    const int64_t n_warps = static_cast<int64_t>(gridDim.x) * (kGThreads / 32);
+    const int64_t warp = static_cast<int64_t>(blockIdx.x) * (kGThreads / 32) + (threadIdx.x >> 5);
+    const IDX upr = static_cast<IDX>((row_len + 15 + 15) / 16 + 1);    // units t = 0..M per row, M <= upr - 1
+    const int64_t r0 = n_rows * warp / n_warps, r1 = n_rows * (warp + 1) / n_warps;
+    const int64_t u_end = r1 * static_cast<int64_t>(upr);
+    const uintptr_t dst_addr = reinterpret_cast<uintptr_t>(dst);
+    const int4* c16 = reinterpret_cast<const int4*>(corpus);
+    const uint32_t pad4 = pad * 0x01010101u;
+    int4 carry = make_int4(0, 0, 0, 0);                             // unit of lane 31, previous group
+    for (int64_t base = r0 * static_cast<int64_t>(upr); base < u_end; base += 32 * kLUnroll) {
+        int4 v[kLUnroll];
+#pragma unroll
+        for (int k = 0; k < kLUnroll; ++k) {
+            const int64_t u = base + k * 32 + lane;
+            v[k] = make_int4(0, 0, 0, 0);
+            if (u < u_end) {
+                const IDX row = static_cast<IDX>(u) / upr;
+                const int t = static_cast<int>(static_cast<IDX>(u) - row * upr);
+                const LineRow p = line_row(starts, n_lines, idx, row, row_len, corpus_bytes, dst_addr);
+                const int64_t q = p.a + t;
+                if (t <= p.m && q >= p.u_lo && q <= p.u_hi) v[k] = ld_host16(c16 + q);
+            }
+        }
+#pragma unroll
+        for (int k = 0; k < kLUnroll; ++k) {
+            int4 prev;
+            prev.x = __shfl_up_sync(0xffffffffu, v[k].x, 1);
+            prev.y = __shfl_up_sync(0xffffffffu, v[k].y, 1);
+            prev.z = __shfl_up_sync(0xffffffffu, v[k].z, 1);
+            prev.w = __shfl_up_sync(0xffffffffu, v[k].w, 1);
+            if (lane == 0) prev = carry;
+            carry.x = __shfl_sync(0xffffffffu, v[k].x, 31);
+            carry.y = __shfl_sync(0xffffffffu, v[k].y, 31);
+            carry.z = __shfl_sync(0xffffffffu, v[k].z, 31);
+            carry.w = __shfl_sync(0xffffffffu, v[k].w, 31);
+            const int64_t u = base + k * 32 + lane;
+            if (u >= u_end) continue;
+            const IDX row = static_cast<IDX>(u) / upr;
+            const int t = static_cast<int>(static_cast<IDX>(u) - row * upr);
+            const LineRow p = line_row(starts, n_lines, idx, row, row_len, corpus_bytes, dst_addr);
+            if (t < 1 || t > p.m) continue;
+            const int64_t j0 = 16 * static_cast<int64_t>(t - 1) - p.d_off;   // row byte of the unit's byte 0
+            const uint32_t w[8] = {static_cast<uint32_t>(prev.x), static_cast<uint32_t>(prev.y),
+                                   static_cast<uint32_t>(prev.z), static_cast<uint32_t>(prev.w),
+                                   static_cast<uint32_t>(v[k].x), static_cast<uint32_t>(v[k].y),
+                                   static_cast<uint32_t>(v[k].z), static_cast<uint32_t>(v[k].w)};
+            uint32_t o[4];
+#pragma unroll
+            for (int e = 0; e < 4; ++e) {
+                int64_t keep = p.len - (j0 + 4 * e);                  // leading bytes of the word that are line bytes
+                keep = keep < 0 ? 0 : (keep > 4 ? 4 : keep);
+                const uint32_t mask = (1u << (4 * static_cast<uint32_t>(keep))) - 1u;
+                o[e] = __byte_perm(window_word(w, p.sh + 4 * e), pad4, (0x3210u & mask) | (0x7654u & ~mask));
+            }
+            uint8_t* out = reinterpret_cast<uint8_t*>((dst_addr + static_cast<uintptr_t>(row * row_len)
+                                                       - p.d_off) & ~static_cast<uintptr_t>(15)) + 16 * (t - 1);
+            if (j0 >= 0 && j0 + 16 <= row_len) {
+                *reinterpret_cast<int4*>(out) = make_int4(static_cast<int>(o[0]), static_cast<int>(o[1]),
+                                                          static_cast<int>(o[2]), static_cast<int>(o[3]));
+            } else {                                                // first / last unit: shared with neighbours
+#pragma unroll
+                for (int b = 0; b < 16; ++b) {
+                    const int64_t j = j0 + b;
+                    if (j >= 0 && j < row_len) out[b] = static_cast<uint8_t>(o[b >> 2] >> (8 * (b & 3)));
+                }
+            }
+        }
+    }
+}
 }  // namespace frl
 
 using namespace frl;
@@ -265,6 +397,37 @@ extern "C" int frl_gather_window_rows(const void* const* batch_ptrs, const int64
             tab, idx_dev, static_cast<uint8_t*>(dst), row_bytes, (bits & 15u) == 0 ? 1 : 0);
     }
     return after_launch("frl_gather_window_rows");
+}
+
+extern "C" int frl_gather_lines(const void* corpus_mapped, int64_t corpus_bytes, int64_t corpus_alloc_bytes,
+                                const int64_t* starts_dev, int64_t n_lines, const int64_t* idx_dev,
+                                void* dst, int64_t n_rows, int64_t row_len, int pad, int max_blocks,
+                                void* stream) {
+    FRL_REQUIRE(n_rows >= 0 && row_len >= 0 && corpus_bytes >= 0 && n_lines >= 1, FRL_E_ARG,
+                "frl_gather_lines: sizes (n_rows %lld, row_len %lld, corpus_bytes %lld, n_lines %lld)",
+                (long long)n_rows, (long long)row_len, (long long)corpus_bytes, (long long)n_lines);
+    FRL_REQUIRE(pad >= 0 && pad <= 255, FRL_E_ARG, "frl_gather_lines: pad %d is not a byte", pad);
+    FRL_REQUIRE(corpus_mapped && starts_dev && idx_dev && dst, FRL_E_ARG, "frl_gather_lines: null pointer");
+    FRL_REQUIRE(corpus_alloc_bytes >= (corpus_bytes + 15) / 16 * 16, FRL_E_ARG,
+                "frl_gather_lines: corpus allocation of %lld bytes is below %lld rounded up to 16",
+                (long long)corpus_alloc_bytes, (long long)corpus_bytes);
+    FRL_REQUIRE(aligned16(corpus_mapped), FRL_E_ALIGN, "frl_gather_lines: corpus pointer not 16-byte aligned");
+    if (n_rows == 0 || row_len == 0) return 0;
+    constexpr int kWarps = kGThreads / 32;
+    int64_t grid = max_blocks > 0 ? max_blocks : 8;
+    const int64_t need = (n_rows + kWarps - 1) / kWarps;            // at least one row per warp
+    if (grid > need) grid = need;
+    const int64_t upr = (row_len + 15 + 15) / 16 + 1;
+    cudaStream_t st = static_cast<cudaStream_t>(stream);
+    if (n_rows * upr + 32 * kLUnroll < (1ll << 32))
+        gather_lines_kernel<uint32_t><<<static_cast<int>(grid), kGThreads, 0, st>>>(
+            static_cast<const uint8_t*>(corpus_mapped), corpus_bytes, starts_dev, n_lines, idx_dev,
+            static_cast<uint8_t*>(dst), n_rows, row_len, static_cast<uint32_t>(pad));
+    else
+        gather_lines_kernel<int64_t><<<static_cast<int>(grid), kGThreads, 0, st>>>(
+            static_cast<const uint8_t*>(corpus_mapped), corpus_bytes, starts_dev, n_lines, idx_dev,
+            static_cast<uint8_t*>(dst), n_rows, row_len, static_cast<uint32_t>(pad));
+    return after_launch("frl_gather_lines");
 }
 
 // TMA (cp.async.bulk) variant of frl_gather_rows: rows must be multiples of 16 bytes.

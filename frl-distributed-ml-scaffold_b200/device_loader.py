@@ -6,6 +6,7 @@ solver_worker.py:462-469, 805-832; transform.py:25-38): host Python per sample, 
 H100 at batch 4096.  A dataset that exposes
 
     pinned_fields     Dict[str, Tensor]   whole raw dataset, one pinned host tensor per field
+                                          (or a ``PaddedLines`` text corpus: ragged rows)
     device_transform  DeviceBatchTransform
 
 is consumed here instead: the index stream comes from the very same sampler/``DataLoader``
@@ -25,6 +26,10 @@ Three ways to move the rows (``FRL_B200_INPUT_PATH``):
                     sources that are not pinned (memory-mapped ``.bin`` files), and the only one
                     that can ship bf16 over PCIe (``FRL_B200_INPUT_WIRE=bf16``).
 
+A ``PaddedLines`` field (lines of a text corpus, each cut or padded to a fixed row) is only
+served by ``kernel``: ``frl_gather_lines`` pulls the lines from the page-locked corpus into uint8
+slots; ``auto`` selects it and ``tma`` / ``host`` are refused.
+
 Alone, every path is bound by PCIe.  Under the training step, CTAs that occupy SMs for the
 length of a batch transfer slow the GEMMs: the TMA kernel's 128 KB of staging takes an SM from
 the GEMMs per CTA, the LSU kernel's CTAs fit beside them.  The host path costs 3x the payload
@@ -35,6 +40,7 @@ default (``kernel``) is not tuned on H100.
 from collections import deque
 from typing import Dict, Iterator, List, Optional, Tuple
 
+import math
 import os
 
 import torch
@@ -77,6 +83,31 @@ def randperm_quiet(n: int, generator: torch.Generator) -> torch.Tensor:
         return torch.randperm(n, generator=generator)
     finally:
         torch.set_num_threads(threads)
+
+
+class PaddedLines:
+    """A ragged byte field in ``pinned_fields``: row ``i`` is line ``i`` of a text corpus,
+    ``corpus[starts[i] : starts[i+1] - 1]``, cut or padded with ``pad`` to ``row_len`` bytes
+    (``text_dataset.TextDataset``).  ``corpus`` provides ``pin() -> device-usable address``,
+    ``n_bytes`` and ``alloc_bytes`` (16-byte aligned, a multiple of 16); ``starts`` is the int64
+    line-start table, uploaded to each device once.  Served by ``frl_gather_lines`` (K8t)."""
+
+    def __init__(self, corpus, starts, row_len: int, pad: int = 0) -> None:
+        self.corpus = corpus
+        self.starts = starts
+        self.row_len = int(row_len)
+        self.pad = int(pad)
+        self._starts_dev: Dict[torch.device, torch.Tensor] = {}
+
+    def starts_on(self, device: torch.device) -> torch.Tensor:
+        if device not in self._starts_dev:
+            self._starts_dev[device] = torch.from_numpy(self.starts).to(device)
+        return self._starts_dev[device]
+
+    def __getstate__(self):
+        state = self.__dict__.copy()
+        state["_starts_dev"] = {}
+        return state
 
 
 def supports_device_batches(dataset) -> bool:
@@ -135,15 +166,23 @@ class DeviceBatchLoader:
             sampler=sampler, num_workers=0, collate_fn=_collate_indices)
         self.sampler = self._index_loader.sampler
         self._fields: Dict[str, torch.Tensor] = dataset.pinned_fields
+        # ragged text fields: only the GPU-pulled LSU kernel (K8t) serves them
+        self._lines: Dict[str, PaddedLines] = {k: v for k, v in self._fields.items() if isinstance(v, PaddedLines)}
         for name, t in self._fields.items():
-            if t.is_cuda or not t.is_contiguous():
+            if name not in self._lines and (t.is_cuda or not t.is_contiguous()):
                 raise ValueError(f"field {name!r} must be a contiguous host tensor")
         # sources the GPU can read directly (pinned, device-mapped) or only the CPU can (e.g. a
         # memory-mapped .bin file: served by the host gather pool)
-        all_pinned = all(t.is_pinned() for t in self._fields.values())
+        all_pinned = all(t.is_pinned() for name, t in self._fields.items() if name not in self._lines)
         # high priority: the next batch's transfer should start as soon as it is submitted
         self._copy_stream = torch.cuda.Stream(device=device, priority=-1)
         self.path = path or os.environ.get("FRL_B200_INPUT_PATH", "auto")
+        if self._lines:
+            if self.path not in ("auto", "kernel"):
+                raise ValueError("input path %r cannot serve the padded text field(s) %s: only the "
+                                 "GPU-pulled kernel path gathers ragged lines"
+                                 % (self.path, ", ".join(repr(k) for k in self._lines)))
+            self.path = "kernel"
         if self.path == "auto":
             self.path = default_input_path() if all_pinned else "host"
         if self.path != "host" and not all_pinned:
@@ -165,6 +204,9 @@ class DeviceBatchLoader:
         tolerant = set(getattr(dataset.device_transform, "bf16_wire_fields", ()) or ())
         self._wire_dtype: Dict[str, torch.dtype] = {}
         for name, t in self._fields.items():
+            if name in self._lines:
+                self._wire_dtype[name] = torch.uint8
+                continue
             cvt = (self.wire in ("auto", "bf16") and out_dtype == torch.bfloat16
                    and t.dtype == torch.float32 and name in tolerant)
             self._wire_dtype[name] = torch.bfloat16 if cvt else t.dtype
@@ -178,17 +220,21 @@ class DeviceBatchLoader:
                 except AttributeError:
                     pass
             for name, t in self._fields.items():
-                if self._wire_dtype[name] != t.dtype:
+                if name not in self._lines and self._wire_dtype[name] != t.dtype:
                     key = (name, t.data_ptr(), self._wire_dtype[name])
                     if key not in cache:
                         cache[key] = t.to(self._wire_dtype[name]).pin_memory()
                     converted[name] = cache[key]
             if converted:
                 self._fields = {k: converted.get(k, v) for k, v in self._fields.items()}
+        # the corpus is page-locked in this (rank) process, its start table uploaded, on first use
+        self._line_src = {name: (f.corpus.pin(), f.starts_on(device)) for name, f in self._lines.items()}
+        row_shape = {name: ((f.row_len,) if name in self._lines else tuple(f.shape[1:]))
+                     for name, f in self._fields.items()}
         self._slots = []
         for _ in range(self.depth):
-            slot = {name: torch.empty((batch_size,) + tuple(t.shape[1:]), dtype=self._wire_dtype[name],
-                                      device=device) for name, t in self._fields.items()}
+            slot = {name: torch.empty((batch_size,) + row_shape[name], dtype=self._wire_dtype[name],
+                                      device=device) for name in self._fields}
             slot["__idx_host"] = torch.empty(batch_size, dtype=torch.int64, pin_memory=True)
             slot["__idx_dev"] = torch.empty(batch_size, dtype=torch.int64, device=device)
             self._slots.append(slot)
@@ -208,8 +254,8 @@ class DeviceBatchLoader:
                                for _ in range(self._n_stage)]
             self._dma_done = [torch.cuda.Event() for _ in range(self._n_stage)]
         self.h2d_bytes_per_batch = sum(
-            t[0].numel() * torch.empty(0, dtype=self._wire_dtype[name]).element_size()
-            for name, t in self._fields.items()) * batch_size + 8 * batch_size
+            math.prod(row_shape[name]) * torch.empty(0, dtype=self._wire_dtype[name]).element_size()
+            for name in self._fields) * batch_size + 8 * batch_size
 
     def __len__(self) -> int:
         return len(self._index_loader)
@@ -256,6 +302,13 @@ class DeviceBatchLoader:
             self._copy_stream.wait_event(self._freed[s])          # previous user of the slot is done
             slot["__idx_dev"][:n].copy_(slot["__idx_host"][:n], non_blocking=True)
             for name, src in self._fields.items():
+                if name in self._lines:
+                    corpus = src.corpus
+                    addr, starts_dev = self._line_src[name]
+                    _native.gather_lines(addr, corpus.n_bytes, corpus.alloc_bytes, starts_dev,
+                                         slot["__idx_dev"][:n], slot[name][:n], pad=src.pad,
+                                         max_blocks=self.blocks)
+                    continue
                 row_bytes = src[0].numel() * src.element_size()
                 wide = row_bytes >= 4096 and row_bytes % 16 == 0
                 if wide and self.path == "tma":

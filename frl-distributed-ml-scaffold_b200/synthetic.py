@@ -10,6 +10,8 @@ as ``frldistml.scaffold`` (oracle only) to run the very same Problem on the refe
 * ``make_resnet_problem`` — config 4 (torchvision resnet18 trunk + one CE head, 11 689 512
   parameters) and config 5 (resnet50 trunk + heads 2048->{1000 CE, 100 CE, 10 MSE, 4 MSE},
   25 790 618 parameters) on synthetic 3xHxW images.
+* ``make_text_problem`` — next-byte prediction over the lines of two ``TextDataset`` corpora
+  (``write_text_corpus`` / ``write_mixed_text_corpus`` write seeded ones).
 """
 import importlib
 from types import SimpleNamespace
@@ -437,3 +439,151 @@ def make_resnet_problem(ns, save_dir: str, config: str = "resnet18", image: int 
     return _problem_class(ns)(tasks, [], fields, save_dir, shift=0.0, scale=1.0, pinned=pinned,
                               base_factory=base_factory,
                               channel_affine=U8_CHANNEL_AFFINE if uint8 else None)
+
+
+# ---- text: next-byte prediction over TextDataset lines ---------------------------------------
+
+def write_text_corpus(path: str, n_lines: int, seed: int, seq_len: int = 32,
+                      max_len: Optional[int] = None) -> None:
+    """A deterministic newline-separated corpus: empty lines and lines shorter than, exactly
+    ``seq_len + 1`` and longer than that, bytes drawn from 0x00-0xFF except ``\\n``, and no
+    trailing newline (so the last line loses two bytes, as in the reference's TextDataset)."""
+    rs = np.random.RandomState(seed)
+    row = seq_len + 1
+    max_len = max_len or 3 * row
+    forced = [0, 1, row - 1, row, row + 1, max_len]
+    lengths = np.concatenate([np.asarray(forced[:n_lines], dtype=np.int64),
+                              rs.randint(0, max_len + 1, size=max(n_lines - len(forced), 0))])
+    values = np.delete(np.arange(256, dtype=np.uint8), 0x0A)
+    body = values[rs.randint(0, 255, size=int(lengths.sum()))]
+    out = np.empty(int(lengths.sum()) + max(n_lines - 1, 0), dtype=np.uint8)
+    pos = src = 0
+    for i, n in enumerate(lengths):
+        out[pos:pos + n] = body[src:src + n]
+        pos += int(n)
+        src += int(n)
+        if i + 1 < n_lines:
+            out[pos] = 0x0A
+            pos += 1
+    with open(path, "wb") as f:
+        f.write(out.tobytes())
+
+
+class PositionsToClasses(nn.Module):
+    """[B, L, C] per-position logits -> [B, C, L], the layout ``nn.CrossEntropyLoss`` takes for
+    per-position classes."""
+
+    def forward(self, x: torch.Tensor) -> torch.Tensor:
+        return x.transpose(1, 2)
+
+
+def _text_device_transform():
+    """Batched twin of the text transform: x = line[:, :-1], y = line[:, 1:] as int64."""
+    from .transform import DeviceBatchTransform
+
+    class NextByteDeviceTransform(DeviceBatchTransform):
+        def apply(self, raw, split, out_dtype):
+            line = raw["line"]
+            return [line[:, :-1].long()], [(line[:, 1:].long(),)]
+
+        def meta(self, raw, index):
+            return {}                      # the per-sample transform's meta has no fields
+
+    return NextByteDeviceTransform()
+
+
+def make_text_problem(ns, save_dir: str, train_path, test_path, seq_len: int = 32,
+                      device_batches: bool = False, hidden: int = 128):
+    """Next-byte prediction on the lines of two text files: Embedding(256, 64), then per position
+    Linear(64, hidden) + ReLU + Linear(hidden, 256), one CrossEntropyLoss(ignore_index=0) task
+    (padding bytes are not predicted).  ``device_batches``: hand the datasets the batched twin
+    of the transform, so the loop serves them through ``DeviceBatchLoader`` (K8t)."""
+    text = importlib.import_module(f"{ns.name}.text_dataset")
+    as_path = getattr(text, "StoragePath", str)          # the reference's TextDataset takes StoragePaths
+
+    class NextByteTask(ns.Task):
+        name = "next_byte"
+
+        @property
+        def network_head(self) -> nn.Module:
+            return nn.Sequential(nn.Linear(hidden, 256), PositionsToClasses())
+
+        @property
+        def criterion(self):
+            return nn.CrossEntropyLoss(ignore_index=0)
+
+        @property
+        def criterion_weight(self) -> float:
+            return 1.0
+
+        def get_target(self, tensors, transform):
+            return (tensors["line"][1:].long(),), NoMeta()
+
+        def compute_batch_metrics(self, meta, target, output):
+            y = target[0]
+            wrong = ((output.argmax(1) != y) & (y != 0)).float().mean(1)
+            return {"byte_err": wrong if wrong.is_cuda else wrong.numpy()}
+
+        @property
+        def rankable_metrics(self):
+            return {("byte_err", ns.Ordering.DESC)}
+
+        def summarize_epoch_metrics(self, batch_metrics):
+            return {"byte_err": float(np.mean(batch_metrics["byte_err"]))}
+
+        def summarize_epoch_samples(self, data, target, meta, output, metric):
+            return []
+
+    class NextByteTransform(ns.MultiTaskTransform):
+        def transform_source_data(self, tensors, split):
+            return [tensors["line"][:-1].long()], NoTransformState()
+
+    class TextProblem(ns.MultiTaskProblem):
+        BatchMetaType = BatchMeta
+
+        def __init__(self) -> None:
+            self._tasks = [NextByteTask()]
+            self.transform = NextByteTransform(self._tasks, NoMeta)
+            kw = {"device_transform": _text_device_transform()} if device_batches else {}
+            self._datasets = [text.TextDataset(split, as_path(str(path)), self.transform, seq_len, **kw)
+                              for split, path in ((ns.Split.TRAIN, train_path), (ns.Split.TEST, test_path))]
+
+        @property
+        def datasets(self):
+            return self._datasets
+
+        @property
+        def save_dir(self) -> str:
+            return save_dir
+
+        @property
+        def anno_param(self):
+            return None
+
+        def get_model_base(self) -> nn.Module:
+            return nn.Sequential(ns.model.ListSelect(sel_index=0, num_elements=1), nn.Embedding(256, 64),
+                                 nn.Linear(64, hidden), nn.ReLU())
+
+        def get_criterion(self):
+            return ns.criteria.ParallelCriterion([t.criterion for t in self._tasks], [1.0],
+                                                 [t.name for t in self._tasks])
+
+    return TextProblem()
+
+
+def write_mixed_text_corpus(path: str, n_bytes: int, seed: int, short_mean: int = 120,
+                            long_mean: int = 2048, long_share: float = 0.1) -> None:
+    """About ``n_bytes`` of seeded text for measurements: line lengths drawn from a mixture of
+    two exponentials (means ``short_mean`` and ``long_mean`` bytes), bytes 0x00-0xFF except
+    ``\\n``."""
+    rs = np.random.RandomState(seed)
+    mean = (1 - long_share) * short_mean + long_share * long_mean
+    n_lines = max(1, int(n_bytes / (mean + 1)))
+    long = rs.rand(n_lines) < long_share
+    lengths = np.where(long, rs.exponential(long_mean, n_lines), rs.exponential(short_mean, n_lines)).astype(np.int64)
+    ends = np.cumsum(lengths + 1) - 1                   # position of each line's newline
+    values = np.delete(np.arange(256, dtype=np.uint8), 0x0A)
+    out = values[rs.randint(0, 255, size=int(ends[-1]))]
+    out[ends[:-1]] = 0x0A
+    with open(path, "wb") as f:
+        f.write(out.tobytes())

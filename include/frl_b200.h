@@ -284,6 +284,18 @@ int frl_gather_window_rows(const void* const* batch_ptrs, const int64_t* batch_r
  * of 16 bytes.  max_blocks <= 0 -> one CTA per SM. */
 int frl_gather_rows_tma(const void* src_mapped, int64_t src_rows, const int64_t* idx_dev, void* dst,
                         int64_t n_rows, int64_t row_bytes, int max_blocks, void* stream);
+/* K8t — padded lines of a newline-separated text corpus in pinned, device-mapped host memory.
+ * Replaces the per-sample TextDataset.get_raw_item + transform + default_collate of the loop
+ * (reference text_dataset.py, solver_worker.py:462-469).  For row r, with i = idx_dev[r]
+ * (an index outside [0, n_lines) reads line 0):
+ *   lo = starts_dev[i], len = clamp(starts_dev[i+1] - 1 - lo, 0, row_len), at most corpus_bytes - lo;
+ *   dst[r, j] = corpus[lo + j] for j < len, else pad.
+ * corpus_mapped: 16-byte aligned, corpus_alloc_bytes >= corpus_bytes rounded up to 16 (the
+ * kernel reads only aligned 16-byte units, each once).  starts_dev: int64 [n_lines + 1] on the
+ * device; dst: uint8 [n_rows, row_len], contiguous, any alignment.  max_blocks <= 0 -> 8 CTAs. */
+int frl_gather_lines(const void* corpus_mapped, int64_t corpus_bytes, int64_t corpus_alloc_bytes,
+                     const int64_t* starts_dev, int64_t n_lines, const int64_t* idx_dev,
+                     void* dst, int64_t n_rows, int64_t row_len, int pad, int max_blocks, void* stream);
 
 /* ------------------------------------------------------------------------------------------
  * Host gather pool — the host half of the input path (no CUDA calls inside).

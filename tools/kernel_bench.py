@@ -240,8 +240,45 @@ def bench_k8(iters):
     return out
 
 
+def bench_k8t(iters):
+    """K8t at batch 4096 over a 256 MB seeded corpus in pinned memory (line lengths: a mixture
+    with means of 120 B and 2 KB, so rows are padded and cut), next to K8 at the same batch and
+    row bytes rounded up to 16 (the fixed-row ceiling).  ``bytes`` = rows delivered to HBM."""
+    import tempfile
+    import numpy as np
+    from frl_b200 import synthetic, text_dataset
+    from frl_b200.types import Split
+    out = []
+    B = 4096
+    with tempfile.TemporaryDirectory() as tmp:
+        path = os.path.join(tmp, "corpus.txt")
+        synthetic.write_mixed_text_corpus(path, 256 << 20, 0)
+        for row_len in (257, 1025):
+            ds = text_dataset.TextDataset(Split.TRAIN, path, lambda raw, split: raw, row_len - 1)
+            field = ds.pinned_fields["line"]
+            addr, starts = field.corpus.pin(), field.starts_on(DEV)
+            g = torch.Generator().manual_seed(row_len)
+            idx = [torch.randint(0, len(ds), (B,), generator=g).to(DEV) for _ in range(8)]
+            lens = np.minimum(np.maximum(np.diff(ds._sample_indices) - 1, 0), row_len)
+            payload = np.mean([lens[i.cpu().numpy()].sum() for i in idx])
+            dst = torch.empty(B, row_len, dtype=torch.uint8, device=DEV)
+            out.append(timed("K8t gather_lines row_len=%d, 8 CTAs" % row_len,
+                             lambda i: _native.gather_lines(addr, field.corpus.n_bytes, field.corpus.alloc_bytes,
+                                                            starts, idx[i % 8], dst, max_blocks=8),
+                             1, B * row_len, iters, "line payload %.0f B/batch; PCIe-bound" % payload))
+            rb = (row_len + 15) // 16 * 16
+            src = torch.zeros((256 << 20) // rb, rb, dtype=torch.uint8, pin_memory=True)
+            ridx = torch.randint(0, src.shape[0], (B,), generator=g).to(DEV)
+            rdst = torch.empty(B, rb, dtype=torch.uint8, device=DEV)
+            out.append(timed("K8 gather_rows row_bytes=%d, 8 CTAs (fixed-row ceiling)" % rb,
+                             lambda i: _native.gather_rows(src, ridx, rdst, max_blocks=8), 1, B * rb, iters,
+                             "PCIe-bound"))
+            del ds, field, src
+    return out
+
+
 BENCHES = {"k2": bench_k2, "k2mt": bench_k2mt, "k3": bench_k3, "k4": bench_k4, "k5": bench_k5, "k6": bench_k6,
-           "k8": bench_k8}
+           "k8": bench_k8, "k8t": bench_k8t}
 
 
 def main():

@@ -2,11 +2,16 @@
 """Stand-alone timing of the candidate host->HBM row-gather paths (one GPU).
 
     python tools/probe_input_path.py [rows_per_batch] [row_elems]
+    python tools/probe_input_path.py --text [batch] [seq_len]
 
 Prints GB/s of: contiguous cudaMemcpyAsync (PCIe reference), frl_gather_rows at several grid
 sizes, frl_gather_rows_tma, the native host gather pool per thread count (plain and with the
 fp32 -> bf16 wire conversion), and the host cost of drawing one index batch from the DataLoader
 machinery.
+
+``--text``: batches/s served by ``DeviceBatchLoader`` (K8t + the batched transform) against the
+per-sample ``DataLoader`` (``TextDataset.__getitem__`` + transform + ``default_collate``) at 4 and
+16 workers, over the same 256 MB seeded corpus, no model; host clock around a device synchronise.
 """
 import os
 import sys
@@ -17,6 +22,47 @@ sys.path.insert(0, REPO)
 import torch  # noqa: E402
 import frl_b200  # noqa: E402,F401
 from frl_b200 import _native  # noqa: E402
+
+
+
+def probe_text(batch: int, seq_len: int, n_batches: int = 40) -> None:
+    import tempfile
+    from frl_b200 import synthetic
+    from frl_b200.device_loader import DeviceBatchLoader
+    ns = synthetic.api_namespace("frl_b200")
+    dev = torch.device("cuda", 0)
+    with tempfile.TemporaryDirectory() as tmp:
+        path = os.path.join(tmp, "corpus.txt")
+        synthetic.write_mixed_text_corpus(path, 256 << 20, 0)
+        fast = synthetic.make_text_problem(ns, tmp, path, path, seq_len=seq_len, device_batches=True)
+        plain = synthetic.make_text_problem(ns, tmp, path, path, seq_len=seq_len)
+        print("text corpus %d lines, batch %d x %d B" % (len(fast.datasets[0]), batch, seq_len + 1))
+
+        def rate(loader, to_device):
+            it = iter(loader)
+            next(it)                                        # warm-up: workers started, first batch
+            torch.cuda.synchronize()
+            t0 = time.perf_counter()
+            for _ in range(n_batches):
+                data, target, _ = next(it)
+                if to_device:
+                    data[0].to(dev, non_blocking=True)
+                    target[0][0].to(dev, non_blocking=True)
+            torch.cuda.synchronize()
+            return n_batches / (time.perf_counter() - t0)
+
+        ld = DeviceBatchLoader(fast.datasets[0], batch_size=batch, sampler=None, device=dev)
+        print("DeviceBatchLoader (K8t, %d CTAs): %8.1f batches/s" % (ld.blocks, rate(ld, False)), flush=True)
+        for workers in (4, 16):
+            dl = torch.utils.data.DataLoader(plain.datasets[0], batch_size=batch, shuffle=True,
+                                             num_workers=workers, pin_memory=True)
+            print("per-sample DataLoader, %2d workers: %8.1f batches/s" % (workers, rate(dl, True)), flush=True)
+
+
+if len(sys.argv) > 1 and sys.argv[1] == "--text":
+    torch.cuda.set_device(0)
+    probe_text(int(sys.argv[2]) if len(sys.argv) > 2 else 4096, int(sys.argv[3]) if len(sys.argv) > 3 else 256)
+    sys.exit(0)
 
 B = int(sys.argv[1]) if len(sys.argv) > 1 else 4096
 W = int(sys.argv[2]) if len(sys.argv) > 2 else 4096
