@@ -16,6 +16,8 @@ LIB_PATH = os.path.join(CSRC_DIR, "libfrl_b200.so")
 
 F32, BF16, U8, I64 = 0, 1, 2, 3
 LOSS_MSE, LOSS_CE = 0, 1
+FP8_E4M3, FP8_E5M2 = 0, 1
+FP8_DTYPE = {FP8_E4M3: torch.float8_e4m3fn, FP8_E5M2: torch.float8_e5m2}
 MAX_TASKS = 8
 
 _DTYPE_CODE = {torch.float32: F32, torch.bfloat16: BF16, torch.uint8: U8, torch.bool: U8,
@@ -86,6 +88,8 @@ SIGNATURES = {
     "frl_nvls_rmsprop": (_i, [_vp, _vp, _vp, _vp, _vp, _i64, _i, _i, _vp, _i, _vp, _i, _d, _d, _d, _d, _d, _d,
                               _vp, _i, _i, _vp]),
     "frl_nvls_barrier": (_i, [_vp, _i, _i, _i, _vp]),
+    "frl_fp8_amax": (_i, [_vp, _i64, _i, _vp, _vp]),
+    "frl_fp8_quantize": (_i, [_vp, _i64, _i64, _i, _vp, _i, _vp, _vp, _vp, _vp]),
 }
 
 _lib: Optional[C.CDLL] = None
@@ -332,6 +336,29 @@ NVLS_EXTERNAL_SYNC = 1
 def nvls_barrier(link, slot: int) -> None:
     _check(lib().frl_nvls_barrier(link.pads_dev, link.rank, link.world, slot, _stream()),
            "frl_nvls_barrier")
+
+
+# ---- K9 -------------------------------------------------------------------------------------
+
+def fp8_amax(src, amax_out) -> None:
+    """amax_out[0] = max |src| (NaN if src holds one) for a contiguous bf16/fp32 device tensor;
+    ``amax_out``: device fp32 scalar, zeroed by the call itself."""
+    assert src.is_contiguous() and amax_out.dtype == torch.float32
+    _check(lib().frl_fp8_amax(_ptr(src), src.numel(), dtype_code(src.dtype), _ptr(amax_out), _stream()),
+           "frl_fp8_amax")
+
+
+def fp8_quantize(src, amax, fmt: int, dst=None, dst_t=None, inv_scale_out=None) -> None:
+    """Codes of the 2-D ``src`` [rows, cols] at the power-of-two scale ``amax`` implies: ``dst``
+    [rows, cols] and/or ``dst_t`` [cols, rows] of the ``fmt`` float8 dtype; ``inv_scale_out``
+    (device fp32 scalar) receives 1 / scale.  See frl_fp8_quantize in include/frl_b200.h."""
+    rows, cols = src.shape
+    want = FP8_DTYPE[fmt]
+    assert src.is_contiguous() and amax.dtype == torch.float32 and inv_scale_out.dtype == torch.float32
+    assert dst is None or (dst.shape == (rows, cols) and dst.dtype == want and dst.is_contiguous())
+    assert dst_t is None or (dst_t.shape == (cols, rows) and dst_t.dtype == want and dst_t.is_contiguous())
+    _check(lib().frl_fp8_quantize(_ptr(src), rows, cols, dtype_code(src.dtype), _ptr(amax), fmt, _ptr(dst),
+                                  _ptr(dst_t), _ptr(inv_scale_out), _stream()), "frl_fp8_quantize")
 
 
 # ---- K8 -------------------------------------------------------------------------------------

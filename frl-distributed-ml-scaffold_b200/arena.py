@@ -111,20 +111,20 @@ class ParamArena:
                     continue
                 if p.dtype != torch.float32:
                     raise TypeError(f"arena expects fp32 parameters at wrap time, got {p.dtype}")
-                uses_lp = is_model and precision == Precision.BF16
+                uses_lp = is_model and precision.bf16_storage
                 self.slots.append(ArenaSlot(p, off, p.numel(), tuple(p.shape), is_model, uses_lp, idx))
                 off = _round_up(off + p.numel(), ALIGN_ELEMS)
             if is_model:
                 self.model_end = off        # padded end of the model-parameter range
         self.numel = off
-        self.grad_dtype = torch.bfloat16 if precision == Precision.BF16 else torch.float32
+        self.grad_dtype = torch.bfloat16 if precision.bf16_storage else torch.float32
 
         def shared(dtype):
             if shared_allocator is not None and self.numel > 0:
                 return shared_allocator(self.numel, dtype)
             return torch.zeros(self.numel, dtype=dtype, device=self.device)
 
-        bf16_mode = precision == Precision.BF16
+        bf16_mode = precision.bf16_storage
         self.master = (torch.zeros(self.numel, dtype=torch.float32, device=self.device)
                        if bf16_mode else shared(torch.float32))
         with torch.no_grad():

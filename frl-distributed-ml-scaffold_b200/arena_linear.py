@@ -24,6 +24,17 @@ Unless ``FRL_B200_FUSE_RELU=0``, a ``nn.Linear`` directly followed by a ``nn.ReL
   backward  dZ = (y > 0) * dY, db = colsum(dZ) ONE pass (``frl_drelu_colsum``, K6b) instead of
                                                threshold_backward + a reduction
             dX = dZ W, dW = dZ^T X             as above
+
+In a ``Precision.FP8`` run a site whose weight lives in the bf16 shadow and whose widths are
+multiples of 16 (``fp8_site_qualifies``) runs its three GEMMs on the FP8 tensor cores
+(``torch._scaled_mm``, tensor-wise scales, bf16 output, fp32 accumulation) for every call whose
+flattened row count is a multiple of 16; other calls take the bf16 Functions above.  Each operand
+is quantised by K9 at a power-of-two scale from its own amax (``frl_fp8_amax`` +
+``frl_fp8_quantize``), one pass giving the row-major copy and, for backward, the transposed one:
+
+  forward   Y  = Xq Wq^T (+ b)        Xq, Wq e4m3; saved for backward: Xq^T, Wq^T (not bf16 X)
+  backward  dX = dZq (Wq^T)^T         dZq e5m2
+            dW = dZq^T (Xq^T)^T       into the arena as above; db as above
 """
 import os
 import types
@@ -35,8 +46,78 @@ import torch.nn as nn
 import torch.nn.functional as F
 
 from . import _native
+from .types import Precision
 
 KERNELS = _native
+
+#: FP8 GEMM operands need K, N (and, for the weight gradient, M) to be multiples of 16
+FP8_MULTIPLE = 16
+
+
+def fp8_site_qualifies(uses_lp: bool, in_features: int, out_features: int) -> bool:
+    """Whether an FP8 run runs a Linear site's GEMMs in FP8 (the row count is checked per call):
+    the weight lives in the bf16 shadow and both widths are multiples of 16."""
+    return bool(uses_lp) and in_features % FP8_MULTIPLE == 0 and out_features % FP8_MULTIPLE == 0
+
+
+def fp8_call_qualifies(x: torch.Tensor) -> bool:
+    """Per call: a bf16/fp32 input whose flattened row count is a positive multiple of 16 and
+    whose rows start on a 16-byte boundary (a contiguous input is quantised in place; any other
+    is copied first)."""
+    if x.dim() == 0 or x.shape[-1] == 0 or x.dtype not in (torch.bfloat16, torch.float32):
+        return False
+    m = x.numel() // x.shape[-1]
+    return m > 0 and m % FP8_MULTIPLE == 0 and (not x.is_contiguous() or x.data_ptr() % 16 == 0)
+
+
+def _fp8_quantize(t2: torch.Tensor, fmt: int, rowmajor: bool, transposed: bool):
+    """(row-major codes or None, transposed codes or None, 1/scale as a device scalar) of the
+    contiguous 2-D ``t2`` at the scale its own amax implies (K9: two launches, no host sync)."""
+    sc = torch.empty(2, dtype=torch.float32, device=t2.device)          # [amax, 1/scale]
+    dt = _native.FP8_DTYPE[fmt]
+    q = torch.empty(t2.shape, dtype=dt, device=t2.device) if rowmajor else None
+    qt = torch.empty((t2.shape[1], t2.shape[0]), dtype=dt, device=t2.device) if transposed else None
+    KERNELS.fp8_amax(t2, sc[:1])
+    KERNELS.fp8_quantize(t2, sc[:1], fmt, q, qt, sc[1:])
+    return q, qt, sc[1]
+
+
+def _fp8_mm(a, b_t, scale_a, scale_b, bias=None, out=None):
+    """a @ b_t^T in bf16 for row-major fp8 ``a`` [M, K] and ``b_t`` [N, K] (b_t.t() is the
+    column-major [K, N] operand ``torch._scaled_mm`` wants)."""
+    return torch._scaled_mm(a, b_t.t(), scale_a, scale_b, bias=bias, out_dtype=torch.bfloat16,
+                            use_fast_accum=False, out=out)
+
+
+def _fp8_operands(x, weight, transposed: bool):
+    x2 = x.reshape(-1, x.shape[-1])
+    if not x2.is_contiguous():
+        x2 = x2.contiguous()
+    xq, xtq, sx = _fp8_quantize(x2, _native.FP8_E4M3, True, transposed)
+    wq, wtq, sw = _fp8_quantize(weight, _native.FP8_E4M3, True, transposed)
+    return xq, xtq, sx, wq, wtq, sw
+
+
+def _fp8_backward(ctx, site, dz2, db_from_dz):
+    """dX and dW of an FP8 site from the bf16 output gradient ``dz2`` (after the ReLU mask).
+    Inside an open pipeline step dW goes to the arena and the bias gradient, unless
+    ``db_from_dz`` is False (already written), is ``frl_colsum(dz2)`` into its slice."""
+    xtq, wtq, sx, sw = ctx.saved_tensors[:4]
+    need_dx = ctx.needs_input_grad[0]
+    dzq, dztq, sdz = _fp8_quantize(dz2, _native.FP8_E5M2, need_dx, True)
+    # dX first: marking the weight's slot ready may launch the bucket's update, which overwrites W
+    dx = _fp8_mm(dzq, wtq, sdz, sw).view(ctx.x_shape) if need_dx else None
+    pipe = site.pipeline
+    if pipe is not None and pipe.step_open:
+        site.weight_grad_fp8(pipe, dztq, xtq, sdz, sx)
+        if db_from_dz and ctx.has_bias and site.bslot is not None:
+            KERNELS.colsum(dz2, pipe.arena.grad_view(site.bslot),
+                           accumulate=not site.bstate.first_touch(pipe.step_id))
+        site.backward_done(pipe)
+        return dx, None, None, None, None
+    dw = _fp8_mm(dztq, xtq, sdz, sx) if ctx.needs_input_grad[1] else None
+    db = dz2.sum(0) if (ctx.has_bias and ctx.needs_input_grad[2]) else None
+    return dx, dw, db, None, None
 
 
 class _ArenaLinearFn(torch.autograd.Function):
@@ -121,6 +202,68 @@ class _ArenaLinearReluFn(torch.autograd.Function):
         dw = dz.t().mm(x2) if ctx.needs_input_grad[1] else None
         db = dz.sum(0) if ctx.needs_input_grad[2] else None
         return dx, dw, db, None
+
+
+class _Fp8LinearFn(torch.autograd.Function):
+    """FP8 form of ``_ArenaLinearFn`` (see the module docstring).  ``for_backward``: whether the
+    call records a graph (grad mode on and an input requires grad); otherwise only the row-major
+    copies the forward GEMM reads are made."""
+
+    @staticmethod
+    def forward(ctx, x, weight, bias, site, for_backward):
+        ctx.site = site
+        ctx.has_bias = bias is not None
+        ctx.x_shape = x.shape
+        xq, xtq, sx, wq, wtq, sw = _fp8_operands(x, weight, for_backward)
+        # the output must not be a view (see _ArenaLinearFn.forward): GEMM into a view of it
+        y = torch.empty(*x.shape[:-1], weight.shape[0], dtype=torch.bfloat16, device=x.device)
+        _fp8_mm(xq, wq, sx, sw, bias=bias, out=y.view(-1, weight.shape[0]))
+        if for_backward:
+            ctx.save_for_backward(xtq, wtq, sx, sw)
+        return y
+
+    @staticmethod
+    @torch.autograd.function.once_differentiable
+    def backward(ctx, dy):
+        dy2 = dy.reshape(-1, dy.shape[-1])
+        if not dy2.is_contiguous():
+            dy2 = dy2.contiguous()
+        return _fp8_backward(ctx, ctx.site, dy2, True)
+
+
+class _Fp8LinearReluFn(torch.autograd.Function):
+    """FP8 form of ``_ArenaLinearReluFn``: the FP8 GEMM with bias, then ReLU; backward runs
+    ``frl_drelu_colsum`` (dZ and the bias gradient in one pass) and then quantises dZ."""
+
+    @staticmethod
+    def forward(ctx, x, weight, bias, site, for_backward):
+        ctx.site = site
+        ctx.has_bias = True
+        ctx.x_shape = x.shape
+        xq, xtq, sx, wq, wtq, sw = _fp8_operands(x, weight, for_backward)
+        y = torch.empty(*x.shape[:-1], weight.shape[0], dtype=torch.bfloat16, device=x.device)
+        _fp8_mm(xq, wq, sx, sw, bias=bias, out=y.view(-1, weight.shape[0]))
+        y.relu_()
+        if for_backward:
+            ctx.save_for_backward(xtq, wtq, sx, sw, y)
+        return y
+
+    @staticmethod
+    @torch.autograd.function.once_differentiable
+    def backward(ctx, dy):
+        y = ctx.saved_tensors[4]
+        site = ctx.site
+        dy2 = dy.reshape(-1, dy.shape[-1])
+        if not dy2.is_contiguous():
+            dy2 = dy2.contiguous()
+        y2 = y.reshape(-1, y.shape[-1])
+        pipe = site.pipeline
+        if pipe is not None and pipe.step_open:
+            dz = torch.empty_like(dy2)
+            KERNELS.drelu_colsum(dy2, y2, dz, pipe.arena.grad_view(site.bslot),
+                                 accumulate=not site.bstate.first_touch(pipe.step_id))
+            return _fp8_backward(ctx, site, dz, False)
+        return _fp8_backward(ctx, site, dy2 * (y2 > 0).to(dy2.dtype), True)
 
 
 class _ArenaMultiHeadFn(torch.autograd.Function):
@@ -277,7 +420,7 @@ class LinearSite:
     site counts its applications in the forward pass (training mode, autograd on) and marks its
     slots ready only when as many backward passes have run; anything left over is marked by
     ``GradBucketPipeline.finish_step`` (after ``backward()`` returned nothing can be missing)."""
-    __slots__ = ("module", "wslot", "bslot", "pipeline", "relu", "wstate", "bstate", "multihead")
+    __slots__ = ("module", "wslot", "bslot", "pipeline", "relu", "wstate", "bstate", "multihead", "fp8")
 
     def __init__(self, module, wslot, bslot, pipeline):
         self.module = module
@@ -286,6 +429,7 @@ class LinearSite:
         self.pipeline = pipeline
         self.relu = None              # the nn.ReLU this layer absorbed (FRL_B200_FUSE_RELU)
         self.multihead = None         # on the first head: the MultiHeadSite of its model
+        self.fp8 = False              # Precision.FP8 and fp8_site_qualifies: FP8 GEMMs per call
         states = pipeline.slot_states
         self.wstate = states.setdefault(wslot.index, SlotState())
         self.bstate = states.setdefault(bslot.index, SlotState()) if bslot is not None else None
@@ -308,6 +452,22 @@ class LinearSite:
         else:
             torch.mm(dz.t(), x2, out=gw)
 
+    def weight_grad_fp8(self, pipe, dztq, xtq, s_dz, s_x) -> None:
+        """``weight_grad`` from the transposed FP8 copies dZ^T [N, M] and X^T [K, M].  A row-split
+        weight takes two GEMMs only if the first block is a multiple of 16 rows."""
+        gw = pipe.arena.grad_view(self.wslot)
+        st = self.wstate
+        if not st.first_touch(pipe.step_id):
+            gw.add_(_fp8_mm(dztq, xtq, s_dz, s_x))
+            return
+        rows = pipe.row_split(self.wslot)
+        if rows and rows % FP8_MULTIPLE == 0 and st.fwd_gen == pipe.forward_gen and st.fwd_count == 1:
+            _fp8_mm(dztq[:rows], xtq, s_dz, s_x, out=gw[:rows])
+            pipe.rows_ready(self.wslot, rows)
+            _fp8_mm(dztq[rows:], xtq, s_dz, s_x, out=gw[rows:])
+        else:
+            _fp8_mm(dztq, xtq, s_dz, s_x, out=gw)
+
     def count_forward(self) -> None:
         pipe = self.pipeline
         if pipe is not None and self.module.training and torch.is_grad_enabled():
@@ -329,14 +489,24 @@ class LinearSite:
                 pipe.defer_ready(self.bslot)
 
 
+def _for_backward(*tensors) -> bool:
+    return torch.is_grad_enabled() and any(t is not None and t.requires_grad for t in tensors)
+
+
 def _forward(self, x):
-    self._frl_site.count_forward()        # here, not inside the Function: grad mode is off in there
-    return _ArenaLinearFn.apply(x, self.weight, self.bias, self._frl_site)
+    site = self._frl_site
+    site.count_forward()                  # here, not inside the Function: grad mode is off in there
+    if site.fp8 and fp8_call_qualifies(x):
+        return _Fp8LinearFn.apply(x, self.weight, self.bias, site, _for_backward(x, self.weight, self.bias))
+    return _ArenaLinearFn.apply(x, self.weight, self.bias, site)
 
 
 def _forward_relu(self, x):
-    self._frl_site.count_forward()
-    return _ArenaLinearReluFn.apply(x, self.weight, self.bias, self._frl_site)
+    site = self._frl_site
+    site.count_forward()
+    if site.fp8 and fp8_call_qualifies(x):
+        return _Fp8LinearReluFn.apply(x, self.weight, self.bias, site, _for_backward(x, self.weight, self.bias))
+    return _ArenaLinearReluFn.apply(x, self.weight, self.bias, site)
 
 
 def _identity(self, x):
@@ -387,10 +557,16 @@ def patch_linears(model: nn.Module, pipeline) -> List[LinearSite]:
         if mod.bias is not None and bslot is None:
             continue                     # frozen bias: leave the module alone
         site = LinearSite(mod, wslot, bslot, pipeline)
+        site.fp8 = (arena.precision is Precision.FP8
+                    and fp8_site_qualifies(wslot.uses_lp, mod.in_features, mod.out_features))
         sites.append(site)
     if os.environ.get("FRL_B200_FUSE_RELU", "1") != "0":
         _fuse_relu_pairs(model, sites)
     _attach_multihead(model, sites, pipeline)
+    for site in sites:
+        if site.multihead is not None:              # the fused task heads stay bf16
+            for h in site.multihead.heads:
+                h.fp8 = False
     repatch_linears(sites)
     return sites
 

@@ -23,7 +23,6 @@ import logging
 import torch
 
 from . import _native
-from .types import Precision
 
 logger = logging.getLogger(__name__)
 
@@ -84,7 +83,7 @@ class _Captured:
     def __init__(self, worker, data, target) -> None:
         self.worker = worker
         w = worker
-        bf16 = w.precision == Precision.BF16
+        bf16 = w.precision.bf16_storage
         self.static_in: List[torch.Tensor] = []
         self.cast_in: List[bool] = []
         for t in data:

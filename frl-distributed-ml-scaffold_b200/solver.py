@@ -300,7 +300,7 @@ class Solver:
         arena = ParamArena(model.parameters(), criterion.parameters(), device=device,
                            precision=args.precision, shared_allocator=symm_alloc,
                            adjacent=head_layout_groups(model))
-        if (args.precision == Precision.BF16 and any(b.is_floating_point() for b in model.buffers())
+        if (args.precision.bf16_storage and any(b.is_floating_point() for b in model.buffers())
                 and not _norm_accepts_fp32_stats(device)):
             # BatchNorm running statistics stay fp32 (what the reference's checkpoints hold: a
             # bf16 EMA with momentum 0.1 stalls on small deltas); only if this torch build
@@ -358,8 +358,8 @@ class Solver:
             # one line per run: which of the alternative paths this configuration took
             logger.info(
                 "frl_b200 step: precision %s | step issue %s | gradient exchange %s | update %s | "
-                "Linear layers with arena-born gradients %d (%d fused with their ReLU) | other "
-                "gradients %s",
+                "Linear layers with arena-born gradients %d (%d fused with their ReLU, %d in FP8) | "
+                "other gradients %s",
                 args.precision.value,
                 "CUDA-graph replay after 2 eager steps" if worker.graphed is not None else "eager launches",
                 ("fused NVLS kernel per bucket (K7), %d buckets" % len(pipeline.buckets)) if pipeline.nvls is not None
@@ -367,6 +367,7 @@ class Solver:
                 else "none (1 GPU)",
                 "per bucket on the side stream" if pipeline.eager else "one tail launch",
                 len(pipeline.linear_sites), sum(s.relu is not None for s in pipeline.linear_sites),
+                sum(s.fp8 for s in pipeline.linear_sites),
                 "read in place through segment tables (K2-mt / one flatten launch per bucket)"
                 if pipeline.mt_enabled else "copied into the arena per tensor")
         scheduler = create_lr_scheduler(run_opts, worker.optimizer,
@@ -576,7 +577,9 @@ class Solver:
 
         ``precision``  ``Precision.FP32`` (default; parity with the reference's arithmetic) or
                        ``Precision.BF16`` (bf16 forward/backward/gradients, fp32 master weights and
-                       optimizer state — the benchmarked configuration).  None: FRL_B200_PRECISION.
+                       optimizer state — the benchmarked configuration) or ``Precision.FP8``
+                       (BF16 with the qualifying Linear layers' GEMMs on the FP8 tensor cores,
+                       see ``types.Precision``).  None: FRL_B200_PRECISION.
         ``graph``      True: replay the training step from a CUDA graph once a batch signature
                        has run 2 eager steps (the Problem's forward must be capturable: static
                        shapes, no host syncs; a failed capture falls back to eager launches).

@@ -697,7 +697,7 @@ class SolverWorker:
         if device.type == "cuda":
             import torch.backends.cudnn as cudnn
             cudnn.benchmark = os.environ.get("FRL_B200_CUDNN_BENCHMARK", "1") != "0"
-            if precision == Precision.FP32:
+            if not precision.bf16_storage:
                 # parity mode: plain fp32 contractions (TF32 is on by default for convolutions)
                 torch.backends.cuda.matmul.allow_tf32 = False
                 cudnn.allow_tf32 = False
@@ -876,7 +876,7 @@ class SolverWorker:
     # one minibatch
     # ------------------------------------------------------------------------------------------
     def _cast_inputs(self, data: Sequence[torch.Tensor]) -> List[torch.Tensor]:
-        if self.precision != Precision.BF16:
+        if not self.precision.bf16_storage:
             return list(data)
         out = []
         for t in data:
@@ -1067,7 +1067,7 @@ class SolverWorker:
             from .device_loader import DeviceBatchLoader, supports_device_batches
             if self.device.type == "cuda" and supports_device_batches(dataset):
                 # raw dataset in pinned host memory: rows pulled by the GPU, transform on device
-                out_dtype = torch.bfloat16 if self.precision == Precision.BF16 else torch.float32
+                out_dtype = torch.bfloat16 if self.precision.bf16_storage else torch.float32
                 loaders[split] = DeviceBatchLoader(dataset, batch_size=batchSize, sampler=sampler,
                                                    device=self.device, out_dtype=out_dtype)
                 ld = loaders[split]

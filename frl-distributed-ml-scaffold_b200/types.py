@@ -56,9 +56,24 @@ class Precision(Enum):
     FP32  - parameters, gradients and optimizer state fp32 (reference parity mode, 1e-5 rel).
     BF16  - bf16 shadow weights + bf16 gradients for forward/backward, fp32 master weights and
             optimizer state in the arena, written by the fused update kernel (1e-2 tolerance).
+    FP8   - BF16 in every respect (storage, gradients, master weights, optimizer state,
+            checkpoints), except that the exact ``nn.Linear`` layers that qualify (weight in the
+            bf16 shadow, in/out features multiples of 16, and per call a row count that is a
+            multiple of 16) run their forward, input-gradient and weight-gradient GEMMs on the
+            FP8 tensor cores: e4m3 activations and weights, e5m2 output gradients, bf16 results.
+            Scaling is current per-tensor scaling: each operand is quantised at a power-of-two
+            scale derived on the device from its own amax in the same step (K9), so the run keeps
+            no scaling state.  Other layers, the fused task heads and calls that do not qualify
+            run exactly as in BF16.
     """
     FP32 = "fp32"
     BF16 = "bf16"
+    FP8 = "fp8"
+
+    @property
+    def bf16_storage(self) -> bool:
+        """bf16 shadow weights and bf16 gradients around fp32 master weights (BF16 and FP8)."""
+        return self is not Precision.FP32
 
 
 # --- records ---------------------------------------------------------------------------------

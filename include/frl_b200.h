@@ -298,6 +298,29 @@ int frl_gather_lines(const void* corpus_mapped, int64_t corpus_bytes, int64_t co
                      void* dst, int64_t n_rows, int64_t row_len, int pad, int max_blocks, void* stream);
 
 /* ------------------------------------------------------------------------------------------
+ * K9 — FP8 operands with current per-tensor scaling, for the Hopper FP8 tensor-core GEMMs of the
+ * FP8 training precision (an extension: the reference trains in fp32 only).  Nothing is kept
+ * between calls: the scale is derived on the device from the tensor being quantised.
+ *
+ * frl_fp8_amax: amax_out[0] = max |src[i]| over n elements of src_dtype (FRL_F32 | FRL_BF16);
+ *   NaN anywhere gives NaN.  The function zeroes amax_out itself on `stream` before the
+ *   reduction (capturable).  src 16-byte aligned, n >= 1.
+ * frl_fp8_quantize: src is row-major [rows, cols] of src_dtype; amax a device scalar (as written
+ *   by frl_fp8_amax).  With FP8_MAX = 448 (FRL_FP8_E4M3, e4m3fn) or 57344 (FRL_FP8_E5M2):
+ *     scale = 2^k, k = floor(log2(FP8_MAX / amax)) clamped to [-126, 126]; scale = 1 if amax == 0;
+ *     scale = NaN if amax is not finite (every code NaN, inv_scale_out NaN);
+ *     q = saturate(round_to_nearest_even(src * scale)), bit for bit torch's
+ *         (x.float() * scale).clamp(-FP8_MAX, FP8_MAX).to(float8);
+ *     dst   [rows, cols] row-major codes, dst_t [cols, rows] (the transposed copy), either may
+ *           be NULL but not both; inv_scale_out[0] = 1 / scale (the dequantisation scale).
+ *   One read of src makes both copies.  Any rows, cols >= 1; src, dst, dst_t 16-byte aligned.
+ * ---------------------------------------------------------------------------------------- */
+enum { FRL_FP8_E4M3 = 0, FRL_FP8_E5M2 = 1 };
+int frl_fp8_amax(const void* src, int64_t n, int src_dtype, float* amax_out, void* stream);
+int frl_fp8_quantize(const void* src, int64_t rows, int64_t cols, int src_dtype, const float* amax,
+                     int fmt, void* dst, void* dst_t, float* inv_scale_out, void* stream);
+
+/* ------------------------------------------------------------------------------------------
  * Host gather pool — the host half of the input path (no CUDA calls inside).
  * Replaces the reference's per-sample __getitem__ + transform + default_collate on the host
  * (reference solver_worker.py:805-832, transform.py:25-38) with native worker threads that copy
