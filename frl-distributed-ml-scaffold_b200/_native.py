@@ -69,6 +69,8 @@ SIGNATURES = {
     "frl_criteria_backward": (_i, [C.POINTER(TaskDesc), _i, _vp, _vp, _vp, _vp]),
     "frl_preproc_affine": (_i, [_vp, _i, _vp, _i, _i64, _i64, _i64, _vp, _vp, _vp]),
     "frl_cast_scale": (_i, [_vp, _i, _vp, _i, _i64, _f, _vp]),
+    "frl_augment_images": (_i, [_vp, _i64, _i, _i, _i, _vp, C.c_uint64, _i, _i, _d, _d, _d, _d, _d, _i, _i,
+                                _vp, _vp, _vp, _i, _i, _i, _vp, _vp]),
     "frl_colsum_scratch_bytes": (_i64, [_i64, _i64]),
     "frl_colsum": (_i, [_vp, _i, _i64, _i64, _vp, _i, _i, _vp, _vp]),
     "frl_drelu_colsum": (_i, [_vp, _vp, _vp, _i, _i64, _i64, _vp, _i, _i, _vp, _vp]),
@@ -261,6 +263,30 @@ def preproc_affine(src, dst, *, inner=1, channels=1, scale=None, bias=None) -> N
     _check(lib().frl_preproc_affine(_ptr(src), dtype_code(src.dtype), _ptr(dst),
                                     dtype_code(dst.dtype), n, inner, channels, _ptr(scale),
                                     _ptr(bias), _stream()), "frl_preproc_affine")
+
+
+AUG_RRC, AUG_PAD_CROP, AUG_CENTER_RESIZE, AUG_CENTER_CROP = 0, 1, 2, 3
+
+
+def augment_images(src, idx, dst, *, seed: int, epoch: int, mode: int, scale_range=(0.08, 1.0),
+                   ratio_range=(3.0 / 4.0, 4.0 / 3.0), eval_crop: float = 0.875, pad: int = 0,
+                   flip: bool = True, scale=None, bias=None, params_out=None) -> None:
+    """K5a: crop box drawn per (seed, epoch, idx[b]), bilinear resize to ``dst``'s [out_h, out_w],
+    optional flip, then ``x * scale[c] + bias[c]``.  ``src`` uint8 [B, C, H, W], ``idx`` device
+    int64 [B], ``dst`` fp32/bf16 [B, C, out_h, out_w], ``params_out`` optional int32 [B, 5]
+    (top, left, h, w, flipped).  See frl_augment_images in include/frl_b200.h."""
+    B, Cc, H, W = src.shape
+    assert src.dtype == torch.uint8 and src.is_contiguous() and dst.is_contiguous()
+    assert dst.dim() == 4 and tuple(dst.shape[:2]) == (B, Cc)
+    assert idx.dtype == torch.int64 and idx.is_contiguous() and idx.numel() == B
+    assert params_out is None or (params_out.dtype == torch.int32 and params_out.is_contiguous()
+                                  and tuple(params_out.shape) == (B, 5))
+    _check(lib().frl_augment_images(_ptr(src), B, Cc, H, W, _ptr(idx), int(seed) & (2 ** 64 - 1), int(epoch),
+                                    int(mode), float(scale_range[0]), float(scale_range[1]),
+                                    float(ratio_range[0]), float(ratio_range[1]), float(eval_crop), int(pad),
+                                    int(bool(flip)), _ptr(scale), _ptr(bias), _ptr(dst), dtype_code(dst.dtype),
+                                    dst.shape[2], dst.shape[3], _ptr(params_out), _stream()),
+           "frl_augment_images")
 
 
 def cast_scale(src, dst, scale: float = 1.0) -> None:

@@ -260,6 +260,11 @@ class DeviceBatchLoader:
     def __len__(self) -> int:
         return len(self._index_loader)
 
+    def set_epoch(self, epoch: int) -> None:
+        """Tell the dataset's transform which epoch the next pass belongs to (its per-sample
+        random draws may be keyed by it)."""
+        self.dataset.device_transform.set_epoch(epoch)
+
     def _index_batches(self) -> Iterator[torch.Tensor]:
         """int64 index tensors, one per minibatch, in the order the reference's
         ``enumerate(DataLoader)`` would serve them — and with the same draws from the global
@@ -407,7 +412,10 @@ class DeviceBatchLoader:
             slot = self._slots[s]
             torch.cuda.current_stream().wait_event(self._ready[s])
             raw = {name: slot[name][:n] for name in self._fields}
-            data, target = transform.apply(raw, split, self.out_dtype)
+            if getattr(transform, "needs_index", False):
+                data, target = transform.apply(raw, split, self.out_dtype, index=slot["__idx_dev"][:n])
+            else:
+                data, target = transform.apply(raw, split, self.out_dtype)
             meta = transform.meta(raw, slot["__idx_dev"][:n])
             # the loop retains targets/meta of the last minibatches for its amortised metrics,
             # the slot is recycled `depth` batches from now: hand out no views of it

@@ -735,6 +735,10 @@ class SolverWorker:
             mark("split start")
             if dist_on:
                 loader.sampler.set_epoch(self.cur_epoch)
+            if hasattr(loader, "set_epoch"):
+                # per-epoch device-side draws (DeviceImageAugment); cur_epoch resumes from the
+                # checkpoint's epoch, so a resumed run continues the same stream
+                loader.set_epoch(self.cur_epoch)
             # the planned order goes to the (null) cache accessor; drawing it also keeps the
             # global RNG stream identical to the reference's (solver_worker.py:431)
             self.accessor.set_sequence_indices(_planned_order(loader.sampler, self.accessor))

@@ -145,12 +145,14 @@ def _pinned_dataset_class(ns):
 
     class PinnedArrayDataset(Base):
         def __init__(self, split, fields, transform, shift, scale, target_fields,
-                     channel_affine=None) -> None:
+                     channel_affine=None, device_transform=None) -> None:
             super().__init__(split, fields, transform)
             pin = torch.cuda.is_available()
             self.pinned_fields = {k: (torch.from_numpy(v).pin_memory() if pin else torch.from_numpy(v))
                                   for k, v in fields.items()}
-            if channel_affine is not None:
+            if device_transform is not None:
+                self.device_transform = device_transform
+            elif channel_affine is not None:
                 self.device_transform = _channel_affine_device_transform(*channel_affine, target_fields)
             else:
                 self.device_transform = _affine_device_transform(shift, scale, target_fields)
@@ -272,18 +274,55 @@ def _problem_class(ns):
         def transform_source_data(self, tensors, split):
             return [tensors["x"].float() * self.scale + self.bias], NoTransformState()
 
+    class CenterCropTransform(ns.MultiTaskTransform):
+        """Per-sample path of an augmenting Problem (``DeviceImageAugment``): the deterministic
+        centre crop of evaluation splits, resized bilinearly, then x * scale[c] + bias[c].  The
+        random crops of the training split exist on the device only."""
+
+        def __init__(self, tasks, augment) -> None:
+            super().__init__(tasks, IndexMeta)
+            self.augment = augment
+            self.scale = torch.tensor(augment.scale or [1.0]).view(-1, 1, 1)
+            self.bias = torch.tensor(augment.bias or [0.0]).view(-1, 1, 1)
+
+        def transform_source_data(self, tensors, split):
+            if split == ns.Split.TRAIN:
+                raise RuntimeError("the training split of an augmenting Problem is served by the device "
+                                   "path only (DeviceBatchLoader + DeviceImageAugment); its per-sample "
+                                   "transform covers the evaluation splits")
+            x = tensors["x"]
+            c, H, W = x.shape
+            aug = self.augment
+            oh, ow = aug.out_size
+            ch, cw = (round(H * aug.eval_crop), round(W * aug.eval_crop)) if aug.mode == "rrc" else (oh, ow)
+            top, left = round((H - ch) / 2), round((W - cw) / 2)
+            crop = torch.zeros(c, ch, cw)           # zero fill where the box leaves the image
+            y0, y1, x0, x1 = max(top, 0), min(top + ch, H), max(left, 0), min(left + cw, W)
+            crop[:, y0 - top:y1 - top, x0 - left:x1 - left] = x[:, y0:y1, x0:x1].float()
+            if (ch, cw) != (oh, ow):
+                crop = nn.functional.interpolate(crop[None], size=(oh, ow), mode="bilinear",
+                                                 align_corners=False, antialias=False)[0]
+            return [crop * self.scale + self.bias], NoTransformState()
+
     class SyntheticMultiTaskProblem(ns.MultiTaskProblem):
         BatchMetaType = BatchMeta
 
         def __init__(self, tasks, trunk_dims: Sequence[int], datasets_fields, save_dir: str,
                      shift: float, scale: float, criterion_kind: str = "parallel",
                      pinned: bool = False, base_factory=None, indexed_dir: Optional[str] = None,
-                     channel_affine=None) -> None:
+                     channel_affine=None, augment=None) -> None:
             self._tasks = tasks
             self._trunk_dims = list(trunk_dims)
             self._base_factory = base_factory
             self._save_dir = save_dir
             self._criterion_kind = criterion_kind
+            if augment is not None:
+                self.transform = CenterCropTransform(tasks, augment)
+                ds_cls = _pinned_dataset_class(ns)
+                self._datasets = [ds_cls(split, fields, self.transform, shift, scale,
+                                         [t._field for t in tasks], device_transform=augment)
+                                  for split, fields in datasets_fields]
+                return
             if channel_affine is not None:
                 self.transform = ChannelAffineTransform(tasks, *channel_affine)
             else:
@@ -416,13 +455,33 @@ def resnet_fields(n: int, image: int, heads, seed: int, uint8: bool = False) -> 
 
 def make_resnet_problem(ns, save_dir: str, config: str = "resnet18", image: int = 224,
                         n_train: int = 64, n_test: int = 0, pinned: bool = False,
-                        uint8: bool = False):
+                        uint8: bool = False, augment: Optional[str] = None,
+                        stored_image: Optional[int] = None):
     """Configs 4/5: a torchvision ResNet trunk (its ``fc`` removed) behind
     ``ListSelect`` and one ``nn.Linear`` head per task; x ~ N(0,1) of shape [3, image, image], or
     (``uint8``) raw 8-bit images normalised per channel by the transform (150 kB/sample over
-    PCIe instead of 602 kB)."""
+    PCIe instead of 602 kB).
+
+    ``augment`` (``uint8`` only): ``"rrc"`` (random resized crop + flip, ImageNet-style) or
+    ``"pad_crop"`` (crop of the image zero-padded by 4 + flip, CIFAR-style) on the device
+    (``transform.DeviceImageAugment``, K5a) from stored ``stored_image`` x ``stored_image`` images
+    to the model's ``image`` x ``image``; evaluation splits take the centre crop.  The datasets are
+    then pinned; their per-sample transform serves the evaluation splits only."""
     import torchvision
+    stored = image if stored_image is None else int(stored_image)
+    if augment is None and stored != image:
+        raise ValueError("stored_image differs from image only for an augmenting Problem (augment=...)")
     arch, heads = RESNET_CONFIGS[config]
+    aug = None
+    if augment is not None:
+        from .transform import DeviceImageAugment
+        if not uint8:
+            raise ValueError("augment works on raw uint8 images: pass uint8=True")
+        if augment not in DeviceImageAugment.MODES:
+            raise ValueError(f"augment must be None or one of {DeviceImageAugment.MODES}, got {augment!r}")
+        aug = DeviceImageAugment("x", [field for _, _, field, _ in heads], mode=augment, out_size=image, pad=4,
+                                 scale=U8_CHANNEL_AFFINE[0], bias=U8_CHANNEL_AFFINE[1])
+        aug.check_image(3, stored, stored)
     feat = {"resnet18": 512, "resnet50": 2048}[arch]
     Reg, Cls = _task_classes(ns)
     tasks = [(Cls if kind == "cls" else Reg)(feat, dim, 1.0, field=field, name=name)
@@ -433,12 +492,12 @@ def make_resnet_problem(ns, save_dir: str, config: str = "resnet18", image: int 
         net.fc = nn.Identity()
         return nn.Sequential(ns.model.ListSelect(sel_index=0, num_elements=1), net)
 
-    fields = [(ns.Split.TRAIN, resnet_fields(n_train, image, heads, 0, uint8))]
+    fields = [(ns.Split.TRAIN, resnet_fields(n_train, stored, heads, 0, uint8))]
     if n_test:
-        fields.append((ns.Split.TEST, resnet_fields(n_test, image, heads, 1, uint8)))
+        fields.append((ns.Split.TEST, resnet_fields(n_test, stored, heads, 1, uint8)))
     return _problem_class(ns)(tasks, [], fields, save_dir, shift=0.0, scale=1.0, pinned=pinned,
                               base_factory=base_factory,
-                              channel_affine=U8_CHANNEL_AFFINE if uint8 else None)
+                              channel_affine=U8_CHANNEL_AFFINE if uint8 else None, augment=aug)
 
 
 # ---- text: next-byte prediction over TextDataset lines ---------------------------------------

@@ -4,9 +4,12 @@
 ``(Sample(data, target), meta)`` and ``__call__`` flattens that to the triple the DataLoader
 collates.  ``DeviceBatchTransform`` is the H100 addition: the same arithmetic applied to a
 whole batch after the raw bytes reached HBM, through the ``frl_preproc_affine`` kernel.
+``DeviceImageAugment`` is a ready-made one for image Problems: crop, resize, flip and normalise in
+one ``frl_augment_images`` pass.
 """
+import math
 from abc import ABC, abstractmethod
-from typing import Any, Dict, Generic, List, NamedTuple, Sequence, Tuple, TypeVar, Union
+from typing import Any, Dict, Generic, List, NamedTuple, Optional, Sequence, Tuple, TypeVar, Union
 
 import numpy as np
 from torch import Tensor
@@ -50,6 +53,10 @@ class DeviceBatchTransform(ABC):
     #: bf16 (``FRL_B200_INPUT_WIRE=bf16``); targets and anything exact must not be listed.
     bf16_wire_fields: Sequence[str] = ()
 
+    #: True: ``apply`` is also given ``index=`` (device int64 [B], the dataset row of each sample),
+    #: e.g. to key per-sample random draws to the sample rather than to its place in the batch.
+    needs_index: bool = False
+
     @abstractmethod
     def apply(self, raw: Dict[str, Tensor], split: Split, out_dtype
               ) -> Tuple[List[Tensor], List[Tuple[Tensor, ...]]]:
@@ -57,3 +64,129 @@ class DeviceBatchTransform(ABC):
 
     def meta(self, raw: Dict[str, Tensor], index: Tensor) -> Dict[str, Any]:
         return {"index": index.clone()}
+
+    def set_epoch(self, epoch: int) -> None:
+        """Called at the start of every split of every epoch (1-based, the loop's epoch)."""
+
+
+def _pair(name: str, value) -> Tuple[float, float]:
+    try:
+        lo, hi = (float(v) for v in value)
+    except (TypeError, ValueError):
+        raise ValueError(f"{name} must be a pair of numbers, got {value!r}") from None
+    if not (0.0 < lo <= hi and math.isfinite(hi)):
+        raise ValueError(f"{name} must satisfy 0 < {name}[0] <= {name}[1], got {value!r}")
+    return lo, hi
+
+
+class DeviceImageAugment(DeviceBatchTransform):
+    """Training-time image augmentation on the device, K5a (``frl_augment_images``): one pass from
+    the raw uint8 images [B, C, H, W] of a batch to the normalised model input.
+
+    ``mode="rrc"``: random resized crop (area share ``crop_scale``, aspect ``crop_ratio``, the
+    torchvision defaults) resized bilinearly to ``out_size``; evaluation splits take the centred
+    ``round(H * eval_crop) x round(W * eval_crop)`` box, resized.
+    ``mode="pad_crop"``: random ``out_size`` crop of the image zero-padded by ``pad`` on every side;
+    evaluation splits take the centred ``out_size`` box.
+    Random modes mirror each sample with p = 1/2 when ``flip``.  The draws are keyed by
+    (``seed``, epoch, dataset index) — not by the batch, its order or the rank — and come from a
+    counter-based generator on the device: torch's global RNG is not touched.
+    Normalisation: ``mean`` / ``std`` in the [0, 1] domain of x / 255 (torchvision's ``Normalize``
+    after ``ToDtype(scale=True)``), or the raw ``scale`` / ``bias`` of ``x * scale[c] + bias[c]``.
+    """
+
+    needs_index = True
+    MODES = ("rrc", "pad_crop")
+
+    def __init__(self, image_field: str, target_fields: Sequence[str], *, mode: str = "rrc",
+                 out_size=224, crop_scale=(0.08, 1.0), crop_ratio=(3.0 / 4.0, 4.0 / 3.0), pad: int = 4,
+                 mean: Optional[Sequence[float]] = None, std: Optional[Sequence[float]] = None,
+                 scale: Optional[Sequence[float]] = None, bias: Optional[Sequence[float]] = None,
+                 seed: int = 0, eval_crop: float = 0.875, flip: bool = True) -> None:
+        if mode not in self.MODES:
+            raise ValueError(f"mode must be one of {self.MODES}, got {mode!r}")
+        oh, ow = (out_size, out_size) if isinstance(out_size, int) else tuple(out_size)
+        if not (int(oh) == oh >= 1 and int(ow) == ow >= 1):
+            raise ValueError(f"out_size must be >= 1, got {out_size!r}")
+        self.image_field = image_field
+        self.target_fields = list(target_fields)
+        self.mode = mode
+        self.out_size = (int(oh), int(ow))
+        self.crop_scale = _pair("crop_scale", crop_scale)
+        self.crop_ratio = _pair("crop_ratio", crop_ratio)
+        if int(pad) != pad or pad < 0:
+            raise ValueError(f"pad must be an integer >= 0, got {pad!r}")
+        self.pad = int(pad)
+        if not (0.0 < float(eval_crop) <= 1.0):
+            raise ValueError(f"eval_crop must be in (0, 1], got {eval_crop!r}")
+        self.eval_crop = float(eval_crop)
+        if int(seed) != seed or not 0 <= seed < 2 ** 64:
+            raise ValueError(f"seed must be an integer in [0, 2**64), got {seed!r}")
+        self.seed = int(seed)
+        self.flip = bool(flip)
+        if (mean is None) != (std is None):
+            raise ValueError("mean and std go together")
+        if mean is not None and (scale is not None or bias is not None):
+            raise ValueError("give mean/std or scale/bias, not both")
+        if mean is not None:
+            if len(mean) != len(std) or not 1 <= len(mean) <= 4:
+                raise ValueError(f"mean and std need one value per channel (1 to 4), got {mean!r}, {std!r}")
+            if any(float(s) <= 0.0 for s in std):
+                raise ValueError(f"std must be > 0, got {std!r}")
+            scale = [1.0 / (255.0 * float(s)) for s in std]
+            bias = [-float(m) / float(s) for m, s in zip(mean, std)]
+        for name, v in (("scale", scale), ("bias", bias)):
+            if v is not None and not 1 <= len(v) <= 4:
+                raise ValueError(f"{name} needs one value per channel (1 to 4), got {v!r}")
+        if scale is not None and bias is not None and len(scale) != len(bias):
+            raise ValueError("scale and bias need the same number of channels")
+        self.scale = None if scale is None else [float(v) for v in scale]
+        self.bias = None if bias is None else [float(v) for v in bias]
+        self.epoch = 0
+        self._coef: Dict[Any, Tuple[Optional[Tensor], Optional[Tensor]]] = {}
+
+    def set_epoch(self, epoch: int) -> None:
+        self.epoch = int(epoch)
+
+    def check_image(self, channels: int, height: int, width: int) -> None:
+        """ValueError unless images of this shape can be served."""
+        if not 1 <= channels <= 4:
+            raise ValueError(f"{self.image_field!r}: images need 1 to 4 channels, got {channels}")
+        for name, v in (("scale", self.scale), ("bias", self.bias)):
+            if v is not None and len(v) != channels:
+                raise ValueError(f"{name} has {len(v)} values for {channels}-channel images")
+        oh, ow = self.out_size
+        if self.mode == "pad_crop" and (oh > height + 2 * self.pad or ow > width + 2 * self.pad):
+            raise ValueError(f"out_size {self.out_size} does not fit {height}x{width} images padded by {self.pad}")
+        if self.mode == "rrc" and (round(height * self.eval_crop) < 1 or round(width * self.eval_crop) < 1):
+            raise ValueError(f"eval_crop {self.eval_crop} leaves no pixel of {height}x{width} images")
+
+    def native_mode(self, split: Split) -> int:
+        from . import _native
+        if split == Split.TRAIN:
+            return _native.AUG_RRC if self.mode == "rrc" else _native.AUG_PAD_CROP
+        return _native.AUG_CENTER_RESIZE if self.mode == "rrc" else _native.AUG_CENTER_CROP
+
+    def augment(self, x: Tensor, index: Tensor, split: Split, out_dtype, params_out=None) -> Tensor:
+        """The normalised, augmented images [B, C, out_h, out_w] of ``out_dtype``."""
+        import torch
+        from . import _native
+        if x.dtype != torch.uint8 or x.dim() != 4:
+            raise ValueError(f"{self.image_field!r} must be uint8 [B, C, H, W], got {x.dtype} {tuple(x.shape)}")
+        self.check_image(*x.shape[1:])
+        if x.device not in self._coef:
+            self._coef[x.device] = tuple(None if v is None else torch.tensor(v, dtype=torch.float32, device=x.device)
+                                         for v in (self.scale, self.bias))
+        sc, bi = self._coef[x.device]
+        out = torch.empty((x.shape[0], x.shape[1]) + self.out_size, dtype=out_dtype, device=x.device)
+        _native.augment_images(x.contiguous(), index, out, seed=self.seed, epoch=self.epoch,
+                               mode=self.native_mode(split), scale_range=self.crop_scale,
+                               ratio_range=self.crop_ratio, eval_crop=self.eval_crop, pad=self.pad,
+                               flip=self.flip, scale=sc, bias=bi, params_out=params_out)
+        return out
+
+    def apply(self, raw, split, out_dtype, index=None):
+        if index is None:
+            raise ValueError("DeviceImageAugment.apply needs index= (the dataset row of every sample)")
+        out = self.augment(raw[self.image_field], index, split, out_dtype)
+        return [out], [(raw[f],) for f in self.target_fields]

@@ -194,6 +194,51 @@ int frl_preproc_affine(const void* src, int src_dtype, void* dst, int dst_dtype,
                        int64_t inner, int64_t channels, const float* scale, const float* bias,
                        void* stream);
 
+/* ------------------------------------------------------------------------------------------
+ * K5a — on-device image augmentation: crop box + bilinear resize + horizontal flip + per-channel
+ * affine in one pass (an extension: the reference's Problems augment per sample on the host,
+ * inside their MultifieldTransform).
+ *   src        uint8 [B, C, H, W] contiguous, 1 <= C <= 4
+ *   idx        int64 [B] (device): the dataset row of each image, keys its random draws
+ *   seed, epoch  the rest of the key; nothing else (batch size, order, rank) enters the draws
+ *   mode       FRL_AUG_RRC         random resized crop, area share in [smin, smax], aspect in [rmin, rmax]
+ *              FRL_AUG_PAD_CROP    random out_h x out_w crop of the image zero-padded by `pad` per side
+ *              FRL_AUG_CENTER_RESIZE  centred round(H*eval_crop) x round(W*eval_crop) box, resized
+ *              FRL_AUG_CENTER_CROP    centred out_h x out_w box (zero fill outside the image)
+ *   flip       0/1: mirror with p = 1/2 (never in the two CENTER modes)
+ *   scale/bias device fp32 [C]; NULL scale = 1, NULL bias = 0
+ *   dst        [B, C, out_h, out_w] of dst_dtype (FRL_F32 | FRL_BF16)
+ *   params_out optional int32 [B, 5]: (top, left, h, w, flipped) of each sample's box
+ *
+ * Sample parameters (oracle/augment_np.py restates them):
+ *   draws: Philox4x32-10, key (lo32(seed), hi32(seed)), counter (lo32(i), hi32(i), epoch, j) for
+ *     block j of sample i = idx[b]; each block gives words w0..w3.
+ *     u(w) = (w >> 8) * 2^-24;  an integer in [0, n) is (uint64(w) * n) >> 32.
+ *   RRC (torchvision RandomResizedCrop.get_params), in double: attempt t = 0..9 uses block t:
+ *     area = H*W * (smin + u(w0)*(smax - smin)); aspect = exp(log rmin + u(w1)*(log rmax - log rmin))
+ *     w = rint(sqrt(area*aspect)), h = rint(sqrt(area/aspect))  (rint: half to even, Python's round)
+ *     accepted if 0 < w <= W and 0 < h <= H: top = int(w2, H-h+1), left = int(w3, W-w+1).
+ *     No attempt accepted: the ratio-clamped centre crop, r = W/H:
+ *       r < rmin: w = W, h = rint(W/rmin); r > rmax: h = H, w = rint(H*rmax); else h = H, w = W;
+ *       h, w at least 1; top = (H-h)/2, left = (W-w)/2 (floor).
+ *   PAD_CROP: block 0: top = int(w0, H+2p-out_h+1) - p, left = int(w1, W+2p-out_w+1) - p; h = out_h, w = out_w.
+ *   CENTER_RESIZE: h = rint(H*eval_crop), w = rint(W*eval_crop); CENTER_CROP: h = out_h, w = out_w;
+ *     both: top = rint((H-h)/2), left = rint((W-w)/2) (torchvision center_crop).
+ *   flip (RRC / PAD_CROP with flip != 0): block 10, flipped = w0 >> 31.
+ * Pixels: bilinear, align_corners=False, no antialiasing (torch interpolate on the crop): per axis
+ *   s = (float)crop / (float)out, src = max(fmaf(s, o + 0.5f, -0.5f), 0) in fp32, taps i0 = (int)src and
+ *   min(i0 + 1, crop - 1), blend in fp32; crop pixels outside the image read 0 (so the normalised
+ *   fill is bias[c]).  A crop the size of the output is an exact copy.  A flipped sample's output
+ *   column x takes the resized column out_w-1-x.  dst = round_nearest(fmaf(v, scale[c], bias[c])).
+ * Graph-capturable: no host reads, no allocation.
+ * ---------------------------------------------------------------------------------------- */
+enum { FRL_AUG_RRC = 0, FRL_AUG_PAD_CROP = 1, FRL_AUG_CENTER_RESIZE = 2, FRL_AUG_CENTER_CROP = 3 };
+int frl_augment_images(const void* src, int64_t batch, int channels, int height, int width,
+                       const int64_t* idx, uint64_t seed, int epoch, int mode,
+                       double smin, double smax, double rmin, double rmax, double eval_crop, int pad,
+                       int flip, const float* scale, const float* bias, void* dst, int dst_dtype,
+                       int out_h, int out_w, int32_t* params_out, void* stream);
+
 /* dtype conversion / scaled copy used by the arena (master -> shadow refresh after a
  * checkpoint load, gradient flatten for modules the arena cannot write into directly):
  * dst = src * scale. */

@@ -3,6 +3,7 @@
 
     python tools/probe_input_path.py [rows_per_batch] [row_elems]
     python tools/probe_input_path.py --text [batch] [seq_len]
+    python tools/probe_input_path.py --augment [batch]
 
 Prints GB/s of: contiguous cudaMemcpyAsync (PCIe reference), frl_gather_rows at several grid
 sizes, frl_gather_rows_tma, the native host gather pool per thread count (plain and with the
@@ -12,6 +13,9 @@ machinery.
 ``--text``: batches/s served by ``DeviceBatchLoader`` (K8t + the batched transform) against the
 per-sample ``DataLoader`` (``TextDataset.__getitem__`` + transform + ``default_collate``) at 4 and
 16 workers, over the same 256 MB seeded corpus, no model; host clock around a device synchronise.
+
+``--augment``: the same comparison for augmented 256 x 256 -> 224 x 224 training images:
+``DeviceBatchLoader`` + K5a against torchvision v2 transforms in a per-sample ``DataLoader``.
 """
 import os
 import sys
@@ -58,6 +62,73 @@ def probe_text(batch: int, seq_len: int, n_batches: int = 40) -> None:
                                              num_workers=workers, pin_memory=True)
             print("per-sample DataLoader, %2d workers: %8.1f batches/s" % (workers, rate(dl, True)), flush=True)
 
+
+class _PerSampleImages(torch.utils.data.Dataset):
+    """uint8 [N, C, H, W] images + labels through a per-sample torchvision transform."""
+
+    def __init__(self, x, y, transform) -> None:
+        self.x, self.y, self.transform = x, y, transform
+
+    def __len__(self) -> int:
+        return len(self.x)
+
+    def __getitem__(self, i):
+        return self.transform(torch.from_numpy(self.x[i])), int(self.y[i])
+
+
+def probe_augment(batch: int = 256, stored: int = 256, out: int = 224, n_batches: int = 20) -> None:
+    """Batches/s of augmented ImageNet-shaped training input, no model: ``DeviceBatchLoader`` with
+    K5a (random resized crop + flip + normalise on the device, bf16 out) against a per-sample
+    ``DataLoader`` running torchvision v2 RandomResizedCrop(antialias=False) + RandomHorizontalFlip +
+    ToDtype + Normalize on the host at 4 and 16 workers (fp32, pinned, copied to the GPU).  Host
+    clock around a device synchronise, after one warm-up batch."""
+    import subprocess
+    import tempfile
+    import torchvision.transforms.v2 as T
+    from frl_b200 import synthetic
+    from frl_b200.device_loader import DeviceBatchLoader
+    print(subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.max.sm", "--format=csv,noheader"],
+                         capture_output=True, text=True).stdout.strip(), flush=True)
+    ns = synthetic.api_namespace("frl_b200")
+    dev = torch.device("cuda", 0)
+    n = batch * (n_batches + 2)
+    with tempfile.TemporaryDirectory() as tmp:
+        prob = synthetic.make_resnet_problem(ns, tmp, "resnet18", image=out, n_train=n, uint8=True,
+                                             augment="rrc", stored_image=stored)
+        train = prob.datasets[0]
+        print("%d images 3x%dx%d uint8 -> 3x%dx%d, batch %d" % (n, stored, stored, out, out, batch), flush=True)
+
+        def rate(loader, to_device):
+            it = iter(loader)
+            next(it)                                        # warm-up: workers started, first batch
+            torch.cuda.synchronize()
+            t0 = time.perf_counter()
+            for _ in range(n_batches):
+                data, target, *_ = next(it)
+                if to_device:
+                    data = data.to(dev, non_blocking=True)
+                    target.to(dev, non_blocking=True)
+            torch.cuda.synchronize()
+            return n_batches / (time.perf_counter() - t0)
+
+        ld = DeviceBatchLoader(train, batch_size=batch, sampler=None, device=dev, out_dtype=torch.bfloat16)
+        ld.set_epoch(1)
+        print("DeviceBatchLoader + K5a (%s path): %8.1f batches/s" % (ld.path, rate(ld, False)), flush=True)
+        tf = T.Compose([T.RandomResizedCrop(out, antialias=False), T.RandomHorizontalFlip(),
+                        T.ToDtype(torch.float32, scale=True),
+                        T.Normalize(list(synthetic.IMAGE_MEAN), list(synthetic.IMAGE_STD))])
+        per_sample = _PerSampleImages(train._fields["x"], train._fields["y_cls"], tf)
+        for workers in (4, 16):
+            dl = torch.utils.data.DataLoader(per_sample, batch_size=batch, shuffle=True, num_workers=workers,
+                                             pin_memory=True)
+            print("per-sample DataLoader (torchvision v2), %2d workers: %8.1f batches/s"
+                  % (workers, rate(dl, True)), flush=True)
+
+
+if len(sys.argv) > 1 and sys.argv[1] == "--augment":
+    torch.cuda.set_device(0)
+    probe_augment(int(sys.argv[2]) if len(sys.argv) > 2 else 256)
+    sys.exit(0)
 
 if len(sys.argv) > 1 and sys.argv[1] == "--text":
     torch.cuda.set_device(0)
