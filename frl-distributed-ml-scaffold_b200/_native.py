@@ -62,6 +62,10 @@ SIGNATURES = {
     "frl_sgd_momentum_mt": (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _i64, _d, _d, _d, _d, _d, _vp, _vp, _i, _vp]),
     "frl_adam_mt": (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _i64, _d, _d, _d, _d, _d, _i64, _d, _vp, _vp, _vp]),
     "frl_rmsprop_mt": (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _i64, _d, _d, _d, _d, _d, _d, _vp, _vp, _vp]),
+    "frl_layerwise_scratch_bytes": (_i64, [_i64, _i64]),
+    "frl_lars_mt": (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _i64, _i64, _vp, _vp, _vp, _d, _d, _d, _d, _vp, _vp, _i, _vp]),
+    "frl_lamb_mt": (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _i64, _i64, _vp, _vp, _vp, _d, _d, _d, _d, _d, _i64,
+                         _d, _vp, _vp, _vp]),
     "frl_reduce_scratch_bytes": (_i64, []),
     "frl_grad_sumsq_clip": (_i, [_vp, _i64, _i, _f, _f, _vp, _vp, _vp]),
     "frl_criteria_scratch_bytes": (_i64, [_i]),
@@ -218,6 +222,48 @@ def rmsprop_mt(p, sq, buf, p_lp, table, *, lr, alpha, eps, wd, mu, grad_scale=1.
     _check(lib().frl_rmsprop_mt(_ptr(p), _ptr(sq), _ptr(buf), _ptr(p_lp), table.segs_dev_ptr,
                                 table.prefix_dev_ptr, table.tile_seg_dev_ptr, table.n_tiles, lr, alpha, eps, wd, mu,
                                 grad_scale, _ptr(grad_scale_dev), _ptr(dyn), _stream()), "frl_rmsprop_mt")
+
+
+# ---- K2-lw: layer-wise adaptive updates (LARS, LAMB) over a segment table -------------------------
+
+LW_ADAPTED, LW_CLIPPED = 1, 2
+
+
+def layerwise_scratch_bytes(n_tiles: int, n_segs: int) -> int:
+    return int(lib().frl_layerwise_scratch_bytes(n_tiles, n_segs))
+
+
+def _check_layerwise(table, flags, ratio, scratch, *vecs) -> None:
+    for t in vecs:
+        if t is not None and not (t.dtype == torch.float32 and t.is_contiguous()):
+            raise NativeLibraryError("layer-wise update: master weights and state must be contiguous fp32")
+    if flags.dtype != torch.int32 or flags.numel() < table.n_segs:
+        raise NativeLibraryError("layer-wise update: seg_flags must be int32 [n_segs]")
+    if ratio.dtype != torch.float32 or ratio.numel() < table.n_segs:
+        raise NativeLibraryError("layer-wise update: ratio must be fp32 [n_segs]")
+    if scratch.numel() * scratch.element_size() < layerwise_scratch_bytes(table.n_tiles, table.n_segs):
+        raise NativeLibraryError("layer-wise update: scratch too small")
+
+
+def lars_mt(p, buf, p_lp, table, flags, ratio, scratch, *, lr, mu, wd, grad_scale=1.0,
+            grad_scale_dev=None, first_step=False, dyn=None) -> None:
+    """K2-lw LARS over the segments of ``table``; ``ratio`` receives each tensor's trust ratio.
+    See frl_lars_mt in include/frl_b200.h."""
+    _check_layerwise(table, flags, ratio, scratch, p, buf)
+    _check(lib().frl_lars_mt(_ptr(p), _ptr(buf), _ptr(p_lp), table.segs_dev_ptr, table.prefix_dev_ptr,
+                             table.tile_seg_dev_ptr, table.n_tiles, table.n_segs, _ptr(flags), _ptr(ratio),
+                             _ptr(scratch), lr, mu, wd, grad_scale, _ptr(grad_scale_dev), _ptr(dyn),
+                             int(first_step), _stream()), "frl_lars_mt")
+
+
+def lamb_mt(p, m, v, p_lp, table, flags, ratio, scratch, *, lr, beta1, beta2, eps, wd, step,
+            grad_scale=1.0, grad_scale_dev=None, dyn=None) -> None:
+    """K2-lw LAMB over the segments of ``table``.  See frl_lamb_mt in include/frl_b200.h."""
+    _check_layerwise(table, flags, ratio, scratch, p, m, v)
+    _check(lib().frl_lamb_mt(_ptr(p), _ptr(m), _ptr(v), _ptr(p_lp), table.segs_dev_ptr, table.prefix_dev_ptr,
+                             table.tile_seg_dev_ptr, table.n_tiles, table.n_segs, _ptr(flags), _ptr(ratio),
+                             _ptr(scratch), lr, beta1, beta2, eps, wd, step, grad_scale, _ptr(grad_scale_dev),
+                             _ptr(dyn), _stream()), "frl_lamb_mt")
 
 
 # ---- K3 -------------------------------------------------------------------------------------

@@ -5,6 +5,8 @@
 (``OptimOpts.momentum`` feeds SGD *and* RMSprop, ``epsilon``/``amsgrad`` feed Adam, weight decay
 is L2-coupled and applies to every parameter).  ``state_dict()`` / ``load_state_dict()`` speak
 torch's per-parameter format so the reference's ``.checkpoint.pth`` files stay interchangeable.
+``FusedLars`` / ``FusedLamb`` (an extension, ``types.LayerAdaptation``) keep SGD's / Adam's state
+format and update whole tensors through the K2-lw kernels.
 
 Known limitation: the step count (Adam's bias corrections) is ONE number for the whole arena.
 ``torch.optim`` keeps one per parameter and does not advance it for a parameter whose gradient
@@ -20,7 +22,7 @@ import torch
 
 from . import _native
 from .arena import ParamArena
-from .types import OptAlgorithm, OptimOpts
+from .types import LayerAdaptation, OptAlgorithm, OptimOpts
 
 # Kernel entry points; tests exercising host logic on CPU swap this for an oracle-backed double.
 KERNELS = _native
@@ -30,6 +32,12 @@ class FusedArenaOptimizer(torch.optim.Optimizer):
     """Base: owns the fp32 state vectors (same layout as the arena) and the step counter."""
 
     STATE_NAMES: Tuple[str, ...] = ()
+
+    @property
+    def needs_whole_tensors(self) -> bool:
+        """True if an update needs every gradient of a tensor at once (per-tensor norms): the
+        pipeline then updates once after backward, never per bucket or per shard."""
+        return False
 
     def __init__(self, arena: ParamArena, defaults: Dict[str, Any]) -> None:
         self.arena = arena
@@ -126,9 +134,12 @@ class FusedArenaOptimizer(torch.optim.Optimizer):
     def _launch(self, lo: int, hi: int, grad_scale: float, coef) -> None:
         raise NotImplementedError
 
-    def apply_table(self, table, *, grad_scale: float = 1.0) -> None:
+    def apply_table(self, table, *, grad_scale: float = 1.0,
+                    clip_coef_dev: Optional[torch.Tensor] = None) -> None:
         """Update every arena slot listed in ``table`` (a ``multi_tensor.GradSegTable`` whose device
         copy is current), reading each gradient where the table says it lies (K2-mt)."""
+        if clip_coef_dev is not None:
+            raise ValueError("K2-mt takes no clip coefficient: clipped updates go through apply_range")
         if table.n_segs:
             self._launch_mt(table, grad_scale)
 
@@ -357,8 +368,139 @@ class FusedRMSprop(FusedArenaOptimizer):
                              g_dtype=KERNELS.dtype_code(self.arena.grad.dtype), dyn=self._dyn)
 
 
-def create_fused_optimizer(arena: ParamArena, optim_opts: OptimOpts) -> FusedArenaOptimizer:
-    """Same dispatch and argument mapping as the reference's ``_create_optimizer``."""
+def is_adapted(slot) -> bool:
+    """Layer-wise adaptation applies to tensors of 2 or more dimensions (``types.LayerAdaptation``)."""
+    return len(slot.shape) >= 2
+
+
+class _LayerwiseMixin:
+    """K2-lw: trust-ratio updates over a segment table (``frl_lars_mt`` / ``frl_lamb_mt``).  The
+    per-table device buffers (adaptation flags, ratios, scratch) are built on first use and kept on
+    the table, so a CUDA-graph capture's table set owns its own."""
+
+    @property
+    def needs_whole_tensors(self) -> bool:
+        return True
+
+    def _lw_buffers(self, table):
+        bufs = getattr(table, "layerwise", None)
+        if bufs is None:
+            dev = self.arena.device
+            flags = torch.tensor([(KERNELS.LW_ADAPTED if is_adapted(s) else 0)
+                                  | (KERNELS.LW_CLIPPED if s.is_model else 0) for s in table.slots],
+                                 dtype=torch.int32).to(dev)
+            ratio = torch.ones(max(table.n_segs, 1), dtype=torch.float32, device=dev)
+            nbytes = KERNELS.layerwise_scratch_bytes(table.n_tiles, table.n_segs)
+            scratch = torch.zeros((nbytes + 15) // 16 * 4, dtype=torch.int32, device=dev)
+            bufs = table.layerwise = (flags, ratio, scratch)
+        return bufs
+
+    def apply_table(self, table, *, grad_scale: float = 1.0,
+                    clip_coef_dev: Optional[torch.Tensor] = None) -> None:
+        """Update every slot of ``table``; ``clip_coef_dev`` multiplies the gradients of model
+        parameters only, as in ``apply_range``."""
+        if table.n_segs:
+            self._launch_lw(table, grad_scale, clip_coef_dev, *self._lw_buffers(table))
+
+    # the flat-bucket and fused NVLS launchers of the base rule see parts of tensors, and read
+    # another ``dyn`` layout: never reached, and refused rather than silently wrong
+    def _launch(self, lo, hi, grad_scale, coef):
+        raise RuntimeError("%s updates whole tensors: use apply_table / apply_range" % type(self).__name__)
+
+    def _launch_mt(self, table, grad_scale):
+        raise RuntimeError("%s updates through the K2-lw kernels: use apply_table" % type(self).__name__)
+
+    def _launch_nvls(self, lo, hi, grad_scale):
+        raise RuntimeError("%s has no fused NVLS step (per-tensor norms need whole tensors)"
+                           % type(self).__name__)
+
+    def last_ratios(self, table) -> torch.Tensor:
+        """Trust ratio of each slot of ``table`` from its last update (device tensor)."""
+        return self._lw_buffers(table)[1][:table.n_segs]
+
+    def apply_range(self, lo: int, hi: int, *, grad_scale: float = 1.0,
+                    clip_coef_dev: Optional[torch.Tensor] = None) -> None:
+        """Whole slots inside ``[lo, hi)``, gradients read from the arena."""
+        from .multi_tensor import GradSegTable
+        tables = self.__dict__.setdefault("_range_tables", {})
+        table = tables.get((lo, hi))
+        if table is None:
+            slots = [s for s in self.arena.slots if lo <= s.offset and s.end <= hi]
+            cut = [s.index for s in self.arena.slots if s.offset < hi and s.end > lo and s not in slots]
+            if cut:
+                raise ValueError("layer-wise updates take whole tensors: [%d, %d) cuts the slots of "
+                                 "parameters %s" % (lo, hi, cut))
+            table = tables[(lo, hi)] = GradSegTable(slots, self.arena.device)
+            g = self.arena.grad
+            for s in slots:
+                table.point(s, g.data_ptr() + s.offset * g.element_size(), g.dtype)
+        table.upload()
+        self.apply_table(table, grad_scale=grad_scale, clip_coef_dev=clip_coef_dev)
+
+
+class FusedLars(_LayerwiseMixin, FusedSGD):
+    """LARS: layer-wise trust ratio on the SGD rule (``types.LayerAdaptation.LARS``).  State and
+    ``state_dict()`` are ``torch.optim.SGD``'s (``momentum_buffer`` in SGD's units)."""
+
+    def __init__(self, arena, lr, momentum=0.0, weight_decay=0.0):
+        super().__init__(arena, lr=lr, momentum=momentum, dampening=0.0, weight_decay=weight_decay)
+
+    def _launch_lw(self, table, grad_scale, coef, flags, ratio, scratch):
+        h = self.hyper
+        mu = float(h["momentum"])
+        KERNELS.lars_mt(self.arena.master, self._state("momentum_buffer") if mu != 0.0 else None,
+                        self.arena.lp, table, flags, ratio, scratch, lr=float(h["lr"]), mu=mu,
+                        wd=float(h["weight_decay"]), grad_scale=grad_scale, grad_scale_dev=coef,
+                        first_step=(self._steps == 0), dyn=self._dyn)
+
+
+class FusedLamb(_LayerwiseMixin, FusedAdam):
+    """LAMB: layer-wise trust ratio on the Adam rule (``types.LayerAdaptation.LAMB``) with
+    DECOUPLED weight decay on adapted tensors (part of the update direction, scaled by the ratio),
+    unlike ``FusedAdam``'s L2-coupled decay.  State and ``state_dict()`` are
+    ``torch.optim.Adam``'s, so checkpoints move between LAMB and Adam in both directions."""
+
+    def __init__(self, arena, lr, betas=(0.9, 0.999), eps=1e-8, weight_decay=0.0):
+        super().__init__(arena, lr=lr, betas=betas, eps=eps, weight_decay=weight_decay, amsgrad=False)
+
+    def _dyn_values(self):
+        h = self.hyper
+        step = self._steps + 1
+        bc1 = 1.0 - float(h["betas"][0]) ** step
+        bc2 = 1.0 - float(h["betas"][1]) ** step
+        return (float(h["lr"]), 1.0 / bc1, bc2 ** 0.5)
+
+    def _launch_lw(self, table, grad_scale, coef, flags, ratio, scratch):
+        h = self.hyper
+        KERNELS.lamb_mt(self.arena.master, self._state("exp_avg"), self._state("exp_avg_sq"), self.arena.lp,
+                        table, flags, ratio, scratch, lr=float(h["lr"]), beta1=float(h["betas"][0]),
+                        beta2=float(h["betas"][1]), eps=float(h["eps"]), wd=float(h["weight_decay"]),
+                        step=self._steps + 1, grad_scale=grad_scale, grad_scale_dev=coef, dyn=self._dyn)
+
+
+def check_layer_adaptation(optim_opts: OptimOpts, layer_adaptation: LayerAdaptation) -> None:
+    """LARS needs the SGD rule, LAMB the Adam rule without amsgrad; anything else is a ValueError."""
+    la = LayerAdaptation(layer_adaptation)
+    ok = (la is LayerAdaptation.NONE
+          or (la is LayerAdaptation.LARS and optim_opts.algo == OptAlgorithm.SGD)
+          or (la is LayerAdaptation.LAMB and optim_opts.algo == OptAlgorithm.ADAM and not optim_opts.amsgrad))
+    if not ok:
+        raise ValueError("layer adaptation %r cannot be combined with optimizer %r%s (LARS needs sgd, "
+                         "LAMB needs adam without amsgrad)"
+                         % (la.value, getattr(optim_opts.algo, "value", optim_opts.algo),
+                            " with amsgrad" if optim_opts.amsgrad else ""))
+
+
+def create_fused_optimizer(arena: ParamArena, optim_opts: OptimOpts,
+                           layer_adaptation: LayerAdaptation = LayerAdaptation.NONE) -> FusedArenaOptimizer:
+    """Same dispatch and argument mapping as the reference's ``_create_optimizer``; with a layer
+    adaptation, its LARS / LAMB counterpart."""
+    check_layer_adaptation(optim_opts, layer_adaptation)
+    if layer_adaptation == LayerAdaptation.LARS:
+        return FusedLars(arena, lr=optim_opts.lr, momentum=optim_opts.momentum,
+                         weight_decay=optim_opts.weightDecay)
+    if layer_adaptation == LayerAdaptation.LAMB:
+        return FusedLamb(arena, lr=optim_opts.lr, weight_decay=optim_opts.weightDecay, eps=optim_opts.epsilon)
     algo = optim_opts.algo
     if algo == OptAlgorithm.RMSPROP:
         return FusedRMSprop(arena, lr=optim_opts.lr, momentum=optim_opts.momentum,

@@ -15,7 +15,9 @@ solver_worker.py:585-592).  Differences that matter on H100:
 * each bucket's all-reduce is issued on a side stream the moment its last gradient is ready and
   its fused update is chained right behind it, overlapping the rest of backward;
 * with clipping enabled the updates wait for the global norm (two-phase tail), computed by one
-  reduction kernel over the model range with no host sync.
+  reduction kernel over the model range with no host sync;
+* an optimizer whose update needs whole tensors (``needs_whole_tensors``: LARS, LAMB) takes the
+  clipping path's shape: per-bucket all-reduce only, then one update over the whole segment table.
 """
 import os
 from typing import Callable, Dict, List, Optional, Tuple
@@ -84,8 +86,11 @@ class GradBucketPipeline:
         # eager: update a bucket on the side stream as soon as it is complete (and reduced) while
         # backward is still running.  Needs no global norm, so clipping turns it off.  On one GPU
         # the caller decides (the persistent cuBLAS GEMMs leave the update few SMs to overlap on,
-        # so a single tail launch is cheaper to issue).
-        self.eager = eager_update and self.clip_norm == 0.0 and (self.distributed or self.on_cuda)
+        # so a single tail launch is cheaper to issue).  An optimizer that needs whole tensors
+        # (per-tensor norms) turns it off as well: its update is one tail over every slot.
+        self.whole_tensors = optimizer.needs_whole_tensors
+        self.eager = (eager_update and self.clip_norm == 0.0 and not self.whole_tensors
+                      and (self.distributed or self.on_cuda))
 
         cap = int(bucket_cap_mb * 1024 * 1024)
         first = int(first_bucket_mb * 1024 * 1024) if (first_bucket_mb and self.distributed) else None
@@ -403,6 +408,20 @@ class GradBucketPipeline:
         self.optimizer.end_step()
 
     def _tail_update(self) -> None:
+        if self.whole_tensors:
+            # one update over the whole table, each gradient read where it lies (1 GPU) or from the
+            # all-reduced arena (world > 1: the stragglers were gathered per bucket)
+            coef = None
+            if self.clip_norm > 0.0:
+                self._flatten_stragglers(self.arena.slots, "all", side=False)
+                coef = self._clip_coef()
+            table = self.tables.whole()
+            self._point(table)
+            table.upload()
+            self._update_table(table, coef)
+            if not self._keep_ext:
+                self._ext.clear()
+            return
         if self.clip_norm > 0.0:
             # the global norm needs every gradient first: gather the stragglers into the arena,
             # then K3 + K2 over the arena (the clip coefficient applies to model parameters only)
@@ -424,16 +443,24 @@ class GradBucketPipeline:
             return
         self._update(0, self.arena.numel, None)
 
-    def _update_table(self, table) -> None:
+    def _update_table(self, table, coef=None) -> None:
+        kw = {} if coef is None else {"clip_coef_dev": coef}
         if self.record_update_events and self.on_cuda:
             e0 = torch.cuda.Event(enable_timing=True)
             e1 = torch.cuda.Event(enable_timing=True)
             e0.record()
-            self.optimizer.apply_table(table, grad_scale=self.grad_scale)
+            self.optimizer.apply_table(table, grad_scale=self.grad_scale, **kw)
             e1.record()
             self.update_events.append((e0, e1, 0, self.arena.numel))
         else:
-            self.optimizer.apply_table(table, grad_scale=self.grad_scale)
+            self.optimizer.apply_table(table, grad_scale=self.grad_scale, **kw)
+
+    def _clip_coef(self):
+        """K3 over the model range of the gradient arena; returns the device clip coefficient."""
+        n_model = self.arena.model_end
+        KERNELS.grad_sumsq_clip(self.arena.grad[:n_model], n_model, pre_scale=self.grad_scale,
+                                max_norm=self.clip_norm, out3=self.clip_out, scratch=self.clip_scratch)
+        return self.clip_out[2:3]
 
     def _finish_partial(self, missing) -> None:
         """world_size == 1 and some parameters got no gradient: torch.optim skips those (no
@@ -445,11 +472,17 @@ class GradBucketPipeline:
             for s in self.arena.slots:
                 if s.index in skip and s.is_model:
                     self.arena.grad[s.offset:s.end].zero_()
-            n_model = self.arena.model_end
-            KERNELS.grad_sumsq_clip(self.arena.grad[:n_model], n_model, pre_scale=self.grad_scale,
-                                    max_norm=self.clip_norm, out3=self.clip_out,
-                                    scratch=self.clip_scratch)
-            coef = self.clip_out[2:3]
+            coef = self._clip_coef()
+        if self.whole_tensors:
+            # a table of the slots that got a gradient (now all in the arena); the others keep
+            # their weights and state
+            present = [s for s in self.arena.slots if s.index not in skip]
+            table = self.tables.flatten(("partial", tuple(s.index for s in present)), present)
+            self._point(table)
+            table.upload()
+            self._update_table(table, coef)
+            self.optimizer.end_step()
+            return
         run_lo = None
         prev_end = None
         for s in self.arena.slots:

@@ -28,19 +28,20 @@ import torch.nn as nn
 
 from .arena import ParamArena
 from .criteria import BaseParallelCriterion
-from .fused_optim import create_fused_optimizer
+from .fused_optim import check_layer_adaptation, create_fused_optimizer, is_adapted
 from .grad_sync import BufferBroadcaster, GradBucketPipeline
 from .lr_scheduler import DropEpochsScheduler, WarmupMultiStepLR
 from .problem import Problem
 from .solver_worker import (FractionalPerformanceSummary, SerializableSampleSummary,
                             SolverWorker)
-from .types import (Device, LRSchedulerAlgorithm, Mode, Precision, RunOpts, SampleSummary,
-                    Split)
+from .types import (Device, LayerAdaptation, LRSchedulerAlgorithm, Mode, Precision, RunOpts,
+                    SampleSummary, Split)
 
 logging.basicConfig(level=logging.INFO, format="%(levelname)s (%(process)d) %(message)s")
 logger = logging.getLogger(__name__)
 
 CHECKPOINT_NAME = ".checkpoint.pth"
+LAYER_ADAPTATION_ENV = "FRL_B200_LAYER_ADAPTATION"   # "none" (default) | "lars" | "lamb"
 PRECISION_ENV = "FRL_B200_PRECISION"      # "fp32" (default, reference parity) | "bf16"
 
 
@@ -94,6 +95,7 @@ class SolverWorkerArgs(NamedTuple):
     precision: Precision = Precision.FP32
     save_every: int = 1
     graph_step: Optional[bool] = None      # None: FRL_B200_CUDA_GRAPH (default off)
+    layer_adaptation: LayerAdaptation = LayerAdaptation.NONE
 
 
 def _torch_load(f, **kw):
@@ -235,6 +237,12 @@ def resolve_precision(explicit: Optional[Precision] = None) -> Precision:
     return Precision(os.environ.get(PRECISION_ENV, "fp32").lower())
 
 
+def resolve_layer_adaptation(explicit: Optional[LayerAdaptation] = None) -> LayerAdaptation:
+    if explicit is not None:
+        return LayerAdaptation(explicit)
+    return LayerAdaptation(os.environ.get(LAYER_ADAPTATION_ENV, "none").lower())
+
+
 class Solver:
     # ------------------------------------------------------------------------------------------
     # per-rank bootstrap (child process)
@@ -293,7 +301,8 @@ class Solver:
         # world > 1 without clipping: arena vectors other ranks reach go to symmetric/multicast
         # memory so all-reduce + update + broadcast can be one NVLS kernel per bucket
         symm_alloc = None
-        if distributed and not run_opts.optim.gradientClip:
+        if (distributed and not run_opts.optim.gradientClip
+                and args.layer_adaptation == LayerAdaptation.NONE):
             from .symm import try_make_allocator
             symm_alloc = try_make_allocator(device, args.world_size)
         from .arena_linear import head_layout_groups
@@ -309,7 +318,7 @@ class Solver:
             for buf in model.buffers():
                 if buf.is_floating_point():
                     buf.data = buf.data.to(torch.bfloat16)
-        optimizer = create_fused_optimizer(arena, run_opts.optim)
+        optimizer = create_fused_optimizer(arena, run_opts.optim, args.layer_adaptation)
         if checkpoint:
             optimizer.load_state_dict(checkpoint.optimizerState)
         nvls_link = None
@@ -359,7 +368,7 @@ class Solver:
             logger.info(
                 "frl_b200 step: precision %s | step issue %s | gradient exchange %s | update %s | "
                 "Linear layers with arena-born gradients %d (%d fused with their ReLU, %d in FP8) | "
-                "other gradients %s",
+                "other gradients %s | layer adaptation %s",
                 args.precision.value,
                 "CUDA-graph replay after 2 eager steps" if worker.graphed is not None else "eager launches",
                 ("fused NVLS kernel per bucket (K7), %d buckets" % len(pipeline.buckets)) if pipeline.nvls is not None
@@ -369,7 +378,10 @@ class Solver:
                 len(pipeline.linear_sites), sum(s.relu is not None for s in pipeline.linear_sites),
                 sum(s.fp8 for s in pipeline.linear_sites),
                 "read in place through segment tables (K2-mt / one flatten launch per bucket)"
-                if pipeline.mt_enabled else "copied into the arena per tensor")
+                if pipeline.mt_enabled else "copied into the arena per tensor",
+                "none" if args.layer_adaptation == LayerAdaptation.NONE else
+                "%s, %d of %d tensors adapted (K2-lw)" % (args.layer_adaptation.value,
+                                                          sum(is_adapted(s) for s in arena.slots), len(arena.slots)))
         scheduler = create_lr_scheduler(run_opts, worker.optimizer,
                                         checkpoint.epoch if checkpoint else -1)
         return worker, scheduler, checkpoint
@@ -571,7 +583,8 @@ class Solver:
     @classmethod
     def solve(cls, run_opts: RunOpts, problem: Problem, *, group_name: Optional[str],
               init_method: str, node_idx: int = 0, node_count: int = 1, memory_quota: int = 0,
-              precision: Optional[Precision] = None, graph: Optional[bool] = None
+              precision: Optional[Precision] = None, graph: Optional[bool] = None,
+              layer_adaptation: Optional[LayerAdaptation] = None
               ) -> Iterator[PerformanceSummary]:
         """The reference's entry point (solver.py:728-739) plus two keyword-only extensions:
 
@@ -584,7 +597,16 @@ class Solver:
                        has run 2 eager steps (the Problem's forward must be capturable: static
                        shapes, no host syncs; a failed capture falls back to eager launches).
                        None: FRL_B200_CUDA_GRAPH (default off).
+        ``layer_adaptation``  ``LayerAdaptation.LARS`` (with ``OptAlgorithm.SGD``) or ``.LAMB`` (with
+                       ``OptAlgorithm.ADAM``, no amsgrad): layer-wise trust-ratio updates for large
+                       batches, see ``types.LayerAdaptation``; any other combination raises
+                       ``ValueError`` before a rank starts.  None: FRL_B200_LAYER_ADAPTATION
+                       (default ``none``).  ``Mode.EVAL`` ignores it.
         """
+        adapt = LayerAdaptation.NONE
+        if run_opts.mode == Mode.TRAIN:
+            adapt = resolve_layer_adaptation(layer_adaptation)
+            check_layer_adaptation(run_opts.optim, adapt)
         n_visible = 0 if run_opts.cpuonly else _cuda_device_count_without_poisoning_fork()
         if n_visible == 0:
             raise RuntimeError(
@@ -622,7 +644,8 @@ class Solver:
                 node_idx=node_idx, node_count=node_count,
                 rank=node_idx * device_count + local_rank, local_rank=local_rank,
                 world_size=world_size, group_name=group_name, init_method=init_method,
-                cache=None, precision=prec, save_every=save_every, graph_step=graph)
+                cache=None, precision=prec, save_every=save_every, graph_step=graph,
+                layer_adaptation=adapt)
             if not run_opts.singleThreaded:
                 parent_conn, child_conn = ctx.Pipe(duplex=False)
                 proc = ctx.Process(target=cls._solver_worker_process,

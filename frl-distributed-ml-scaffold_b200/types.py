@@ -76,6 +76,45 @@ class Precision(Enum):
         return self is not Precision.FP32
 
 
+class LayerAdaptation(Enum):
+    """Extension (not in the reference): layer-wise learning-rate adaptation for large-batch
+    training, chosen with ``Solver.solve(..., layer_adaptation=...)`` or
+    ``FRL_B200_LAYER_ADAPTATION``.  Per arena slot, in fp32, with ``g^ = g * grad_scale`` (times the
+    clip coefficient when ``gradientClip`` is on, model parameters only), ``w`` the fp32 master
+    weights before the update and ``lr`` the scheduled rate.
+
+    A tensor is ADAPTED if it has 2 or more dimensions (Linear and conv weights, embeddings).  0-
+    and 1-D tensors (biases, normalisation affine parameters, criterion parameters) get ratio 1
+    and no weight decay.  The rule is fixed.
+
+    NONE - the plain ``OptimOpts.algo`` update.
+    LARS - layer adaptation on the SGD rule (You et al. 2017); needs ``algo == SGD``.  Trust
+           coefficient eta = 0.001 (fixed), mu = ``momentum``, no dampening:
+             adapted:     ratio = eta*||w|| / (||g^|| + wd*||w||) if ||w|| > 0 and ||g^|| > 0, else 1;
+                          d = ratio * (g^ + wd*w)
+             not adapted: d = g^
+             buf = d on the first step, else mu*buf + d;  w -= lr*buf   (mu = 0: no buffer)
+           The buffer has torch SGD's units: checkpoints load into ``torch.optim.SGD``.
+    LAMB - layer adaptation on the Adam rule (You et al. 2019); needs ``algo == ADAM`` and
+           ``amsgrad == False``.  beta = (0.9, 0.999), eps = ``epsilon``, lam = ``weightDecay`` if
+           adapted else 0, t = the arena's step count (as for the fused Adam):
+             m = m + (1-beta1)*(g^ - m);  v = beta2*v + (1-beta2)*g^^2
+             u = (m / bc1) / (sqrt(v) / sqrt(bc2) + eps) + lam*w          bc_i = 1 - beta_i^t
+             ratio = ||w|| / ||u|| if adapted and ||w|| > 0 and ||u|| > 0, else 1;  w -= lr*ratio*u
+           The weight decay is DECOUPLED (part of u), unlike the L2-coupled decay of this
+           package's Adam.  The state is Adam's: checkpoints load into ``torch.optim.Adam`` and an
+           Adam checkpoint resumes under LAMB.
+
+    A non-finite gradient still gives non-finite weights (the ratio-1 branch passes a NaN on), so
+    the NaN-loss check fires.  Both run as two tile-parallel kernels over whole tensors (K2-lw), so
+    the gradients are all-reduced per bucket and the update runs once after backward: no eager
+    per-bucket update and no fused NVLS step.  ``Mode.EVAL`` ignores the setting.
+    """
+    NONE = "none"
+    LARS = "lars"
+    LAMB = "lamb"
+
+
 # --- records ---------------------------------------------------------------------------------
 
 class SampleSummary(NamedTuple):
@@ -104,6 +143,9 @@ class OptimOpts(NamedTuple):
     amsgrad       Adam: adds the running maximum of the second moment (a third state vector)
     gradientClip  > 0: global-norm clip of the MODEL parameters' gradients (K3 computes the
                   coefficient on the device, K2 applies it); turns the fused NVLS step off
+
+    Layer-wise adaptation (LARS on SGD, LAMB on Adam) is not a field here but a keyword of
+    ``Solver.solve``: see ``LayerAdaptation``.
     """
     algo: OptAlgorithm
     lr: float = 0.001

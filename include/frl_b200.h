@@ -126,6 +126,49 @@ int frl_rmsprop_mt(float* p, float* sq, float* buf, void* p_lp, const frl_grad_s
                    const float* dyn, void* stream);
 
 /* ------------------------------------------------------------------------------------------
+ * K2-lw — layer-wise adaptive updates over a segment table (an extension: the reference offers
+ * SGD, Adam and RMSprop only).  LARS (You et al. 2017) is layer adaptation on the SGD rule, LAMB
+ * (You et al. 2019) on the Adam rule.  Segment table, p / state / p_lp and the other arguments
+ * as in frl_*_mt; additionally
+ *   n_segs         segments in the table
+ *   seg_flags_dev  int32 [n_segs]: FRL_LW_ADAPTED = the tensor is adapted (2 or more dimensions:
+ *                  Linear / conv weights, embeddings; 0-/1-D tensors such as biases, normalisation
+ *                  affine and criterion parameters get ratio 1 and no weight decay);
+ *                  FRL_LW_CLIPPED = grad_scale_dev multiplies this segment's gradient (model
+ *                  parameters under global-norm clipping; criterion parameters are not clipped)
+ *   ratio_dev      fp32 [n_segs], written: the trust ratio each tensor was updated with
+ *   scratch        frl_layerwise_scratch_bytes(n_tiles, n_segs) bytes, zero-initialised once
+ * Per segment, fp32, with g^ = g * grad_scale (* *grad_scale_dev if FRL_LW_CLIPPED), w the master
+ * weights before the update, lr the scheduled rate:
+ *   LARS (trust coefficient eta = 0.001, fixed; mu = momentum; no dampening):
+ *     adapted:     ratio = eta*||w|| / (||g^|| + wd*||w||) if ||w|| > 0 and ||g^|| > 0, else 1;
+ *                  d = ratio * (g^ + wd*w)
+ *     not adapted: d = g^   (ratio 1, no weight decay)
+ *     buf = first_step ? d : mu*buf + d ; w -= lr*buf        (mu == 0: w -= lr*d, buf may be NULL)
+ *   LAMB (lam = wd if adapted else 0; t = step, >= 1):
+ *     m = m + (1-beta1)*(g^ - m) ; v = beta2*v + (1-beta2)*g^^2
+ *     u = (m / bc1) / (sqrt(v) / sqrt(bc2) + eps) + lam*w     bc_i = 1 - beta_i^t
+ *     ratio = ||w|| / ||u|| if adapted and ||w|| > 0 and ||u|| > 0, else 1 ;  w -= lr*ratio*u
+ *     The weight decay is DECOUPLED (part of u), unlike frl_adam's L2-coupled decay.
+ * A non-finite gradient yields non-finite weights (a NaN norm takes the ratio-1 branch, which
+ * passes the NaN on).  Norms: fp32 per tile, folded per tensor in double in tile order (no float
+ * atomics, deterministic).  Two launches: stats (LAMB writes m, v here) and apply.
+ *   dyn  LARS: dyn[0] = lr ;  LAMB: dyn[0] = lr, dyn[1] = 1/(1-beta1^t), dyn[2] = sqrt(1-beta2^t).
+ * ---------------------------------------------------------------------------------------- */
+enum { FRL_LW_ADAPTED = 1, FRL_LW_CLIPPED = 2 };
+int64_t frl_layerwise_scratch_bytes(int64_t n_tiles, int64_t n_segs);
+int frl_lars_mt(float* p, float* buf, void* p_lp, const frl_grad_seg* segs_dev,
+                const int64_t* tile_prefix_dev, const int32_t* tile_seg_dev, int64_t n_tiles,
+                int64_t n_segs, const int32_t* seg_flags_dev, float* ratio_dev, void* scratch,
+                double lr, double mu, double wd, double grad_scale, const float* grad_scale_dev,
+                const float* dyn, int first_step, void* stream);
+int frl_lamb_mt(float* p, float* m, float* v, void* p_lp, const frl_grad_seg* segs_dev,
+                const int64_t* tile_prefix_dev, const int32_t* tile_seg_dev, int64_t n_tiles,
+                int64_t n_segs, const int32_t* seg_flags_dev, float* ratio_dev, void* scratch,
+                double lr, double beta1, double beta2, double eps, double wd, int64_t step,
+                double grad_scale, const float* grad_scale_dev, const float* dyn, void* stream);
+
+/* ------------------------------------------------------------------------------------------
  * K3 — global gradient norm for clipping.
  * Replaces torch.nn.utils.clip_grad_norm_ (reference solver_worker.py:588-591): one pass
  * over the model-parameter range of the gradient arena.
