@@ -66,6 +66,7 @@ SIGNATURES = {
     "frl_lars_mt": (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _i64, _i64, _vp, _vp, _vp, _d, _d, _d, _d, _vp, _vp, _i, _vp]),
     "frl_lamb_mt": (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _i64, _i64, _vp, _vp, _vp, _d, _d, _d, _d, _d, _i64,
                          _d, _vp, _vp, _vp]),
+    "frl_grad_accumulate_mt": (_i, [_vp, _vp, _vp, _vp, _i64, _d, _i, _vp, _vp]),
     "frl_reduce_scratch_bytes": (_i64, []),
     "frl_grad_sumsq_clip": (_i, [_vp, _i64, _i, _f, _f, _vp, _vp, _vp]),
     "frl_criteria_scratch_bytes": (_i64, [_i]),
@@ -264,6 +265,22 @@ def lamb_mt(p, m, v, p_lp, table, flags, ratio, scratch, *, lr, beta1, beta2, ep
                              table.tile_seg_dev_ptr, table.n_tiles, table.n_segs, _ptr(flags), _ptr(ratio),
                              _ptr(scratch), lr, beta1, beta2, eps, wd, step, grad_scale, _ptr(grad_scale_dev),
                              _ptr(dyn), _stream()), "frl_lamb_mt")
+
+
+# ---- K10: gradient accumulation over a segment table ----------------------------------------------
+
+def grad_accumulate_mt(acc, table, *, w: float = 1.0, first: bool = False, dyn=None) -> None:
+    """acc[slot] = (first ? 0 : acc[slot]) + w * g for every slot of ``table`` (a
+    ``multi_tensor.GradSegTable`` whose device copy is current; a slot pointed at address 0
+    contributes nothing).  ``dyn``: optional device fp32 [2] = (w, first) overriding the
+    arguments.  See frl_grad_accumulate_mt in include/frl_b200.h."""
+    if acc.dtype != torch.float32 or not acc.is_contiguous():
+        raise NativeLibraryError("gradient accumulation: the accumulator must be contiguous fp32")
+    if dyn is not None and (dyn.dtype != torch.float32 or dyn.numel() < 2):
+        raise NativeLibraryError("gradient accumulation: dyn must be fp32 [2]")
+    _check(lib().frl_grad_accumulate_mt(_ptr(acc), table.segs_dev_ptr, table.prefix_dev_ptr, table.tile_seg_dev_ptr,
+                                        table.n_tiles, float(w), int(bool(first)), _ptr(dyn), _stream()),
+           "frl_grad_accumulate_mt")
 
 
 # ---- K3 -------------------------------------------------------------------------------------

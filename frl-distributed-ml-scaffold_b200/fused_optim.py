@@ -52,6 +52,7 @@ class FusedArenaOptimizer(torch.optim.Optimizer):
         # replayed from a CUDA graph, where by-value kernel arguments are frozen at capture
         self._dyn: Optional[torch.Tensor] = None
         self._dyn_last: Optional[Tuple[float, ...]] = None
+        self._grad_src: Optional[torch.Tensor] = None      # apply_range(grad_src=...)
         # fused NVLS step (world > 1): set by the pipeline; each rank then updates only its
         # 1/world shard of every bucket (master + state), the weights arrive by multicast
         self.nvls = None
@@ -117,19 +118,25 @@ class FusedArenaOptimizer(torch.optim.Optimizer):
         self._in_step = False
 
     def apply_range(self, lo: int, hi: int, *, grad_scale: float = 1.0,
-                    clip_coef_dev: Optional[torch.Tensor] = None) -> None:
+                    clip_coef_dev: Optional[torch.Tensor] = None,
+                    grad_src: Optional[torch.Tensor] = None) -> None:
         """Update arena elements ``[lo, hi)``.  ``clip_coef_dev`` (a device scalar written by
         the norm kernel) multiplies model-parameter gradients only — the reference clips
         ``model.parameters()`` and leaves criterion parameters alone
-        (reference solver_worker.py:588-591)."""
+        (reference solver_worker.py:588-591).  ``grad_src``: an arena-shaped gradient vector read
+        instead of ``arena.grad`` (the fp32 gradient accumulator)."""
         if hi <= lo:
             return
-        split = self.arena.model_end
-        if clip_coef_dev is not None and lo < split < hi:
-            self._launch(lo, split, grad_scale, clip_coef_dev)
-            self._launch(split, hi, grad_scale, None)
-        else:
-            self._launch(lo, hi, grad_scale, clip_coef_dev if lo < split else None)
+        self._grad_src = grad_src
+        try:
+            split = self.arena.model_end
+            if clip_coef_dev is not None and lo < split < hi:
+                self._launch(lo, split, grad_scale, clip_coef_dev)
+                self._launch(split, hi, grad_scale, None)
+            else:
+                self._launch(lo, hi, grad_scale, clip_coef_dev if lo < split else None)
+        finally:
+            self._grad_src = None
 
     def _launch(self, lo: int, hi: int, grad_scale: float, coef) -> None:
         raise NotImplementedError
@@ -194,7 +201,8 @@ class FusedArenaOptimizer(torch.optim.Optimizer):
     def _slices(self, lo: int, hi: int):
         a = self.arena
         lp = a.lp[lo:hi] if (a.lp is not None and lo < a.model_end) else None
-        return a.master[lo:hi], a.grad[lo:hi], lp
+        g = a.grad if self._grad_src is None else self._grad_src
+        return a.master[lo:hi], g[lo:hi], lp
 
     # -- torch-format (de)serialisation ----------------------------------------------------------
     def _per_param_extra(self) -> Dict[str, Any]:

@@ -17,10 +17,13 @@ solver_worker.py:585-592).  Differences that matter on H100:
 * with clipping enabled the updates wait for the global norm (two-phase tail), computed by one
   reduction kernel over the model range with no host sync;
 * an optimizer whose update needs whole tensors (``needs_whole_tensors``: LARS, LAMB) takes the
-  clipping path's shape: per-bucket all-reduce only, then one update over the whole segment table.
+  clipping path's shape: per-bucket all-reduce only, then one update over the whole segment table;
+* with gradient accumulation (k > 1) no bucket is launched during backward: one K10 launch per
+  microbatch folds every gradient into an fp32 accumulator, and the microbatch that closes a group
+  all-reduces the accumulator per bucket, clips and updates from it.
 """
 import os
-from typing import Callable, Dict, List, Optional, Tuple
+from typing import Callable, Dict, List, NamedTuple, Optional, Tuple
 
 import torch
 import torch.distributed as dist
@@ -31,6 +34,37 @@ from .arena import ParamArena
 from .fused_optim import FusedArenaOptimizer
 
 KERNELS = _native     # swapped by CPU tests of the host logic
+
+
+class MicroBatch(NamedTuple):
+    """Position of one microbatch of a training split under gradient accumulation."""
+    first: bool        # opens a group: K10 overwrites the accumulator
+    closes: bool       # closes a group: the update runs after its backward
+    rows: int          # n_i
+    weight: float      # w_i = n_i / B
+    group_rows: int    # N: rows of the group it belongs to
+
+
+def accumulation_plan(n_batches: int, k: int, batch_size: int = 1,
+                      n_samples: Optional[int] = None) -> List[MicroBatch]:
+    """Groups of ``k`` consecutive microbatches of one split.  Microbatch ``j`` closes a group if
+    ``(j + 1) % k == 0`` or it is the split's last, so the last group may be short; no group
+    crosses a split.  Every microbatch has ``batch_size`` rows except the last, which has what
+    is left of ``n_samples`` (default: a full one)."""
+    if n_batches <= 0:
+        return []
+    last = batch_size if n_samples is None else n_samples - (n_batches - 1) * batch_size
+    if not 0 < last <= batch_size:
+        raise ValueError("%r samples do not make %d batches of %d" % (n_samples, n_batches, batch_size))
+    rows = [batch_size] * (n_batches - 1) + [last]
+    plan: List[MicroBatch] = []
+    for lo in range(0, n_batches, k):
+        group = rows[lo:lo + k]
+        n_group = sum(group)
+        for i, n in enumerate(group):
+            plan.append(MicroBatch(first=i == 0, closes=i == len(group) - 1, rows=n,
+                                   weight=n / batch_size, group_rows=n_group))
+    return plan
 
 
 class _TableSet:
@@ -74,7 +108,7 @@ class GradBucketPipeline:
     def __init__(self, arena: ParamArena, optimizer: FusedArenaOptimizer, *,
                  process_group=None, world_size: int = 1, clip_norm: float = 0.0,
                  bucket_cap_mb: float = 25.0, first_bucket_mb: Optional[float] = 1.0,
-                 eager_update: bool = True, nvls_link=None) -> None:
+                 eager_update: bool = True, nvls_link=None, accumulation: int = 1) -> None:
         self.arena = arena
         self.optimizer = optimizer
         self.pg = process_group
@@ -83,14 +117,18 @@ class GradBucketPipeline:
         self.grad_scale = 1.0 / world_size
         self.distributed = world_size > 1
         self.on_cuda = arena.device.type == "cuda"
+        if isinstance(accumulation, bool) or int(accumulation) != accumulation or accumulation < 1:
+            raise ValueError("gradient accumulation must be an integer >= 1, got %r" % (accumulation,))
+        self.accumulation = int(accumulation)
         # eager: update a bucket on the side stream as soon as it is complete (and reduced) while
         # backward is still running.  Needs no global norm, so clipping turns it off.  On one GPU
         # the caller decides (the persistent cuBLAS GEMMs leave the update few SMs to overlap on,
         # so a single tail launch is cheaper to issue).  An optimizer that needs whole tensors
-        # (per-tensor norms) turns it off as well: its update is one tail over every slot.
+        # (per-tensor norms) turns it off as well: its update is one tail over every slot.  So does
+        # gradient accumulation: a microbatch's gradients go into the accumulator, not to an update.
         self.whole_tensors = optimizer.needs_whole_tensors
         self.eager = (eager_update and self.clip_norm == 0.0 and not self.whole_tensors
-                      and (self.distributed or self.on_cuda))
+                      and self.accumulation == 1 and (self.distributed or self.on_cuda))
 
         cap = int(bucket_cap_mb * 1024 * 1024)
         first = int(first_bucket_mb * 1024 * 1024) if (first_bucket_mb and self.distributed) else None
@@ -180,6 +218,59 @@ class GradBucketPipeline:
         # timing taps (bench): list of (start_event, end_event, lo, hi) for update launches
         self.record_update_events = False
         self.update_events: List[Tuple[torch.cuda.Event, torch.cuda.Event, int, int]] = []
+        self.accumulate_events: List[Tuple[torch.cuda.Event, torch.cuda.Event]] = []     # K10 launches
+
+        # gradient accumulation (k > 1): after each microbatch's backward ONE K10 launch folds every
+        # gradient, weighted, into an fp32 arena-shaped accumulator; the microbatch that closes a
+        # group runs the exchange and the update from it.  k == 1 allocates and launches nothing.
+        self.acc: Optional[torch.Tensor] = None
+        if self.accumulation > 1:
+            self.acc = torch.zeros(arena.numel, dtype=torch.float32, device=arena.device)
+            # (w, first) of the next K10 launch, device-resident so one captured graph serves
+            # every position inside a group; uploaded from a pinned ring like the optimizer's scalars
+            # (1, 1) until set_microbatch() says otherwise, as the by-value defaults below: a caller
+            # that never sets a position gets one microbatch per group (weight 1), never a zero update
+            self._acc_dyn = torch.ones(2, dtype=torch.float32, device=arena.device)
+            self._acc_dyn_host = torch.zeros(self._ACC_RING, 2, dtype=torch.float32, pin_memory=self.on_cuda)
+            self._acc_dyn_slot = 0
+            self._acc_dyn_last: Optional[Tuple[float, float]] = (1.0, 1.0)
+            self._acc_tables: Dict[Tuple[int, ...], object] = {}     # update tables reading the accumulator
+        self._acc_first = True
+        self._acc_closes = True
+        self._acc_weight = 1.0
+        self._acc_scale = self.grad_scale
+        self._acc_seen = set()         # slots that got a gradient in some microbatch of the open group
+        self.last_ready: frozenset = frozenset()
+
+    _ACC_RING = 16
+
+    @property
+    def accumulator_bytes(self) -> int:
+        return 0 if self.acc is None else self.acc.numel() * 4
+
+    def set_microbatch(self, *, first: bool, closes: bool, weight: float = 1.0,
+                       group_scale: float = 1.0) -> None:
+        """Position of the next microbatch in its accumulation group (k > 1; call before its
+        forward, never inside a CUDA-graph capture).  ``first``: it opens the group (K10 overwrites
+        the accumulator); ``closes``: the update runs after its backward; ``weight``: n_i / B, its
+        rows over the batch size; ``group_scale``: B / N, the batch size over the group's rows."""
+        if self.acc is None:
+            return
+        self._acc_first, self._acc_closes = bool(first), bool(closes)
+        self._acc_weight = float(weight)
+        self._acc_scale = float(group_scale) / self.world
+        if first:
+            self._acc_seen.clear()
+        vals = (self._acc_weight, 1.0 if first else 0.0)
+        if vals != self._acc_dyn_last:
+            if self.on_cuda:
+                row = self._acc_dyn_host[self._acc_dyn_slot % self._ACC_RING]
+                self._acc_dyn_slot += 1
+                row[0], row[1] = vals
+                self._acc_dyn.copy_(row, non_blocking=True)
+            else:
+                self._acc_dyn.copy_(torch.tensor(vals, dtype=torch.float32))
+            self._acc_dyn_last = vals
 
     # -- step protocol ---------------------------------------------------------------------------
     def begin_step(self) -> None:
@@ -263,7 +354,7 @@ class GradBucketPipeline:
             if b.launched:                    # the first half of a row-split weight went ahead
                 continue
             b.pending -= 1
-            if b.pending == 0 and (self.distributed or self.eager):
+            if b.pending == 0 and (self.distributed or self.eager) and self.acc is None:
                 self._launch_bucket(b)
 
     def row_split(self, slot) -> int:
@@ -350,6 +441,15 @@ class GradBucketPipeline:
         self.forward_gen += 1
         self._step_open = False
         self._tail_deferred = False
+        if self.acc is not None and not (self.distributed and self._ready != self._n_slots):
+            # k > 1: fold this microbatch into the accumulator; the group's last one updates.
+            # Inside a capture the K10 launch is recorded and the update is left to run_tail().
+            self._accumulate_microbatch(keep_refs=defer_tail)
+            if defer_tail:
+                self._tail_deferred = True
+            elif self._acc_closes:
+                self._update_from_accumulator()
+            return
         if self._ready != self._n_slots:
             missing = [s.index for s in self.arena.slots if id(s.param) not in self._ready_ids]
             if self.distributed:
@@ -392,10 +492,18 @@ class GradBucketPipeline:
         """True if a step ends with tail launches (not everything is updated eagerly)."""
         return not self.eager
 
-    def run_tail(self, grad_refs=None, tables=None) -> None:
+    def run_tail(self, grad_refs=None, tables=None, ready=None) -> None:
         """The deferred part of ``finish_step(defer_tail=True)``; also what a CUDA-graph replay
         of the captured step is followed by (then with the capture's gradient references and
-        segment tables: the replayed backward wrote to exactly those addresses)."""
+        segment tables: the replayed backward wrote to exactly those addresses).  With gradient
+        accumulation: the update from the accumulator if this microbatch closes its group;
+        ``ready`` names the slots the replayed K10 launch accumulated."""
+        if self.acc is not None:
+            if ready is not None:
+                self._acc_seen |= ready
+            if self._acc_closes:
+                self._update_from_accumulator()
+            return
         if grad_refs is not None:
             mine = (self._ext, self.tables)
             self._ext, self.tables, self._keep_ext = grad_refs, tables, True
@@ -483,19 +591,108 @@ class GradBucketPipeline:
             self._update_table(table, coef)
             self.optimizer.end_step()
             return
-        run_lo = None
-        prev_end = None
+        for lo, hi in self._runs(lambda s: s.index not in skip
+                                 and not any(a <= s.offset < z for a, z in done)):
+            self._update(lo, hi, coef)
+        self.optimizer.end_step()
+
+    def _runs(self, keep) -> List[Tuple[int, int]]:
+        """Arena ranges ``[lo, hi)`` of the maximal runs of consecutive slots with ``keep(slot)``."""
+        runs: List[Tuple[int, int]] = []
+        run_lo = prev_end = None
         for s in self.arena.slots:
-            if s.index in skip or any(lo <= s.offset < hi for lo, hi in done):
+            if not keep(s):
                 if run_lo is not None:
-                    self._update(run_lo, prev_end, coef)
+                    runs.append((run_lo, prev_end))
                     run_lo = None
                 continue
             if run_lo is None:
                 run_lo = s.offset
             prev_end = s.end
         if run_lo is not None:
-            self._update(run_lo, prev_end, coef)
+            runs.append((run_lo, prev_end))
+        return runs
+
+    # -- gradient accumulation (k > 1) -------------------------------------------------------------
+    def _accumulate_microbatch(self, keep_refs: bool = False) -> None:
+        """ONE K10 launch over the whole table: every gradient of this microbatch, where it lies,
+        times n_i / B into the accumulator; slots without a gradient point at NULL (nothing added,
+        zeroed when the microbatch opens its group)."""
+        table = self.tables.whole()
+        g_arena = self.arena.grad
+        esz = g_arena.element_size()
+        base = g_arena.data_ptr()
+        ready = []
+        for s in table.slots:
+            if id(s.param) not in self._ready_ids:
+                table.point(s, 0, g_arena.dtype)
+                continue
+            ready.append(s.index)
+            g = self._ext.get(s.index)
+            if g is None:
+                table.point(s, base + s.offset * esz, g_arena.dtype)
+            else:
+                table.point(s, g.data_ptr(), g.dtype)
+        self.last_ready = frozenset(ready)
+        self._acc_seen.update(ready)
+        table.upload()
+        timed = self.record_update_events and self.on_cuda
+        if timed:
+            e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+            e0.record()
+        KERNELS.grad_accumulate_mt(self.acc, table, w=self._acc_weight, first=self._acc_first,
+                                   dyn=self._acc_dyn)
+        if timed:
+            e1.record()
+            self.accumulate_events.append((e0, e1))
+        if not keep_refs:
+            self._ext.clear()            # the launch is enqueued: stream order protects the reads
+
+    def _acc_table(self, slots):
+        """Segment table of ``slots`` pointing into the accumulator (fp32), built once per set."""
+        key = tuple(s.index for s in slots)
+        t = self._acc_tables.get(key)
+        if t is None:
+            from .multi_tensor import GradSegTable
+            t = self._acc_tables[key] = GradSegTable(slots, self.arena.device)
+            for s in slots:
+                t.point(s, self.acc.data_ptr() + 4 * s.offset, torch.float32)
+        t.upload()
+        return t
+
+    def _update_from_accumulator(self) -> None:
+        """The group is closed: exchange the accumulator (fp32, per bucket), clip, update once.
+        ``_acc_scale`` = B / (world * N) turns the weighted sum into the group's mean gradient."""
+        acc, scale = self.acc, self._acc_scale
+        if self.distributed:
+            for b in self.buckets:
+                dist.all_reduce(acc[b.lo:b.hi], op=dist.ReduceOp.SUM, group=self.pg)
+            present = list(self.arena.slots)
+        else:
+            # one GPU: a slot that got no gradient in any microbatch keeps its weights and state
+            present = [s for s in self.arena.slots if s.index in self._acc_seen]
+        timed = self.record_update_events and self.on_cuda
+        if timed:
+            e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+            e0.record()
+        coef = None
+        if self.clip_norm > 0.0:
+            n_model = self.arena.model_end
+            KERNELS.grad_sumsq_clip(acc[:n_model], n_model, pre_scale=scale, max_norm=self.clip_norm,
+                                    out3=self.clip_out, scratch=self.clip_scratch)
+            coef = self.clip_out[2:3]
+        if self.whole_tensors:
+            if present:
+                self.optimizer.apply_table(self._acc_table(present), grad_scale=scale, clip_coef_dev=coef)
+        elif len(present) == len(self.arena.slots):
+            self.optimizer.apply_range(0, self.arena.numel, grad_scale=scale, clip_coef_dev=coef, grad_src=acc)
+        else:
+            seen = {s.index for s in present}
+            for lo, hi in self._runs(lambda s: s.index in seen):
+                self.optimizer.apply_range(lo, hi, grad_scale=scale, clip_coef_dev=coef, grad_src=acc)
+        if timed:
+            e1.record()
+            self.update_events.append((e0, e1, 0, self.arena.numel))
         self.optimizer.end_step()
 
     # -- one-time synchronisation ----------------------------------------------------------------

@@ -11,7 +11,8 @@ CUDA graph and replayed with a single launch.
 What stays outside the graph (cheap, and needs per-step values):
   * filling the static input buffers (the cast kernel writes them directly in BF16 mode);
   * per-step scalars (lr, Adam bias corrections): uploaded to the optimizer's ``dyn`` block,
-    which the captured update kernels read from device memory;
+    which the captured update kernels read from device memory; with gradient accumulation the
+    K10 launch's (weight, first) likewise, and the group-closing update runs after the replay;
   * on one GPU the tail update (and the clip-norm kernel) so it can be timed and tuned alone;
   * the 4*(1+T)-byte copy of the loss vector into the pinned loss log.
 """
@@ -111,6 +112,7 @@ class _Captured:
         # tables that name them now belong to this graph: the replayed backward writes to exactly
         # those addresses, the tail update / the captured flatten launches read them there
         self.grad_refs, self.tables = w.pipeline.detach_grad_refs()
+        self.ready = w.pipeline.last_ready     # slots the captured K10 launch accumulates (k > 1)
         # capture executed nothing on the device, but begin_step() counted a step: undo it, the
         # replay performs the step for real (finish_step(defer_tail=True) left the optimizer's
         # step counter to run_tail())
@@ -143,7 +145,8 @@ class _Captured:
         global REPLAYED_LAUNCHES
         REPLAYED_LAUNCHES += self.frl_kernels
         w.pipeline.step_id += 1
-        w.pipeline.run_tail(self.grad_refs, self.tables)   # tail update (1 GPU / clipping) + step counter
+        # tail update (1 GPU / clipping) + step counter; with accumulation the group's update
+        w.pipeline.run_tail(self.grad_refs, self.tables, self.ready)
         if sink_row is not None:
             row = self._loss_vec
             if row is None:

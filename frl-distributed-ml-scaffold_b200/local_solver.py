@@ -20,7 +20,8 @@ class LocalSolver:
     @classmethod
     def solve(cls, run_opts: RunOpts, problem: Problem, save_notebook: bool = False,
               precision: Optional[Precision] = None, graph: Optional[bool] = None, *,
-              layer_adaptation: Optional[LayerAdaptation] = None) -> PerformanceSummary:
+              layer_adaptation: Optional[LayerAdaptation] = None,
+              grad_accumulation: Optional[int] = None) -> PerformanceSummary:
         if save_notebook:
             logger.warning("save_notebook is not supported by frl_b200 (visualisation only)")
         # a stale rendezvous file from a crashed run would poison the file:// store
@@ -32,6 +33,7 @@ class LocalSolver:
         last: Optional[PerformanceSummary] = None
         for last in Solver.solve(run_opts, problem, group_name=group_name,
                                  init_method="file://" + SYNC_FILE, precision=precision,
-                                 graph=graph, layer_adaptation=layer_adaptation):
+                                 graph=graph, layer_adaptation=layer_adaptation,
+                                 grad_accumulation=grad_accumulation):
             pass
         return last

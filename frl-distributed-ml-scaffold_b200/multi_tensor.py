@@ -73,7 +73,7 @@ class GradSegTable:
     def point(self, slot, ptr: int, dtype: torch.dtype) -> None:
         row = self._segs[self._row_of[slot.index]]
         code = _native.dtype_code(dtype)
-        if row.g != ptr or row.g_dtype != code:
+        if (row.g or 0) != ptr or row.g_dtype != code:       # ctypes reads a NULL pointer as None
             row.g = ptr
             row.g_dtype = code
             self._dirty = True

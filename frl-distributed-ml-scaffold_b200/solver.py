@@ -43,6 +43,7 @@ logger = logging.getLogger(__name__)
 CHECKPOINT_NAME = ".checkpoint.pth"
 LAYER_ADAPTATION_ENV = "FRL_B200_LAYER_ADAPTATION"   # "none" (default) | "lars" | "lamb"
 PRECISION_ENV = "FRL_B200_PRECISION"      # "fp32" (default, reference parity) | "bf16"
+GRAD_ACCUM_ENV = "FRL_B200_GRAD_ACCUM"     # microbatches per optimizer update, default 1
 
 
 class SingleSampleSummary(NamedTuple):
@@ -96,6 +97,7 @@ class SolverWorkerArgs(NamedTuple):
     save_every: int = 1
     graph_step: Optional[bool] = None      # None: FRL_B200_CUDA_GRAPH (default off)
     layer_adaptation: LayerAdaptation = LayerAdaptation.NONE
+    grad_accumulation: int = 1
 
 
 def _torch_load(f, **kw):
@@ -243,6 +245,21 @@ def resolve_layer_adaptation(explicit: Optional[LayerAdaptation] = None) -> Laye
     return LayerAdaptation(os.environ.get(LAYER_ADAPTATION_ENV, "none").lower())
 
 
+def resolve_grad_accumulation(explicit: Optional[int] = None) -> int:
+    """Microbatches per optimizer update: ``explicit``, else FRL_B200_GRAD_ACCUM, else 1.  Anything
+    but an integer >= 1 (``0``, negatives, ``2.5``, ``True``, non-numeric strings) is a ValueError."""
+    value: Any = explicit
+    if value is None:
+        raw = os.environ.get(GRAD_ACCUM_ENV, "1")
+        try:
+            value = int(raw.strip())
+        except ValueError:
+            raise ValueError("%s=%r: gradient accumulation must be an integer >= 1" % (GRAD_ACCUM_ENV, raw)) from None
+    if isinstance(value, bool) or not isinstance(value, (int, np.integer)) or value < 1:
+        raise ValueError("grad_accumulation=%r: gradient accumulation must be an integer >= 1" % (value,))
+    return int(value)
+
+
 class Solver:
     # ------------------------------------------------------------------------------------------
     # per-rank bootstrap (child process)
@@ -293,6 +310,12 @@ class Solver:
             model.load_state_dict(checkpoint.modelState)
         model.to(device)
         criterion: BaseParallelCriterion = problem.get_criterion().to(device)
+        from .criteria import GradNormWeightedCriterion
+        accum = args.grad_accumulation if run_opts.mode == Mode.TRAIN else 1
+        if accum > 1 and isinstance(criterion, GradNormWeightedCriterion):
+            # GradNorm learns its task weights from each step's own gradients
+            raise ValueError("grad_accumulation=%d cannot be combined with GradNormWeightedCriterion: "
+                             "its task weights are learnt per step, not per accumulated group" % accum)
 
         distributed = args.world_size > 1
         if distributed:
@@ -302,7 +325,7 @@ class Solver:
         # memory so all-reduce + update + broadcast can be one NVLS kernel per bucket
         symm_alloc = None
         if (distributed and not run_opts.optim.gradientClip
-                and args.layer_adaptation == LayerAdaptation.NONE):
+                and args.layer_adaptation == LayerAdaptation.NONE and accum == 1):
             from .symm import try_make_allocator
             symm_alloc = try_make_allocator(device, args.world_size)
         from .arena_linear import head_layout_groups
@@ -343,10 +366,10 @@ class Solver:
                                                "24" if nvls_link is not None else "48")),
             first_bucket_mb=None,
             eager_update=os.environ.get("FRL_B200_EAGER_UPDATE",
-                                        "1" if args.world_size > 1 else "0") != "0")
+                                        "1" if args.world_size > 1 else "0") != "0",
+            accumulation=accum)
         # GradNorm differentiates through the layers' backward (create_graph=True) and debugGrad
         # calls autograd.grad on them: those runs keep the stock nn.Linear autograd path
-        from .criteria import GradNormWeightedCriterion
         if (os.environ.get("FRL_B200_DIRECT_GRADS", "1") != "0" and not run_opts.debugGrad
                 and not isinstance(criterion, GradNormWeightedCriterion)):
             pipeline.patch_linears(model)
@@ -368,7 +391,7 @@ class Solver:
             logger.info(
                 "frl_b200 step: precision %s | step issue %s | gradient exchange %s | update %s | "
                 "Linear layers with arena-born gradients %d (%d fused with their ReLU, %d in FP8) | "
-                "other gradients %s | layer adaptation %s",
+                "other gradients %s | layer adaptation %s | gradient accumulation %s",
                 args.precision.value,
                 "CUDA-graph replay after 2 eager steps" if worker.graphed is not None else "eager launches",
                 ("fused NVLS kernel per bucket (K7), %d buckets" % len(pipeline.buckets)) if pipeline.nvls is not None
@@ -381,7 +404,10 @@ class Solver:
                 if pipeline.mt_enabled else "copied into the arena per tensor",
                 "none" if args.layer_adaptation == LayerAdaptation.NONE else
                 "%s, %d of %d tensors adapted (K2-lw)" % (args.layer_adaptation.value,
-                                                          sum(is_adapted(s) for s in arena.slots), len(arena.slots)))
+                                                          sum(is_adapted(s) for s in arena.slots), len(arena.slots)),
+                "none" if accum == 1 else
+                "%d microbatches per update (K10, fp32 accumulator %.1f MiB)" % (
+                    accum, pipeline.accumulator_bytes / 2 ** 20))
         scheduler = create_lr_scheduler(run_opts, worker.optimizer,
                                         checkpoint.epoch if checkpoint else -1)
         return worker, scheduler, checkpoint
@@ -584,7 +610,8 @@ class Solver:
     def solve(cls, run_opts: RunOpts, problem: Problem, *, group_name: Optional[str],
               init_method: str, node_idx: int = 0, node_count: int = 1, memory_quota: int = 0,
               precision: Optional[Precision] = None, graph: Optional[bool] = None,
-              layer_adaptation: Optional[LayerAdaptation] = None
+              layer_adaptation: Optional[LayerAdaptation] = None,
+              grad_accumulation: Optional[int] = None
               ) -> Iterator[PerformanceSummary]:
         """The reference's entry point (solver.py:728-739) plus two keyword-only extensions:
 
@@ -602,11 +629,32 @@ class Solver:
                        batches, see ``types.LayerAdaptation``; any other combination raises
                        ``ValueError`` before a rank starts.  None: FRL_B200_LAYER_ADAPTATION
                        (default ``none``).  ``Mode.EVAL`` ignores it.
+        ``grad_accumulation``  k >= 1 microbatches per optimizer update (gradient accumulation).
+                       ``batchSize`` stays the rows of one per-rank microbatch.  Within a training
+                       split the microbatches are grouped k at a time: microbatch j closes a group
+                       if (j + 1) % k == 0 or it is the split's last, so the last group may be
+                       short; no group crosses a split or epoch boundary (checkpoints keep their
+                       format and a resumed run is exact).  With g_i the gradient of microbatch i's
+                       (mean-reduced) loss, n_i its rows, B = batchSize and N the group's rows, the
+                       update uses  G = (1/world) * sum_ranks sum_i (n_i/B) * g_i * (B/N),  summed
+                       on the device into an fp32 accumulator (K10).  For MSE and cross-entropy
+                       without ignored targets G is the gradient of one batch of N rows; with
+                       ``ignore_index`` or a masked loss it is the row-weighted mean of the
+                       per-microbatch means, as in every framework's accumulation.  Adam's / LAMB's
+                       step count and the optimizer state dict count updates; the NaN guard, loss
+                       log rows, ``lossLoggingFreq``, metrics, the watchdog, BatchNorm statistics
+                       and the buffer broadcast stay per microbatch; the LR schedule stays per
+                       epoch.  Not combinable with ``GradNormWeightedCriterion`` (ValueError).
+                       None: FRL_B200_GRAD_ACCUM (default 1: no accumulator, today's step).  Any
+                       value but an integer >= 1 raises ``ValueError`` before a rank starts.
+                       ``Mode.EVAL`` ignores it.
         """
         adapt = LayerAdaptation.NONE
+        accum = 1
         if run_opts.mode == Mode.TRAIN:
             adapt = resolve_layer_adaptation(layer_adaptation)
             check_layer_adaptation(run_opts.optim, adapt)
+            accum = resolve_grad_accumulation(grad_accumulation)
         n_visible = 0 if run_opts.cpuonly else _cuda_device_count_without_poisoning_fork()
         if n_visible == 0:
             raise RuntimeError(
@@ -645,7 +693,7 @@ class Solver:
                 rank=node_idx * device_count + local_rank, local_rank=local_rank,
                 world_size=world_size, group_name=group_name, init_method=init_method,
                 cache=None, precision=prec, save_every=save_every, graph_step=graph,
-                layer_adaptation=adapt)
+                layer_adaptation=adapt, grad_accumulation=accum)
             if not run_opts.singleThreaded:
                 parent_conn, child_conn = ctx.Pipe(duplex=False)
                 proc = ctx.Process(target=cls._solver_worker_process,

@@ -39,7 +39,7 @@ from . import _native
 from .arena import ParamArena
 from .criteria import BaseParallelCriterion, GradNormWeightedCriterion
 from .fused_optim import FusedArenaOptimizer
-from .grad_sync import BufferBroadcaster, GradBucketPipeline
+from .grad_sync import BufferBroadcaster, GradBucketPipeline, accumulation_plan
 from .model import MultiTaskModel
 from .problem import BatchMetrics, Ordering, Problem
 from .sampler import ScaffoldSampler
@@ -756,6 +756,11 @@ class SolverWorker:
                 problem, len(loader.sampler), len(dataset), self.device,
                 max(self.run_opts.numVisualizedSamples, MODEL_CONVERSION_TEST_SAMPLE_CT))
             n_batches = len(loader)
+            # gradient accumulation: which microbatches open / close a group, and their weights
+            plan = None
+            if training and self.pipeline.accumulation > 1:
+                plan = accumulation_plan(n_batches, self.pipeline.accumulation, loader.batch_size,
+                                         len(loader.sampler))
             log = LossLog(n_tasks, n_batches, self.device)
             checked = 0
             batch_start = time.time()
@@ -777,6 +782,13 @@ class SolverWorker:
                                     for t in head) for head in target]
                     self.criterion.set_step_sink(log.row(minibatch_idx), log.nan_flag)
                     self.criterion._sink_written = False
+                    if plan is not None:
+                        mb = plan[minibatch_idx]
+                        if data[0].shape[0] != mb.rows:
+                            raise RuntimeError("gradient accumulation: minibatch %d has %d rows, the loader "
+                                               "promised %d" % (minibatch_idx, data[0].shape[0], mb.rows))
+                        self.pipeline.set_microbatch(first=mb.first, closes=mb.closes, weight=mb.weight,
+                                                     group_scale=loader.batch_size / mb.group_rows)
                     output, total_loss, sub_loss, grad_norms = self._pass_one_minibatch(
                         minibatch_idx, data_type, data, target)
                     self._finish_loss_row(log, minibatch_idx, total_loss, sub_loss)

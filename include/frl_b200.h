@@ -169,6 +169,23 @@ int frl_lamb_mt(float* p, float* m, float* v, void* p_lp, const frl_grad_seg* se
                 double grad_scale, const float* grad_scale_dev, const float* dyn, void* stream);
 
 /* ------------------------------------------------------------------------------------------
+ * K10 — gradient accumulation (an extension: the reference has no accumulation).  Several
+ * microbatches per optimizer update: after each microbatch's backward, one launch folds every
+ * gradient of a K2-mt segment table into an fp32 accumulator.
+ *   acc[seg.arena_off + i] = (first ? 0 : acc[seg.arena_off + i]) + w * g[i]   for every segment,
+ *   fp32, computed as fmaf(w, g, base); a segment with g == NULL contributes 0 (so `first`
+ *   zeroes it, and without `first` it is not touched).
+ * acc: fp32 arena-shaped vector, 16-byte aligned, covering every segment's arena_off + numel
+ * rounded up to 4; segment table as in K2-mt (any mix of FRL_F32 / FRL_BF16 gradients,
+ * arena-resident or read in place).  Elements outside every segment are untouched.
+ * dyn: optional device fp32[2] overriding the by-value arguments: dyn[0] = w, dyn[1] != 0 -> first.
+ * Graph-capturable: no host reads, no allocation.  n_tiles == 0: returns 0, launches nothing.
+ * ---------------------------------------------------------------------------------------- */
+int frl_grad_accumulate_mt(float* acc, const frl_grad_seg* segs_dev, const int64_t* tile_prefix_dev,
+                           const int32_t* tile_seg_dev, int64_t n_tiles, double w, int first,
+                           const float* dyn, void* stream);
+
+/* ------------------------------------------------------------------------------------------
  * K3 — global gradient norm for clipping.
  * Replaces torch.nn.utils.clip_grad_norm_ (reference solver_worker.py:588-591): one pass
  * over the model-parameter range of the gradient arena.

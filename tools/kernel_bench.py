@@ -213,6 +213,39 @@ def bench_k2lw(iters):
     return out
 
 
+def bench_k10(iters):
+    """K10 gradient accumulation over the headline MLP's 10 tensors (54.7 M parameters) as the solver
+    builds it: one segment table over the arena's slots, bf16 gradients in the arena, an fp32
+    accumulator, timed from a CUDA graph.  Gradients (109 MB) and accumulator (219 MB) are far larger
+    than L2, so every launch streams from HBM.  Bytes per parameter: first = 1 reads g and writes acc
+    (6); first = 0 reads g and acc and writes acc (10)."""
+    from frl_b200.multi_tensor import GradSegTable
+
+    class Slot:
+        def __init__(self, index, offset, numel):
+            self.index, self.offset, self.numel = index, offset, numel
+
+    sizes = [4096 * 4096, 4096] * 3 + [1000 * 4096, 1000, 64 * 4096, 64]
+    slots, off = [], 0
+    for i, n in enumerate(sizes):
+        slots.append(Slot(i, off, n))
+        off = (off + n + 7) // 8 * 8
+    n, n_real = off, sum(sizes)
+    grad = torch.randn(n, device=DEV).bfloat16()
+    table = GradSegTable(slots, DEV)
+    for s in slots:
+        table.point(s, grad.data_ptr() + 2 * s.offset, grad.dtype)
+    table.upload()
+    acc = torch.zeros(n, device=DEV)
+    out = []
+    for first, bpp in ((True, 6), (False, 10)):
+        out.append(timed("K10 grad_accumulate_mt mlp bf16-grad first=%d (%d tensors, %d params)"
+                         % (first, len(slots), n_real),
+                         lambda i, first=first: _native.grad_accumulate_mt(acc, table, w=1.0, first=first),
+                         1, bpp * n_real, iters, "accumulator %d MB" % (4 * n >> 20), graph=True))
+    return out
+
+
 def bench_k3(iters):
     n = 54_703_144
     out = []
@@ -426,7 +459,7 @@ def bench_k9(iters):
 
 BENCHES = {"k2": bench_k2, "k2mt": bench_k2mt, "k2lw": bench_k2lw, "k3": bench_k3, "k4": bench_k4, "k5": bench_k5, "k5a": bench_k5a,
            "k6": bench_k6,
-           "k8": bench_k8, "k8t": bench_k8t, "k9": bench_k9}
+           "k8": bench_k8, "k8t": bench_k8t, "k9": bench_k9, "k10": bench_k10}
 
 
 def main():
