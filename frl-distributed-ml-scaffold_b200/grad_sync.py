@@ -68,28 +68,26 @@ def accumulation_plan(n_batches: int, k: int, batch_size: int = 1,
 
 
 class _TableSet:
-    """Segment tables of one pipeline, built on first use: the whole arena (1-GPU tail update that
-    reads gradients in place) and, per (bucket, set of straggler slots), the flatten tables.
-    A CUDA-graph capture gets a set of its own: captured uploads read the set's pinned rows at
-    every replay, so nothing else may ever rewrite them."""
+    """Segment tables of one pipeline, built on first use, one per (use, set of slots): the step's
+    gradients of every slot (K10, the 1-GPU update that reads them in place), per bucket the
+    stragglers to flatten, the end-of-step update of the slots that got a gradient, the
+    accumulator.  A CUDA-graph capture gets a set of its own: captured uploads read the set's
+    pinned rows at every replay, so nothing else may ever rewrite them."""
 
     def __init__(self, arena) -> None:
         self.arena = arena
-        self._whole = None
-        self._flatten: Dict[Tuple, object] = {}
+        self._tables: Dict[Tuple, object] = {}
 
-    def whole(self):
-        if self._whole is None:
-            from .multi_tensor import GradSegTable
-            self._whole = GradSegTable(self.arena.slots, self.arena.device)
-        return self._whole
-
-    def flatten(self, key, slots):
-        t = self._flatten.get(key)
+    def get(self, use, slots):
+        key = (use, tuple(s.index for s in slots))
+        t = self._tables.get(key)
         if t is None:
             from .multi_tensor import GradSegTable
-            t = self._flatten[key] = GradSegTable(slots, self.arena.device)
+            t = self._tables[key] = GradSegTable(slots, self.arena.device)
         return t
+
+    def whole(self):
+        return self.get("grads", self.arena.slots)
 
 
 class _Bucket:
@@ -234,7 +232,6 @@ class GradBucketPipeline:
             self._acc_dyn_host = torch.zeros(self._ACC_RING, 2, dtype=torch.float32, pin_memory=self.on_cuda)
             self._acc_dyn_slot = 0
             self._acc_dyn_last: Optional[Tuple[float, float]] = (1.0, 1.0)
-            self._acc_tables: Dict[Tuple[int, ...], object] = {}     # update tables reading the accumulator
         self._acc_first = True
         self._acc_closes = True
         self._acc_weight = 1.0
@@ -307,17 +304,23 @@ class GradBucketPipeline:
         return hook
 
     # -- multi-tensor plumbing ---------------------------------------------------------------------
-    def _point(self, table) -> None:
-        """This step's gradient locations into ``table`` (arena slice unless a straggler)."""
-        g_arena = self.arena.grad
-        esz = g_arena.element_size()
-        base = g_arena.data_ptr()
-        for s in table.slots:
-            g = self._ext.get(s.index)
-            if g is None:
-                table.point(s, base + s.offset * esz, g_arena.dtype)
+    def _table(self, use, slots, acc: bool = False, ready=None):
+        """The table of ``slots`` for ``use``, pointed at this step's gradients and uploaded: each
+        slot's slice of the accumulator (``acc``), else the gradient autograd left outside the
+        arena (a straggler) or the arena slice; NULL for a slot whose index is not in ``ready``."""
+        table = self.tables.get(use, slots)
+        g = self.acc if acc else self.arena.grad
+        base, esz = g.data_ptr(), g.element_size()
+        for s in slots:
+            ext = None if acc else self._ext.get(s.index)
+            if ready is not None and s.index not in ready:
+                table.point(s, 0, g.dtype)
+            elif ext is not None:
+                table.point(s, ext.data_ptr(), ext.dtype)
             else:
-                table.point(s, g.data_ptr(), g.dtype)
+                table.point(s, base + s.offset * esz, g.dtype)
+        table.upload()
+        return table
 
     def _flatten_stragglers(self, slots, key, side: bool) -> None:
         """ONE launch: gather the listed slots' out-of-arena gradients into their arena slices
@@ -325,10 +328,7 @@ class GradBucketPipeline:
         ext = [s for s in slots if s.index in self._ext]
         if not ext:
             return
-        table = self.tables.flatten((key, tuple(s.index for s in ext)), ext)
-        self._point(table)
-        table.upload()
-        KERNELS.flatten_grads(table, self.arena.grad, scale=1.0)
+        KERNELS.flatten_grads(self._table(key, ext), self.arena.grad, scale=1.0)
         for s in ext:
             g = self._ext.pop(s.index) if not self._keep_ext else self._ext[s.index]
             if side:
@@ -389,45 +389,45 @@ class GradBucketPipeline:
         try:
             if self._ext:
                 self._flatten_stragglers(b.slots, id(b), side=self.on_cuda)
-            if self.nvls is not None and not b.replicated:
-                nv = self.nvls
-                grid = nv.max_blocks
-                if b is self._last_bucket:            # runs alone: backward has nothing left to issue
-                    nv.max_blocks = nv.tail_blocks
-                try:
-                    self._update(b.lo, b.hi, None)    # K7: reduce + update + broadcast
-                finally:
-                    nv.max_blocks = grid
-            elif self.distributed:
+            fused = self.nvls is not None and not b.replicated      # K7: reduce + update + broadcast
+            if self.distributed and not fused:
                 b.work = dist.all_reduce(self.arena.grad[b.lo:b.hi], op=dist.ReduceOp.SUM,
                                          group=self.pg, async_op=True)
                 if self.eager:
                     b.work.wait()             # stream-level wait, the host does not block
-                    self._update(b.lo, b.hi, None)
-            elif self.eager:
-                self._update(b.lo, b.hi, None)
+            if self.eager:
+                tap = self._tap()
+                if fused:
+                    nv = self.nvls
+                    grid = nv.max_blocks
+                    if b is self._last_bucket:        # runs alone: backward has nothing left to issue
+                        nv.max_blocks = nv.tail_blocks
+                    try:
+                        self.optimizer.apply_range_nvls(b.lo, b.hi, grad_scale=self.grad_scale)
+                    finally:
+                        nv.max_blocks = grid
+                else:
+                    self.optimizer.apply_range(b.lo, b.hi, grad_scale=self.grad_scale)
+                self._tap_end(tap, self.update_events, b.lo, b.hi)
         finally:
             if self.on_cuda:
                 torch.cuda.set_stream(cur)
         b.launched = True
 
-    def _apply(self, lo: int, hi: int, coef) -> None:
-        if self.nvls is not None and lo < self.arena.model_end or \
-                (self.nvls is not None and self.arena.lp is None):
-            self.optimizer.apply_range_nvls(lo, hi, grad_scale=self.grad_scale)
-        else:
-            self.optimizer.apply_range(lo, hi, grad_scale=self.grad_scale, clip_coef_dev=coef)
+    def _tap(self):
+        """Timing tap (bench): a pair of events, the first recorded now, or None while it is off."""
+        if not (self.record_update_events and self.on_cuda):
+            return None
+        tap = (torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True))
+        tap[0].record()
+        return tap
 
-    def _update(self, lo: int, hi: int, coef) -> None:
-        if self.record_update_events and self.on_cuda:
-            e0 = torch.cuda.Event(enable_timing=True)
-            e1 = torch.cuda.Event(enable_timing=True)
-            e0.record()
-            self._apply(lo, hi, coef)
-            e1.record()
-            self.update_events.append((e0, e1, lo, hi))
-        else:
-            self._apply(lo, hi, coef)
+    @staticmethod
+    def _tap_end(tap, events, *span) -> None:
+        """Close a ``_tap()`` window: record its end event and append ``(start, end, *span)``."""
+        if tap is not None:
+            tap[1].record()
+            events.append(tap + span)
 
     def finish_step(self, defer_tail: bool = False) -> None:
         """Call after ``backward()`` returned: reduces/updates whatever is still outstanding and
@@ -440,52 +440,34 @@ class GradBucketPipeline:
         self._deferred.clear()
         self.forward_gen += 1
         self._step_open = False
-        self._tail_deferred = False
-        if self.acc is not None and not (self.distributed and self._ready != self._n_slots):
+        partial = self._ready != self._n_slots
+        if partial and self.distributed:
+            missing = [s.index for s in self.arena.slots if id(s.param) not in self._ready_ids]
+            # same contract as DDP with find_unused_parameters=False (the reference's setting)
+            raise RuntimeError(
+                "Expected to have finished reduction for every parameter, but parameters at "
+                f"indices {missing} did not receive a gradient in this step")
+        if self.acc is not None:
             # k > 1: fold this microbatch into the accumulator; the group's last one updates.
             # Inside a capture the K10 launch is recorded and the update is left to run_tail().
             self._accumulate_microbatch(keep_refs=defer_tail)
-            if defer_tail:
-                self._tail_deferred = True
-            elif self._acc_closes:
-                self._update_from_accumulator()
-            return
-        if self._ready != self._n_slots:
-            missing = [s.index for s in self.arena.slots if id(s.param) not in self._ready_ids]
-            if self.distributed:
-                # same contract as DDP with find_unused_parameters=False (the reference's setting)
-                raise RuntimeError(
-                    "Expected to have finished reduction for every parameter, but parameters at "
-                    f"indices {missing} did not receive a gradient in this step")
-            if self.eager and self.on_cuda:
-                torch.cuda.current_stream().wait_stream(self.side_stream)
-            self._flatten_stragglers(self.arena.slots, "all", side=False)
-            self._finish_partial(missing)
-            return
-        if self.distributed or self.eager:
-            if self.on_cuda:
-                cur = torch.cuda.current_stream()
-                if self.distributed and not self.eager:
+        else:
+            if self.distributed and not self.eager:
+                cur = torch.cuda.current_stream() if self.on_cuda else None
+                if cur is not None:
                     torch.cuda.set_stream(self.side_stream)
-                    for b in self.buckets:
-                        b.work.wait()
-                    torch.cuda.set_stream(cur)
-                cur.wait_stream(self.side_stream)
-            elif self.distributed and not self.eager:
                 for b in self.buckets:
                     b.work.wait()
-            if defer_tail:
-                self._tail_deferred = True
+                if cur is not None:
+                    torch.cuda.set_stream(cur)
+            if self.on_cuda and (self.distributed or self.eager):
+                torch.cuda.current_stream().wait_stream(self.side_stream)
+            if partial:
+                # one GPU, some parameters got no gradient: updated at once, capture or not
+                self._end_update([s for s in self.arena.slots if id(s.param) in self._ready_ids])
                 return
-            if not self.eager:
-                self._tail_update()
-        else:
-            if defer_tail:
-                self._tail_deferred = True
-                return
-            self._tail_update()
-        self._ext.clear()
-        self.optimizer.end_step()
+        if not defer_tail:
+            self.run_tail()
 
     @property
     def has_tail(self) -> bool:
@@ -502,98 +484,73 @@ class GradBucketPipeline:
             if ready is not None:
                 self._acc_seen |= ready
             if self._acc_closes:
-                self._update_from_accumulator()
+                self._end_update(acc=True)
             return
         if grad_refs is not None:
             mine = (self._ext, self.tables)
             self._ext, self.tables, self._keep_ext = grad_refs, tables, True
         try:
             if self.has_tail:
-                self._tail_update()
+                self._end_update()
+            else:
+                self.optimizer.end_step()
         finally:
             if grad_refs is not None:
                 (self._ext, self.tables), self._keep_ext = mine, False
-        self.optimizer.end_step()
 
-    def _tail_update(self) -> None:
-        if self.whole_tensors:
-            # one update over the whole table, each gradient read where it lies (1 GPU) or from the
-            # all-reduced arena (world > 1: the stragglers were gathered per bucket)
-            coef = None
-            if self.clip_norm > 0.0:
-                self._flatten_stragglers(self.arena.slots, "all", side=False)
-                coef = self._clip_coef()
-            table = self.tables.whole()
-            self._point(table)
-            table.upload()
-            self._update_table(table, coef)
-            if not self._keep_ext:
-                self._ext.clear()
-            return
-        if self.clip_norm > 0.0:
-            # the global norm needs every gradient first: gather the stragglers into the arena,
-            # then K3 + K2 over the arena (the clip coefficient applies to model parameters only)
-            self._flatten_stragglers(self.arena.slots, "all", side=False)
-            n_model = self.arena.model_end
-            KERNELS.grad_sumsq_clip(self.arena.grad[:n_model], n_model, pre_scale=self.grad_scale,
-                                    max_norm=self.clip_norm, out3=self.clip_out,
-                                    scratch=self.clip_scratch)
-            self._update(0, self.arena.numel, self.clip_out[2:3])
-            return
-        if self._ext and not self.distributed:
-            # one GPU: the update reads every gradient where it lies — no flatten pass
-            table = self.tables.whole()
-            self._point(table)
-            table.upload()
-            self._update_table(table)
-            if not self._keep_ext:
-                self._ext.clear()
-            return
-        self._update(0, self.arena.numel, None)
-
-    def _update_table(self, table, coef=None) -> None:
-        kw = {} if coef is None else {"clip_coef_dev": coef}
-        if self.record_update_events and self.on_cuda:
-            e0 = torch.cuda.Event(enable_timing=True)
-            e1 = torch.cuda.Event(enable_timing=True)
-            e0.record()
-            self.optimizer.apply_table(table, grad_scale=self.grad_scale, **kw)
-            e1.record()
-            self.update_events.append((e0, e1, 0, self.arena.numel))
+    def _end_update(self, present=None, acc: bool = False) -> None:
+        """Every update that is not a bucket's eager one, then the optimizer's step count.
+        ``present``: the slots that got a gradient (default: all) -- torch.optim skips the others
+        (no weight decay, no momentum decay), so they keep their weights and state.  ``acc``: the
+        group is closed, update from the accumulator (fp32; exchanged per bucket on several GPUs)
+        at ``_acc_scale`` = B / (world * N), which turns the weighted sum into the group's mean."""
+        slots, n = self.arena.slots, self.arena.numel
+        if acc:
+            grads, scale = self.acc, self._acc_scale
+            if self.distributed:
+                for b in self.buckets:
+                    dist.all_reduce(grads[b.lo:b.hi], op=dist.ReduceOp.SUM, group=self.pg)
+            else:
+                present = [s for s in slots if s.index in self._acc_seen]
         else:
-            self.optimizer.apply_table(table, grad_scale=self.grad_scale, **kw)
-
-    def _clip_coef(self):
-        """K3 over the model range of the gradient arena; returns the device clip coefficient."""
-        n_model = self.arena.model_end
-        KERNELS.grad_sumsq_clip(self.arena.grad[:n_model], n_model, pre_scale=self.grad_scale,
-                                max_norm=self.clip_norm, out3=self.clip_out, scratch=self.clip_scratch)
-        return self.clip_out[2:3]
-
-    def _finish_partial(self, missing) -> None:
-        """world_size == 1 and some parameters got no gradient: torch.optim skips those (no
-        weight decay, no momentum decay), so update only the contiguous runs that did."""
-        skip = set(missing)
-        done = [(b.lo, b.hi) for b in self.buckets if b.launched and self.eager]
+            grads, scale = self.arena.grad, self.grad_scale
+        have = {s.index for s in (slots if present is None else present)}
+        every = len(have) == len(slots)
+        window = self._tap() if acc else None     # accumulation: ONE timed window, K3 included
         coef = None
+        if not acc and (self.clip_norm > 0.0 or not every):
+            # the norm and the runs' flat updates read the arena: gather the stragglers into it
+            self._flatten_stragglers(slots, "all", side=False)
         if self.clip_norm > 0.0:
-            for s in self.arena.slots:
-                if s.index in skip and s.is_model:
-                    self.arena.grad[s.offset:s.end].zero_()
-            coef = self._clip_coef()
-        if self.whole_tensors:
-            # a table of the slots that got a gradient (now all in the arena); the others keep
-            # their weights and state
-            present = [s for s in self.arena.slots if s.index not in skip]
-            table = self.tables.flatten(("partial", tuple(s.index for s in present)), present)
-            self._point(table)
-            table.upload()
-            self._update_table(table, coef)
-            self.optimizer.end_step()
-            return
-        for lo, hi in self._runs(lambda s: s.index not in skip
-                                 and not any(a <= s.offset < z for a, z in done)):
-            self._update(lo, hi, coef)
+            # the global norm over the model range only (criterion parameters are not clipped);
+            # a missing gradient counts as zero
+            if not acc:
+                for s in slots:
+                    if s.index not in have and s.is_model:
+                        grads[s.offset:s.end].zero_()
+            n_model = self.arena.model_end
+            KERNELS.grad_sumsq_clip(grads[:n_model], n_model, pre_scale=scale, max_norm=self.clip_norm,
+                                    out3=self.clip_out, scratch=self.clip_scratch)
+            coef = self.clip_out[2:3]
+        if self.whole_tensors or (not acc and self._ext and coef is None and not self.distributed):
+            # one update over a table of the present slots: whole tensors (per-tensor norms), or on
+            # one GPU every gradient read where it lies -- no flatten pass
+            table = self._table("acc" if acc else "grads", [s for s in slots if s.index in have], acc=acc)
+            tap = None if acc else self._tap()
+            self.optimizer.apply_table(table, grad_scale=scale, clip_coef_dev=coef)
+            self._tap_end(tap, self.update_events, 0, n)
+        else:
+            done = [(b.lo, b.hi) for b in self.buckets if b.launched and self.eager]
+            runs = [(0, n)] if every else self._runs(
+                lambda s: s.index in have and not any(a <= s.offset < z for a, z in done))
+            for lo, hi in runs:
+                tap = None if acc else self._tap()
+                self.optimizer.apply_range(lo, hi, grad_scale=scale, clip_coef_dev=coef,
+                                           grad_src=grads if acc else None)
+                self._tap_end(tap, self.update_events, lo, hi)
+        self._tap_end(window, self.update_events, 0, n)
+        if not self._keep_ext:
+            self._ext.clear()
         self.optimizer.end_step()
 
     def _runs(self, keep) -> List[Tuple[int, int]]:
@@ -618,82 +575,16 @@ class GradBucketPipeline:
         """ONE K10 launch over the whole table: every gradient of this microbatch, where it lies,
         times n_i / B into the accumulator; slots without a gradient point at NULL (nothing added,
         zeroed when the microbatch opens its group)."""
-        table = self.tables.whole()
-        g_arena = self.arena.grad
-        esz = g_arena.element_size()
-        base = g_arena.data_ptr()
-        ready = []
-        for s in table.slots:
-            if id(s.param) not in self._ready_ids:
-                table.point(s, 0, g_arena.dtype)
-                continue
-            ready.append(s.index)
-            g = self._ext.get(s.index)
-            if g is None:
-                table.point(s, base + s.offset * esz, g_arena.dtype)
-            else:
-                table.point(s, g.data_ptr(), g.dtype)
-        self.last_ready = frozenset(ready)
-        self._acc_seen.update(ready)
-        table.upload()
-        timed = self.record_update_events and self.on_cuda
-        if timed:
-            e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-            e0.record()
+        slots = self.arena.slots
+        self.last_ready = frozenset(s.index for s in slots if id(s.param) in self._ready_ids)
+        self._acc_seen |= self.last_ready
+        table = self._table("grads", slots, ready=self.last_ready)
+        tap = self._tap()
         KERNELS.grad_accumulate_mt(self.acc, table, w=self._acc_weight, first=self._acc_first,
                                    dyn=self._acc_dyn)
-        if timed:
-            e1.record()
-            self.accumulate_events.append((e0, e1))
+        self._tap_end(tap, self.accumulate_events)
         if not keep_refs:
             self._ext.clear()            # the launch is enqueued: stream order protects the reads
-
-    def _acc_table(self, slots):
-        """Segment table of ``slots`` pointing into the accumulator (fp32), built once per set."""
-        key = tuple(s.index for s in slots)
-        t = self._acc_tables.get(key)
-        if t is None:
-            from .multi_tensor import GradSegTable
-            t = self._acc_tables[key] = GradSegTable(slots, self.arena.device)
-            for s in slots:
-                t.point(s, self.acc.data_ptr() + 4 * s.offset, torch.float32)
-        t.upload()
-        return t
-
-    def _update_from_accumulator(self) -> None:
-        """The group is closed: exchange the accumulator (fp32, per bucket), clip, update once.
-        ``_acc_scale`` = B / (world * N) turns the weighted sum into the group's mean gradient."""
-        acc, scale = self.acc, self._acc_scale
-        if self.distributed:
-            for b in self.buckets:
-                dist.all_reduce(acc[b.lo:b.hi], op=dist.ReduceOp.SUM, group=self.pg)
-            present = list(self.arena.slots)
-        else:
-            # one GPU: a slot that got no gradient in any microbatch keeps its weights and state
-            present = [s for s in self.arena.slots if s.index in self._acc_seen]
-        timed = self.record_update_events and self.on_cuda
-        if timed:
-            e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-            e0.record()
-        coef = None
-        if self.clip_norm > 0.0:
-            n_model = self.arena.model_end
-            KERNELS.grad_sumsq_clip(acc[:n_model], n_model, pre_scale=scale, max_norm=self.clip_norm,
-                                    out3=self.clip_out, scratch=self.clip_scratch)
-            coef = self.clip_out[2:3]
-        if self.whole_tensors:
-            if present:
-                self.optimizer.apply_table(self._acc_table(present), grad_scale=scale, clip_coef_dev=coef)
-        elif len(present) == len(self.arena.slots):
-            self.optimizer.apply_range(0, self.arena.numel, grad_scale=scale, clip_coef_dev=coef, grad_src=acc)
-        else:
-            seen = {s.index for s in present}
-            for lo, hi in self._runs(lambda s: s.index in seen):
-                self.optimizer.apply_range(lo, hi, grad_scale=scale, clip_coef_dev=coef, grad_src=acc)
-        if timed:
-            e1.record()
-            self.update_events.append((e0, e1, 0, self.arena.numel))
-        self.optimizer.end_step()
 
     # -- one-time synchronisation ----------------------------------------------------------------
     def broadcast_parameters(self, src: int = 0) -> None:
