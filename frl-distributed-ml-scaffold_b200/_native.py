@@ -67,6 +67,7 @@ SIGNATURES = {
     "frl_lamb_mt": (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _i64, _i64, _vp, _vp, _vp, _d, _d, _d, _d, _d, _i64,
                          _d, _vp, _vp, _vp]),
     "frl_grad_accumulate_mt": (_i, [_vp, _vp, _vp, _vp, _i64, _d, _i, _vp, _vp]),
+    "frl_weight_ema": (_i, [_vp, _vp, _i64, _d, _vp]),
     "frl_reduce_scratch_bytes": (_i64, []),
     "frl_grad_sumsq_clip": (_i, [_vp, _i64, _i, _f, _f, _vp, _vp, _vp]),
     "frl_criteria_scratch_bytes": (_i64, [_i]),
@@ -281,6 +282,19 @@ def grad_accumulate_mt(acc, table, *, w: float = 1.0, first: bool = False, dyn=N
     _check(lib().frl_grad_accumulate_mt(_ptr(acc), table.segs_dev_ptr, table.prefix_dev_ptr, table.tile_seg_dev_ptr,
                                         table.n_tiles, float(w), int(bool(first)), _ptr(dyn), _stream()),
            "frl_grad_accumulate_mt")
+
+
+# ---- K11: weight EMA ------------------------------------------------------------------------------
+
+def weight_ema(ema, p, w: float) -> None:
+    """ema = lerp(ema, p, w) in fp32, torch's formula, over ``ema.numel()`` elements of two
+    contiguous fp32 device vectors (``p`` at least as long).  See frl_weight_ema in
+    include/frl_b200.h."""
+    if ema.dtype != torch.float32 or p.dtype != torch.float32 or not (ema.is_contiguous() and p.is_contiguous()):
+        raise NativeLibraryError("weight EMA: ema and p must be contiguous fp32")
+    if p.numel() < ema.numel():
+        raise NativeLibraryError("weight EMA: p has %d elements, ema %d" % (p.numel(), ema.numel()))
+    _check(lib().frl_weight_ema(_ptr(ema), _ptr(p), ema.numel(), float(w), _stream()), "frl_weight_ema")
 
 
 # ---- K3 -------------------------------------------------------------------------------------

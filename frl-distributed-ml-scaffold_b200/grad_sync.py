@@ -20,7 +20,10 @@ solver_worker.py:585-592).  Differences that matter on H100:
   clipping path's shape: per-bucket all-reduce only, then one update over the whole segment table;
 * with gradient accumulation (k > 1) no bucket is launched during backward: one K10 launch per
   microbatch folds every gradient into an fp32 accumulator, and the microbatch that closes a group
-  all-reduces the accumulator per bucket, clips and updates from it.
+  all-reduces the accumulator per bucket, clips and updates from it;
+* with a weight EMA (``ema.WeightEMA``) every optimizer update is followed by one K11 launch on the
+  compute stream, behind the update and, with eager per-bucket updates, behind the join with the
+  side stream; never inside a captured graph (the tail runs after the replay).
 """
 import os
 from typing import Callable, Dict, List, NamedTuple, Optional, Tuple
@@ -106,7 +109,7 @@ class GradBucketPipeline:
     def __init__(self, arena: ParamArena, optimizer: FusedArenaOptimizer, *,
                  process_group=None, world_size: int = 1, clip_norm: float = 0.0,
                  bucket_cap_mb: float = 25.0, first_bucket_mb: Optional[float] = 1.0,
-                 eager_update: bool = True, nvls_link=None, accumulation: int = 1) -> None:
+                 eager_update: bool = True, nvls_link=None, accumulation: int = 1, ema=None) -> None:
         self.arena = arena
         self.optimizer = optimizer
         self.pg = process_group
@@ -197,6 +200,10 @@ class GradBucketPipeline:
         self.nvls = nvls_link if use_nvls else None
         if self.nvls is not None:
             optimizer.nvls = self.nvls
+        # weight EMA: needs the whole master on every rank, which the fused NVLS step does not keep
+        if ema is not None and self.nvls is not None:
+            raise ValueError("a weight EMA cannot be combined with the fused NVLS step (K7)")
+        self.ema = ema
         self._step_open = False
         self.step_id = 0
         self.linear_sites = []
@@ -463,8 +470,10 @@ class GradBucketPipeline:
             if self.on_cuda and (self.distributed or self.eager):
                 torch.cuda.current_stream().wait_stream(self.side_stream)
             if partial:
-                # one GPU, some parameters got no gradient: updated at once, capture or not
-                self._end_update([s for s in self.arena.slots if id(s.param) in self._ready_ids])
+                # one GPU, some parameters got no gradient: updated at once, capture or not (inside
+                # a capture without the EMA step: run_tail() updates again and steps the EMA)
+                self._end_update([s for s in self.arena.slots if id(s.param) in self._ready_ids],
+                                 ema=not defer_tail)
                 return
         if not defer_tail:
             self.run_tail()
@@ -494,12 +503,15 @@ class GradBucketPipeline:
                 self._end_update()
             else:
                 self.optimizer.end_step()
+                if self.ema is not None:
+                    self.ema.update()
         finally:
             if grad_refs is not None:
                 (self._ext, self.tables), self._keep_ext = mine, False
 
-    def _end_update(self, present=None, acc: bool = False) -> None:
-        """Every update that is not a bucket's eager one, then the optimizer's step count.
+    def _end_update(self, present=None, acc: bool = False, ema: bool = True) -> None:
+        """Every update that is not a bucket's eager one, then the optimizer's step count and
+        (``ema``) the weight EMA's step.
         ``present``: the slots that got a gradient (default: all) -- torch.optim skips the others
         (no weight decay, no momentum decay), so they keep their weights and state.  ``acc``: the
         group is closed, update from the accumulator (fp32; exchanged per bucket on several GPUs)
@@ -552,6 +564,8 @@ class GradBucketPipeline:
         if not self._keep_ext:
             self._ext.clear()
         self.optimizer.end_step()
+        if ema and self.ema is not None:
+            self.ema.update()
 
     def _runs(self, keep) -> List[Tuple[int, int]]:
         """Arena ranges ``[lo, hi)`` of the maximal runs of consecutive slots with ``keep(slot)``."""

@@ -21,7 +21,8 @@ class LocalSolver:
     def solve(cls, run_opts: RunOpts, problem: Problem, save_notebook: bool = False,
               precision: Optional[Precision] = None, graph: Optional[bool] = None, *,
               layer_adaptation: Optional[LayerAdaptation] = None,
-              grad_accumulation: Optional[int] = None) -> PerformanceSummary:
+              grad_accumulation: Optional[int] = None,
+              ema_decay: Optional[float] = None) -> PerformanceSummary:
         if save_notebook:
             logger.warning("save_notebook is not supported by frl_b200 (visualisation only)")
         # a stale rendezvous file from a crashed run would poison the file:// store
@@ -34,6 +35,6 @@ class LocalSolver:
         for last in Solver.solve(run_opts, problem, group_name=group_name,
                                  init_method="file://" + SYNC_FILE, precision=precision,
                                  graph=graph, layer_adaptation=layer_adaptation,
-                                 grad_accumulation=grad_accumulation):
+                                 grad_accumulation=grad_accumulation, ema_decay=ema_decay):
             pass
         return last

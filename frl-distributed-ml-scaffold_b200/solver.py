@@ -28,6 +28,7 @@ import torch.nn as nn
 
 from .arena import ParamArena
 from .criteria import BaseParallelCriterion
+from .ema import EMA_STATE_KEY
 from .fused_optim import check_layer_adaptation, create_fused_optimizer, is_adapted
 from .grad_sync import BufferBroadcaster, GradBucketPipeline
 from .lr_scheduler import DropEpochsScheduler, WarmupMultiStepLR
@@ -44,6 +45,8 @@ CHECKPOINT_NAME = ".checkpoint.pth"
 LAYER_ADAPTATION_ENV = "FRL_B200_LAYER_ADAPTATION"   # "none" (default) | "lars" | "lamb"
 PRECISION_ENV = "FRL_B200_PRECISION"      # "fp32" (default, reference parity) | "bf16"
 GRAD_ACCUM_ENV = "FRL_B200_GRAD_ACCUM"     # microbatches per optimizer update, default 1
+EMA_DECAY_ENV = "FRL_B200_EMA_DECAY"       # weight EMA decay in [0, 1), default 0 (off)
+EMA_SUFFIX = ".ema"                        # <checkpoint>.ema: the weight EMA next to a checkpoint
 
 
 class SingleSampleSummary(NamedTuple):
@@ -97,6 +100,8 @@ class SolverWorkerArgs(NamedTuple):
     save_every: int = 1
     graph_step: Optional[bool] = None      # None: FRL_B200_CUDA_GRAPH (default off)
     layer_adaptation: LayerAdaptation = LayerAdaptation.NONE
+    # weight EMA decay, 0 = off; placed before grad_accumulation, which stays the last field
+    ema_decay: float = 0.0
     grad_accumulation: int = 1
 
 
@@ -260,6 +265,41 @@ def resolve_grad_accumulation(explicit: Optional[int] = None) -> int:
     return int(value)
 
 
+def resolve_ema_decay(explicit: Optional[float] = None) -> float:
+    """Weight EMA decay: ``explicit``, else FRL_B200_EMA_DECAY, else 0 (no EMA).  Anything but a
+    real number in [0, 1) (``True``, negatives, ``1.0``, NaN, non-numeric strings) is a ValueError."""
+    value: Any = explicit
+    if value is None:
+        raw = os.environ.get(EMA_DECAY_ENV, "0")
+        try:
+            value = float(raw.strip())
+        except ValueError:
+            raise ValueError("%s=%r: the EMA decay must be a real number in [0, 1)" % (EMA_DECAY_ENV, raw)) from None
+    if (isinstance(value, bool) or not isinstance(value, (int, float, np.integer, np.floating))
+            or not 0.0 <= float(value) < 1.0):
+        raise ValueError("ema_decay=%r: the EMA decay must be a real number in [0, 1)" % (value,))
+    return float(value)
+
+
+def load_ema_checkpoint(ema, path: str, epoch: int) -> bool:
+    """Resume ``ema`` (an ``ema.WeightEMA``) from the ``<checkpoint>.ema`` file at ``path`` if it
+    exists and belongs to the checkpoint being resumed (saved at the same ``epoch``).  A file of
+    another epoch (left by a later run without an EMA, or a save cut short between the two files) is
+    not used: the EMA then starts from the loaded weights with 0 updates.  Returns True if loaded."""
+    if not os.path.exists(path):
+        return False
+    blob = _torch_load(path, map_location="cpu")
+    if int(blob["epoch"]) != int(epoch):
+        logger.warning("%s was saved at epoch %d, the checkpoint being resumed at epoch %d: not used, "
+                       "the weight EMA starts from the loaded weights", path, int(blob["epoch"]), int(epoch))
+        return False
+    if float(blob["decay"]) != ema.decay:
+        logger.warning("%s was averaged with decay %r; continuing with %r", path, blob["decay"], ema.decay)
+    ema.load_state_dict(blob)
+    logger.info("Loaded the weight EMA from %s (%d updates)", path, ema.updates)
+    return True
+
+
 class Solver:
     # ------------------------------------------------------------------------------------------
     # per-rank bootstrap (child process)
@@ -323,9 +363,10 @@ class Solver:
 
         # world > 1 without clipping: arena vectors other ranks reach go to symmetric/multicast
         # memory so all-reduce + update + broadcast can be one NVLS kernel per bucket
+        ema_decay = args.ema_decay if run_opts.mode == Mode.TRAIN else 0.0
         symm_alloc = None
         if (distributed and not run_opts.optim.gradientClip
-                and args.layer_adaptation == LayerAdaptation.NONE and accum == 1):
+                and args.layer_adaptation == LayerAdaptation.NONE and accum == 1 and ema_decay == 0.0):
             from .symm import try_make_allocator
             symm_alloc = try_make_allocator(device, args.world_size)
         from .arena_linear import head_layout_groups
@@ -344,6 +385,14 @@ class Solver:
         optimizer = create_fused_optimizer(arena, run_opts.optim, args.layer_adaptation)
         if checkpoint:
             optimizer.load_state_dict(checkpoint.optimizerState)
+        ema = None
+        if ema_decay > 0.0:
+            # after the buffers took their final dtype; starts from the weights just loaded
+            from .ema import WeightEMA
+            ema = WeightEMA(arena, model, ema_decay)
+            if checkpoint and run_opts.initialModelPath is None:
+                load_ema_checkpoint(ema, os.path.join(args.save_dir, CHECKPOINT_NAME + EMA_SUFFIX),
+                                    checkpoint.epoch)
         nvls_link = None
         if symm_alloc is not None:
             from .symm import make_link
@@ -367,7 +416,7 @@ class Solver:
             first_bucket_mb=None,
             eager_update=os.environ.get("FRL_B200_EAGER_UPDATE",
                                         "1" if args.world_size > 1 else "0") != "0",
-            accumulation=accum)
+            accumulation=accum, ema=ema)
         # GradNorm differentiates through the layers' backward (create_graph=True) and debugGrad
         # calls autograd.grad on them: those runs keep the stock nn.Linear autograd path
         if (os.environ.get("FRL_B200_DIRECT_GRADS", "1") != "0" and not run_opts.debugGrad
@@ -384,14 +433,15 @@ class Solver:
                               pipeline=pipeline, buffers=buffers, precision=args.precision,
                               serialize_state=(args.local_rank == 0),
                               graph_step=(args.graph_step if args.graph_step is not None
-                                          else os.environ.get("FRL_B200_CUDA_GRAPH", "0") == "1"))
+                                          else os.environ.get("FRL_B200_CUDA_GRAPH", "0") == "1"),
+                              ema=ema)
         worker.save_every = args.save_every
         if args.rank == 0:
             # one line per run: which of the alternative paths this configuration took
             logger.info(
                 "frl_b200 step: precision %s | step issue %s | gradient exchange %s | update %s | "
                 "Linear layers with arena-born gradients %d (%d fused with their ReLU, %d in FP8) | "
-                "other gradients %s | layer adaptation %s | gradient accumulation %s",
+                "other gradients %s | layer adaptation %s | gradient accumulation %s | weight EMA %s",
                 args.precision.value,
                 "CUDA-graph replay after 2 eager steps" if worker.graphed is not None else "eager launches",
                 ("fused NVLS kernel per bucket (K7), %d buckets" % len(pipeline.buckets)) if pipeline.nvls is not None
@@ -407,7 +457,10 @@ class Solver:
                                                           sum(is_adapted(s) for s in arena.slots), len(arena.slots)),
                 "none" if accum == 1 else
                 "%d microbatches per update (K10, fp32 accumulator %.1f MiB)" % (
-                    accum, pipeline.accumulator_bytes / 2 ** 20))
+                    accum, pipeline.accumulator_bytes / 2 ** 20),
+                "none" if ema is None else
+                "decay %r, one K11 launch per update (%.1f MiB), held-out splits evaluated with it" % (
+                    ema_decay, ema.nbytes / 2 ** 20))
         scheduler = create_lr_scheduler(run_opts, worker.optimizer,
                                         checkpoint.epoch if checkpoint else -1)
         return worker, scheduler, checkpoint
@@ -540,6 +593,7 @@ class Solver:
                        for i in range(len(test_io[0].output))]
         model = _torch_load(io.BytesIO(donor.modelBuffer), map_location="cpu")
         optimizer_state = _torch_load(io.BytesIO(donor.optimizerStateBuffer), map_location="cpu")
+        ema = optimizer_state.pop(EMA_STATE_KEY, None)       # the main checkpoint keeps its format
 
         logger.info("==> saving checkpoint to %s", str(save_dir))
         stem = os.path.join(save_dir, base_filename)
@@ -553,6 +607,10 @@ class Solver:
             torch.save(model, f_model)       # whole module: loadable without the class layout
             torch.save({"test_input": test_input, "test_output": test_output}, f_data)
             torch.save(problem.anno_param._asdict() if problem.anno_param else {}, f_anno)
+            if ema is not None:
+                with open(stem + EMA_SUFFIX, "wb") as f_ema:
+                    torch.save({"epoch": epoch, "decay": ema["decay"], "updates": ema["updates"],
+                                "state_dict": ema["state_dict"]}, f_ema)
 
     # ------------------------------------------------------------------------------------------
     # parent side: collecting per-epoch results from the ranks
@@ -611,7 +669,8 @@ class Solver:
               init_method: str, node_idx: int = 0, node_count: int = 1, memory_quota: int = 0,
               precision: Optional[Precision] = None, graph: Optional[bool] = None,
               layer_adaptation: Optional[LayerAdaptation] = None,
-              grad_accumulation: Optional[int] = None
+              grad_accumulation: Optional[int] = None,
+              ema_decay: Optional[float] = None
               ) -> Iterator[PerformanceSummary]:
         """The reference's entry point (solver.py:728-739) plus two keyword-only extensions:
 
@@ -648,13 +707,43 @@ class Solver:
                        None: FRL_B200_GRAD_ACCUM (default 1: no accumulator, today's step).  Any
                        value but an integer >= 1 raises ``ValueError`` before a rank starts.
                        ``Mode.EVAL`` ignores it.
+        ``ema_decay``  d in [0, 1): keep an exponential moving average (EMA) of the weights; 0 is
+                       off.  The same values as ``AveragedModel(model, multi_avg_fn=
+                       get_ema_multi_avg_fn(d), use_buffers=True)`` with ``update_parameters``
+                       called after every ``optimizer.step()``.  It covers the model's trainable
+                       parameters (arena range ``[0, model_end)``; criterion parameters are not
+                       averaged) and is updated once per optimizer update (with gradient
+                       accumulation by the microbatch that closes a group): the first update
+                       copies the fp32 master weights, every later one is
+                       ``ema = lerp(ema, w, 1 - d)`` in fp32 on them, torch's lerp formula with
+                       ``1 - d`` formed in double (K11, one launch).  Floating buffers (BatchNorm
+                       statistics) get the same lerp through ``torch._foreach_lerp_``,
+                       non-floating ones are copied.  In a TRAIN run every split other than
+                       ``Split.TRAIN`` is evaluated with the EMA weights and buffers (swapped
+                       into the arena and the bf16 shadow for the split, swapped back bit for
+                       bit after it), so its losses, metrics and ``testIO`` samples, and hence
+                       ``<stem>.test_data``, belong to the EMA model.  Every checkpoint gets a
+                       ``<stem>.ema`` next to it: ``{"epoch", "decay", "updates",
+                       "state_dict"}``, the state dict keyed like the main checkpoint's, so
+                       ``initialModelPath=<stem>.ema`` with ``Mode.EVAL`` evaluates the EMA model;
+                       the main checkpoint and ``<stem>.model`` keep the live weights and their
+                       format.  A resume loads ``<save_dir>/.checkpoint.pth.ema`` if it exists
+                       and was saved at the checkpoint's epoch (bit-exact continuation); without
+                       it, with one of another epoch, or with ``initialModelPath``, the EMA starts
+                       from the loaded weights with 0 updates.  Several GPUs: the EMA
+                       turns the fused NVLS step (K7) off, every rank keeps the same averaged
+                       parameters (buffers: see INTEGRATION.md; rank 0's are saved).
+                       None: FRL_B200_EMA_DECAY (default 0).  Any value but a real number in
+                       [0, 1) raises ``ValueError`` before a rank starts.  ``Mode.EVAL`` ignores it.
         """
         adapt = LayerAdaptation.NONE
         accum = 1
+        decay = 0.0
         if run_opts.mode == Mode.TRAIN:
             adapt = resolve_layer_adaptation(layer_adaptation)
             check_layer_adaptation(run_opts.optim, adapt)
             accum = resolve_grad_accumulation(grad_accumulation)
+            decay = resolve_ema_decay(ema_decay)
         n_visible = 0 if run_opts.cpuonly else _cuda_device_count_without_poisoning_fork()
         if n_visible == 0:
             raise RuntimeError(
@@ -693,7 +782,7 @@ class Solver:
                 rank=node_idx * device_count + local_rank, local_rank=local_rank,
                 world_size=world_size, group_name=group_name, init_method=init_method,
                 cache=None, precision=prec, save_every=save_every, graph_step=graph,
-                layer_adaptation=adapt, grad_accumulation=accum)
+                layer_adaptation=adapt, grad_accumulation=accum, ema_decay=decay)
             if not run_opts.singleThreaded:
                 parent_conn, child_conn = ctx.Pipe(duplex=False)
                 proc = ctx.Process(target=cls._solver_worker_process,

@@ -16,7 +16,7 @@ host with the device:
 * one watchdog thread per split is kicked per step instead of spawning a Timer per step.
 """
 import bisect
-from contextlib import contextmanager
+from contextlib import contextmanager, nullcontext
 import heapq
 import io
 import os
@@ -38,6 +38,7 @@ import torch.utils.data
 from . import _native
 from .arena import ParamArena
 from .criteria import BaseParallelCriterion, GradNormWeightedCriterion
+from .ema import EMA_STATE_KEY
 from .fused_optim import FusedArenaOptimizer
 from .grad_sync import BufferBroadcaster, GradBucketPipeline, accumulation_plan
 from .model import MultiTaskModel
@@ -666,7 +667,7 @@ class SolverWorker:
                  pipeline: Optional[GradBucketPipeline] = None,
                  buffers: Optional[BufferBroadcaster] = None,
                  precision: Precision = Precision.FP32,
-                 serialize_state: bool = True, graph_step: bool = False) -> None:
+                 serialize_state: bool = True, graph_step: bool = False, ema=None) -> None:
         self.model = model
         self.criterion = criterion
         self.optimizer = optimizer
@@ -678,6 +679,7 @@ class SolverWorker:
         self.pipeline = pipeline or GradBucketPipeline(
             self.arena, optimizer, clip_norm=run_opts.optim.gradientClip)
         self.buffers = buffers
+        self.ema = ema                 # ema.WeightEMA: held-out splits of a TRAIN run evaluate with it
         self.cur_epoch = 0
         self._node_idx = node_idx
         self._node_count = node_count
@@ -762,6 +764,9 @@ class SolverWorker:
                 plan = accumulation_plan(n_batches, self.pipeline.accumulation, loader.batch_size,
                                          len(loader.sampler))
             log = LossLog(n_tasks, n_batches, self.device)
+            # with a weight EMA, the splits a TRAIN run only evaluates run on the averaged weights
+            weights = (self.ema.swapped() if self.ema is not None and mode == Mode.TRAIN
+                       and data_type != Split.TRAIN else nullcontext())
             checked = 0
             batch_start = time.time()
             mark("setup done")
@@ -772,7 +777,7 @@ class SolverWorker:
             # an epoch is then served late).  A step leaves no reference cycles behind
             # (its autograd graph is dropped explicitly below); FRL_B200_GC_IN_LOOP=1 keeps the
             # collector on for Problems whose hooks do.
-            with StepWatchdog(self.run_opts.minibatchTimeoutMs) as dog, sampler_state, _gc_paused():
+            with weights, StepWatchdog(self.run_opts.minibatchTimeoutMs) as dog, sampler_state, _gc_paused():
                 for minibatch_idx, (data, target, raw_meta) in enumerate(loader):
                     dog.kick()
                     if minibatch_idx < 3:
@@ -1031,6 +1036,9 @@ class SolverWorker:
                     for k, v in entry.items():
                         if torch.is_tensor(v):
                             entry[k] = v.cpu()
+                if self.ema is not None:
+                    # travels to the parent with the optimizer state, which writes it to <stem>.ema
+                    state[EMA_STATE_KEY] = self.ema.state_dict()
                 torch.save(state, buf)
                 optim_bytes = buf.getvalue()
             self.model.train(was_training)

@@ -186,6 +186,20 @@ int frl_grad_accumulate_mt(float* acc, const frl_grad_seg* segs_dev, const int64
                            const float* dyn, void* stream);
 
 /* ------------------------------------------------------------------------------------------
+ * K11 — weight EMA (an extension: the reference has no EMA).  Replaces the
+ * torch.optim.swa_utils.AveragedModel(..., multi_avg_fn=get_ema_multi_avg_fn(decay))
+ * .update_parameters(model) call a user would add after optimizer.step() (reference
+ * solver_worker.py:592): one streaming pass over the model range of the fp32 master weights,
+ *   ema[i] = lerp(ema[i], p[i], (float)w)   for i < n,
+ * with torch's lerp formula  |w| < 0.5 ? e + w*(p - e) : p - (p - e)*(1 - w),  each branch one
+ * fmaf.  The caller passes w = 1 - decay (formed in double).  12 B per element.
+ * ema, p: fp32, 16-byte aligned (FRL_E_ALIGN); n >= 0 and 0 <= w <= 1 (FRL_E_ARG); every check
+ * is made before any launch.  Graph-capturable: no host reads, no allocation.  n == 0: returns 0,
+ * launches nothing.
+ * ---------------------------------------------------------------------------------------- */
+int frl_weight_ema(float* ema, const float* p, int64_t n, double w, void* stream);
+
+/* ------------------------------------------------------------------------------------------
  * K3 — global gradient norm for clipping.
  * Replaces torch.nn.utils.clip_grad_norm_ (reference solver_worker.py:588-591): one pass
  * over the model-parameter range of the gradient arena.

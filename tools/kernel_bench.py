@@ -246,6 +246,22 @@ def bench_k10(iters):
     return out
 
 
+def bench_k11(iters):
+    """K11 weight EMA over the headline MLP's model range (54.7 M parameters, its arena as the solver
+    lays it out), timed from a CUDA graph.  Two operand sets (EMA + master, 438 MB each) alternate,
+    so every launch streams from HBM with L2 cold.  Bytes per parameter: read ema and p, write ema
+    (12)."""
+    sizes = [4096 * 4096, 4096] * 3 + [1000 * 4096, 1000, 64 * 4096, 64]
+    n = 0
+    for s in sizes:
+        n = (n + s + 7) // 8 * 8
+    ns = sets_for(8 * n)
+    sets = [(torch.randn(n, device=DEV), torch.randn(n, device=DEV)) for _ in range(ns)]
+    return [timed("K11 weight_ema mlp model range (%d elems)" % n,
+                  lambda i: _native.weight_ema(sets[i][0], sets[i][1], 1e-4), ns, 12 * n, iters,
+                  "%d rotating sets of %d MB" % (ns, 8 * n >> 20), graph=True)]
+
+
 def bench_k3(iters):
     n = 54_703_144
     out = []
@@ -459,7 +475,7 @@ def bench_k9(iters):
 
 BENCHES = {"k2": bench_k2, "k2mt": bench_k2mt, "k2lw": bench_k2lw, "k3": bench_k3, "k4": bench_k4, "k5": bench_k5, "k5a": bench_k5a,
            "k6": bench_k6,
-           "k8": bench_k8, "k8t": bench_k8t, "k9": bench_k9, "k10": bench_k10}
+           "k8": bench_k8, "k8t": bench_k8t, "k9": bench_k9, "k10": bench_k10, "k11": bench_k11}
 
 
 def main():
