@@ -12,8 +12,9 @@
 //   backward: grid (blocks, T).  dout_i = (gl[0] + gl[1+i]) * w_i * dL_i/dout_i, reading
 //             each logit once and writing each gradient once.
 // MaskedLoss (reference criteria.py:267-287) becomes a predicate on the reduction instead of a
-// boolean gather; an empty mask gives the reference's value (0 for MSE, log C for CE) and a
-// zero gradient, again without the mask.sum() host sync.
+// boolean gather; an empty mask gives the reference's value (0 for MSE; for CE log C, or NaN
+// when ignore_index == 0 because every label of tgt - tgt is then ignored) and a zero gradient,
+// again without the mask.sum() host sync.
 #include "frl_common.cuh"
 
 namespace frl {
@@ -293,8 +294,11 @@ criteria_fwd_kernel(const __grid_constant__ CritParams P, float* __restrict__ lo
             const frl_task_desc& q = P.t[i];
             float Li;
             if (q.mask != nullptr && dsel == 0.0) {
-                // reference MaskedLoss with an empty mask: inner(out-out, tgt-tgt)
-                Li = (q.kind == FRL_LOSS_MSE) ? 0.f : logf(static_cast<float>(q.cols));
+                // reference MaskedLoss with an empty mask: inner(out-out, tgt-tgt).  tgt-tgt makes
+                // every CE label 0, so with ignore_index == 0 every row is ignored: 0/0 = NaN
+                if (q.kind == FRL_LOSS_MSE)     Li = 0.f;
+                else if (q.ignore_index == 0)   Li = __int_as_float(0x7fc00000);
+                else                            Li = logf(static_cast<float>(q.cols));
             } else {
                 Li = static_cast<float>(ds / dvalid);       // 0/0 -> NaN, as torch
             }

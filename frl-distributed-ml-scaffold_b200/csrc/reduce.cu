@@ -76,7 +76,10 @@ sumsq_clip_kernel(const GVec* __restrict__ g, int64_t n, float pre_scale, float 
         const float norm = sqrtf(ss);
         out3[0] = ss;
         out3[1] = norm;
-        out3[2] = fminf(1.f, max_norm / (norm + 1e-6f));
+        // torch's clamp(max=1), not fminf: a NaN norm gives a NaN coefficient, so a NaN
+        // gradient anywhere turns every clipped gradient NaN, as clip_grad_norm_ does
+        const float coef = max_norm / (norm + 1e-6f);
+        out3[2] = coef > 1.f ? 1.f : coef;
         sc->ticket = 0;      // ready for the next launch on this stream
     }
 }

@@ -205,6 +205,8 @@ int frl_weight_ema(float* ema, const float* p, int64_t n, double w, void* stream
  * over the model-parameter range of the gradient arena.
  *   out[0] = sum(g^2) * pre_scale^2,  out[1] = sqrt(out[0]),
  *   out[2] = min(1, max_norm / (out[1] + 1e-6))   (the coefficient K2 reads)
+ * As in clip_grad_norm_ (clamp(max=1)), a NaN gradient makes out[2] NaN, so every clipped
+ * gradient becomes NaN; an inf gradient makes it 0 (NaN only where the gradient was inf).
  * scratch: >= frl_reduce_scratch_floats() floats + 1 uint32 ticket, zero-initialised once.
  * Deterministic: fixed-order two-stage reduction.
  * ---------------------------------------------------------------------------------------- */
@@ -218,6 +220,12 @@ int frl_grad_sumsq_clip(const void* g, int64_t n, int g_dtype, float pre_scale, 
  * nn.MSELoss / nn.CrossEntropyLoss kernels underneath, MaskedLoss's gather
  * (criteria.py:267-287) and the isnan()/item() syncs of the loop (solver_worker.py:486-487,
  * 569).
+ * A task whose mask selects nothing gives the reference's inner(out - out, tgt - tgt): 0 for MSE,
+ * log C for CE, or NaN for CE with ignore_index == 0 (every label of tgt - tgt is 0, so every
+ * row is ignored), with a zero gradient.  Two differences remain, both only with non-finite
+ * outputs: the reference's out - out is NaN where an output is inf or NaN, which makes that loss
+ * NaN, but the kernels never read a masked-out output, so they still give 0 / log C; and torch's
+ * gradient of a NaN row whose label is ignore_index is NaN, where the kernels write 0.
  * ---------------------------------------------------------------------------------------- */
 #define FRL_MAX_TASKS 8
 enum { FRL_LOSS_MSE = 0, FRL_LOSS_CE = 1 };

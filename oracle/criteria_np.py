@@ -25,7 +25,8 @@ def mse(out, tgt, mask=None):
 
 def cross_entropy(logits, labels, mask=None, ignore_index=-100):
     """mean over selected, non-ignored rows of (logsumexp(x) - x[y]); an all-False mask gives
-    log(C) with zero gradient (reference MaskedLoss: CE(out - out, tgt - tgt))."""
+    log(C) with zero gradient (reference MaskedLoss: CE(out - out, tgt - tgt)), or NaN when
+    ignore_index == 0, since tgt - tgt makes every label 0 and so every row is ignored."""
     x = logits.astype(np.float64)
     B, C = x.shape
     m = x.max(axis=1, keepdims=True)
@@ -33,7 +34,7 @@ def cross_entropy(logits, labels, mask=None, ignore_index=-100):
     sel = np.ones(B, dtype=bool) if mask is None else mask.astype(bool)
     grad = np.zeros_like(x)
     if mask is not None and sel.sum() == 0:
-        return float(np.log(C)), grad
+        return (np.nan if ignore_index == 0 else float(np.log(C))), grad
     valid = sel & (labels != ignore_index)
     n = int(valid.sum())
     if n == 0:

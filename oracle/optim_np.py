@@ -61,9 +61,11 @@ def rmsprop_step(p, g, sq, buf, *, lr, alpha, eps, wd, mu, grad_scale=1.0):
 
 
 def clip_coef(g_model, max_norm, pre_scale=1.0):
-    """torch.nn.utils.clip_grad_norm_: min(1, max_norm / (||g||_2 + 1e-6))."""
+    """torch.nn.utils.clip_grad_norm_: clamp(max_norm / (||g||_2 + 1e-6), max=1).  A NaN norm
+    gives a NaN coefficient (Python's min(1.0, nan) would give 1.0)."""
     norm = float(np.sqrt(np.sum((g_model.astype(np.float64) * pre_scale) ** 2)))
-    return min(1.0, max_norm / (norm + 1e-6)), norm
+    coef = max_norm / (norm + 1e-6)
+    return (1.0 if coef > 1.0 else coef), norm
 
 
 def bf16_round(x):
