@@ -4,7 +4,7 @@ The reference lets autograd allocate ``weight.grad`` wherever the caching alloca
 DDP then copies it into a bucket, pre-divides, all-reduces and copies it back (reference
 solver.py:287-289 -> torch Reducer).  For exact ``nn.Linear`` modules — the layers where a
 Problem's forward really is a dense contraction — the solver swaps the module's ``forward`` for
-this autograd Function while the model is wrapped:
+one autograd Function, ``_ArenaLinearFn``, while the model is wrapped:
 
   forward   y = x W^T + b                      (cuBLAS, unchanged)
   backward  dX = dY W                          (cuBLAS)
@@ -28,13 +28,19 @@ Unless ``FRL_B200_FUSE_RELU=0``, a ``nn.Linear`` directly followed by a ``nn.ReL
 In a ``Precision.FP8`` run a site whose weight lives in the bf16 shadow and whose widths are
 multiples of 16 (``fp8_site_qualifies``) runs its three GEMMs on the FP8 tensor cores
 (``torch._scaled_mm``, tensor-wise scales, bf16 output, fp32 accumulation) for every call whose
-flattened row count is a multiple of 16; other calls take the bf16 Functions above.  Each operand
+flattened row count is a multiple of 16; other calls take the bf16 GEMMs above.  Each operand
 is quantised by K9 at a power-of-two scale from its own amax (``frl_fp8_amax`` +
 ``frl_fp8_quantize``), one pass giving the row-major copy and, for backward, the transposed one:
 
   forward   Y  = Xq Wq^T (+ b)        Xq, Wq e4m3; saved for backward: Xq^T, Wq^T (not bf16 X)
   backward  dX = dZq (Wq^T)^T         dZq e5m2
             dW = dZq^T (Xq^T)^T       into the arena as above; db as above
+
+Whatever the variant, backward runs one protocol: form dZ (on a ReLU site inside a step,
+``frl_drelu_colsum`` writes the bias gradient with it), compute dX, and only then write dW
+(``LinearSite.weight_grad``), the bias gradient if not yet written, and mark the slots ready
+(``LinearSite.backward_done``): marking a slot ready can launch the bucket's update, which
+overwrites W.
 """
 import os
 import types
@@ -98,172 +104,120 @@ def _fp8_operands(x, weight, transposed: bool):
     return xq, xtq, sx, wq, wtq, sw
 
 
-def _fp8_backward(ctx, site, dz2, db_from_dz):
-    """dX and dW of an FP8 site from the bf16 output gradient ``dz2`` (after the ReLU mask).
-    Inside an open pipeline step dW goes to the arena and the bias gradient, unless
-    ``db_from_dz`` is False (already written), is ``frl_colsum(dz2)`` into its slice."""
-    xtq, wtq, sx, sw = ctx.saved_tensors[:4]
-    need_dx = ctx.needs_input_grad[0]
-    dzq, dztq, sdz = _fp8_quantize(dz2, _native.FP8_E5M2, need_dx, True)
-    # dX first: marking the weight's slot ready may launch the bucket's update, which overwrites W
-    dx = _fp8_mm(dzq, wtq, sdz, sw).view(ctx.x_shape) if need_dx else None
-    pipe = site.pipeline
-    if pipe is not None and pipe.step_open:
-        site.weight_grad_fp8(pipe, dztq, xtq, sdz, sx)
-        if db_from_dz and ctx.has_bias and site.bslot is not None:
-            KERNELS.colsum(dz2, pipe.arena.grad_view(site.bslot),
-                           accumulate=not site.bstate.first_touch(pipe.step_id))
-        site.backward_done(pipe)
-        return dx, None, None, None, None
-    dw = _fp8_mm(dztq, xtq, sdz, sx) if ctx.needs_input_grad[1] else None
-    db = dz2.sum(0) if (ctx.has_bias and ctx.needs_input_grad[2]) else None
-    return dx, dw, db, None, None
+class _DenseGemms:
+    """dX and dW of a dense (bf16/fp32) site from its saved (X, W) and dZ [M, N]."""
+    row_multiple = 1
+
+    def __init__(self, saved, dz, need_dx):
+        x, self.weight = saved[0], saved[1]
+        self.x2 = x.reshape(-1, x.shape[-1])
+        self.dz, self.dzt = dz, dz.t()
+
+    def dx(self):
+        return self.dz.matmul(self.weight)
+
+    def dw(self, dzt, out=None):
+        """Rows of dW = dZ^T X for the rows ``dzt`` of dZ^T."""
+        return torch.mm(dzt, self.x2, out=out)
+
+    def dw_add(self, gw):
+        gw.addmm_(self.dzt, self.x2)
+
+
+class _Fp8Gemms:
+    """The same on the FP8 tensor cores from the saved Xq^T, Wq^T and their scales: dZ is quantised
+    to e5m2, the row-major copy only if dX is needed.  A row block of dW must be a multiple of 16
+    rows."""
+    row_multiple = FP8_MULTIPLE
+
+    def __init__(self, saved, dz, need_dx):
+        self.xtq, self.wtq, self.sx, self.sw = saved[:4]
+        self.dzq, self.dzt, self.sdz = _fp8_quantize(dz, _native.FP8_E5M2, need_dx, True)
+
+    def dx(self):
+        return _fp8_mm(self.dzq, self.wtq, self.sdz, self.sw)
+
+    def dw(self, dzt, out=None):
+        return _fp8_mm(dzt, self.xtq, self.sdz, self.sx, out=out)
+
+    def dw_add(self, gw):
+        gw.add_(self.dw(self.dzt))
 
 
 class _ArenaLinearFn(torch.autograd.Function):
+    """One Linear site, with the ReLU it absorbed if it has one (``site.relu``), with dense or FP8
+    (``fp8``) GEMMs; see the module docstring.  ``for_backward`` (FP8 only): whether the call
+    records a graph (grad mode on and an input requires grad); otherwise nothing is saved and only
+    the row-major copies the forward GEMM reads are made."""
+
     @staticmethod
-    def forward(ctx, x, weight, bias, site):
-        ctx.site = site
-        ctx.has_bias = bias is not None
-        ctx.save_for_backward(x, weight)
-        if x.dim() <= 2:
+    def forward(ctx, x, weight, bias, site, fp8, for_backward):
+        ctx.site, ctx.fp8, ctx.has_bias, ctx.x_shape = site, fp8, bias is not None, x.shape
+        relu = site.relu is not None
+        if not (fp8 or relu) and x.dim() <= 2:
+            ctx.save_for_backward(x, weight)
             return F.linear(x, weight, bias)
         # N-D input: F.linear would return a VIEW of its 2-D result, and autograd forbids in-place
         # ops (nn.ReLU(inplace=True)) on a view created inside a custom Function: write the GEMM
         # into a 2-D view of a fresh N-D tensor instead and return that tensor
-        y = torch.empty(*x.shape[:-1], weight.shape[0], dtype=x.dtype, device=x.device)
-        x2 = x.reshape(-1, x.shape[-1])
-        if bias is not None:
-            torch.addmm(bias, x2, weight.t(), out=y.view(-1, weight.shape[0]))
+        y = torch.empty(*x.shape[:-1], weight.shape[0], dtype=torch.bfloat16 if fp8 else x.dtype,
+                        device=x.device)
+        y2 = y.view(-1, weight.shape[0])
+        if fp8:
+            xq, xtq, sx, wq, wtq, sw = _fp8_operands(x, weight, for_backward)
+            _fp8_mm(xq, wq, sx, sw, bias=bias, out=y2)
+            if relu:
+                y.relu_()
+            saved = (xtq, wtq, sx, sw) if for_backward else ()
         else:
-            torch.mm(x2, weight.t(), out=y.view(-1, weight.shape[0]))
+            x2 = x.reshape(-1, x.shape[-1])
+            if relu:
+                torch._addmm_activation(bias, x2, weight.t(), use_gelu=False, out=y2)
+            elif bias is not None:
+                torch.addmm(bias, x2, weight.t(), out=y2)
+            else:
+                torch.mm(x2, weight.t(), out=y2)
+            saved = (x, weight)
+        if relu and saved:
+            saved += (y,)
+        ctx.save_for_backward(*saved)
         return y
 
     @staticmethod
     @torch.autograd.function.once_differentiable
     def backward(ctx, dy):
-        x, weight = ctx.saved_tensors
-        site = ctx.site
-        # dX first: marking the weight's slot ready may launch the bucket's update on the side
-        # stream, and that update overwrites the very weight dX = dY W reads
-        dx = dy.matmul(weight) if ctx.needs_input_grad[0] else None
-        dy2 = dy.reshape(-1, dy.shape[-1])
-        x2 = x.reshape(-1, x.shape[-1])
+        site, saved = ctx.site, ctx.saved_tensors
+        relu = site.relu is not None
         pipe = site.pipeline
-        if pipe is not None and pipe.step_open:
-            site.weight_grad(pipe, dy2, x2)
-            if ctx.has_bias and site.bslot is not None:
-                if not dy2.is_contiguous():
-                    dy2 = dy2.contiguous()
-                KERNELS.colsum(dy2, pipe.arena.grad_view(site.bslot),
+        in_step = pipe is not None and pipe.step_open
+        dz = dy.reshape(-1, dy.shape[-1])
+        if relu or ctx.fp8:
+            dz = dz.contiguous()
+        db_written = False
+        if relu:
+            y2 = saved[-1].reshape(-1, dz.shape[1])
+            if in_step:                              # dZ and the bias gradient in one pass
+                dz_relu = torch.empty_like(dz)
+                KERNELS.drelu_colsum(dz, y2, dz_relu, pipe.arena.grad_view(site.bslot),
+                                     accumulate=not site.bstate.first_touch(pipe.step_id))
+                dz, db_written = dz_relu, True
+            else:
+                dz = dz * (y2 > 0).to(dz.dtype)
+        need_dx = ctx.needs_input_grad[0]
+        gemms = (_Fp8Gemms if ctx.fp8 else _DenseGemms)(saved, dz, need_dx)
+        # dX first: marking the weight's slot ready may launch the bucket's update on the side
+        # stream, and that update overwrites the very weight dX = dZ W reads
+        dx = gemms.dx().view(ctx.x_shape) if need_dx else None
+        if in_step:
+            site.weight_grad(pipe, gemms)
+            if ctx.has_bias and not db_written and site.bslot is not None:
+                KERNELS.colsum(dz.contiguous(), pipe.arena.grad_view(site.bslot),
                                accumulate=not site.bstate.first_touch(pipe.step_id))
             site.backward_done(pipe)
-            return dx, None, None, None
-        dw = dy2.t().mm(x2) if ctx.needs_input_grad[1] else None
-        db = dy2.sum(0) if (ctx.has_bias and ctx.needs_input_grad[2]) else None
-        return dx, dw, db, None
-
-
-class _ArenaLinearReluFn(torch.autograd.Function):
-    """relu(linear(x)) as one unit; see the module docstring."""
-
-    @staticmethod
-    def forward(ctx, x, weight, bias, site):
-        ctx.site = site
-        x2 = x.reshape(-1, x.shape[-1])
-        # the output must not be a view (see _ArenaLinearFn.forward): GEMM into a view of it
-        y = torch.empty(*x.shape[:-1], weight.shape[0], dtype=x.dtype, device=x.device)
-        torch._addmm_activation(bias, x2, weight.t(), use_gelu=False, out=y.view(-1, weight.shape[0]))
-        ctx.save_for_backward(x, weight, y)
-        return y
-
-    @staticmethod
-    @torch.autograd.function.once_differentiable
-    def backward(ctx, dy):
-        x, weight, y = ctx.saved_tensors
-        site = ctx.site
-        dy2 = dy.reshape(-1, dy.shape[-1])
-        if not dy2.is_contiguous():
-            dy2 = dy2.contiguous()
-        y2 = y.reshape(-1, y.shape[-1])
-        x2 = x.reshape(-1, x.shape[-1])
-        pipe = site.pipeline
-        if pipe is not None and pipe.step_open and (dy2.is_cuda or KERNELS is not _native):
-            dz = torch.empty_like(dy2)
-            KERNELS.drelu_colsum(dy2, y2, dz, pipe.arena.grad_view(site.bslot),
-                                 accumulate=not site.bstate.first_touch(pipe.step_id))
-            # dX before any slot is marked ready (the bucket's update overwrites W)
-            dx = dz.matmul(weight).view_as(x) if ctx.needs_input_grad[0] else None
-            site.weight_grad(pipe, dz, x2)
-            site.backward_done(pipe)
-            return dx, None, None, None
-        dz = dy2 * (y2 > 0).to(dy2.dtype)
-        dx = dz.matmul(weight).view_as(x) if ctx.needs_input_grad[0] else None
-        dw = dz.t().mm(x2) if ctx.needs_input_grad[1] else None
-        db = dz.sum(0) if ctx.needs_input_grad[2] else None
-        return dx, dw, db, None
-
-
-class _Fp8LinearFn(torch.autograd.Function):
-    """FP8 form of ``_ArenaLinearFn`` (see the module docstring).  ``for_backward``: whether the
-    call records a graph (grad mode on and an input requires grad); otherwise only the row-major
-    copies the forward GEMM reads are made."""
-
-    @staticmethod
-    def forward(ctx, x, weight, bias, site, for_backward):
-        ctx.site = site
-        ctx.has_bias = bias is not None
-        ctx.x_shape = x.shape
-        xq, xtq, sx, wq, wtq, sw = _fp8_operands(x, weight, for_backward)
-        # the output must not be a view (see _ArenaLinearFn.forward): GEMM into a view of it
-        y = torch.empty(*x.shape[:-1], weight.shape[0], dtype=torch.bfloat16, device=x.device)
-        _fp8_mm(xq, wq, sx, sw, bias=bias, out=y.view(-1, weight.shape[0]))
-        if for_backward:
-            ctx.save_for_backward(xtq, wtq, sx, sw)
-        return y
-
-    @staticmethod
-    @torch.autograd.function.once_differentiable
-    def backward(ctx, dy):
-        dy2 = dy.reshape(-1, dy.shape[-1])
-        if not dy2.is_contiguous():
-            dy2 = dy2.contiguous()
-        return _fp8_backward(ctx, ctx.site, dy2, True)
-
-
-class _Fp8LinearReluFn(torch.autograd.Function):
-    """FP8 form of ``_ArenaLinearReluFn``: the FP8 GEMM with bias, then ReLU; backward runs
-    ``frl_drelu_colsum`` (dZ and the bias gradient in one pass) and then quantises dZ."""
-
-    @staticmethod
-    def forward(ctx, x, weight, bias, site, for_backward):
-        ctx.site = site
-        ctx.has_bias = True
-        ctx.x_shape = x.shape
-        xq, xtq, sx, wq, wtq, sw = _fp8_operands(x, weight, for_backward)
-        y = torch.empty(*x.shape[:-1], weight.shape[0], dtype=torch.bfloat16, device=x.device)
-        _fp8_mm(xq, wq, sx, sw, bias=bias, out=y.view(-1, weight.shape[0]))
-        y.relu_()
-        if for_backward:
-            ctx.save_for_backward(xtq, wtq, sx, sw, y)
-        return y
-
-    @staticmethod
-    @torch.autograd.function.once_differentiable
-    def backward(ctx, dy):
-        y = ctx.saved_tensors[4]
-        site = ctx.site
-        dy2 = dy.reshape(-1, dy.shape[-1])
-        if not dy2.is_contiguous():
-            dy2 = dy2.contiguous()
-        y2 = y.reshape(-1, y.shape[-1])
-        pipe = site.pipeline
-        if pipe is not None and pipe.step_open:
-            dz = torch.empty_like(dy2)
-            KERNELS.drelu_colsum(dy2, y2, dz, pipe.arena.grad_view(site.bslot),
-                                 accumulate=not site.bstate.first_touch(pipe.step_id))
-            return _fp8_backward(ctx, site, dz, False)
-        return _fp8_backward(ctx, site, dy2 * (y2 > 0).to(dy2.dtype), True)
+            return dx, None, None, None, None, None
+        dw = gemms.dw(gemms.dzt) if ctx.needs_input_grad[1] else None
+        db = dz.sum(0) if (ctx.has_bias and ctx.needs_input_grad[2]) else None
+        return dx, dw, db, None, None, None
 
 
 class _ArenaMultiHeadFn(torch.autograd.Function):
@@ -434,39 +388,25 @@ class LinearSite:
         self.wstate = states.setdefault(wslot.index, SlotState())
         self.bstate = states.setdefault(bslot.index, SlotState()) if bslot is not None else None
 
-    def weight_grad(self, pipe, dz: torch.Tensor, x2: torch.Tensor) -> None:
-        """dW = dZ^T X into the weight's arena slice (store on the step's first touch, accumulate
-        after).  A weight the pipeline exchanges in two row blocks (``row_split``: the layer whose
-        dW ends backward) is computed as two GEMMs and the first block handed over in between,
-        provided this is the parameter's only application in the step."""
+    def weight_grad(self, pipe, gemms) -> None:
+        """dW = dZ^T X by ``gemms`` (``_DenseGemms`` / ``_Fp8Gemms``) into the weight's arena slice
+        (store on the step's first touch, accumulate after).  A weight the pipeline exchanges in two
+        row blocks (``row_split``: the layer whose dW ends backward) is computed as two GEMMs and
+        the first block handed over in between, provided this is the parameter's only application
+        in the step and the block is a multiple of ``gemms.row_multiple`` rows."""
         gw = pipe.arena.grad_view(self.wslot)
         st = self.wstate
         if not st.first_touch(pipe.step_id):
-            gw.addmm_(dz.t(), x2)
+            gemms.dw_add(gw)
             return
         rows = pipe.row_split(self.wslot)
-        if rows and st.fwd_gen == pipe.forward_gen and st.fwd_count == 1:
-            torch.mm(dz[:, :rows].t(), x2, out=gw[:rows])
+        if (rows and rows % gemms.row_multiple == 0 and st.fwd_gen == pipe.forward_gen
+                and st.fwd_count == 1):
+            gemms.dw(gemms.dzt[:rows], out=gw[:rows])
             pipe.rows_ready(self.wslot, rows)
-            torch.mm(dz[:, rows:].t(), x2, out=gw[rows:])
+            gemms.dw(gemms.dzt[rows:], out=gw[rows:])
         else:
-            torch.mm(dz.t(), x2, out=gw)
-
-    def weight_grad_fp8(self, pipe, dztq, xtq, s_dz, s_x) -> None:
-        """``weight_grad`` from the transposed FP8 copies dZ^T [N, M] and X^T [K, M].  A row-split
-        weight takes two GEMMs only if the first block is a multiple of 16 rows."""
-        gw = pipe.arena.grad_view(self.wslot)
-        st = self.wstate
-        if not st.first_touch(pipe.step_id):
-            gw.add_(_fp8_mm(dztq, xtq, s_dz, s_x))
-            return
-        rows = pipe.row_split(self.wslot)
-        if rows and rows % FP8_MULTIPLE == 0 and st.fwd_gen == pipe.forward_gen and st.fwd_count == 1:
-            _fp8_mm(dztq[:rows], xtq, s_dz, s_x, out=gw[:rows])
-            pipe.rows_ready(self.wslot, rows)
-            _fp8_mm(dztq[rows:], xtq, s_dz, s_x, out=gw[rows:])
-        else:
-            _fp8_mm(dztq, xtq, s_dz, s_x, out=gw)
+            gemms.dw(gemms.dzt, out=gw)
 
     def count_forward(self) -> None:
         pipe = self.pipeline
@@ -496,17 +436,9 @@ def _for_backward(*tensors) -> bool:
 def _forward(self, x):
     site = self._frl_site
     site.count_forward()                  # here, not inside the Function: grad mode is off in there
-    if site.fp8 and fp8_call_qualifies(x):
-        return _Fp8LinearFn.apply(x, self.weight, self.bias, site, _for_backward(x, self.weight, self.bias))
-    return _ArenaLinearFn.apply(x, self.weight, self.bias, site)
-
-
-def _forward_relu(self, x):
-    site = self._frl_site
-    site.count_forward()
-    if site.fp8 and fp8_call_qualifies(x):
-        return _Fp8LinearReluFn.apply(x, self.weight, self.bias, site, _for_backward(x, self.weight, self.bias))
-    return _ArenaLinearReluFn.apply(x, self.weight, self.bias, site)
+    fp8 = site.fp8 and fp8_call_qualifies(x)
+    return _ArenaLinearFn.apply(x, self.weight, self.bias, site, fp8,
+                                fp8 and _for_backward(x, self.weight, self.bias))
 
 
 def _identity(self, x):
@@ -606,11 +538,9 @@ def unpatch_linears(sites: List[LinearSite]) -> None:
 def repatch_linears(sites: List[LinearSite]) -> None:
     for site in sites:
         site.module._frl_site = site
+        site.module.forward = types.MethodType(_forward, site.module)
         if site.relu is not None:
-            site.module.forward = types.MethodType(_forward_relu, site.module)
             site.relu.forward = types.MethodType(_identity, site.relu)
-        else:
-            site.module.forward = types.MethodType(_forward, site.module)
         if site.multihead is not None:
             site.multihead.model._frl_heads = site.multihead
             site.multihead.model.forward = types.MethodType(_multihead_forward, site.multihead.model)

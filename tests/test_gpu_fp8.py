@@ -140,15 +140,15 @@ def _dequant(x2, fmt):
 
 @pytest.mark.parametrize("relu", [False, True])
 @pytest.mark.parametrize("xshape", [(256, 512), (4, 64, 512)])
-def test_fp8_site_matches_fp32_on_its_dequantised_operands(relu, xshape):
+def test_fp8_linear_fn_matches_fp32_on_its_dequantised_operands(relu, xshape):
     torch.manual_seed(3)
     K, N = xshape[-1], 384
     x = torch.randn(xshape, device=DEV).bfloat16().requires_grad_(True)
     w = (torch.randn(N, K, device=DEV) / K ** 0.5).bfloat16().requires_grad_(True)
     b = torch.randn(N, device=DEV).bfloat16().requires_grad_(True)
-    site = types.SimpleNamespace(pipeline=None)             # outside a pipeline step: ordinary grads
-    fn = arena_linear._Fp8LinearReluFn if relu else arena_linear._Fp8LinearFn
-    y = fn.apply(x, w, b, site, True)
+    # outside a pipeline step: ordinary grads
+    site = types.SimpleNamespace(pipeline=None, relu=nn.ReLU() if relu else None)
+    y = arena_linear._ArenaLinearFn.apply(x, w, b, site, True, True)
     assert y.dtype == torch.bfloat16 and y.shape == xshape[:-1] + (N,)
     dy = torch.randn(y.shape, device=DEV).bfloat16()
     y.backward(dy)
@@ -388,7 +388,7 @@ def test_fp8_checkpoints_have_the_bf16_layout_and_resume():
         assert _layout(final["state_dict"]) == _layout(ckpt["state_dict"])
 
 
-def test_ragged_minibatch_falls_back_to_the_bf16_function(monkeypatch):
+def test_ragged_minibatch_falls_back_to_bf16_gemms(monkeypatch):
     ns = synthetic.api_namespace("frl_b200")
     t = ns.types
     save_dir = tempfile.mkdtemp(prefix="frl_b200_fp8_")
@@ -400,13 +400,12 @@ def test_ragged_minibatch_falls_back_to_the_bf16_function(monkeypatch):
     worker.model.train()
     assert sum(s.fp8 for s in worker.pipeline.linear_sites) == 2
     calls = {"fp8": 0, "bf16": 0}
-    for cls, key in ((arena_linear._Fp8LinearReluFn, "fp8"), (arena_linear._ArenaLinearReluFn, "bf16")):
-        orig = cls.apply
+    orig = arena_linear._ArenaLinearFn.apply
 
-        def counted(*a, _orig=orig, _key=key):
-            calls[_key] += 1
-            return _orig(*a)
-        monkeypatch.setattr(cls, "apply", counted)
+    def counted(x, weight, bias, site, fp8, for_backward):
+        calls["fp8" if fp8 else "bf16"] += 1
+        return orig(x, weight, bias, site, fp8, for_backward)
+    monkeypatch.setattr(arena_linear._ArenaLinearFn, "apply", counted)
     g = torch.Generator().manual_seed(7)
     for step, (rows, want) in enumerate(((32, {"fp8": 2, "bf16": 0}), (24, {"fp8": 2, "bf16": 2}))):
         x = torch.randn(rows, 64, generator=g).cuda()
