@@ -15,7 +15,7 @@ CSRC_DIR = os.path.join(_HERE, "csrc")
 LIB_PATH = os.path.join(CSRC_DIR, "libfrl_b200.so")
 
 F32, BF16, U8, I64 = 0, 1, 2, 3
-LOSS_MSE, LOSS_CE = 0, 1
+LOSS_MSE, LOSS_CE, LOSS_CE_PROB = 0, 1, 2
 FP8_E4M3, FP8_E5M2 = 0, 1
 FP8_DTYPE = {FP8_E4M3: torch.float8_e4m3fn, FP8_E5M2: torch.float8_e5m2}
 MAX_TASKS = 8
@@ -35,7 +35,7 @@ class TaskDesc(C.Structure):
         ("ignore_index", C.c_int32),
         ("out", C.c_void_p), ("tgt", C.c_void_p), ("mask", C.c_void_p), ("dout", C.c_void_p),
         ("rows", C.c_int64), ("cols", C.c_int64), ("mask_inner", C.c_int64),
-        ("weight", C.c_float), ("_pad", C.c_float),
+        ("weight", C.c_float), ("label_smoothing", C.c_float),
     ]
 
 
@@ -77,6 +77,9 @@ SIGNATURES = {
     "frl_cast_scale": (_i, [_vp, _i, _vp, _i, _i64, _f, _vp]),
     "frl_augment_images": (_i, [_vp, _i64, _i, _i, _i, _vp, C.c_uint64, _i, _i, _d, _d, _d, _d, _d, _i, _i,
                                 _vp, _vp, _vp, _i, _i, _i, _vp, _vp]),
+    "frl_augment_mix_images": (_i, [_vp, _i64, _i, _i, _i, _vp, C.c_uint64, _i, _i, _d, _d, _d, _d, _d, _i, _i,
+                                    _vp, _vp, _vp, _i, _i, _i, _vp, _i, _f, _i, _i, _i, _i, _vp]),
+    "frl_mix_targets": (_i, [_vp, _i, _i64, _i64, _i, _f, _vp, _vp]),
     "frl_colsum_scratch_bytes": (_i64, [_i64, _i64]),
     "frl_colsum": (_i, [_vp, _i, _i64, _i64, _vp, _i, _i, _vp, _vp]),
     "frl_drelu_colsum": (_i, [_vp, _vp, _vp, _i, _i64, _i64, _vp, _i, _i, _vp, _vp]),
@@ -345,6 +348,24 @@ def preproc_affine(src, dst, *, inner=1, channels=1, scale=None, bias=None) -> N
 AUG_RRC, AUG_PAD_CROP, AUG_CENTER_RESIZE, AUG_CENTER_CROP = 0, 1, 2, 3
 
 
+MIX_MIXUP, MIX_CUTMIX = 1, 2
+
+
+def _augment_args(src, idx, dst, seed, epoch, mode, scale_range, ratio_range, eval_crop, pad, flip, scale, bias,
+                  params_out):
+    B, Cc, H, W = src.shape
+    assert src.dtype == torch.uint8 and src.is_contiguous() and dst.is_contiguous()
+    assert dst.dim() == 4 and tuple(dst.shape[:2]) == (B, Cc)
+    assert idx.dtype == torch.int64 and idx.is_contiguous() and idx.numel() == B
+    assert params_out is None or (params_out.dtype == torch.int32 and params_out.is_contiguous()
+                                  and tuple(params_out.shape) == (B, 5))
+    return [_ptr(src), B, Cc, H, W, _ptr(idx), int(seed) & (2 ** 64 - 1), int(epoch),
+            int(mode), float(scale_range[0]), float(scale_range[1]),
+            float(ratio_range[0]), float(ratio_range[1]), float(eval_crop), int(pad),
+            int(bool(flip)), _ptr(scale), _ptr(bias), _ptr(dst), dtype_code(dst.dtype),
+            dst.shape[2], dst.shape[3], _ptr(params_out)]
+
+
 def augment_images(src, idx, dst, *, seed: int, epoch: int, mode: int, scale_range=(0.08, 1.0),
                    ratio_range=(3.0 / 4.0, 4.0 / 3.0), eval_crop: float = 0.875, pad: int = 0,
                    flip: bool = True, scale=None, bias=None, params_out=None) -> None:
@@ -352,18 +373,40 @@ def augment_images(src, idx, dst, *, seed: int, epoch: int, mode: int, scale_ran
     optional flip, then ``x * scale[c] + bias[c]``.  ``src`` uint8 [B, C, H, W], ``idx`` device
     int64 [B], ``dst`` fp32/bf16 [B, C, out_h, out_w], ``params_out`` optional int32 [B, 5]
     (top, left, h, w, flipped).  See frl_augment_images in include/frl_b200.h."""
-    B, Cc, H, W = src.shape
-    assert src.dtype == torch.uint8 and src.is_contiguous() and dst.is_contiguous()
-    assert dst.dim() == 4 and tuple(dst.shape[:2]) == (B, Cc)
-    assert idx.dtype == torch.int64 and idx.is_contiguous() and idx.numel() == B
-    assert params_out is None or (params_out.dtype == torch.int32 and params_out.is_contiguous()
-                                  and tuple(params_out.shape) == (B, 5))
-    _check(lib().frl_augment_images(_ptr(src), B, Cc, H, W, _ptr(idx), int(seed) & (2 ** 64 - 1), int(epoch),
-                                    int(mode), float(scale_range[0]), float(scale_range[1]),
-                                    float(ratio_range[0]), float(ratio_range[1]), float(eval_crop), int(pad),
-                                    int(bool(flip)), _ptr(scale), _ptr(bias), _ptr(dst), dtype_code(dst.dtype),
-                                    dst.shape[2], dst.shape[3], _ptr(params_out), _stream()),
-           "frl_augment_images")
+    args = _augment_args(src, idx, dst, seed, epoch, mode, scale_range, ratio_range, eval_crop, pad, flip, scale,
+                         bias, params_out)
+    _check(lib().frl_augment_images(*args, _stream()), "frl_augment_images")
+
+
+def augment_mix_images(src, idx, dst, *, mix_mode: int, lam: float, box=(0, 0, 0, 0), seed: int, epoch: int,
+                       mode: int, scale_range=(0.08, 1.0), ratio_range=(3.0 / 4.0, 4.0 / 3.0),
+                       eval_crop: float = 0.875, pad: int = 0, flip: bool = True, scale=None, bias=None,
+                       params_out=None) -> None:
+    """K5a with Mixup (``mix_mode=MIX_MIXUP``) or CutMix (``MIX_CUTMIX``, ``box`` = (y0, y1, x0, x1)
+    on the output image) of sample p with sample B-1-p, in the same pass.  Other arguments as
+    ``augment_images``.  See frl_augment_mix_images in include/frl_b200.h."""
+    args = _augment_args(src, idx, dst, seed, epoch, mode, scale_range, ratio_range, eval_crop, pad, flip, scale,
+                         bias, params_out)
+    y0, y1, x0, x1 = (int(v) for v in box)
+    _check(lib().frl_augment_mix_images(*args, int(mix_mode), float(lam), y0, y1, x0, x1, _stream()),
+           "frl_augment_mix_images")
+
+
+def mix_targets(src, dst, lam: float, n_classes: int = 0) -> None:
+    """The batch's target field mixed with partner B-1-i: int64 labels [B] -> fp32 ``dst`` [B,
+    n_classes] (lam at y_i plus 1-lam at y_j, NaN rows for labels outside [0, n_classes)), or a
+    floating field [B, ...] -> ``dst`` of its dtype and shape.  See frl_mix_targets in
+    include/frl_b200.h."""
+    assert src.is_contiguous() and dst.is_contiguous() and src.dim() >= 1
+    B = src.shape[0]
+    if src.dtype == torch.int64:
+        assert src.dim() == 1 and dst.dtype == torch.float32 and tuple(dst.shape) == (B, n_classes)
+        inner = 1
+    else:
+        assert dst.dtype == src.dtype and dst.shape == src.shape
+        inner = src[0].numel() if B else 1
+    _check(lib().frl_mix_targets(_ptr(src), dtype_code(src.dtype), B, inner, int(n_classes), float(lam), _ptr(dst),
+                                 _stream()), "frl_mix_targets")
 
 
 def cast_scale(src, dst, scale: float = 1.0) -> None:

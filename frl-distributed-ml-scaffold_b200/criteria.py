@@ -8,10 +8,12 @@ Public classes and semantics are the reference's:
 * ``MaskedLoss``                   inner loss over the entries selected by a boolean mask
 
 When the outputs are CUDA tensors and every loss module is one the kernels implement
-(``nn.MSELoss``/``nn.CrossEntropyLoss`` with mean reduction, optionally inside ``MaskedLoss``)
-the T per-task losses, their weighting and the total are ONE forward launch and ONE backward
+(``nn.MSELoss``/``nn.CrossEntropyLoss`` with mean reduction, optionally inside ``MaskedLoss``;
+cross-entropy with any ``label_smoothing`` and with class-index or ``[N, C]`` probability
+targets) the T per-task losses, their weighting and the total are ONE forward launch and ONE backward
 launch (``frl_criteria_forward`` / ``frl_criteria_backward``) with no host synchronisation.  Any
-other loss module is the user's plugin code and is simply called, as the reference does.
+other loss module is the user's plugin code and is simply called, as the reference does; so are
+class-weighted cross-entropy and per-position (``out.dim() > 2``) probability targets.
 """
 from abc import ABC, abstractmethod
 from typing import Dict, List, Optional, Sequence, Tuple
@@ -60,12 +62,13 @@ class MaskedLoss(L._Loss):
 # =============================================================================================
 
 class _TaskPlan:
-    __slots__ = ("kind", "masked", "ignore_index")
+    __slots__ = ("kind", "masked", "ignore_index", "label_smoothing")
 
-    def __init__(self, kind: int, masked: bool, ignore_index: int = -100):
+    def __init__(self, kind: int, masked: bool, ignore_index: int = -100, label_smoothing: float = 0.0):
         self.kind = kind
         self.masked = masked
         self.ignore_index = ignore_index
+        self.label_smoothing = label_smoothing
 
 
 def _classify(module: nn.Module) -> Optional[_TaskPlan]:
@@ -78,8 +81,9 @@ def _classify(module: nn.Module) -> Optional[_TaskPlan]:
     if type(module) is nn.MSELoss and module.reduction == "mean":
         return _TaskPlan(_native.LOSS_MSE, masked)
     if (type(module) is nn.CrossEntropyLoss and module.reduction == "mean"
-            and module.weight is None and module.label_smoothing == 0.0):
-        return _TaskPlan(_native.LOSS_CE, masked, int(module.ignore_index))
+            and module.weight is None and 0.0 <= module.label_smoothing <= 1.0):
+        # LOSS_CE here; _plan_for turns it into LOSS_CE_PROB for a probability target
+        return _TaskPlan(_native.LOSS_CE, masked, int(module.ignore_index), float(module.label_smoothing))
     return None
 
 
@@ -129,6 +133,13 @@ def _plan_for(modules: Sequence[nn.Module], outputs: Sequence[torch.Tensor],
             if mask is not None:
                 if mask.dim() > out.dim() or tuple(out.shape[:mask.dim()]) != tuple(mask.shape):
                     return None
+        elif tgt.is_floating_point():
+            # probability targets [N, C] (per-position ones stay with the composed ops)
+            if out.dim() != 2 or tgt.dtype not in _FLOAT_OK or tgt.shape != out.shape:
+                return None
+            if mask is not None and mask.shape != out.shape[:1]:
+                return None
+            tp.kind = _native.LOSS_CE_PROB
         elif out.dim() > 2 and mask is None:
             # per-position classes, torch's [N, C, d1, ...] layout with targets [N, d1, ...]: the
             # kernels see the rows of out.movedim(1, -1) as [N * d1 * ..., C]
@@ -181,6 +192,7 @@ def _descs(plan: _Plan, outs: Sequence[torch.Tensor], douts: Optional[Sequence[t
         d.out_dtype = _native.dtype_code(out.dtype)
         d.tgt_dtype = _native.dtype_code(tgt.dtype)
         d.ignore_index = tp.ignore_index
+        d.label_smoothing = tp.label_smoothing
         d.out = out.data_ptr()
         d.tgt = tgt.data_ptr()
         if tp.kind == _native.LOSS_MSE:
@@ -211,7 +223,9 @@ class _FusedLosses(torch.autograd.Function):
         dev = outs[0].device
         losses = torch.empty(1 + plan.n, dtype=torch.float32, device=dev)
         aux = torch.empty(plan.n, dtype=torch.float32, device=dev)
-        n_lse = sum(o.shape[0] for o, tp in zip(outs, plan.tasks) if tp.kind == _native.LOSS_CE)
+        # per-row slots: the log-sum-exp, and for probability targets also sum(q')
+        n_lse = sum(o.shape[0] * (2 if tp.kind == _native.LOSS_CE_PROB else 1)
+                    for o, tp in zip(outs, plan.tasks) if tp.kind != _native.LOSS_MSE)
         lse = torch.empty(max(n_lse, 1), dtype=torch.float32, device=dev)
         arr, keep = _descs(plan, outs, None)
         KERNELS.criteria_forward(arr, plan.n, losses, aux, lse, plan.sink, plan.nan_flag,
@@ -247,7 +261,8 @@ def _log_path_once(modules, fused: bool) -> None:
             "criterion path for loss modules %s: %s", list(key[0]),
             "fused kernels (frl_criteria_forward / _backward, one launch each)" if fused else
             "composed torch ops — outside the fused kernels' domain (MSE / CrossEntropy with mean "
-            "reduction, optionally inside MaskedLoss)")
+            "reduction, optionally inside MaskedLoss; not class-weighted CrossEntropy or per-position "
+            "probability targets)")
 
 
 def fused_task_losses(modules, outputs, targets, weights=None, sink=None, nan_flag=None

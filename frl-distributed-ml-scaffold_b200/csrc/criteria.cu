@@ -11,6 +11,9 @@
 //             raises an optional NaN flag — no host sync, deterministic.
 //   backward: grid (blocks, T).  dout_i = (gl[0] + gl[1+i]) * w_i * dL_i/dout_i, reading
 //             each logit once and writing each gradient once.
+// Label smoothing and probability targets (CE_PROB) take a soft-row branch of the same loops: the
+// target row streams through the chunk loop next to the logits, and the class-index rows with
+// label_smoothing == 0 run the arithmetic they always ran.
 // MaskedLoss (reference criteria.py:267-287) becomes a predicate on the reduction instead of a
 // boolean gather; an empty mask gives the reference's value (0 for MSE; for CE log C, or NaN
 // when ignore_index == 0 because every label of tgt - tgt is then ignored) and a zero gradient,
@@ -30,7 +33,7 @@ struct CritParams {
     int nblk[FRL_MAX_TASKS];        // CTAs working on task i
     int blk_start[FRL_MAX_TASKS];   // first CTA (of the 1-D grid) of task i
     int part_off[FRL_MAX_TASKS];    // first partial slot of task i
-    int64_t lse_off[FRL_MAX_TASKS]; // offset of task i's rows in the lse array (CE only)
+    int64_t lse_off[FRL_MAX_TASKS]; // offset of task i's rows in the lse array (CE / CE_PROB only)
     int n_tasks;
     int total_blocks;
 };
@@ -125,18 +128,32 @@ __device__ __forceinline__ void mse_partial(const frl_task_desc& t, int blk, int
     nsel = c;
 }
 
-template <typename OT>
+// the smoothed target weight q'_c of column c of a soft row: CE_PROB (1-eps) q_c + eps/C, class
+// index (1-eps) [c == y] + eps/C
+__device__ __forceinline__ float soft_w(const frl_task_desc& t, bool prob, int64_t r0, int64_t c, int64_t y,
+                                       float keep, float eps_c) {
+    if (prob) return fmaf(keep, ld_any(t.tgt, t.tgt_dtype, r0 + c), eps_c);
+    return (c == y ? keep : 0.f) + eps_c;
+}
+
+template <typename OT, bool SOFT>
 __device__ __forceinline__ void ce_partial(const frl_task_desc& t, int blk, int nblk, float* lse_out,
                                            float& sum, float& nsel, float& nvalid) {
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
     const int64_t C = t.cols;
     const bool vec = vec_ok(t);
     const int64_t* labels = static_cast<const int64_t*>(t.tgt);
+    // soft rows (probability targets or label smoothing) also form aw = sum_c q'_c (m - x_c) and
+    // sw = sum_c q'_c, so that the row loss sum_c q'_c (lse - x_c) is aw + sw * log(se)
+    const bool prob = SOFT && t.kind == FRL_LOSS_CE_PROB;
+    const bool soft = SOFT && (prob || t.label_smoothing != 0.f);
+    const float keep = 1.f - t.label_smoothing, eps_c = t.label_smoothing / static_cast<float>(C);
     float s_loss = 0.f, s_sel = 0.f, s_valid = 0.f;
     for (int64_t row = static_cast<int64_t>(blk) * kCWarps + warp; row < t.rows;
          row += static_cast<int64_t>(nblk) * kCWarps) {
         const int64_t r0 = row * C;
-        float m = -INFINITY, se = 0.f;
+        const int64_t ys = soft && !prob ? labels[row] : -1;
+        float m = -INFINITY, se = 0.f, aw = 0.f, sw = 0.f;
         bool has_nan = false;
         if (vec && C <= kCRowChunk) {
             // the whole row in registers: every lane issues its (up to) 8 loads back to back, one
@@ -161,6 +178,15 @@ __device__ __forceinline__ void ce_partial(const frl_task_desc& t, int blk, int 
                     const f32x4 v = cvt4(q[j]);
                     has_nan |= (v.x != v.x) | (v.y != v.y) | (v.z != v.z) | (v.w != v.w);
                     se += expf(v.x - m) + expf(v.y - m) + expf(v.z - m) + expf(v.w - m);
+                    if (soft) {          // the target row streams from memory, never held
+                        const int64_t c = lane * 4 + j * 128;
+                        const float w0 = soft_w(t, prob, r0, c, ys, keep, eps_c);
+                        const float w1 = soft_w(t, prob, r0, c + 1, ys, keep, eps_c);
+                        const float w2 = soft_w(t, prob, r0, c + 2, ys, keep, eps_c);
+                        const float w3 = soft_w(t, prob, r0, c + 3, ys, keep, eps_c);
+                        aw += w0 * (m - v.x) + w1 * (m - v.y) + w2 * (m - v.z) + w3 * (m - v.w);
+                        sw += (w0 + w1) + (w2 + w3);
+                    }
                 }
             }
         } else if (vec) {
@@ -180,11 +206,21 @@ __device__ __forceinline__ void ce_partial(const frl_task_desc& t, int blk, int 
                     ml = fmaxf(fmaxf(ml, fmaxf(v[j].x, v[j].y)), fmaxf(v[j].z, v[j].w));
                 const float mn = fmaxf(mr, ml);
                 float add = 0.f;
+                if (soft && mr != -INFINITY) aw = fmaf(sw, mn - mr, aw);    // rebase aw on mn
 #pragma unroll
                 for (int j = 0; j < kCVecPerLane; ++j) {
                     if (cb + lane * 4 + j * 128 < C) {
                         has_nan |= (v[j].x != v[j].x) | (v[j].y != v[j].y) | (v[j].z != v[j].z) | (v[j].w != v[j].w);
                         add += expf(v[j].x - mn) + expf(v[j].y - mn) + expf(v[j].z - mn) + expf(v[j].w - mn);
+                        if (soft) {
+                            const int64_t c = cb + lane * 4 + j * 128;
+                            const float w0 = soft_w(t, prob, r0, c, ys, keep, eps_c);
+                            const float w1 = soft_w(t, prob, r0, c + 1, ys, keep, eps_c);
+                            const float w2 = soft_w(t, prob, r0, c + 2, ys, keep, eps_c);
+                            const float w3 = soft_w(t, prob, r0, c + 3, ys, keep, eps_c);
+                            aw += w0 * (mn - v[j].x) + w1 * (mn - v[j].y) + w2 * (mn - v[j].z) + w3 * (mn - v[j].w);
+                            sw += (w0 + w1) + (w2 + w3);
+                        }
                     }
                 }
                 sr = (mn == -INFINITY) ? 0.f : fmaf(sr, expf(mr - mn), add);
@@ -192,6 +228,8 @@ __device__ __forceinline__ void ce_partial(const frl_task_desc& t, int blk, int 
             }
             m = warp_max(mr);
             se = (mr == -INFINITY) ? 0.f : sr * expf(mr - m);
+            if (soft && mr != -INFINITY) aw = fmaf(sw, m - mr, aw);
+
         } else {
             for (int64_t c = lane; c < C; c += 32) m = fmaxf(m, ldf<OT>(t.out, r0 + c));
             m = warp_max(m);
@@ -199,16 +237,41 @@ __device__ __forceinline__ void ce_partial(const frl_task_desc& t, int blk, int 
                 const float x = ldf<OT>(t.out, r0 + c);
                 has_nan |= (x != x);
                 se += expf(x - m);
+                if (soft) {
+                    const float w = soft_w(t, prob, r0, c, ys, keep, eps_c);
+                    aw = fmaf(w, m - x, aw);
+                    sw += w;
+                }
             }
         }
         se = warp_sum(se);
         has_nan = __any_sync(0xffffffffu, has_nan);
         float lse = m + logf(se);
         if (has_nan) lse = __int_as_float(0x7fc00000);   // fmaxf drops NaNs; keep them visible
+        if (soft) {
+            aw = warp_sum(aw);
+            sw = warp_sum(sw);
+        }
         if (lane == 0) {
             lse_out[row] = lse;
             const bool sel = (t.mask == nullptr) || (t.mask[row] != 0);
-            if (sel) {
+            if (prob) {
+                lse_out[t.rows + row] = sw;          // the backward's softmax factor
+                if (sel) {
+                    s_sel += 1.f;
+                    s_valid += 1.f;
+                    s_loss += has_nan ? __int_as_float(0x7fc00000) : fmaf(sw, logf(se), aw);
+                }
+            } else if (soft) {
+                if (sel) {
+                    s_sel += 1.f;
+                    if (ys != static_cast<int64_t>(t.ignore_index)) {
+                        s_valid += 1.f;
+                        s_loss += (ys >= 0 && ys < C && !has_nan) ? fmaf(sw, logf(se), aw)
+                                                                 : __int_as_float(0x7fc00000);
+                    }
+                }
+            } else if (sel) {
                 s_sel += 1.f;
                 const int64_t y = labels[row];
                 if (y != static_cast<int64_t>(t.ignore_index)) {
@@ -224,6 +287,8 @@ __device__ __forceinline__ void ce_partial(const frl_task_desc& t, int blk, int 
     nvalid = s_valid;
 }
 
+// SOFT = false: no task has soft rows, and the kernel is the one that ran before soft targets
+template <bool SOFT>
 __global__ void __launch_bounds__(kCThreads, 5)
 criteria_fwd_kernel(const __grid_constant__ CritParams P, float* __restrict__ losses,
                     float* __restrict__ aux, float* __restrict__ lse,
@@ -249,8 +314,8 @@ criteria_fwd_kernel(const __grid_constant__ CritParams P, float* __restrict__ lo
         nvalid = nsel;
     } else {
         float* lse_t = lse + P.lse_off[ti];
-        if (t.out_dtype == FRL_F32) ce_partial<float>(t, blk, P.nblk[ti], lse_t, s, nsel, nvalid);
-        else                        ce_partial<__nv_bfloat16>(t, blk, P.nblk[ti], lse_t, s, nsel, nvalid);
+        if (t.out_dtype == FRL_F32) ce_partial<float, SOFT>(t, blk, P.nblk[ti], lse_t, s, nsel, nvalid);
+        else                        ce_partial<__nv_bfloat16, SOFT>(t, blk, P.nblk[ti], lse_t, s, nsel, nvalid);
     }
     s = block_sum(s, smem);
     nsel = block_sum(nsel, smem);
@@ -296,7 +361,9 @@ criteria_fwd_kernel(const __grid_constant__ CritParams P, float* __restrict__ lo
             if (q.mask != nullptr && dsel == 0.0) {
                 // reference MaskedLoss with an empty mask: inner(out-out, tgt-tgt).  tgt-tgt makes
                 // every CE label 0, so with ignore_index == 0 every row is ignored: 0/0 = NaN
+                // (CE_PROB: every q is 0, so q' = eps/C and the loss is eps * log C)
                 if (q.kind == FRL_LOSS_MSE)     Li = 0.f;
+                else if (SOFT && q.kind == FRL_LOSS_CE_PROB) Li = q.label_smoothing * logf(static_cast<float>(q.cols));
                 else if (q.ignore_index == 0)   Li = __int_as_float(0x7fc00000);
                 else                            Li = logf(static_cast<float>(q.cols));
             } else {
@@ -332,22 +399,56 @@ __device__ __forceinline__ void mse_bwd(const frl_task_desc& t, int blk, int nbl
     }
 }
 
-template <typename OT>
+template <typename OT, bool SOFT>
 __device__ __forceinline__ void ce_bwd(const frl_task_desc& t, int blk, int nblk, const float* lse,
                                        float coef) {
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
     const int64_t C = t.cols;
     const bool vec = vec_ok(t);
     const int64_t* labels = static_cast<const int64_t*>(t.tgt);
+    // soft rows: d/dx = (softmax * sum(q') - q') * coef, sum(q') = 1 for a class index
+    const bool prob = SOFT && t.kind == FRL_LOSS_CE_PROB;
+    const bool soft = SOFT && (prob || t.label_smoothing != 0.f);
+    const float keep = 1.f - t.label_smoothing, eps_c = t.label_smoothing / static_cast<float>(C);
     for (int64_t row = static_cast<int64_t>(blk) * kCWarps + warp; row < t.rows;
          row += static_cast<int64_t>(nblk) * kCWarps) {
         const int64_t r0 = row * C;
-        const int64_t y = labels[row];
+        const int64_t y = prob ? -1 : labels[row];
         const bool use = ((t.mask == nullptr) || (t.mask[row] != 0)) &&
-                         (y != static_cast<int64_t>(t.ignore_index));
+                         (prob || y != static_cast<int64_t>(t.ignore_index));
         const float k = use ? coef : 0.f;
         const float l = lse[row];
-        if (vec) {
+        if (soft) {
+            const float sq = prob ? lse[t.rows + row] : 1.f;
+            if (vec) {
+                for (int64_t cb = 0; cb < C; cb += kCRowChunk) {
+                    f32x4 v[kCVecPerLane];
+#pragma unroll
+                    for (int j = 0; j < kCVecPerLane; ++j) {
+                        const int64_t c = cb + lane * 4 + j * 128;
+                        if (c < C) v[j] = ld4<OT>(t.out, r0 + c);
+                    }
+#pragma unroll
+                    for (int j = 0; j < kCVecPerLane; ++j) {
+                        const int64_t c = cb + lane * 4 + j * 128;
+                        if (c >= C) break;
+                        f32x4 q = v[j];
+                        q.x = (expf(q.x - l) * sq - soft_w(t, prob, r0, c + 0, y, keep, eps_c)) * k;
+                        q.y = (expf(q.y - l) * sq - soft_w(t, prob, r0, c + 1, y, keep, eps_c)) * k;
+                        q.z = (expf(q.z - l) * sq - soft_w(t, prob, r0, c + 2, y, keep, eps_c)) * k;
+                        q.w = (expf(q.w - l) * sq - soft_w(t, prob, r0, c + 3, y, keep, eps_c)) * k;
+                        if (!use) q = f32x4{0.f, 0.f, 0.f, 0.f};
+                        st4<OT>(t.dout, r0 + c, q);
+                    }
+                }
+            } else {
+                for (int64_t c = lane; c < C; c += 32) {
+                    const float x = ldf<OT>(t.out, r0 + c);
+                    stf<OT>(t.dout, r0 + c,
+                            use ? (expf(x - l) * sq - soft_w(t, prob, r0, c, y, keep, eps_c)) * k : 0.f);
+                }
+            }
+        } else if (vec) {
             for (int64_t cb = 0; cb < C; cb += kCRowChunk) {
                 f32x4 v[kCVecPerLane];
 #pragma unroll
@@ -377,6 +478,7 @@ __device__ __forceinline__ void ce_bwd(const frl_task_desc& t, int blk, int nblk
     }
 }
 
+template <bool SOFT>
 __global__ void __launch_bounds__(kCThreads, 5)
 criteria_bwd_kernel(const __grid_constant__ CritParams P, const float* __restrict__ gl,
                     const float* __restrict__ aux, const float* __restrict__ lse) {
@@ -393,22 +495,28 @@ criteria_bwd_kernel(const __grid_constant__ CritParams P, const float* __restric
         else                        mse_bwd<__nv_bfloat16>(t, blk, P.nblk[ti], coef);
     } else {
         const float* lse_t = lse + P.lse_off[ti];
-        if (t.out_dtype == FRL_F32) ce_bwd<float>(t, blk, P.nblk[ti], lse_t, scale);
-        else                        ce_bwd<__nv_bfloat16>(t, blk, P.nblk[ti], lse_t, scale);
+        if (t.out_dtype == FRL_F32) ce_bwd<float, SOFT>(t, blk, P.nblk[ti], lse_t, scale);
+        else                        ce_bwd<__nv_bfloat16, SOFT>(t, blk, P.nblk[ti], lse_t, scale);
     }
 }
 
 static int build_params(const frl_task_desc* tasks, int T, bool backward, CritParams& P, int& max_blk,
-                        const char* name) {
+                        bool& soft, const char* name) {
     FRL_REQUIRE(tasks != nullptr && T >= 1, FRL_E_ARG, "%s: no tasks", name);
     FRL_REQUIRE(T <= FRL_MAX_TASKS, FRL_E_TOO_MANY, "%s: at most %d tasks", name, FRL_MAX_TASKS);
     int off = 0;
     int64_t lse_off = 0;
     max_blk = 1;
+    soft = false;
     P.n_tasks = T;
     for (int i = 0; i < T; ++i) {
         const frl_task_desc& t = tasks[i];
-        FRL_REQUIRE(t.kind == FRL_LOSS_MSE || t.kind == FRL_LOSS_CE, FRL_E_ARG, "%s: task %d kind", name, i);
+        FRL_REQUIRE(t.kind == FRL_LOSS_MSE || t.kind == FRL_LOSS_CE || t.kind == FRL_LOSS_CE_PROB, FRL_E_ARG,
+                    "%s: task %d kind", name, i);
+        FRL_REQUIRE(t.label_smoothing >= 0.f && t.label_smoothing <= 1.f, FRL_E_ARG,
+                    "%s: task %d label_smoothing must be in [0, 1], got %g", name, i, t.label_smoothing);
+        FRL_REQUIRE(t.kind != FRL_LOSS_MSE || t.label_smoothing == 0.f, FRL_E_ARG,
+                    "%s: task %d label_smoothing on an MSE task", name, i);
         FRL_REQUIRE(t.out_dtype == FRL_F32 || t.out_dtype == FRL_BF16, FRL_E_DTYPE, "%s: task %d out dtype", name, i);
         FRL_REQUIRE(t.rows >= 0 && t.cols >= 1, FRL_E_ARG, "%s: task %d shape", name, i);
         FRL_REQUIRE(t.rows == 0 || (t.out && t.tgt), FRL_E_ARG, "%s: task %d null out/tgt", name, i);
@@ -416,10 +524,15 @@ static int build_params(const frl_task_desc* tasks, int T, bool backward, CritPa
         if (t.kind == FRL_LOSS_MSE) {
             FRL_REQUIRE(t.tgt_dtype == FRL_F32 || t.tgt_dtype == FRL_BF16, FRL_E_DTYPE, "%s: task %d tgt dtype", name, i);
             FRL_REQUIRE(!t.mask || t.mask_inner >= 1, FRL_E_ARG, "%s: task %d mask_inner", name, i);
+        } else if (t.kind == FRL_LOSS_CE_PROB) {
+            FRL_REQUIRE(t.tgt_dtype == FRL_F32 || t.tgt_dtype == FRL_BF16, FRL_E_DTYPE,
+                        "%s: task %d CE probability targets must be FRL_F32 or FRL_BF16", name, i);
+            FRL_REQUIRE(!t.mask || t.mask_inner == t.cols, FRL_E_ARG, "%s: task %d CE mask is per row", name, i);
         } else {
             FRL_REQUIRE(t.tgt_dtype == FRL_I64, FRL_E_DTYPE, "%s: task %d CE labels must be int64", name, i);
             FRL_REQUIRE(!t.mask || t.mask_inner == t.cols, FRL_E_ARG, "%s: task %d CE mask is per row", name, i);
         }
+        soft |= t.kind == FRL_LOSS_CE_PROB || t.label_smoothing != 0.f;
         P.t[i] = t;
         int64_t work_blocks;
         if (t.kind == FRL_LOSS_MSE) work_blocks = (t.rows * t.cols + kCThreads * 8 - 1) / (kCThreads * 8);
@@ -431,6 +544,7 @@ static int build_params(const frl_task_desc* tasks, int T, bool backward, CritPa
         off += kCMaxBlocksPerTask;
         P.lse_off[i] = lse_off;
         if (t.kind == FRL_LOSS_CE) lse_off += t.rows;
+        if (t.kind == FRL_LOSS_CE_PROB) lse_off += 2 * t.rows;     // lse, then sum(q') per row
         if (P.nblk[i] > max_blk) max_blk = P.nblk[i];
     }
     int total = 0;
@@ -456,15 +570,18 @@ extern "C" int frl_criteria_forward(const frl_task_desc* tasks_host, int n_tasks
                                     int32_t* nan_flag_mapped, void* scratch, void* stream) {
     CritParams P;
     int max_blk = 1;
-    const int rc = build_params(tasks_host, n_tasks, false, P, max_blk, "frl_criteria_forward");
+    bool soft = false;
+    const int rc = build_params(tasks_host, n_tasks, false, P, max_blk, soft, "frl_criteria_forward");
     if (rc) return rc;
     FRL_REQUIRE(losses && aux && scratch, FRL_E_ARG, "frl_criteria_forward: null outputs");
     bool any_ce = false;
-    for (int i = 0; i < n_tasks; ++i) any_ce |= (tasks_host[i].kind == FRL_LOSS_CE);
+    for (int i = 0; i < n_tasks; ++i) any_ce |= (tasks_host[i].kind != FRL_LOSS_MSE);
     FRL_REQUIRE(!any_ce || lse, FRL_E_ARG, "frl_criteria_forward: CE task needs lse buffer");
     const int grid = P.total_blocks;        // one CTA per unit of work: no empty CTAs, one wave
-    criteria_fwd_kernel<<<grid, kCThreads, 0, static_cast<cudaStream_t>(stream)>>>(
-        P, losses, aux, lse, sink_mapped, nan_flag_mapped, static_cast<CritScratchHeader*>(scratch));
+    cudaStream_t st = static_cast<cudaStream_t>(stream);
+    CritScratchHeader* hdr = static_cast<CritScratchHeader*>(scratch);
+    if (soft) criteria_fwd_kernel<true><<<grid, kCThreads, 0, st>>>(P, losses, aux, lse, sink_mapped, nan_flag_mapped, hdr);
+    else      criteria_fwd_kernel<false><<<grid, kCThreads, 0, st>>>(P, losses, aux, lse, sink_mapped, nan_flag_mapped, hdr);
     return after_launch("frl_criteria_forward");
 }
 
@@ -473,10 +590,13 @@ extern "C" int frl_criteria_backward(const frl_task_desc* tasks_host, int n_task
                                      void* stream) {
     CritParams P;
     int max_blk = 1;
-    const int rc = build_params(tasks_host, n_tasks, true, P, max_blk, "frl_criteria_backward");
+    bool soft = false;
+    const int rc = build_params(tasks_host, n_tasks, true, P, max_blk, soft, "frl_criteria_backward");
     if (rc) return rc;
     FRL_REQUIRE(grad_losses && aux, FRL_E_ARG, "frl_criteria_backward: null inputs");
     const int grid = P.total_blocks;
-    criteria_bwd_kernel<<<grid, kCThreads, 0, static_cast<cudaStream_t>(stream)>>>(P, grad_losses, aux, lse);
+    cudaStream_t st = static_cast<cudaStream_t>(stream);
+    if (soft) criteria_bwd_kernel<true><<<grid, kCThreads, 0, st>>>(P, grad_losses, aux, lse);
+    else      criteria_bwd_kernel<false><<<grid, kCThreads, 0, st>>>(P, grad_losses, aux, lse);
     return after_launch("frl_criteria_backward");
 }

@@ -216,8 +216,9 @@ def _task_classes(ns):
 
     class ClassificationTask(ns.Task):
         def __init__(self, in_dim: int, n_classes: int, weight: float, field: str = "y_cls",
-                     name: str = "cls") -> None:
+                     name: str = "cls", label_smoothing: float = 0.0) -> None:
             self._in, self._out, self._w, self._field, self.name = in_dim, n_classes, weight, field, name
+            self.label_smoothing = float(label_smoothing)
 
         @property
         def network_head(self) -> nn.Module:
@@ -225,7 +226,7 @@ def _task_classes(ns):
 
         @property
         def criterion(self):
-            return nn.CrossEntropyLoss()
+            return nn.CrossEntropyLoss(label_smoothing=self.label_smoothing)
 
         @property
         def criterion_weight(self) -> float:
@@ -235,7 +236,10 @@ def _task_classes(ns):
             return (tensors[self._field],), NoMeta()
 
         def compute_batch_metrics(self, meta, target, output):
-            wrong = (output.argmax(1) != target[0]).float()
+            y = target[0]
+            if y.is_floating_point() and y.dim() == 2:
+                y = y.argmax(1)           # mixed (probability) targets: the dominant class
+            wrong = (output.argmax(1) != y).float()
             return {self.name + "_err": wrong if wrong.is_cuda else wrong.numpy()}
 
         @property
@@ -456,7 +460,8 @@ def resnet_fields(n: int, image: int, heads, seed: int, uint8: bool = False) -> 
 def make_resnet_problem(ns, save_dir: str, config: str = "resnet18", image: int = 224,
                         n_train: int = 64, n_test: int = 0, pinned: bool = False,
                         uint8: bool = False, augment: Optional[str] = None,
-                        stored_image: Optional[int] = None):
+                        stored_image: Optional[int] = None, mixup_alpha: float = 0.0,
+                        cutmix_alpha: float = 0.0, label_smoothing: float = 0.0):
     """Configs 4/5: a torchvision ResNet trunk (its ``fc`` removed) behind
     ``ListSelect`` and one ``nn.Linear`` head per task; x ~ N(0,1) of shape [3, image, image], or
     (``uint8``) raw 8-bit images normalised per channel by the transform (150 kB/sample over
@@ -466,13 +471,23 @@ def make_resnet_problem(ns, save_dir: str, config: str = "resnet18", image: int 
     ``"pad_crop"`` (crop of the image zero-padded by 4 + flip, CIFAR-style) on the device
     (``transform.DeviceImageAugment``, K5a) from stored ``stored_image`` x ``stored_image`` images
     to the model's ``image`` x ``image``; evaluation splits take the centre crop.  The datasets are
-    then pinned; their per-sample transform serves the evaluation splits only."""
+    then pinned; their per-sample transform serves the evaluation splits only.
+    ``mixup_alpha`` / ``cutmix_alpha`` (need ``augment``): Mixup / CutMix of the training batches
+    (``transform.BatchMix`` over every head's target field) in the augmentation pass.
+    ``label_smoothing``: the classification heads' ``CrossEntropyLoss(label_smoothing=...)``."""
     import torchvision
     stored = image if stored_image is None else int(stored_image)
     if augment is None and stored != image:
         raise ValueError("stored_image differs from image only for an augmenting Problem (augment=...)")
     arch, heads = RESNET_CONFIGS[config]
     aug = None
+    mix = None
+    if mixup_alpha or cutmix_alpha:
+        from .transform import BatchMix
+        if augment is None:
+            raise ValueError("mixup_alpha / cutmix_alpha mix on the device augmentation path: pass augment=...")
+        mix = BatchMix({field: dim for kind, dim, field, _ in heads if kind == "cls"},
+                       mixup_alpha=mixup_alpha, cutmix_alpha=cutmix_alpha)
     if augment is not None:
         from .transform import DeviceImageAugment
         if not uint8:
@@ -480,11 +495,12 @@ def make_resnet_problem(ns, save_dir: str, config: str = "resnet18", image: int 
         if augment not in DeviceImageAugment.MODES:
             raise ValueError(f"augment must be None or one of {DeviceImageAugment.MODES}, got {augment!r}")
         aug = DeviceImageAugment("x", [field for _, _, field, _ in heads], mode=augment, out_size=image, pad=4,
-                                 scale=U8_CHANNEL_AFFINE[0], bias=U8_CHANNEL_AFFINE[1])
+                                 scale=U8_CHANNEL_AFFINE[0], bias=U8_CHANNEL_AFFINE[1], mix=mix)
         aug.check_image(3, stored, stored)
     feat = {"resnet18": 512, "resnet50": 2048}[arch]
     Reg, Cls = _task_classes(ns)
-    tasks = [(Cls if kind == "cls" else Reg)(feat, dim, 1.0, field=field, name=name)
+    tasks = [Cls(feat, dim, 1.0, field=field, name=name, label_smoothing=label_smoothing) if kind == "cls"
+             else Reg(feat, dim, 1.0, field=field, name=name)
              for kind, dim, field, name in heads]
 
     def base_factory() -> nn.Module:

@@ -222,28 +222,40 @@ int frl_grad_sumsq_clip(const void* g, int64_t n, int g_dtype, float pre_scale, 
  * 569).
  * A task whose mask selects nothing gives the reference's inner(out - out, tgt - tgt): 0 for MSE,
  * log C for CE, or NaN for CE with ignore_index == 0 (every label of tgt - tgt is 0, so every
- * row is ignored), with a zero gradient.  Two differences remain, both only with non-finite
- * outputs: the reference's out - out is NaN where an output is inf or NaN, which makes that loss
- * NaN, but the kernels never read a masked-out output, so they still give 0 / log C; and torch's
- * gradient of a NaN row whose label is ignore_index is NaN, where the kernels write 0.
+ * row is ignored), eps * log C for CE_PROB, with a zero gradient.  Two differences remain, both
+ * only with non-finite outputs: the reference's out - out is NaN where an output is inf or NaN,
+ * which makes that loss NaN, but the kernels never read a masked-out output, so they still give
+ * 0 / log C; and torch's gradient of a NaN row whose label is ignore_index is NaN, where the
+ * kernels write 0.
+ * Cross-entropy with label smoothing eps (torch's F.cross_entropy, mean reduction; x a row's
+ * logits, lse its log-sum-exp, C = cols):
+ *   FRL_LOSS_CE, class index y:  row loss = lse - (1-eps) x_y - (eps/C) sum_c x_c, summed over the
+ *     selected rows whose label is not ignore_index and divided by their count;
+ *     gradient = (softmax - (1-eps) e_y - eps/C) * coef.
+ *   FRL_LOSS_CE_PROB, probabilities q (rows not renormalised), q' = (1-eps) q + eps/C:
+ *     row loss = sum_c q'_c (lse - x_c), divided by the number of selected rows;
+ *     gradient = (softmax * sum_c q'_c - q') * coef.
+ *   With eps == 0 and class indices the kernels compute what they computed before soft targets.
+ * Left to the caller's composed torch ops: class weights, and per-position probability targets.
  * ---------------------------------------------------------------------------------------- */
 #define FRL_MAX_TASKS 8
-enum { FRL_LOSS_MSE = 0, FRL_LOSS_CE = 1 };
+enum { FRL_LOSS_MSE = 0, FRL_LOSS_CE = 1, FRL_LOSS_CE_PROB = 2 };
 
 typedef struct frl_task_desc {
-    int32_t     kind;         /* FRL_LOSS_MSE | FRL_LOSS_CE */
+    int32_t     kind;         /* FRL_LOSS_MSE | FRL_LOSS_CE | FRL_LOSS_CE_PROB */
     int32_t     out_dtype;    /* FRL_F32 | FRL_BF16 : dtype of `out` (and of `dout`) */
-    int32_t     tgt_dtype;    /* MSE: FRL_F32 | FRL_BF16 ; CE: FRL_I64 */
+    int32_t     tgt_dtype;    /* MSE, CE_PROB: FRL_F32 | FRL_BF16 ; CE: FRL_I64 */
     int32_t     ignore_index; /* CE only (torch default -100) */
     const void* out;          /* model output  [rows, cols] row-major contiguous */
-    const void* tgt;          /* MSE: [rows, cols] ; CE: int64 class index [rows] */
-    const uint8_t* mask;      /* optional (MaskedLoss): nonzero = use ; numel = rows*cols/mask_inner */
+    const void* tgt;          /* MSE, CE_PROB: [rows, cols] ; CE: int64 class index [rows] */
+    const uint8_t* mask;      /* optional (MaskedLoss): nonzero = use ; numel = rows*cols/mask_inner
+                                 (CE / CE_PROB: one entry per row) */
     void*       dout;         /* backward only: gradient wrt out, same shape/dtype as out */
     int64_t     rows;
     int64_t     cols;
     int64_t     mask_inner;   /* elements of `out` covered by one mask entry (1 or cols ...) */
     float       weight;       /* loss weight w_i */
-    float       _pad;
+    float       label_smoothing;  /* eps in [0, 1], CE / CE_PROB only (0 for MSE) */
 } frl_task_desc;
 
 /* scratch bytes for T tasks (partials + ticket); zero-initialise once */
@@ -251,9 +263,14 @@ int64_t frl_criteria_scratch_bytes(int n_tasks);
 
 /* forward: losses[0] = sum_i w_i*L_i (left-to-right), losses[1+i] = w_i*L_i.
  *   aux[i]      = 1/count_i (0 if nothing selected) for the backward
- *   lse[...]    = per-row log-sum-exp of every CE task, rows concatenated in task order
+ *   lse[...]    = per-row slots of every CE / CE_PROB task, in task order: rows floats (the
+ *                 log-sum-exp) for a CE task, 2 * rows for a CE_PROB task (the log-sum-exp of
+ *                 every row, then sum_c q'_c of every row); sum(rows) + sum(rows of CE_PROB) in all
  *   sink_mapped = optional second destination of losses[0..T] (e.g. a row of a pinned loss
- *                 log), nan_flag_mapped = optional int set to 1 when losses[0] is NaN. */
+ *                 log), nan_flag_mapped = optional int set to 1 when losses[0] is NaN.
+ * Argument errors (before any launch): a kind other than the three, eps outside [0, 1], eps != 0
+ * on an MSE task, a CE_PROB target that is not FRL_F32 / FRL_BF16, a CE / CE_PROB mask that is
+ * not per row. */
 int frl_criteria_forward(const frl_task_desc* tasks_host, int n_tasks,
                          float* losses, float* aux, float* lse,
                          float* sink_mapped, int32_t* nan_flag_mapped,
@@ -320,6 +337,38 @@ int frl_augment_images(const void* src, int64_t batch, int channels, int height,
                        double smin, double smax, double rmin, double rmax, double eval_crop, int pad,
                        int flip, const float* scale, const float* bias, void* dst, int dst_dtype,
                        int out_h, int out_w, int32_t* params_out, void* stream);
+
+/* K5a with Mixup / CutMix in the same pass (an extension: the usual large-batch ImageNet recipe,
+ * Zhang et al. 2018 / Yun et al. 2019).  Arguments as frl_augment_images, plus
+ *   mix_mode   FRL_MIX_MIXUP or FRL_MIX_CUTMIX;  lam in [0, 1];  lam1 = 1 - (double)lam rounded once
+ *              to fp32
+ *   box_*      CutMix box [box_y0, box_y1) x [box_x0, box_x1) on the output image (inside it;
+ *              ignored by Mixup)
+ * Sample p is paired with sample j = B-1-p.  With a_p, a_j the fp32 values K5a would round to the
+ * output dtype for the same pixel (the same boxes, drawn as K5a draws them):
+ *   Mixup:  out_p = __fadd_rn(__fmul_rn(lam, a_p), __fmul_rn(lam1, a_j))
+ *   CutMix: out_p = a_j inside the box, a_p outside
+ * and only that final store rounds.  The middle sample of an odd batch, and params_out, are
+ * written exactly as by frl_augment_images.  Grid (ceil(B/2), ceil(out_h/8)): one CTA per pair.
+ *
+ * frl_mix_targets: the target fields of the same batch, one launch per field, partner j = B-1-i.
+ *   src_dtype FRL_I64: src int64 [B] labels of n_classes >= 2 classes (inner must be 1); dst fp32
+ *     [B, n_classes] = lam at y_i plus lam1 at y_j (fp32 adds onto 0); a row whose y_i or y_j lies
+ *     outside [0, n_classes) is NaN, so a NaN-loss check fires without a host read.
+ *   src_dtype FRL_F32 | FRL_BF16: src [B, inner], dst of the same dtype and shape =
+ *     round(__fadd_rn(__fmul_rn(lam, t_i), __fmul_rn(lam1, t_j))).
+ *   lam = 1 gives one-hot rows (labels) and t_i (finite values): the targets of an unmixed batch.
+ * Graph-capturable: no host reads, no allocation.  Every argument check comes before any launch.
+ * ---------------------------------------------------------------------------------------- */
+enum { FRL_MIX_MIXUP = 1, FRL_MIX_CUTMIX = 2 };
+int frl_augment_mix_images(const void* src, int64_t batch, int channels, int height, int width,
+                           const int64_t* idx, uint64_t seed, int epoch, int mode,
+                           double smin, double smax, double rmin, double rmax, double eval_crop, int pad,
+                           int flip, const float* scale, const float* bias, void* dst, int dst_dtype,
+                           int out_h, int out_w, int32_t* params_out, int mix_mode, float lam,
+                           int box_y0, int box_y1, int box_x0, int box_x1, void* stream);
+int frl_mix_targets(const void* src, int src_dtype, int64_t batch, int64_t inner, int n_classes, float lam,
+                    void* dst, void* stream);
 
 /* dtype conversion / scaled copy used by the arena (master -> shadow refresh after a
  * checkpoint load, gradient flatten for modules the arena cannot write into directly):

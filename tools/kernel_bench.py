@@ -372,6 +372,74 @@ def bench_k5a(iters):
                   "bytes: touched source lines of the drawn boxes + output", graph=True)]
 
 
+def bench_k5m(iters):
+    """K5a alone, fused with Mixup and fused with CutMix (frl_augment_mix_images) at the K5a shape,
+    same sets and boxes: the mix reads both samples' taps in one CTA per pair, so its bytes are
+    K5a's (each sample's taps are read once, each output written once)."""
+    B, Cc, S, O = 256, 3, 256, 224
+    ns = sets_for(B * Cc * (S * S + 2 * O * O))
+    src = [torch.randint(0, 256, (B, Cc, S, S), device=DEV, dtype=torch.uint8) for _ in range(ns)]
+    dst = [torch.empty(B, Cc, O, O, device=DEV, dtype=torch.bfloat16) for _ in range(ns)]
+    idx = [torch.arange(B, device=DEV, dtype=torch.int64) + i * B for i in range(ns)]
+    sc, bi = torch.rand(Cc, device=DEV), torch.rand(Cc, device=DEV)
+    params = torch.empty(B, 5, dtype=torch.int32, device=DEV)
+    read = 0
+    for i in range(ns):
+        _native.augment_images(src[i], idx[i], dst[i], seed=0, epoch=1, mode=_native.AUG_RRC, scale=sc, bias=bi,
+                               params_out=params)
+        read += sum(Cc * _taps_touched(int(h), O) * _taps_touched(int(w), O) for h, w in params[:, 2:4].tolist())
+    nbytes = read // ns + B * Cc * O * O * 2
+    kw = dict(seed=0, epoch=1, mode=_native.AUG_RRC, scale=sc, bias=bi)
+    out = [timed("K5a augment_images RRC u8 [256,3,256,256] -> bf16 [256,3,224,224]",
+                 lambda i: _native.augment_images(src[i], idx[i], dst[i], **kw), ns, nbytes, iters,
+                 "bytes: touched source lines of the drawn boxes + output", graph=True)]
+    out.append(timed("K5a + Mixup augment_mix_images (lam 0.7), same shape",
+                     lambda i: _native.augment_mix_images(src[i], idx[i], dst[i], mix_mode=_native.MIX_MIXUP,
+                                                          lam=0.7, **kw), ns, nbytes, iters, "bytes as K5a",
+                     graph=True))
+    out.append(timed("K5a + CutMix augment_mix_images (box 112x112), same shape",
+                     lambda i: _native.augment_mix_images(src[i], idx[i], dst[i], mix_mode=_native.MIX_CUTMIX,
+                                                          lam=0.75, box=(56, 168, 56, 168), **kw),
+                     ns, nbytes, iters, "bytes as K5a", graph=True))
+    return out
+
+
+def bench_k4s(iters):
+    """K4 forward + backward at [4096, 1000] bf16 logits: class indices with eps = 0 and eps = 0.1,
+    fp32 probability targets; beside them the composed torch ops label smoothing took before
+    (F.cross_entropy forward + autograd backward).  Bytes: logits read twice (forward, backward),
+    gradient written once, targets read once per pass (8 B labels or a 4 B-per-class row)."""
+    B, C = 4096, 1000
+    out = []
+    import torch.nn.functional as F
+    for label, eps, prob in (("eps=0", 0.0, False), ("eps=0.1", 0.1, False), ("fp32 probabilities", 0.0, True)):
+        tb = B * C * 4 if prob else B * 8
+        per = 3 * B * C * 2 + 2 * tb + B * 8
+        ns = sets_for(per)
+        mods = [torch.nn.CrossEntropyLoss(label_smoothing=eps)]
+        sets = []
+        for _ in range(ns):
+            lo = torch.randn(B, C, device=DEV).to(torch.bfloat16).requires_grad_(True)
+            tgt = (torch.rand(B, C, device=DEV).softmax(1) if prob else torch.randint(0, C, (B,), device=DEV))
+            sets.append((lo, tgt))
+
+        def step(i):
+            lo, tgt = sets[i]
+            criteria.fused_task_losses(mods, [lo], [(tgt,)])[0].backward()
+            lo.grad = None
+
+        out.append(timed("K4 forward+backward bf16 [4096,1000] CE %s" % label, step, ns, per, iters,
+                         "includes autograd dispatch"))
+        if eps > 0:
+            def composed(i):
+                lo, tgt = sets[i]
+                F.cross_entropy(lo, tgt, label_smoothing=eps).backward()
+                lo.grad = None
+            out.append(timed("composed torch F.cross_entropy forward+backward bf16 [4096,1000] %s" % label,
+                             composed, ns, per, iters, "the path label smoothing took before K4 handled it"))
+    return out
+
+
 def bench_k6(iters):
     out = []
     rows = cols = 4096
@@ -474,7 +542,7 @@ def bench_k9(iters):
 
 
 BENCHES = {"k2": bench_k2, "k2mt": bench_k2mt, "k2lw": bench_k2lw, "k3": bench_k3, "k4": bench_k4, "k5": bench_k5, "k5a": bench_k5a,
-           "k6": bench_k6,
+           "k5m": bench_k5m, "k4s": bench_k4s, "k6": bench_k6,
            "k8": bench_k8, "k8t": bench_k8t, "k9": bench_k9, "k10": bench_k10, "k11": bench_k11}
 
 
