@@ -38,7 +38,10 @@ struct AdamRule {
         m = fmaf(w1, g - m, m);                       // exp_avg.lerp_(g, 1-beta1), weight < 0.5 branch
         v = fmaf(w2 * g, g, v * beta2);               // mul_(beta2).addcmul_(g, g, 1-beta2)
         float vv = v;
-        if (AMSGRAD) { vmax = fmaxf(vmax, v); vv = vmax; }
+        if (AMSGRAD) {                                // torch.maximum: NaN in either operand wins
+            vmax = (v > vmax || v != v) ? v : vmax;   // (fmaxf would drop it)
+            vv = vmax;
+        }
         const float denom = sqrtf(vv) / bc2_sqrt + eps;
         p = fmaf(neg_step_size, m / denom, p);        // addcdiv_(m, denom, -step_size)
     }
