@@ -15,9 +15,7 @@ host with the device:
   always False, reference solver_worker.py:829);
 * one watchdog thread per split is kicked per step instead of spawning a Timer per step.
 """
-import bisect
 from contextlib import contextmanager, nullcontext
-import heapq
 import io
 import os
 import queue
@@ -27,9 +25,8 @@ import json
 import logging
 import random
 import time
-from collections import defaultdict
 from math import ceil
-from typing import Any, DefaultDict, Dict, Iterator, List, NamedTuple, Optional, Sequence, Tuple, Union
+from typing import Any, Dict, Iterator, List, NamedTuple, Optional, Sequence, Tuple, Union
 
 import numpy as np
 import torch
@@ -64,19 +61,6 @@ class SingleSample(NamedTuple):
     meta: Dict[str, Any]
     output: List[torch.Tensor]
     metric: Dict[str, float]
-
-    # heap entries are (score, sample): never let tuple comparison fall through to tensors
-    def __lt__(self, other: Any) -> bool:
-        return False
-
-    def __gt__(self, other: Any) -> bool:
-        return False
-
-    def __eq__(self, other: Any) -> bool:
-        return False
-
-    def __ne__(self, other: Any) -> bool:
-        return True
 
 
 class SerializableSampleSummary(NamedTuple):
@@ -223,7 +207,12 @@ class _MetricWorker:
 
 class SamplerState:
     """Keeps the last few minibatches on the device and folds them into per-sample metrics,
-    a random sample set and the worst-k samples (reference solver_worker.py:189-374)."""
+    a random sample set and the worst-k samples (reference solver_worker.py:189-374).
+
+    Each window is folded by tensor ops on the device of its outputs, whatever the Problem's hook
+    returns: the metrics go into per-split columns, the random picks are row-gathered by
+    host-known positions, the worst-k set is a running buffer merged per window with ``topk``.
+    Nothing is read back until ``finish()`` reads everything at once."""
 
     def __init__(self, problem: Problem, n_samples: int, dataset_len: int,
                  device: torch.device, n_vis: int) -> None:
@@ -234,8 +223,6 @@ class SamplerState:
         n_random = min(max(self._n_vis, MODEL_CONVERSION_TEST_SAMPLE_CT), n_samples)
         self._random_indices = frozenset(random.sample(range(n_samples), n_random))
         self._cur_samples = 0
-        self._random_samples: List[SingleSample] = []
-        self._worst_samples: List[Tuple[float, SingleSample]] = []
         self._rankable_metric, self._ordering = problem.get_rankable_metric()
         self._allow_non_positive_definite = ("MSE" not in self._rankable_metric
                                              and "EucDist" not in self._rankable_metric)
@@ -243,12 +230,11 @@ class SamplerState:
         self._data: List[List[torch.Tensor]] = []
         self._targets: List[List[Tuple[torch.Tensor, ...]]] = []
         self._outputs: List[List[torch.Tensor]] = []
-        self._data_metric: DefaultDict[str, list] = defaultdict(list)
         # Where the fold runs.  The reference calls the Problem's hooks synchronously on the
         # training thread (solver_worker.py:286-312) and so does this loop by default; a hook that
         # returns host arrays then costs one pipeline drain per window.  Two ways around it:
-        #   * the hook returns DEVICE tensors (``_fold_device``): nothing is read back until the
-        #     split ends, the fold stays on the training thread/stream and never blocks it;
+        #   * the hook returns DEVICE tensors (``metrics_on_device``): the fold is pure device
+        #     work, it stays on the training thread/stream and never blocks it;
         #   * the Problem declares ``metric_hooks_thread_safe = True`` (or FRL_B200_ASYNC_METRICS=1):
         #     host-returning hooks run on a worker thread + side stream.  Opt-in, because hooks
         #     that touch the model, global RNGs or backend flags would race with the next steps.
@@ -258,13 +244,16 @@ class SamplerState:
             want_async = "1" if getattr(problem, "metric_hooks_thread_safe", False) else "0"
         if device.type == "cuda" and want_async != "0":
             self._runner = _MetricWorker(device)
-        # device-side state (hooks returning device tensors)
-        self._dev_mode: Optional[bool] = None
-        self._dev_cols: Dict[str, torch.Tensor] = {}
-        self._dev_meta: Dict[str, torch.Tensor] = {}
-        self._host_meta: DefaultDict[str, list] = defaultdict(list)
+        self._dev_mode = False               # the hook returned device tensors (``metrics_on_device``)
+        # per-sample metric columns and meta (tensor columns, or host lists), over the split
+        self._cols: Dict[str, torch.Tensor] = {}
+        self._meta: Dict[str, Union[torch.Tensor, list]] = {}
         self._dev_random: List[Dict[str, Any]] = []
         self._dev_worst: Optional[Dict[str, Any]] = None
+        # filled by finish()
+        self._data_metric: Dict[str, np.ndarray] = {}
+        self._random_samples: List[SingleSample] = []
+        self._worst_samples: List[SingleSample] = []
 
     @staticmethod
     def _cat_metas(metas: List[RawMetas]) -> RawMetas:
@@ -285,22 +274,16 @@ class SamplerState:
         self._outputs.append([t.detach() for t in outputs])
         self._targets.append([tuple(t.detach() for t in head) for head in targets])
 
-    def _one(self, i, data_batches, starts, target, output, meta, sample_metric) -> SingleSample:
-        # the inputs of the retained minibatches are never concatenated (at batch 4096 that is
-        # a 0.3 GB copy per amortisation window for at most a handful of picked samples): find
-        # the minibatch sample ``i`` of the window came from and index into it
-        b = bisect.bisect_right(starts, i) - 1
-        j = i - starts[b]
-        return SingleSample(
-            data=[t[j].cpu() for t in data_batches[b]],
-            target=[tuple(t[i].cpu() for t in head) for head in target],
-            meta={k: None if v is None else v[i] for k, v in meta._asdict().items()},
-            output=[t[i].float().cpu() for t in output],
-            metric={k: v[i] for k, v in sample_metric.items()})
+    @property
+    def metrics_on_device(self) -> bool:
+        """The Problem's hook returned device tensors: folding a window is pure device work
+        (no host read), so it needs no worker thread and can be queued behind the last steps."""
+        return self._dev_mode
 
     def compute_metrics(self) -> None:
-        """Fold the retained minibatches (a 'window') into the split's metrics.  On CUDA the
-        fold runs on the metric thread/stream and this returns at once; ``finish()`` joins."""
+        """Fold the retained minibatches (a 'window') into the split's metrics.  With a metric
+        worker the fold of a host-returning hook runs on its thread/stream and this returns at
+        once; ``finish()`` joins."""
         if not self._data:
             return
         window = (self._metas, self._data, self._outputs, self._targets)
@@ -320,70 +303,8 @@ class SamplerState:
             self._runner.close()
             self._runner = None
 
-    def finish(self) -> None:
-        """All windows folded (re-raises what a fold raised); call before reading results."""
-        if self._runner is not None:
-            self._runner.drain()
-            self._runner.close()
-            self._runner = None
-        if self._dev_mode:
-            self._finish_device()
-
-    def _fold(self, metas, data_batches, outputs, targets) -> None:
-        meta = self._problem.refine_batch_meta(self._cat_metas(metas))
-        n_heads = len(outputs[0])
-        target = [tuple(torch.cat([t[h][j] for t in targets])
-                        for j in range(len(targets[0][h]))) for h in range(n_heads)]
-        output = [torch.cat([o[h] for o in outputs]) for h in range(n_heads)]
-        output = [o.float() if o.dtype == torch.bfloat16 else o for o in output]
-        sizes = [len(d[0]) for d in data_batches]
-        starts = [0] + list(itertools.accumulate(sizes))[:-1]
-        n_group = sum(sizes)
-
-        sample_metric = self._problem.compute_batch_metrics(
-            meta=meta, target=target, output=output, device=self._device)
-        if self._dev_mode is None:
-            self._dev_mode = bool(sample_metric) and all(
-                torch.is_tensor(v) and v.is_cuda for v in sample_metric.values())
-        if self._dev_mode:
-            self._fold_device(meta, data_batches, starts, n_group, target, output, sample_metric)
-            self._cur_samples += n_group
-            return
-        if sample_metric is not None:
-            for k, v in sample_metric.items():
-                self._data_metric[k].append(np.asarray(v))     # joined once, at the epoch's end
-
-        if self._n_vis > 0 and sample_metric is not None:
-            base = self._cur_samples
-            for i in sorted(j - base for j in self._random_indices if base <= j < base + n_group):
-                self._random_samples.append(
-                    self._one(i, data_batches, starts, target, output, meta, sample_metric))
-            # worst-k: only the k most extreme samples of this group can enter the heap
-            scores = np.asarray(sample_metric[self._rankable_metric], dtype=np.float64).copy()
-            valid = np.ones(n_group, dtype=bool) if self._allow_non_positive_definite else scores >= 0
-            if self._ordering == Ordering.DESC:
-                scores = -scores
-            cand = np.flatnonzero(valid)
-            if len(cand) > self._n_vis:
-                top = np.argpartition(scores[cand], len(cand) - self._n_vis)[-self._n_vis:]
-                cand = np.sort(cand[top])
-            for i in cand:
-                score = float(scores[i])
-                if len(self._worst_samples) < self._n_vis:
-                    heapq.heappush(self._worst_samples, (score, self._one(
-                        int(i), data_batches, starts, target, output, meta, sample_metric)))
-                elif score > self._worst_samples[0][0]:
-                    heapq.heappushpop(self._worst_samples, (score, self._one(
-                        int(i), data_batches, starts, target, output, meta, sample_metric)))
-        self._cur_samples += n_group
-
-    # -- device-side fold -----------------------------------------------------------------------
-    # The Problem's hook returned per-sample metrics as DEVICE tensors: they go into
-    # [n_samples] device columns, the random picks are row-gathered by host-known positions, the
-    # worst-k set is kept as running device buffers merged per window with ``topk`` — no
-    # device-to-host read, no host sync until ``finish()`` reads everything back once.
     @staticmethod
-    def _gather_rows(batches: List[torch.Tensor], starts: List[int], idx: torch.Tensor) -> torch.Tensor:
+    def _gather_rows(batches: List[torch.Tensor], idx: torch.Tensor) -> torch.Tensor:
         """Rows ``idx`` (device int64, window-relative) of the retained minibatch list.  The host
         does not know ``idx`` (it comes out of a device ``topk``) and the minibatches are separate
         tensors: K8w (``frl_gather_window_rows``) walks a table of their base pointers — one launch,
@@ -393,48 +314,48 @@ class SamplerState:
             return _native.gather_window_rows([b if b.is_contiguous() else b.contiguous() for b in batches], idx)
         return (batches[0] if len(batches) == 1 else torch.cat(batches)).index_select(0, idx)
 
-    def _pick(self, idx: torch.Tensor, data_batches, starts, target, output, meta, sample_metric):
+    def _pick(self, idx: torch.Tensor, base: int, data_batches, target, output) -> Dict[str, Any]:
         """Rows ``idx`` (window-relative, device) of everything a ``SingleSample`` shows; metrics
         and meta are looked up by global position from the per-split columns at the end."""
         n_fields = len(data_batches[0])
-        return {"pos": idx + self._cur_samples,
-                "data": [self._gather_rows([d[f] for d in data_batches], starts, idx) for f in range(n_fields)],
+        return {"pos": idx + base,
+                "data": [self._gather_rows([d[f] for d in data_batches], idx) for f in range(n_fields)],
                 "target": [tuple(t.index_select(0, idx) for t in head) for head in target],
                 "output": [o.index_select(0, idx) for o in output]}
 
-    @staticmethod
-    def _cat_picks(a, b):
-        return {"pos": torch.cat([a["pos"], b["pos"]]),
-                "data": [torch.cat([x, y]) for x, y in zip(a["data"], b["data"])],
-                "target": [tuple(torch.cat([x, y]) for x, y in zip(ha, hb))
-                           for ha, hb in zip(a["target"], b["target"])],
-                "output": [torch.cat([x, y]) for x, y in zip(a["output"], b["output"])]}
+    def _fold(self, metas, data_batches, outputs, targets) -> None:
+        meta = self._problem.refine_batch_meta(self._cat_metas(metas))
+        n_heads = len(outputs[0])
+        target = [tuple(torch.cat([t[h][j] for t in targets])
+                        for j in range(len(targets[0][h]))) for h in range(n_heads)]
+        output = [torch.cat([o[h] for o in outputs]) for h in range(n_heads)]
+        output = [o.float() if o.dtype == torch.bfloat16 else o for o in output]
+        base, n_group, dev = self._cur_samples, sum(len(d[0]) for d in data_batches), output[0].device
+        self._cur_samples += n_group
 
-    @staticmethod
-    def _take(p, sel):
-        return {"pos": p["pos"].index_select(0, sel),
-                "data": [x.index_select(0, sel) for x in p["data"]],
-                "target": [tuple(x.index_select(0, sel) for x in head) for head in p["target"]],
-                "output": [x.index_select(0, sel) for x in p["output"]]}
-
-    def _fold_device(self, meta, data_batches, starts, n_group, target, output, sample_metric) -> None:
-        base, dev = self._cur_samples, self._device
-        for k, v in sample_metric.items():
-            col = self._dev_cols.get(k)
-            if col is None:
-                col = self._dev_cols[k] = torch.zeros(self._n_samples, dtype=torch.float32, device=dev)
-            col[base:base + n_group] = v.reshape(n_group).float()
+        sample_metric = self._problem.compute_batch_metrics(
+            meta=meta, target=target, output=output, device=self._device)
         for k, v in meta._asdict().items():
-            if v is None:
-                continue
-            if torch.is_tensor(v) and v.is_cuda:
-                col = self._dev_meta.get(k)
+            if torch.is_tensor(v):
+                col = self._meta.get(k)
                 if col is None:
-                    col = self._dev_meta[k] = torch.zeros((self._n_samples,) + tuple(v.shape[1:]),
-                                                          dtype=v.dtype, device=dev)
+                    col = self._meta[k] = torch.zeros((self._n_samples,) + tuple(v.shape[1:]),
+                                                      dtype=v.dtype, device=v.device)
                 col[base:base + n_group] = v
-            else:            # host-side meta (names, ids as lists / CPU tensors): kept for the split
-                self._host_meta[k].extend(v.tolist() if torch.is_tensor(v) else list(v))
+            else:            # names, ids as lists; a None field stays None per sample
+                self._meta.setdefault(k, []).extend([None] * n_group if v is None else v)
+        if not sample_metric:
+            return
+        self._dev_mode = all(torch.is_tensor(v) and v.is_cuda for v in sample_metric.values())
+        for k, v in sample_metric.items():
+            # host arrays are uploaded (a few KB: the hook has just synchronised to produce them)
+            v = torch.as_tensor(v, device=dev).reshape(n_group)
+            if v.dtype in (torch.bfloat16, torch.float16):
+                v = v.float()
+            col = self._cols.get(k)
+            if col is None:
+                col = self._cols[k] = torch.zeros(self._n_samples, dtype=v.dtype, device=dev)
+            col[base:base + n_group] = v
         if self._n_vis <= 0:
             return
         picks = sorted(j - base for j in self._random_indices if base <= j < base + n_group)
@@ -442,38 +363,37 @@ class SamplerState:
             # a few int64s from pageable memory: the driver stages them, the host does not wait
             # for the device (a pinned allocation here would cost a system call)
             idx = torch.tensor(picks, dtype=torch.int64, device=dev)
-            self._dev_random.append(self._pick(idx, data_batches, starts, target, output, meta, sample_metric))
-        # worst-k of this window, merged into the running set: all on the device
-        scores = sample_metric[self._rankable_metric].reshape(n_group).float()
-        if self._ordering == Ordering.DESC:
-            valid = torch.ones_like(scores, dtype=torch.bool) if self._allow_non_positive_definite else scores >= 0
-            scores = -scores
-        else:
-            valid = torch.ones_like(scores, dtype=torch.bool) if self._allow_non_positive_definite else scores >= 0
-        scores = torch.where(valid, scores, torch.full_like(scores, float("-inf")))
-        k = min(self._n_vis, n_group)
-        top_scores, top_idx = torch.topk(scores, k)
-        cand = self._pick(top_idx, data_batches, starts, target, output, meta, sample_metric)
-        cand["score"] = top_scores
-        if self._dev_worst is None:
-            self._dev_worst = cand
-        else:
-            merged = self._cat_picks(self._dev_worst, cand)
-            merged_scores = torch.cat([self._dev_worst["score"], top_scores])
-            keep_scores, sel = torch.topk(merged_scores, min(self._n_vis, merged_scores.numel()))
-            self._dev_worst = self._take(merged, sel)
-            self._dev_worst["score"] = keep_scores
+            self._dev_random.append(self._pick(idx, base, data_batches, target, output))
+        # worst-k of this window, merged into the running set, ranked in float64
+        metric = self._cols[self._rankable_metric][base:base + n_group].double()
+        valid = (torch.ones_like(metric, dtype=torch.bool) if self._allow_non_positive_definite
+                 else metric >= 0)
+        score = -metric if self._ordering == Ordering.DESC else metric
+        # every valid sample outranks every invalid one, also a valid one that ranks as -inf
+        score = torch.where(valid, score.clamp(min=torch.finfo(torch.float64).min), float("-inf"))
+        top_score, top_idx = torch.topk(score, min(self._n_vis, n_group))
+        cand = self._pick(top_idx, base, data_batches, target, output)
+        cand["score"], cand["valid"] = top_score, valid.index_select(0, top_idx)
+        if self._dev_worst is not None:
+            merged = _tree_map(lambda a, b: torch.cat([a, b]), self._dev_worst, cand)
+            sel = torch.topk(merged["score"], min(self._n_vis, merged["score"].numel()))[1]
+            cand = _tree_map(lambda t: t.index_select(0, sel), merged)
+        self._dev_worst = cand
 
-    def _finish_device(self) -> None:
-        """The split's single device-to-host read: metric columns, the picks, the worst-k set —
-        every copy issued asynchronously into pinned memory, ONE stream synchronisation."""
+    def finish(self) -> None:
+        """All windows folded (re-raises what a fold raised); call before reading results.
+
+        The split's single device-to-host read: metric columns, meta, the picks, the worst-k
+        set — every copy issued asynchronously into pinned memory, ONE stream synchronisation."""
+        if self._runner is not None:
+            self._runner.drain()
+            self._runner.close()
+            self._runner = None
         pending: List[Tuple[torch.Tensor, torch.Tensor]] = []
         requests: List[torch.Tensor] = []
 
         def host(t: torch.Tensor) -> int:
             """Queue ``t`` for the read-back; returns its ticket."""
-            if t.dtype == torch.bfloat16:
-                t = t.float()
             requests.append(t.contiguous())
             return len(requests) - 1
 
@@ -498,25 +418,20 @@ class SamplerState:
             if total == 0:
                 return [torch.empty(t.shape, dtype=t.dtype) for t in requests]
             packed = torch.cat(parts)
-            # (host tensors only when a test drives the fold logic without a device)
+            # (host tensors only when the fold ran without a device)
             stage = _pinned_block(total) if packed.is_cuda else torch.empty(total, dtype=torch.uint8)
             stage[:total].copy_(packed, non_blocking=True)
             pending.append((stage, packed))               # keep the source alive until the sync
             return [stage[o:o + t.numel() * t.element_size()].view(t.dtype).view(t.shape)
                     for t, o in zip(requests, offs)]
 
-        def host_pick(p):
-            return {"pos": host(p["pos"]), "data": [host(x) for x in p["data"]],
-                    "target": [tuple(host(x) for x in head) for head in p["target"]],
-                    "output": [host(x) for x in p["output"]],
-                    "score": host(p["score"]) if "score" in p else None}
-
         t_begin = time.perf_counter()
         n = self._cur_samples
-        cols_h = {k: host(v[:n]) for k, v in self._dev_cols.items()}
-        meta_h = {k: host(v[:n]) for k, v in self._dev_meta.items()}
-        random_h = [host_pick(p) for p in self._dev_random]
-        worst_h = host_pick(self._dev_worst) if self._dev_worst is not None else None
+        cols_h = {k: host(v[:n]) for k, v in self._cols.items()}
+        # device meta joins the read-back; host meta (CPU columns, lists) is already here
+        meta_h = {k: host(v[:n]) for k, v in self._meta.items() if torch.is_tensor(v) and v.is_cuda}
+        random_h = [_tree_map(host, p) for p in self._dev_random]
+        worst_h = [_tree_map(host, self._dev_worst)] if self._dev_worst is not None else []
         t_q = time.perf_counter()
         landed = flush()
         t_f = time.perf_counter()
@@ -534,52 +449,36 @@ class SamplerState:
                 prof = cProfile.Profile()
                 prof.enable()
 
-        def resolve(x):
-            if isinstance(x, int):
-                return landed[x]
-            if isinstance(x, dict):
-                return {k: resolve(v) for k, v in x.items()}
-            if isinstance(x, (list, tuple)):
-                return type(x)(resolve(v) for v in x)
-            return x
+        cols_h, meta_h, random_h, worst_h = _tree_map(landed.__getitem__, (cols_h, meta_h, random_h, worst_h))
 
-        cols_h, meta_h, random_h, worst_h = resolve(cols_h), resolve(meta_h), resolve(random_h), resolve(worst_h)
         def own(t: torch.Tensor) -> torch.Tensor:
             # a pageable copy out of the staging block by plain memcpy.  ``clone()``/``copy_`` of a
             # CPU tensor above ATen's grain size (32 768 elements) is an OpenMP parallel region:
             # waking a 128-thread pool that sleeps between epochs costs milliseconds PER CALL;
-            # numpy's copy is single-threaded
+            # numpy's copy is single-threaded (numpy has no bfloat16: those go as their int16 bits)
+            if t.dtype == torch.bfloat16:
+                return own(t.view(torch.int16)).view(torch.bfloat16)
             return torch.from_numpy(t.numpy().copy())
 
-        cols = {k: v.numpy().copy() for k, v in cols_h.items()}
-        for k, v in cols.items():
-            self._data_metric[k] = [v]
-        dev_meta = {k: own(v) for k, v in meta_h.items()}
+        self._data_metric = {k: v.numpy().copy() for k, v in cols_h.items()}
+        meta = {k: own(meta_h[k]) if k in meta_h else v for k, v in self._meta.items()}
 
-        def samples_of(p, keep=None) -> List[SingleSample]:
-            out = []
-            for r, g in enumerate(p["pos"].tolist()):
-                if keep is not None and not keep[r]:
-                    continue
-                meta = {k: v[g] for k, v in dev_meta.items()}
-                meta.update({k: v[g] for k, v in self._host_meta.items()})
-                out.append(SingleSample(data=[own(x[r]) for x in p["data"]],
-                                        target=[tuple(own(x[r]) for x in h) for h in p["target"]],
-                                        meta=meta, output=[own(x[r]) for x in p["output"]],
-                                        metric={k: cols[k][g] for k in cols}))
-            return out
+        def samples_of(p, rows) -> List[SingleSample]:
+            pos = p["pos"].tolist()
+            return [SingleSample(data=[own(x[r]) for x in p["data"]],
+                                 target=[tuple(own(x[r]) for x in h) for h in p["target"]],
+                                 meta={k: v[pos[r]] for k, v in meta.items()},
+                                 output=[own(x[r]) for x in p["output"]],
+                                 metric={k: v[pos[r]] for k, v in self._data_metric.items()})
+                    for r in rows]
 
         for p in random_h:
-            self._random_samples.extend(samples_of(p))
-        if worst_h is not None:
-            scores = worst_h["score"].tolist()
-            finite = [s != float("-inf") for s in scores]          # -inf = filtered out (invalid metric)
-            kept = samples_of(worst_h, finite)
-            kept_scores = [s for s, f in zip(scores, finite) if f]
-            # heap order of the host path is unspecified beyond "the k most extreme": ascending by
-            # score, as a drained min-heap would come out
-            order = sorted(range(len(kept)), key=lambda i: kept_scores[i])
-            self._worst_samples = [(kept_scores[i], kept[i]) for i in order]
+            self._random_samples.extend(samples_of(p, range(p["pos"].numel())))
+        for p in worst_h:
+            # the valid ones, ascending by score (the order a drained min-heap would give)
+            ranked = sorted((s, r) for r, (s, ok) in enumerate(zip(p["score"].tolist(), p["valid"].tolist()))
+                            if ok)
+            self._worst_samples = samples_of(p, [r for _, r in ranked])
         self._dev_random, self._dev_worst = [], None
         if tracing:
             logger.info("finish trace: host-side assembly after the sync %.2f ms", 1e3 * (time.perf_counter() - t_s))
@@ -601,14 +500,24 @@ class SamplerState:
 
     @property
     def worst_samples(self) -> List[SingleSample]:
-        return [s for _, s in self._worst_samples]
+        """Ascending by rank score: the most extreme sample last."""
+        return self._worst_samples
 
     @property
     def data_metric(self) -> Dict[str, np.ndarray]:
         """Per-sample metrics of the whole split, one array per metric (the reference grows
         Python lists of scalars per sample, solver_worker.py:318-319; same length and order)."""
-        return {k: (np.concatenate([np.atleast_1d(a) for a in v]) if v else np.zeros(0))
-                for k, v in self._data_metric.items()}
+        return self._data_metric
+
+
+def _tree_map(fn, *trees):
+    """``fn`` over the matching leaves of nested dicts / lists / tuples of the same shape."""
+    first = trees[0]
+    if isinstance(first, dict):
+        return {k: _tree_map(fn, *(t[k] for t in trees)) for k in first}
+    if isinstance(first, (list, tuple)):
+        return type(first)(_tree_map(fn, *xs) for xs in zip(*trees))
+    return fn(*trees)
 
 
 def _planned_order(sampler, accessor) -> List[int]:
@@ -835,7 +744,7 @@ class SolverWorker:
                 # pure device work, no host read) so the stream drains once, not twice; a NaN in
                 # the last steps is still raised first — the fold's results are simply dropped
                 # with the exception
-                fold_early = bool(sampler_state._dev_mode)
+                fold_early = sampler_state.metrics_on_device
                 if fold_early:
                     sampler_state.compute_metrics()
                     mark("last window folded")

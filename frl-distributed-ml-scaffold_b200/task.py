@@ -57,9 +57,12 @@ class Task(Generic[TransformT, SampleMetaT, BatchMetaT]):
     @abstractmethod
     def compute_batch_metrics(self, meta: BatchMetaT, target: Tuple[torch.Tensor, ...],
                               output: torch.Tensor) -> "Dict[str, object]":
-        """Per-sample metrics of a window of retained minibatches (device tensors in, host arrays
-        out).  Called every ``metricAmortizationSchedule`` minibatches on the metric worker
-        thread and stream: it may synchronise freely, the training thread does not wait."""
+        """Per-sample metrics of a window of retained minibatches: device tensors in, host arrays
+        or device tensors out.  Called every ``metricAmortizationSchedule`` minibatches on the
+        training thread.  Device tensors keep the fold on the device, so the training thread
+        does not wait; host arrays end in a device-to-host read that drains the launch pipeline,
+        unless the Problem sets ``metric_hooks_thread_safe`` and the hook runs on the metric
+        worker thread and stream instead."""
         ...
 
     @property

@@ -181,14 +181,11 @@ def test_model_helpers():
 
 
 
-@pytest.mark.parametrize("config", ["err_MSE_DESC", "score_ASC", "score_DESC"])
-def test_sampler_state_host_path_matches_reference_fixture(golden_dir, config):
-    """tests/golden/sampler_state.json = what the unmodified reference's SamplerState produced for
-    the shared scenario (oracle/make_sampler_state_golden.py): per-sample metrics, random picks
-    and worst-k set of this repo's class must be the same (host arrays from the hook)."""
+def _fold_sampler_state_scenario(golden_dir, config, as_numpy):
+    """The shared scenario (oracle/make_sampler_state_golden.py) folded by this repo's class with a
+    hook that returns numpy arrays or tensors; the fixture recorded from the reference for it."""
     import json
     import random
-    import numpy as np
     import torch
     import frl_b200.solver_worker as sw
     from frl_b200.problem import Ordering
@@ -197,47 +194,45 @@ def test_sampler_state_host_path_matches_reference_fixture(golden_dir, config):
     name, ordering = config.rsplit("_", 1)
     batches, total = gen.scenario()
     random.seed(gen.PY_SEED)
-    mine = sw.SamplerState(gen.make_problem(Ordering, name, ordering), total, total, torch.device("cpu"),
-                           gen.N_VIS)
+    mine = sw.SamplerState(gen.make_problem(Ordering, name, ordering, as_numpy=as_numpy), total, total,
+                           torch.device("cpu"), gen.N_VIS)
     gen.drive(mine, batches)
-    mine.finish()
+    return mine, want, batches
+
+
+def _assert_matches_fixture(mine, want, batches):
+    import numpy as np
+    import torch
     for k, v in want["metrics"].items():
         np.testing.assert_array_equal(np.asarray(mine.data_metric[k], dtype=np.float64), np.asarray(v))
     assert [int(s.meta["index"]) for s in mine.random_samples] == want["random_ids"]
     assert sorted(int(s.meta["index"]) for s in mine.worst_samples) == want["worst_ids"]
-
-
-@pytest.mark.parametrize("config", ["err_MSE_DESC", "score_ASC", "score_DESC"])
-def test_sampler_state_device_fold_logic_on_host_tensors(golden_dir, config):
-    """The device-side fold (per-sample columns, random picks by position, running top-k merged per
-    window, ONE packed read-back) is tensor logic that does not care where the tensors live: driven
-    here with host tensors (the hook returns tensors, ``_dev_mode`` forced) against the same
-    reference fixtures; ``tests/test_gpu_solver.py`` runs it on the device."""
-    import json
-    import random
-    import numpy as np
-    import torch
-    import frl_b200.solver_worker as sw
-    from frl_b200.problem import Ordering
-    from oracle import make_sampler_state_golden as gen
-    want = json.load(open(os.path.join(golden_dir, "sampler_state.json")))[config]
-    name, ordering = config.rsplit("_", 1)
-    batches, total = gen.scenario()
-    random.seed(gen.PY_SEED)
-    mine = sw.SamplerState(gen.make_problem(Ordering, name, ordering, as_numpy=False), total, total,
-                           torch.device("cpu"), gen.N_VIS)
-    mine._dev_mode = True
-    gen.drive(mine, batches)
-    assert not mine.random_samples and not mine.worst_samples and mine._dev_worst is not None
-    mine.finish()
-    for k, v in want["metrics"].items():
-        np.testing.assert_allclose(np.asarray(mine.data_metric[k], dtype=np.float64), np.asarray(v),
-                                   rtol=1e-6, atol=1e-7)
-    assert [int(s.meta["index"]) for s in mine.random_samples] == want["random_ids"]
-    assert sorted(int(s.meta["index"]) for s in mine.worst_samples) == want["worst_ids"]
+    # the captured samples are the scenario's rows, bit for bit
     rows = {int(i): (b["data"][0][j], b["outputs"][0][j], b["targets"][1][0][j])
             for b in batches for j, i in enumerate(b["meta"]["index"])}
     for smp in mine.random_samples + mine.worst_samples:
         d, o, t = rows[int(smp.meta["index"])]
         assert torch.equal(smp.data[0], d) and torch.equal(smp.output[0], o) and torch.equal(smp.target[1][0], t)
+
+
+@pytest.mark.parametrize("config", ["err_MSE_DESC", "score_ASC", "score_DESC"])
+def test_sampler_state_host_path_matches_reference_fixture(golden_dir, config):
+    """tests/golden/sampler_state.json = what the unmodified reference's SamplerState produced for
+    the shared scenario (oracle/make_sampler_state_golden.py): per-sample metrics, random picks
+    and worst-k set of this repo's class must be the same (host arrays from the hook)."""
+    mine, want, batches = _fold_sampler_state_scenario(golden_dir, config, as_numpy=True)
+    mine.finish()
+    _assert_matches_fixture(mine, want, batches)
+
+
+@pytest.mark.parametrize("config", ["err_MSE_DESC", "score_ASC", "score_DESC"])
+def test_sampler_state_device_fold_logic_on_host_tensors(golden_dir, config):
+    """The hook returns tensors: per-sample columns, random picks by position, running top-k
+    merged per window, ONE packed read-back in ``finish()`` — tensor logic that does not care
+    where the tensors live, driven here with host tensors against the same reference fixtures;
+    ``tests/test_gpu_solver.py`` runs it on the device."""
+    mine, want, batches = _fold_sampler_state_scenario(golden_dir, config, as_numpy=False)
+    assert not mine.random_samples and not mine.worst_samples and mine._dev_worst is not None
+    mine.finish()
+    _assert_matches_fixture(mine, want, batches)
 

@@ -336,7 +336,7 @@ def test_fused_linear_relu_units_keep_reference_parity(ns, golden_dir, monkeypat
 def test_device_side_sampler_state_matches_reference_fixture(golden_dir, config):
     """The Problem's hook returns DEVICE tensors; per-sample metrics stay in HBM
     columns, the worst-k set is a running device buffer merged with topk per window, everything is
-    read back once at the end of the split.  Same fixtures as the host path: the reference's own
+    read back once at the end of the split.  Same fixtures as the numpy-returning hook: the reference's own
     SamplerState on the same scenario (oracle/make_sampler_state_golden.py)."""
     import json
     import random
@@ -355,7 +355,7 @@ def test_device_side_sampler_state_matches_reference_fixture(golden_dir, config)
     mine = sw.SamplerState(gen.make_problem(Ordering, name, ordering, as_numpy=False), total, total, dev,
                            gen.N_VIS)
     gen.drive(mine, cuda_batches)
-    assert mine._dev_mode is True and mine._runner is None        # no worker thread, no host read so far
+    assert mine.metrics_on_device and mine._runner is None        # no worker thread, no host read so far
     assert not mine.random_samples and not mine.worst_samples
     mine.finish()
     for k, v in want["metrics"].items():
