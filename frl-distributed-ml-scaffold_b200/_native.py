@@ -435,7 +435,8 @@ def colsum(x, out, accumulate: bool = False) -> None:
 
 
 def drelu_colsum(dy, act, dz, out, accumulate: bool = False) -> None:
-    """dz = where(act > 0, dy, 0); out[c] (+)= sum_r dz[r, c] — one pass (contiguous 2-D inputs)."""
+    """dz = threshold_backward(dy, act, 0) (dy unless act <= 0); out[c] (+)= sum_r dz[r, c] — one
+    pass (contiguous 2-D inputs)."""
     rows, cols = dy.shape
     assert act.shape == dy.shape == dz.shape and act.dtype == dy.dtype == dz.dtype
     assert dy.is_contiguous() and act.is_contiguous() and dz.is_contiguous()

@@ -21,8 +21,8 @@ Unless ``FRL_B200_FUSE_RELU=0``, a ``nn.Linear`` directly followed by a ``nn.ReL
   forward   y = relu(x W^T + b)                one cuBLASLt GEMM with the bias+ReLU epilogue
                                                (``torch._addmm_activation``); the ReLU module
                                                becomes a pass-through
-  backward  dZ = (y > 0) * dY, db = colsum(dZ) ONE pass (``frl_drelu_colsum``, K6b) instead of
-                                               threshold_backward + a reduction
+  backward  dZ = threshold_backward(dY, y, 0), ONE pass (``frl_drelu_colsum``, K6b) instead of
+            db = colsum(dZ)                    threshold_backward + a reduction
             dX = dZ W, dW = dZ^T X             as above
 
 In a ``Precision.FP8`` run a site whose weight lives in the bf16 shadow and whose widths are
@@ -202,7 +202,7 @@ class _ArenaLinearFn(torch.autograd.Function):
                                      accumulate=not site.bstate.first_touch(pipe.step_id))
                 dz, db_written = dz_relu, True
             else:
-                dz = dz * (y2 > 0).to(dz.dtype)
+                dz = torch.ops.aten.threshold_backward(dz, y2, 0)     # stock ReLU backward, NaN/inf included
         need_dx = ctx.needs_input_grad[0]
         gemms = (_Fp8Gemms if ctx.fp8 else _DenseGemms)(saved, dz, need_dx)
         # dX first: marking the weight's slot ready may launch the bucket's update on the side

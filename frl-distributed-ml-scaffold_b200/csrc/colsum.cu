@@ -72,9 +72,10 @@ template <> __device__ __forceinline__ void store8<__nv_bfloat16>(__nv_bfloat16*
 }
 
 // partial layout: [tile][split][kSCols] floats, after the per-tile tickets.
-// MASK (K6b): x is dY of a ReLU layer, `act` its forward output; dZ = act > 0 ? dY : 0 is written
+// MASK (K6b): x is dY of a ReLU layer, `act` its forward output; dZ = act <= 0 ? 0 : dY is written
 // to `dz` on the way and the column sums are those of dZ — ReLU's backward and the bias-gradient
-// reduction in the one pass over dY that the reduction needs anyway.
+// reduction in the one pass over dY that the reduction needs anyway.  The predicate is torch's
+// threshold_backward(dY, act, 0): a NaN activation passes dY through (act > 0 would drop it).
 template <typename XT, typename OT, bool VEC, bool MASK, int kSRowsInFlight>
 __global__ void __launch_bounds__(kSThreads, 4)
 colsum_kernel(const XT* __restrict__ x, const XT* __restrict__ act, XT* __restrict__ dz, int64_t rows,
@@ -115,7 +116,7 @@ colsum_kernel(const XT* __restrict__ x, const XT* __restrict__ act, XT* __restri
                         float a[8];
                         unpack8(qa[u], a);
 #pragma unroll
-                        for (int k = 0; k < 8; ++k) v[k] = a[k] > 0.f ? v[k] : 0.f;
+                        for (int k = 0; k < 8; ++k) v[k] = a[k] <= 0.f ? 0.f : v[k];
                         store8<XT>(dz + r * cols + c0, v);
                     }
 #pragma unroll
@@ -131,7 +132,7 @@ colsum_kernel(const XT* __restrict__ x, const XT* __restrict__ act, XT* __restri
                 if (c0 + k < cols) {
                     float v = ld1<XT>(x + r * cols + c0 + k);
                     if (MASK) {
-                        v = ld1<XT>(act + r * cols + c0 + k) > 0.f ? v : 0.f;
+                        v = ld1<XT>(act + r * cols + c0 + k) <= 0.f ? 0.f : v;
                         st1<XT>(dz + r * cols + c0 + k, v);
                     }
                     acc[k] += v;
@@ -191,14 +192,15 @@ extern "C" int64_t frl_colsum_scratch_bytes(int64_t rows, int64_t cols) {
            tiles * kSMaxSplits * kSCols * static_cast<int64_t>(sizeof(float));
 }
 
-static int launch_colsum(const void* x, const void* act, void* dz, int x_dtype, int64_t rows, int64_t cols,
-                         void* out, int out_dtype, int accumulate, void* scratch, void* stream,
+// rows == 0 is a valid launch (an empty batch): the matrices may then be null, and out[c] is
+// stored as 0, or left as it is when accumulating
+static int launch_colsum(const void* x, const void* act, void* dz, bool mask, int x_dtype, int64_t rows,
+                         int64_t cols, void* out, int out_dtype, int accumulate, void* scratch, void* stream,
                          const char* name) {
-    FRL_REQUIRE(x && out && scratch && rows >= 0 && cols >= 1, FRL_E_ARG, "%s: bad args", name);
+    FRL_REQUIRE((x || rows == 0) && out && scratch && rows >= 0 && cols >= 1, FRL_E_ARG, "%s: bad args", name);
     FRL_REQUIRE((x_dtype == FRL_F32 || x_dtype == FRL_BF16) && (out_dtype == FRL_F32 || out_dtype == FRL_BF16),
                 FRL_E_DTYPE, "%s: dtype", name);
-    const bool mask = act != nullptr;
-    FRL_REQUIRE(!mask || dz != nullptr, FRL_E_ARG, "%s: dz is required with act", name);
+    FRL_REQUIRE(!mask || rows == 0 || (act && dz), FRL_E_ARG, "%s: act and dz are required", name);
     const int64_t tiles = colsum_tiles(cols);
     const int splits = colsum_splits(rows, tiles);
     unsigned int* tickets = static_cast<unsigned int*>(scratch);
@@ -241,14 +243,13 @@ static int launch_colsum(const void* x, const void* act, void* dz, int x_dtype, 
 
 extern "C" int frl_colsum(const void* x, int x_dtype, int64_t rows, int64_t cols, void* out,
                           int out_dtype, int accumulate, void* scratch, void* stream) {
-    return launch_colsum(x, nullptr, nullptr, x_dtype, rows, cols, out, out_dtype, accumulate, scratch,
+    return launch_colsum(x, nullptr, nullptr, false, x_dtype, rows, cols, out, out_dtype, accumulate, scratch,
                          stream, "frl_colsum");
 }
 
 extern "C" int frl_drelu_colsum(const void* dy, const void* act, void* dz, int dtype, int64_t rows,
                                 int64_t cols, void* out, int out_dtype, int accumulate, void* scratch,
                                 void* stream) {
-    FRL_REQUIRE(act && dz, FRL_E_ARG, "frl_drelu_colsum: act and dz are required");
-    return launch_colsum(dy, act, dz, dtype, rows, cols, out, out_dtype, accumulate, scratch, stream,
+    return launch_colsum(dy, act, dz, true, dtype, rows, cols, out, out_dtype, accumulate, scratch, stream,
                          "frl_drelu_colsum");
 }

@@ -381,14 +381,17 @@ int frl_cast_scale(const void* src, int src_dtype, void* dst, int dst_dtype, int
  * The bias gradient of a linear layer, written straight into the gradient arena; replaces the
  * generic reduction autograd runs inside `total_loss.backward()` (reference
  * solver_worker.py:586).  accumulate != 0 adds to `out` (a layer applied twice in one step).
+ * rows == 0 (an empty batch; the matrices may then be null) stores 0, or leaves `out` as it is
+ * when accumulating.
  * scratch: frl_colsum_scratch_bytes(rows, cols) bytes, zero-initialised once; deterministic.
  * ---------------------------------------------------------------------------------------- */
 int64_t frl_colsum_scratch_bytes(int64_t rows, int64_t cols);
 int frl_colsum(const void* x, int x_dtype, int64_t rows, int64_t cols, void* out, int out_dtype,
                int accumulate, void* scratch, void* stream);
 /* K6b — the same pass with ReLU's backward folded in, for a Linear+ReLU pair: dz[r,c] =
- * act[r,c] > 0 ? dy[r,c] : 0 (act = the layer's forward output; dy, act, dz share dtype and the
- * [rows, cols] layout; dz may alias dy) and out[c] (+)= sum_r dz[r,c].  Replaces autograd's
+ * threshold_backward(dy, act, 0)[r,c] = act[r,c] <= 0 ? 0 : dy[r,c], so a NaN activation passes dy
+ * through as torch's ReLU backward does (act = the layer's forward output; dy, act, dz share dtype
+ * and the [rows, cols] layout; dz may alias dy) and out[c] (+)= sum_r dz[r,c].  Replaces autograd's
  * threshold_backward kernel plus the bias-gradient reduction (reference solver_worker.py:586). */
 int frl_drelu_colsum(const void* dy, const void* act, void* dz, int dtype, int64_t rows, int64_t cols,
                      void* out, int out_dtype, int accumulate, void* scratch, void* stream);

@@ -136,7 +136,8 @@ class KernelDouble:
         out.copy_((out.float() + tot if accumulate else tot).to(out.dtype))
 
     def drelu_colsum(self, dy, act, dz, out, accumulate=False):
+        import torch
         self.calls.append(("drelu_colsum", dy.shape[1]))
-        dz.copy_(dy * (act > 0).to(dy.dtype))
+        dz.copy_(torch.ops.aten.threshold_backward(dy, act, 0))     # ReLU's backward: dy unless act <= 0
         tot = dz.float().sum(0)
         out.copy_((out.float() + tot if accumulate else tot).to(out.dtype))

@@ -369,27 +369,8 @@ def test_launch_counter_counts_our_kernels():
 
 
 # ------------------------------------------------------------------------------------------------
-# K6 + nn.Linear gradients born in the arena
+# nn.Linear gradients born in the arena (K6 and K6b themselves: test_gpu_colsum_paths.py)
 # ------------------------------------------------------------------------------------------------
-
-@pytest.mark.parametrize("rows,cols", [(1, 1), (7, 13), (4096, 4096), (4096, 1000), (333, 264), (5, 4104)])
-@pytest.mark.parametrize("xdt,odt", [(torch.float32, torch.float32), (torch.bfloat16, torch.bfloat16),
-                                     (torch.bfloat16, torch.float32)])
-def test_colsum_matches_float64_sum(rows, cols, xdt, odt):
-    x = torch.randn(rows, cols, device=DEV).to(xdt)
-    out = torch.full((cols,), 3.0, dtype=odt, device=DEV)
-    want = x.double().sum(0)
-    _native.colsum(x, out)
-    tol = dict(rtol=2e-2, atol=2e-1) if odt == torch.bfloat16 else dict(rtol=1e-5, atol=1e-4 * max(rows, 1) ** 0.5)
-    torch.testing.assert_close(out.double(), want, **tol)
-    before = out.clone()
-    _native.colsum(x, out, accumulate=True)
-    torch.testing.assert_close(out.double(), before.double() + want, **tol)
-    _native.colsum(x, out)                        # deterministic: same bits on a second launch
-    again = out.clone()
-    _native.colsum(x, out)
-    assert torch.equal(out, again)
-
 
 @pytest.mark.parametrize("precision", ["fp32", "bf16"])
 def test_linear_gradients_are_written_into_the_arena(precision, monkeypatch):
@@ -501,31 +482,8 @@ def test_tma_gather_rejects_rows_that_are_not_multiples_of_16_bytes():
 
 
 # ------------------------------------------------------------------------------------------------
-# K6b + Linear/ReLU units (FRL_B200_FUSE_RELU)
+# Linear/ReLU units (FRL_B200_FUSE_RELU)
 # ------------------------------------------------------------------------------------------------
-
-@pytest.mark.parametrize("rows,cols", [(1, 1), (7, 13), (4096, 4096), (333, 264), (5, 4104)])
-@pytest.mark.parametrize("xdt,odt", [(torch.float32, torch.float32), (torch.bfloat16, torch.bfloat16),
-                                     (torch.bfloat16, torch.float32)])
-def test_drelu_colsum_matches_threshold_backward_plus_sum(rows, cols, xdt, odt):
-    dy = torch.randn(rows, cols, device=DEV).to(xdt)
-    act = torch.relu(torch.randn(rows, cols, device=DEV)).to(xdt)          # ~half zeros, as a ReLU output
-    dz = torch.full_like(dy, 7.0)
-    out = torch.full((cols,), 3.0, dtype=odt, device=DEV)
-    _native.drelu_colsum(dy, act, dz, out)
-    want_dz = torch.where(act > 0, dy, torch.zeros_like(dy))                # aten threshold_backward
-    assert torch.equal(dz, want_dz)                                        # a select: exact
-    want = want_dz.double().sum(0)
-    tol = dict(rtol=2e-2, atol=2e-1) if odt == torch.bfloat16 else dict(rtol=1e-5, atol=1e-4 * max(rows, 1) ** 0.5)
-    torch.testing.assert_close(out.double(), want, **tol)
-    before = out.clone()
-    _native.drelu_colsum(dy, act, dz, out, accumulate=True)
-    torch.testing.assert_close(out.double(), before.double() + want, **tol)
-    # in place (dz aliasing dy) gives the same result
-    dy2 = dy.clone()
-    _native.drelu_colsum(dy2, act, dy2, out)
-    assert torch.equal(dy2, want_dz)
-
 
 @pytest.mark.parametrize("precision", ["fp32", "bf16"])
 def test_fused_linear_relu_units_match_the_unfused_modules(precision, monkeypatch):
