@@ -57,6 +57,9 @@ SIGNATURES = {
     "frl_sgd_momentum": (_i, [_vp, _vp, _vp, _vp, _i64, _d, _d, _d, _d, _d, _vp, _vp, _i, _i, _vp]),
     "frl_adam": (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _i64, _d, _d, _d, _d, _d, _i64, _d, _vp, _vp, _i, _vp]),
     "frl_rmsprop": (_i, [_vp, _vp, _vp, _vp, _vp, _i64, _d, _d, _d, _d, _d, _d, _vp, _vp, _i, _vp]),
+    "frl_dw_gemm": (_i, [_vp, _i64, _vp, _i64, _i64, _i64, _i64, _vp, _vp]),
+    "frl_dw_gemm_sgd": (_i, [_vp, _i64, _vp, _i64, _i64, _i64, _i64, _vp, _vp, _vp, _vp, _d, _d, _d, _d, _d,
+                             _vp, _i, _vp]),
     "frl_mt_tile_elems": (_i64, []),
     "frl_flatten_grads": (_i, [_vp, _vp, _vp, _i64, _vp, _i, _d, _vp]),
     "frl_sgd_momentum_mt": (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _i64, _d, _d, _d, _d, _d, _vp, _vp, _i, _vp]),
@@ -191,6 +194,36 @@ def rmsprop(p, g, sq, buf, p_lp, n, *, lr, alpha, eps, wd, mu, grad_scale=1.0,
     _check(lib().frl_rmsprop(_ptr(p), _ptr(g), _ptr(sq), _ptr(buf), _ptr(p_lp), n, lr, alpha,
                              eps, wd, mu, grad_scale, _ptr(grad_scale_dev), _ptr(dyn),
                              dtype_code(g.dtype), _stream()), "frl_rmsprop")
+
+
+# ---- K12: weight-gradient GEMM, optionally with the SGD update in its epilogue ----------------------
+
+DW_TILE = (128, 256, 64)      # (out, in, rows) multiples K12 needs
+
+
+def dw_gemm_fits(dz, x, gw) -> bool:
+    """Whether K12 can compute gw = dz^T x: bf16 operands with unit column stride, rows 16-byte
+    aligned, a contiguous bf16 output and shapes that are multiples of ``DW_TILE``."""
+    tm, tn, tk = DW_TILE
+    return (dz.dim() == 2 and x.dim() == 2 and dz.dtype == x.dtype == gw.dtype == torch.bfloat16
+            and dz.stride(1) == 1 and x.stride(1) == 1 and dz.stride(0) % 8 == 0 and x.stride(0) % 8 == 0
+            and dz.data_ptr() % 16 == 0 and x.data_ptr() % 16 == 0 and gw.data_ptr() % 16 == 0
+            and gw.is_contiguous() and dz.shape[0] == x.shape[0] and tuple(gw.shape) == (dz.shape[1], x.shape[1])
+            and dz.shape[1] % tm == 0 and x.shape[1] % tn == 0 and dz.shape[0] % tk == 0 and dz.shape[0] > 0)
+
+
+def dw_gemm(dz, x, gw) -> None:
+    """gw = dz^T x (bf16, fp32 accumulation) for dz [rows, out], x [rows, in]."""
+    _check(lib().frl_dw_gemm(_ptr(dz), dz.stride(0), _ptr(x), x.stride(0), dz.shape[0], dz.shape[1], x.shape[1],
+                             _ptr(gw), _stream()), "frl_dw_gemm")
+
+
+def dw_gemm_sgd(dz, x, gw, p, buf, p_lp, *, lr, mu, dampening, wd, grad_scale=1.0, first_step=False,
+                dyn=None) -> None:
+    """gw = dz^T x, then ``sgd_momentum``'s update of the [out, in] slices p / buf / p_lp from it."""
+    _check(lib().frl_dw_gemm_sgd(_ptr(dz), dz.stride(0), _ptr(x), x.stride(0), dz.shape[0], dz.shape[1],
+                                 x.shape[1], _ptr(gw), _ptr(p), _ptr(buf), _ptr(p_lp), lr, mu, dampening, wd,
+                                 grad_scale, _ptr(dyn), int(first_step), _stream()), "frl_dw_gemm_sgd")
 
 
 # ---- K2-mt / K1: multi-tensor forms (gradients read where autograd left them) ---------------------

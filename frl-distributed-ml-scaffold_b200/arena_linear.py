@@ -40,7 +40,9 @@ Whatever the variant, backward runs one protocol: form dZ (on a ReLU site inside
 ``frl_drelu_colsum`` writes the bias gradient with it), compute dX, and only then write dW
 (``LinearSite.weight_grad``), the bias gradient if not yet written, and mark the slots ready
 (``LinearSite.backward_done``): marking a slot ready can launch the bucket's update, which
-overwrites W.
+overwrites W.  So can the dW GEMM itself: on one GPU with SGD (``GradBucketPipeline.fused_dw_update``)
+a bf16 weight applied once per forward whose shape fits the tile gets its gradient and its update
+from one kernel (``frl_dw_gemm_sgd``, K12).
 """
 import os
 import types
@@ -400,11 +402,14 @@ class LinearSite:
             gemms.dw_add(gw)
             return
         rows = pipe.row_split(self.wslot)
-        if (rows and rows % gemms.row_multiple == 0 and st.fwd_gen == pipe.forward_gen
-                and st.fwd_count == 1):
+        only_use = st.fwd_gen == pipe.forward_gen and st.fwd_count == 1
+        if rows and rows % gemms.row_multiple == 0 and only_use:
             gemms.dw(gemms.dzt[:rows], out=gw[:rows])
             pipe.rows_ready(self.wslot, rows)
             gemms.dw(gemms.dzt[rows:], out=gw[rows:])
+        elif (pipe.fused_dw_update and only_use and not rows and type(gemms) is _DenseGemms
+              and self.wslot.uses_lp and _native.dw_gemm_fits(gemms.dz, gemms.x2, gw)):
+            pipe.update_in_dw_gemm(self.wslot, gemms.dz, gemms.x2, gw)
         else:
             gemms.dw(gemms.dzt, out=gw)
 

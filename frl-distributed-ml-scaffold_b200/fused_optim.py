@@ -265,6 +265,18 @@ class FusedSGD(FusedArenaOptimizer):
                              grad_scale=grad_scale, grad_scale_dev=coef,
                              first_step=(self._steps == 0), dyn=self._dyn)
 
+    def update_in_dw_gemm(self, slot, dz, x, gw, *, grad_scale: float = 1.0) -> None:
+        """K12: the weight gradient gw = dz^T x of ``slot`` and, in the same kernel, this step's
+        update of the slot from exactly that bf16 gradient (what ``_launch`` over the slot does)."""
+        h = self.hyper
+        a = self.arena
+        mu = float(h["momentum"])
+        buf = self._state("momentum_buffer")[slot.offset:slot.end] if mu != 0.0 else None
+        KERNELS.dw_gemm_sgd(dz, x, gw, a.master[slot.offset:slot.end], buf, a.lp[slot.offset:slot.end],
+                            lr=float(h["lr"]), mu=mu, dampening=float(h["dampening"]),
+                            wd=float(h["weight_decay"]), grad_scale=grad_scale,
+                            first_step=(self._steps == 0), dyn=self._dyn)
+
     def _launch_mt(self, table, grad_scale):
         h = self.hyper
         mu = float(h["momentum"])

@@ -23,7 +23,11 @@ solver_worker.py:585-592).  Differences that matter on H100:
   all-reduces the accumulator per bucket, clips and updates from it;
 * with a weight EMA (``ema.WeightEMA``) every optimizer update is followed by one K11 launch on the
   compute stream, behind the update and, with eager per-bucket updates, behind the join with the
-  side stream; never inside a captured graph (the tail runs after the replay).
+  side stream; never inside a captured graph (the tail runs after the replay);
+* on one GPU with SGD and bf16 shadow weights (``fused_dw_update``), a Linear layer whose dW GEMM
+  qualifies (``arena_linear.LinearSite.weight_grad``) updates its weight in that GEMM's epilogue
+  (K12), under the tensor-core work of the following tiles; the tail then updates only the slots
+  K12 did not (heads, biases, anything else).
 """
 import os
 from typing import Callable, Dict, List, NamedTuple, Optional, Tuple
@@ -34,7 +38,8 @@ import torch.nn as nn
 
 from . import _native
 from .arena import ParamArena
-from .fused_optim import FusedArenaOptimizer
+from .fused_optim import FusedArenaOptimizer, FusedSGD
+from .types import Precision
 
 KERNELS = _native     # swapped by CPU tests of the host logic
 
@@ -245,6 +250,14 @@ class GradBucketPipeline:
         self._acc_scale = self.grad_scale
         self._acc_seen = set()         # slots that got a gradient in some microbatch of the open group
         self.last_ready: frozenset = frozenset()
+        # K12: one GPU, one tail update (eager per-bucket updates would race the GEMM for the same
+        # weights' state), no global norm, no accumulator, plain SGD on bf16 shadow weights
+        self.fused_dw_update = (
+            not self.distributed and not self.eager and self.clip_norm == 0.0 and self.accumulation == 1
+            and type(optimizer) is FusedSGD and arena.precision is Precision.BF16
+            and hasattr(KERNELS, "dw_gemm_sgd") and (self.on_cuda or KERNELS is not _native)
+            and os.environ.get("FRL_B200_FUSED_DW_UPDATE", "1") != "0")
+        self.dw_updated: set = set()      # slot indices K12 updated in this step
 
     _ACC_RING = 16
 
@@ -287,6 +300,7 @@ class GradBucketPipeline:
             b.work = None
             b.launched = False
         self.optimizer.begin_step()
+        self.dw_updated = set()        # a new set: a captured step keeps the one it filled
         self.step_id += 1
         self._step_open = True
 
@@ -379,6 +393,12 @@ class GradBucketPipeline:
             if not b.launched and b.hi <= done and b.pending == 1:
                 b.pending = 0
                 self._launch_bucket(b)
+
+    def update_in_dw_gemm(self, slot, dz, x, gw) -> None:
+        """K12: gw = dz^T x into the slot's gradient and the slot's update from it, in one kernel
+        (``fused_dw_update``; the caller checked the shapes).  The tail leaves the slot alone."""
+        self.optimizer.update_in_dw_gemm(slot, dz, x, gw, grad_scale=self.grad_scale)
+        self.dw_updated.add(slot.index)
 
     def defer_ready(self, slot) -> None:
         """The slot's gradient was written but more contributions are expected in this backward;
@@ -483,12 +503,13 @@ class GradBucketPipeline:
         """True if a step ends with tail launches (not everything is updated eagerly)."""
         return not self.eager
 
-    def run_tail(self, grad_refs=None, tables=None, ready=None) -> None:
+    def run_tail(self, grad_refs=None, tables=None, ready=None, dw_updated=None) -> None:
         """The deferred part of ``finish_step(defer_tail=True)``; also what a CUDA-graph replay
         of the captured step is followed by (then with the capture's gradient references and
         segment tables: the replayed backward wrote to exactly those addresses).  With gradient
         accumulation: the update from the accumulator if this microbatch closes its group;
-        ``ready`` names the slots the replayed K10 launch accumulated."""
+        ``ready`` names the slots the replayed K10 launch accumulated; ``dw_updated`` the slots
+        the replayed K12 launches updated."""
         if self.acc is not None:
             if ready is not None:
                 self._acc_seen |= ready
@@ -496,8 +517,10 @@ class GradBucketPipeline:
                 self._end_update(acc=True)
             return
         if grad_refs is not None:
-            mine = (self._ext, self.tables)
+            mine = (self._ext, self.tables, self.dw_updated)
             self._ext, self.tables, self._keep_ext = grad_refs, tables, True
+            if dw_updated is not None:
+                self.dw_updated = dw_updated
         try:
             if self.has_tail:
                 self._end_update()
@@ -507,7 +530,7 @@ class GradBucketPipeline:
                     self.ema.update()
         finally:
             if grad_refs is not None:
-                (self._ext, self.tables), self._keep_ext = mine, False
+                (self._ext, self.tables, self.dw_updated), self._keep_ext = mine, False
 
     def _end_update(self, present=None, acc: bool = False, ema: bool = True) -> None:
         """Every update that is not a bucket's eager one, then the optimizer's step count and
@@ -544,6 +567,8 @@ class GradBucketPipeline:
             KERNELS.grad_sumsq_clip(grads[:n_model], n_model, pre_scale=scale, max_norm=self.clip_norm,
                                     out3=self.clip_out, scratch=self.clip_scratch)
             coef = self.clip_out[2:3]
+        if not acc:
+            have -= self.dw_updated               # K12 updated these inside their dW GEMMs
         if self.whole_tensors or (not acc and self._ext and coef is None and not self.distributed):
             # one update over a table of the present slots: whole tensors (per-tensor norms), or on
             # one GPU every gradient read where it lies -- no flatten pass
@@ -553,7 +578,7 @@ class GradBucketPipeline:
             self._tap_end(tap, self.update_events, 0, n)
         else:
             done = [(b.lo, b.hi) for b in self.buckets if b.launched and self.eager]
-            runs = [(0, n)] if every else self._runs(
+            runs = [(0, n)] if len(have) == len(slots) else self._runs(
                 lambda s: s.index in have and not any(a <= s.offset < z for a, z in done))
             for lo, hi in runs:
                 tap = None if acc else self._tap()

@@ -113,6 +113,7 @@ class _Captured:
         # those addresses, the tail update / the captured flatten launches read them there
         self.grad_refs, self.tables = w.pipeline.detach_grad_refs()
         self.ready = w.pipeline.last_ready     # slots the captured K10 launch accumulates (k > 1)
+        self.dw_updated = w.pipeline.dw_updated    # slots the captured K12 launches update
         # capture executed nothing on the device, but begin_step() counted a step: undo it, the
         # replay performs the step for real (finish_step(defer_tail=True) left the optimizer's
         # step counter to run_tail())
@@ -146,7 +147,7 @@ class _Captured:
         REPLAYED_LAUNCHES += self.frl_kernels
         w.pipeline.step_id += 1
         # tail update (1 GPU / clipping) + step counter; with accumulation the group's update
-        w.pipeline.run_tail(self.grad_refs, self.tables, self.ready)
+        w.pipeline.run_tail(self.grad_refs, self.tables, self.ready, self.dw_updated)
         if sink_row is not None:
             row = self._loss_vec
             if row is None:

@@ -447,7 +447,9 @@ class Solver:
                 ("fused NVLS kernel per bucket (K7), %d buckets" % len(pipeline.buckets)) if pipeline.nvls is not None
                 else ("ncclAllReduce in place + K2 per bucket, %d buckets" % len(pipeline.buckets)) if distributed
                 else "none (1 GPU)",
-                "per bucket on the side stream" if pipeline.eager else "one tail launch",
+                "per bucket on the side stream" if pipeline.eager else
+                "in the dW GEMM's epilogue (K12) for trunk Linear weights that qualify, one tail launch for the rest"
+                if pipeline.fused_dw_update else "one tail launch",
                 len(pipeline.linear_sites), sum(s.relu is not None for s in pipeline.linear_sites),
                 sum(s.fp8 for s in pipeline.linear_sites),
                 "read in place through segment tables (K2-mt / one flatten launch per bucket)"

@@ -83,6 +83,25 @@ int frl_rmsprop(float* p, const void* g, float* sq, float* buf, void* p_lp, int6
              void* stream);
 
 /* ------------------------------------------------------------------------------------------
+ * K12 — weight-gradient GEMM gw = dz^T x on the tensor cores (persistent, TMA + WGMMA), with
+ * an optional SGD update of the same weights in its epilogue.
+ *   dz [rows, out] (leading dimension ld_dz), x [rows, in] (ld_x): row-major bf16;
+ *   gw [out, in]: contiguous bf16, written in both forms (fp32 accumulation, rounded once).
+ *   out % 128 == 0, in % 256 == 0, rows % 64 == 0 (FRL_E_ARG); every pointer 16-byte aligned
+ *   and ld_dz, ld_x multiples of 8 (FRL_E_ALIGN / FRL_E_ARG).
+ * frl_dw_gemm     : gw only (what torch.mm(dz.t(), x, out=gw) computes).
+ * frl_dw_gemm_sgd : gw, then frl_sgd_momentum's update of p / buf / p_lp ([out, in], contiguous)
+ *                   applied to exactly the bf16 gw just written: bit-identical to frl_dw_gemm
+ *                   followed by frl_sgd_momentum(g_dtype = FRL_BF16) over the slice.
+ * ---------------------------------------------------------------------------------------- */
+int frl_dw_gemm(const void* dz, int64_t ld_dz, const void* x, int64_t ld_x, int64_t rows,
+                int64_t out, int64_t in, void* gw, void* stream);
+int frl_dw_gemm_sgd(const void* dz, int64_t ld_dz, const void* x, int64_t ld_x, int64_t rows,
+                    int64_t out, int64_t in, void* gw, float* p, float* buf, void* p_lp,
+                    double lr, double mu, double dampening, double wd, double grad_scale,
+                    const float* dyn, int first_step, void* stream);
+
+/* ------------------------------------------------------------------------------------------
  * K2-mt / K1 — multi-tensor forms of the update and the bucket flatten.
  * Replaces the DDP reducer's per-tensor bucket copy-in / copy-out (reference solver.py:287-289 ->
  * torch Reducer) for parameters whose gradients autograd allocates itself (convolutions,
