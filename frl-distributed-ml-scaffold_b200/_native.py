@@ -69,6 +69,11 @@ SIGNATURES = {
     "frl_lars_mt": (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _i64, _i64, _vp, _vp, _vp, _d, _d, _d, _d, _vp, _vp, _i, _vp]),
     "frl_lamb_mt": (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _i64, _i64, _vp, _vp, _vp, _d, _d, _d, _d, _d, _i64,
                          _d, _vp, _vp, _vp]),
+    "frl_q8_tables": (None, [_vp, _vp]),
+    "frl_adam8_mt": (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _i64, _i64, _vp, _vp, _d, _d, _d, _d, _d,
+                          _i64, _d, _vp, _vp, _vp]),
+    "frl_q8_encode_mt": (_i, [_vp, _vp, _vp, _i, _vp, _vp, _vp, _i64, _i64, _vp, _vp]),
+    "frl_q8_decode_mt": (_i, [_vp, _vp, _vp, _i, _vp, _vp, _vp, _i64, _i64, _vp, _vp]),
     "frl_grad_accumulate_mt": (_i, [_vp, _vp, _vp, _vp, _i64, _d, _i, _vp, _vp]),
     "frl_weight_ema": (_i, [_vp, _vp, _i64, _d, _vp]),
     "frl_reduce_scratch_bytes": (_i64, []),
@@ -302,6 +307,64 @@ def lamb_mt(p, m, v, p_lp, table, flags, ratio, scratch, *, lr, beta1, beta2, ep
                              table.tile_seg_dev_ptr, table.n_tiles, table.n_segs, _ptr(flags), _ptr(ratio),
                              _ptr(scratch), lr, beta1, beta2, eps, wd, step, grad_scale, _ptr(grad_scale_dev),
                              _ptr(dyn), _stream()), "frl_lamb_mt")
+
+
+# ---- K2-q8: Adam with 8-bit block-wise state over a segment table ---------------------------------
+
+Q8_BLOCK = 256                        # elements per quantisation block (FRL_Q8_BLOCK)
+Q8_EXP_AVG, Q8_EXP_AVG_SQ = 0, 1
+
+
+def q8_device_tables():
+    """The library's (MAG7, MAG8) tables as fp32 CPU tensors of 128 and 256 entries."""
+    mag7, mag8 = torch.zeros(128, dtype=torch.float32), torch.zeros(256, dtype=torch.float32)
+    lib().frl_q8_tables(_ptr(mag7), _ptr(mag8))
+    return mag7, mag8
+
+
+def _check_q8(table, qbase, flags=None, codes=(), absmax=(), fp32=()) -> None:
+    for t in fp32:
+        if t is not None and not (t.dtype == torch.float32 and t.is_contiguous()):
+            raise NativeLibraryError("8-bit state: master weights and fp32 state must be contiguous fp32")
+    for q in codes:
+        if not (q.dtype == torch.uint8 and q.is_contiguous()):
+            raise NativeLibraryError("8-bit state: codes must be contiguous uint8 (one byte per arena element)")
+    for a in absmax:
+        if not (a.dtype == torch.float32 and a.is_contiguous()):
+            raise NativeLibraryError("8-bit state: absmax must be contiguous fp32")
+    if qbase.dtype != torch.int64 or qbase.numel() < table.n_segs:
+        raise NativeLibraryError("8-bit state: qbase must be int64 [n_segs]")
+    if flags is not None and (flags.dtype != torch.int32 or flags.numel() < table.n_segs):
+        raise NativeLibraryError("8-bit state: seg_flags must be int32 [n_segs]")
+
+
+def adam8_mt(p, m_q, v_q, m_absmax, v_absmax, p_lp, table, qbase, flags, *, lr, beta1, beta2, eps, wd, step,
+             grad_scale=1.0, grad_scale_dev=None, dyn=None) -> None:
+    """K2-q8 Adam over the segments of ``table`` with 8-bit block-wise ``exp_avg`` / ``exp_avg_sq``.
+    See frl_adam8_mt in include/frl_b200.h."""
+    _check_q8(table, qbase, flags, codes=(m_q, v_q), absmax=(m_absmax, v_absmax), fp32=(p,))
+    _check(lib().frl_adam8_mt(_ptr(p), _ptr(m_q), _ptr(v_q), _ptr(m_absmax), _ptr(v_absmax), _ptr(p_lp),
+                              table.segs_dev_ptr, table.prefix_dev_ptr, table.tile_seg_dev_ptr, table.n_tiles,
+                              table.n_segs, _ptr(qbase), _ptr(flags), lr, beta1, beta2, eps, wd, step, grad_scale,
+                              _ptr(grad_scale_dev), _ptr(dyn), _stream()), "frl_adam8_mt")
+
+
+def q8_encode_mt(x, q, absmax, state: int, table, qbase) -> None:
+    """Codes and absmax of the fp32 arena-shaped ``x`` over the segments of ``table`` (``state``:
+    ``Q8_EXP_AVG`` or ``Q8_EXP_AVG_SQ``).  See frl_q8_encode_mt in include/frl_b200.h."""
+    _check_q8(table, qbase, codes=(q,), absmax=(absmax,), fp32=(x,))
+    _check(lib().frl_q8_encode_mt(_ptr(x), _ptr(q), _ptr(absmax), int(state), table.segs_dev_ptr,
+                                  table.prefix_dev_ptr, table.tile_seg_dev_ptr, table.n_tiles, table.n_segs,
+                                  _ptr(qbase), _stream()), "frl_q8_encode_mt")
+
+
+def q8_decode_mt(q, absmax, x, state: int, table, qbase) -> None:
+    """fp32 values of the codes over the segments of ``table`` into the arena-shaped ``x``.  See
+    frl_q8_decode_mt in include/frl_b200.h."""
+    _check_q8(table, qbase, codes=(q,), absmax=(absmax,), fp32=(x,))
+    _check(lib().frl_q8_decode_mt(_ptr(q), _ptr(absmax), _ptr(x), int(state), table.segs_dev_ptr,
+                                  table.prefix_dev_ptr, table.tile_seg_dev_ptr, table.n_tiles, table.n_segs,
+                                  _ptr(qbase), _stream()), "frl_q8_decode_mt")
 
 
 # ---- K10: gradient accumulation over a segment table ----------------------------------------------

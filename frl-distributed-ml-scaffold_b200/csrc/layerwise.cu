@@ -42,10 +42,6 @@ struct LambParams {
     }
 };
 
-__device__ __forceinline__ float seg_scale(int flags, float gscale, const float* gscale_dev) {
-    return (gscale_dev != nullptr && (flags & FRL_LW_CLIPPED)) ? gscale * __ldg(gscale_dev) : gscale;
-}
-
 // sum of a and of b over the block, fixed order; valid in thread 0.  smem: 64 T.
 template <typename T>
 __device__ __forceinline__ void block_sum2(T& a, T& b, T* smem) {

@@ -1,5 +1,6 @@
 // Tiling shared by the streaming update kernels: the flat K2 update and the segment-table forms
-// (K2-mt, K1 flatten in optim.cu; the layer-wise LARS / LAMB kernels in layerwise.cu).
+// (K2-mt, K1 flatten in optim.cu; the layer-wise LARS / LAMB kernels in layerwise.cu; the 8-bit
+// state Adam kernels in adam8.cu).
 #pragma once
 #include "frl_common.cuh"
 
@@ -62,6 +63,12 @@ __device__ __forceinline__ f32x4 seg_load4(const SegView& sv, int64_t e) {
             t[k] = sv.g_dtype == FRL_F32 ? static_cast<const float*>(sv.g)[e + k]
                                          : __bfloat162float(static_cast<const __nv_bfloat16*>(sv.g)[e + k]);
     return f32x4{t[0], t[1], t[2], t[3]};
+}
+
+// gradient scale of a segment: the device clip coefficient multiplies the segments flagged
+// FRL_LW_CLIPPED (model parameters) only
+__device__ __forceinline__ float seg_scale(int flags, float gscale, const float* gscale_dev) {
+    return (gscale_dev != nullptr && (flags & FRL_LW_CLIPPED)) ? gscale * __ldg(gscale_dev) : gscale;
 }
 
 // grid over tiles: one resident wave (CTAs that fit per SM for this kernel x SM count), capped by

@@ -6,7 +6,9 @@
 is L2-coupled and applies to every parameter).  ``state_dict()`` / ``load_state_dict()`` speak
 torch's per-parameter format so the reference's ``.checkpoint.pth`` files stay interchangeable.
 ``FusedLars`` / ``FusedLamb`` (an extension, ``types.LayerAdaptation``) keep SGD's / Adam's state
-format and update whole tensors through the K2-lw kernels.
+format and update whole tensors through the K2-lw kernels.  ``FusedAdam8bit`` (an extension,
+``types.OptimizerState``) keeps Adam's moments as 8-bit block-wise codes (K2-q8) and speaks
+``torch.optim.Adam``'s format in its state dict.
 
 Known limitation: the step count (Adam's bias corrections) is ONE number for the whole arena.
 ``torch.optim`` keeps one per parameter and does not advance it for a parameter whose gradient
@@ -18,11 +20,12 @@ receive a gradient every step — every configuration of BASELINE.json — are u
 """
 from typing import Any, Dict, List, Optional, Tuple
 
+import numpy as np
 import torch
 
 from . import _native
 from .arena import ParamArena
-from .types import LayerAdaptation, OptAlgorithm, OptimOpts
+from .types import LayerAdaptation, OptAlgorithm, OptimizerState, OptimOpts
 
 # Kernel entry points; tests exercising host logic on CPU swap this for an oracle-backed double.
 KERNELS = _native
@@ -393,14 +396,48 @@ def is_adapted(slot) -> bool:
     return len(slot.shape) >= 2
 
 
-class _LayerwiseMixin:
-    """K2-lw: trust-ratio updates over a segment table (``frl_lars_mt`` / ``frl_lamb_mt``).  The
-    per-table device buffers (adaptation flags, ratios, scratch) are built on first use and kept on
-    the table, so a CUDA-graph capture's table set owns its own."""
+class _WholeTensorMixin:
+    """An update over whole tensors through a segment table (``apply_table``): the pipeline runs it
+    once after backward.  The flat-bucket and fused NVLS launchers of the base rule see parts of
+    tensors: never reached, and refused rather than silently wrong."""
 
     @property
     def needs_whole_tensors(self) -> bool:
         return True
+
+    def _launch(self, lo, hi, grad_scale, coef):
+        raise RuntimeError("%s updates whole tensors: use apply_table / apply_range" % type(self).__name__)
+
+    def _launch_mt(self, table, grad_scale):
+        raise RuntimeError("%s updates through its own segment-table kernel: use apply_table" % type(self).__name__)
+
+    def _launch_nvls(self, lo, hi, grad_scale):
+        raise RuntimeError("%s has no fused NVLS step (its update needs whole tensors)" % type(self).__name__)
+
+    def apply_range(self, lo: int, hi: int, *, grad_scale: float = 1.0,
+                    clip_coef_dev: Optional[torch.Tensor] = None) -> None:
+        """Whole slots inside ``[lo, hi)``, gradients read from the arena."""
+        from .multi_tensor import GradSegTable
+        tables = self.__dict__.setdefault("_range_tables", {})
+        table = tables.get((lo, hi))
+        if table is None:
+            slots = [s for s in self.arena.slots if lo <= s.offset and s.end <= hi]
+            cut = [s.index for s in self.arena.slots if s.offset < hi and s.end > lo and s not in slots]
+            if cut:
+                raise ValueError("%s takes whole tensors: [%d, %d) cuts the slots of parameters %s"
+                                 % (type(self).__name__, lo, hi, cut))
+            table = tables[(lo, hi)] = GradSegTable(slots, self.arena.device)
+            g = self.arena.grad
+            for s in slots:
+                table.point(s, g.data_ptr() + s.offset * g.element_size(), g.dtype)
+        table.upload()
+        self.apply_table(table, grad_scale=grad_scale, clip_coef_dev=clip_coef_dev)
+
+
+class _LayerwiseMixin(_WholeTensorMixin):
+    """K2-lw: trust-ratio updates over a segment table (``frl_lars_mt`` / ``frl_lamb_mt``).  The
+    per-table device buffers (adaptation flags, ratios, scratch) are built on first use and kept on
+    the table, so a CUDA-graph capture's table set owns its own."""
 
     def _lw_buffers(self, table):
         bufs = getattr(table, "layerwise", None)
@@ -422,40 +459,9 @@ class _LayerwiseMixin:
         if table.n_segs:
             self._launch_lw(table, grad_scale, clip_coef_dev, *self._lw_buffers(table))
 
-    # the flat-bucket and fused NVLS launchers of the base rule see parts of tensors, and read
-    # another ``dyn`` layout: never reached, and refused rather than silently wrong
-    def _launch(self, lo, hi, grad_scale, coef):
-        raise RuntimeError("%s updates whole tensors: use apply_table / apply_range" % type(self).__name__)
-
-    def _launch_mt(self, table, grad_scale):
-        raise RuntimeError("%s updates through the K2-lw kernels: use apply_table" % type(self).__name__)
-
-    def _launch_nvls(self, lo, hi, grad_scale):
-        raise RuntimeError("%s has no fused NVLS step (per-tensor norms need whole tensors)"
-                           % type(self).__name__)
-
     def last_ratios(self, table) -> torch.Tensor:
         """Trust ratio of each slot of ``table`` from its last update (device tensor)."""
         return self._lw_buffers(table)[1][:table.n_segs]
-
-    def apply_range(self, lo: int, hi: int, *, grad_scale: float = 1.0,
-                    clip_coef_dev: Optional[torch.Tensor] = None) -> None:
-        """Whole slots inside ``[lo, hi)``, gradients read from the arena."""
-        from .multi_tensor import GradSegTable
-        tables = self.__dict__.setdefault("_range_tables", {})
-        table = tables.get((lo, hi))
-        if table is None:
-            slots = [s for s in self.arena.slots if lo <= s.offset and s.end <= hi]
-            cut = [s.index for s in self.arena.slots if s.offset < hi and s.end > lo and s not in slots]
-            if cut:
-                raise ValueError("layer-wise updates take whole tensors: [%d, %d) cuts the slots of "
-                                 "parameters %s" % (lo, hi, cut))
-            table = tables[(lo, hi)] = GradSegTable(slots, self.arena.device)
-            g = self.arena.grad
-            for s in slots:
-                table.point(s, g.data_ptr() + s.offset * g.element_size(), g.dtype)
-        table.upload()
-        self.apply_table(table, grad_scale=grad_scale, clip_coef_dev=clip_coef_dev)
 
 
 class FusedLars(_LayerwiseMixin, FusedSGD):
@@ -498,6 +504,149 @@ class FusedLamb(_LayerwiseMixin, FusedAdam):
                         step=self._steps + 1, grad_scale=grad_scale, grad_scale_dev=coef, dyn=self._dyn)
 
 
+# ---- 8-bit block-wise Adam state (K2-q8) ----------------------------------------------------------
+
+Q8_BLOCK = 256           # elements per quantisation block; blocks start at each tensor's first element
+_DECADES = (1e-6, 1e-5, 1e-4, 1e-3, 1e-2, 1e-1, 1.0)
+
+
+def q8_tables() -> Tuple[np.ndarray, np.ndarray]:
+    """The storage format's two code tables (the dynamic tree map), fp32, increasing:
+    ``MAG7`` (128 entries, ``exp_avg`` magnitudes: code = sign bit << 7 | index) and ``MAG8``
+    (256 entries, ``exp_avg_sq``).  Each entry is formed in float64 and rounded once to fp32; both
+    hold 0 and 1.  csrc/adam8.cu builds the same tables from the same expression."""
+    mag7, mag8 = [0.0], [0.0]
+    for i, dec in enumerate(_DECADES):
+        n7, n8 = 1 << i, 2 << i
+        mag7 += [dec * (0.1 + 0.9 * (j + 0.5) / n7) for j in range(n7)]
+        mag8 += [dec * (0.1 + 0.9 * (j + 0.5) / n8) for j in range(n8)]
+    mag7[-1] = 1.0                      # replaces the largest, 0.99296875
+    mag8.append(1.0)
+    return np.asarray(mag7, dtype=np.float32), np.asarray(mag8, dtype=np.float32)
+
+
+def q8_block_bases(slots) -> Tuple[Dict[int, int], int]:
+    """Global index of each slot's first block (by slot index): a prefix sum of ceil(numel / 256)
+    over ``slots`` in arena order, and the total number of blocks."""
+    bases, n = {}, 0
+    for s in sorted(slots, key=lambda s: s.offset):
+        bases[s.index] = n
+        n += (s.numel + Q8_BLOCK - 1) // Q8_BLOCK
+    return bases, n
+
+
+class FusedAdam8bit(_WholeTensorMixin, FusedAdam):
+    """Adam (``FusedAdam``'s rule and hyper-parameters, no amsgrad) with ``exp_avg`` /
+    ``exp_avg_sq`` kept as 8-bit block-wise codes (``types.OptimizerState.Q8``): one byte per
+    arena element per state plus one fp32 absmax per 256-element block, updated by one K2-q8 launch
+    over a segment table after backward.  ``state_dict()`` writes ``torch.optim.Adam``'s format with
+    the decoded fp32 moments; ``load_state_dict()`` encodes them, so checkpoints move between
+    ``torch.optim.Adam``, ``FusedAdam`` and this optimizer in both directions, and a run resumed
+    from its own checkpoint continues bit for bit (decode-then-encode returns the same codes)."""
+
+    STATE_NAMES = (("exp_avg", "exp_avg"), ("exp_avg_sq", "exp_avg_sq"))
+
+    def __init__(self, arena, lr, betas=(0.9, 0.999), eps=1e-8, weight_decay=0.0):
+        super().__init__(arena, lr=lr, betas=betas, eps=eps, weight_decay=weight_decay, amsgrad=False)
+        self._qbase, self.q8_blocks = q8_block_bases(arena.slots)
+        dev = arena.device
+        self.codes = {n: torch.zeros(arena.numel, dtype=torch.uint8, device=dev) for n, _ in self.STATE_NAMES}
+        self.absmax = {n: torch.zeros(max(self.q8_blocks, 1), dtype=torch.float32, device=dev)
+                       for n, _ in self.STATE_NAMES}
+        self._all_table = None
+
+    @property
+    def state_bytes(self) -> int:
+        """Device bytes of the optimizer state (codes and absmax of both moments)."""
+        return sum(t.numel() * t.element_size() for d in (self.codes, self.absmax) for t in d.values())
+
+    @property
+    def fp32_state_bytes(self) -> int:
+        """What ``FusedAdam`` keeps for the same arena: two fp32 arena-shaped vectors."""
+        return 2 * 4 * self.arena.numel
+
+    def _q8_buffers(self, table):
+        """Per-table device arrays, kept on the table: each slot's first block, and its flags
+        (``LW_CLIPPED``: model parameters take the clip coefficient)."""
+        bufs = getattr(table, "adam8", None)
+        if bufs is None:
+            dev = self.arena.device
+            qbase = torch.tensor([self._qbase[s.index] for s in table.slots] or [0], dtype=torch.int64).to(dev)
+            flags = torch.tensor([KERNELS.LW_CLIPPED if s.is_model else 0 for s in table.slots] or [0],
+                                 dtype=torch.int32).to(dev)
+            bufs = table.adam8 = (qbase, flags)
+        return bufs
+
+    def apply_table(self, table, *, grad_scale: float = 1.0,
+                    clip_coef_dev: Optional[torch.Tensor] = None) -> None:
+        """Update every slot of ``table`` (K2-q8); ``clip_coef_dev`` multiplies the gradients of
+        model parameters only, as in ``apply_range``."""
+        if not table.n_segs:
+            return
+        h = self.hyper
+        qbase, flags = self._q8_buffers(table)
+        KERNELS.adam8_mt(self.arena.master, self.codes["exp_avg"], self.codes["exp_avg_sq"],
+                         self.absmax["exp_avg"], self.absmax["exp_avg_sq"], self.arena.lp, table, qbase, flags,
+                         lr=float(h["lr"]), beta1=float(h["betas"][0]), beta2=float(h["betas"][1]),
+                         eps=float(h["eps"]), wd=float(h["weight_decay"]), step=self._steps + 1,
+                         grad_scale=grad_scale, grad_scale_dev=clip_coef_dev, dyn=self._dyn)
+
+    def _every_slot(self):
+        if self._all_table is None:
+            from .multi_tensor import GradSegTable
+            self._all_table = GradSegTable(self.arena.slots, self.arena.device)     # gradients not read
+            self._all_table.upload()
+        return self._all_table, self._q8_buffers(self._all_table)[0]
+
+    def decoded(self, name: str) -> torch.Tensor:
+        """``exp_avg`` or ``exp_avg_sq`` decoded into a fresh fp32 arena-shaped vector."""
+        table, qbase = self._every_slot()
+        out = self.arena.new_state()
+        KERNELS.q8_decode_mt(self.codes[name], self.absmax[name], out, self._state_code(name), table, qbase)
+        return out
+
+    def _encode(self, name: str, x: torch.Tensor) -> None:
+        table, qbase = self._every_slot()
+        KERNELS.q8_encode_mt(x, self.codes[name], self.absmax[name], self._state_code(name), table, qbase)
+
+    @staticmethod
+    def _state_code(name: str) -> int:
+        return KERNELS.Q8_EXP_AVG if name == "exp_avg" else KERNELS.Q8_EXP_AVG_SQ
+
+    def state_dict(self) -> Dict[str, Any]:
+        self._vec = {n: self.decoded(n) for n, _ in self.STATE_NAMES} if self._steps > 0 else {}
+        try:
+            return super().state_dict()
+        finally:
+            self._vec = {}
+
+    def load_state_dict(self, state_dict: Dict[str, Any]) -> None:
+        for g in state_dict["param_groups"]:
+            if g.get("amsgrad", False):
+                raise ValueError("8-bit Adam state holds no max_exp_avg_sq: an amsgrad state dict cannot be loaded")
+        self._vec = {}
+        try:
+            super().load_state_dict(state_dict)       # fills fp32 vectors through _state()
+            for name, _ in self.STATE_NAMES:
+                self._encode(name, self._vec[name] if name in self._vec else self.arena.new_state())
+        finally:
+            self._vec = {}
+
+
+def check_optimizer_state(optim_opts: OptimOpts, layer_adaptation: LayerAdaptation,
+                          optimizer_state: OptimizerState) -> None:
+    """8-bit state needs Adam without amsgrad and without layer adaptation; anything else is a
+    ValueError naming the values."""
+    st = OptimizerState(optimizer_state)
+    la = LayerAdaptation(layer_adaptation)
+    if st is OptimizerState.Q8 and not (optim_opts.algo == OptAlgorithm.ADAM and not optim_opts.amsgrad
+                                        and la is LayerAdaptation.NONE):
+        raise ValueError("optimizer state %r cannot be combined with optimizer %r%s and layer adaptation %r "
+                         "(8-bit state needs adam without amsgrad and layer adaptation none)"
+                         % (st.value, getattr(optim_opts.algo, "value", optim_opts.algo),
+                            " with amsgrad" if optim_opts.amsgrad else "", la.value))
+
+
 def check_layer_adaptation(optim_opts: OptimOpts, layer_adaptation: LayerAdaptation) -> None:
     """LARS needs the SGD rule, LAMB the Adam rule without amsgrad; anything else is a ValueError."""
     la = LayerAdaptation(layer_adaptation)
@@ -512,10 +661,14 @@ def check_layer_adaptation(optim_opts: OptimOpts, layer_adaptation: LayerAdaptat
 
 
 def create_fused_optimizer(arena: ParamArena, optim_opts: OptimOpts,
-                           layer_adaptation: LayerAdaptation = LayerAdaptation.NONE) -> FusedArenaOptimizer:
+                           layer_adaptation: LayerAdaptation = LayerAdaptation.NONE,
+                           optimizer_state: OptimizerState = OptimizerState.FP32) -> FusedArenaOptimizer:
     """Same dispatch and argument mapping as the reference's ``_create_optimizer``; with a layer
-    adaptation, its LARS / LAMB counterpart."""
+    adaptation, its LARS / LAMB counterpart; with 8-bit optimizer state, ``FusedAdam8bit``."""
     check_layer_adaptation(optim_opts, layer_adaptation)
+    check_optimizer_state(optim_opts, layer_adaptation, optimizer_state)
+    if OptimizerState(optimizer_state) is OptimizerState.Q8:
+        return FusedAdam8bit(arena, lr=optim_opts.lr, weight_decay=optim_opts.weightDecay, eps=optim_opts.epsilon)
     if layer_adaptation == LayerAdaptation.LARS:
         return FusedLars(arena, lr=optim_opts.lr, momentum=optim_opts.momentum,
                          weight_decay=optim_opts.weightDecay)

@@ -9,7 +9,7 @@ from typing import Optional
 
 from .problem import Problem
 from .solver import PerformanceSummary, Solver
-from .types import LayerAdaptation, Precision, RunOpts
+from .types import LayerAdaptation, OptimizerState, Precision, RunOpts
 
 logger = logging.getLogger(__name__)
 
@@ -22,7 +22,8 @@ class LocalSolver:
               precision: Optional[Precision] = None, graph: Optional[bool] = None, *,
               layer_adaptation: Optional[LayerAdaptation] = None,
               grad_accumulation: Optional[int] = None,
-              ema_decay: Optional[float] = None) -> PerformanceSummary:
+              ema_decay: Optional[float] = None,
+              optimizer_state: Optional[OptimizerState] = None) -> PerformanceSummary:
         if save_notebook:
             logger.warning("save_notebook is not supported by frl_b200 (visualisation only)")
         # a stale rendezvous file from a crashed run would poison the file:// store
@@ -35,6 +36,7 @@ class LocalSolver:
         for last in Solver.solve(run_opts, problem, group_name=group_name,
                                  init_method="file://" + SYNC_FILE, precision=precision,
                                  graph=graph, layer_adaptation=layer_adaptation,
-                                 grad_accumulation=grad_accumulation, ema_decay=ema_decay):
+                                 grad_accumulation=grad_accumulation, ema_decay=ema_decay,
+                                 optimizer_state=optimizer_state):
             pass
         return last

@@ -29,13 +29,14 @@ import torch.nn as nn
 from .arena import ParamArena
 from .criteria import BaseParallelCriterion
 from .ema import EMA_STATE_KEY
-from .fused_optim import check_layer_adaptation, create_fused_optimizer, is_adapted
+from .fused_optim import (FusedAdam8bit, check_layer_adaptation, check_optimizer_state, create_fused_optimizer,
+                          is_adapted)
 from .grad_sync import BufferBroadcaster, GradBucketPipeline
 from .lr_scheduler import DropEpochsScheduler, WarmupMultiStepLR
 from .problem import Problem
 from .solver_worker import (FractionalPerformanceSummary, SerializableSampleSummary,
                             SolverWorker)
-from .types import (Device, LayerAdaptation, LRSchedulerAlgorithm, Mode, Precision, RunOpts,
+from .types import (Device, LayerAdaptation, LRSchedulerAlgorithm, Mode, OptimizerState, Precision, RunOpts,
                     SampleSummary, Split)
 
 logging.basicConfig(level=logging.INFO, format="%(levelname)s (%(process)d) %(message)s")
@@ -46,6 +47,7 @@ LAYER_ADAPTATION_ENV = "FRL_B200_LAYER_ADAPTATION"   # "none" (default) | "lars"
 PRECISION_ENV = "FRL_B200_PRECISION"      # "fp32" (default, reference parity) | "bf16"
 GRAD_ACCUM_ENV = "FRL_B200_GRAD_ACCUM"     # microbatches per optimizer update, default 1
 EMA_DECAY_ENV = "FRL_B200_EMA_DECAY"       # weight EMA decay in [0, 1), default 0 (off)
+OPTIMIZER_STATE_ENV = "FRL_B200_OPTIMIZER_STATE"   # "fp32" (default) | "8bit"
 EMA_SUFFIX = ".ema"                        # <checkpoint>.ema: the weight EMA next to a checkpoint
 
 
@@ -100,6 +102,8 @@ class SolverWorkerArgs(NamedTuple):
     save_every: int = 1
     graph_step: Optional[bool] = None      # None: FRL_B200_CUDA_GRAPH (default off)
     layer_adaptation: LayerAdaptation = LayerAdaptation.NONE
+    # Adam's state storage; placed before ema_decay and grad_accumulation, which stay the last fields
+    optimizer_state: OptimizerState = OptimizerState.FP32
     # weight EMA decay, 0 = off; placed before grad_accumulation, which stays the last field
     ema_decay: float = 0.0
     grad_accumulation: int = 1
@@ -250,6 +254,14 @@ def resolve_layer_adaptation(explicit: Optional[LayerAdaptation] = None) -> Laye
     return LayerAdaptation(os.environ.get(LAYER_ADAPTATION_ENV, "none").lower())
 
 
+def resolve_optimizer_state(explicit: Optional[OptimizerState] = None) -> OptimizerState:
+    """Adam's state storage: ``explicit``, else FRL_B200_OPTIMIZER_STATE, else fp32.  An unknown value
+    is a ValueError."""
+    if explicit is not None:
+        return OptimizerState(explicit)
+    return OptimizerState(os.environ.get(OPTIMIZER_STATE_ENV, "fp32").lower())
+
+
 def resolve_grad_accumulation(explicit: Optional[int] = None) -> int:
     """Microbatches per optimizer update: ``explicit``, else FRL_B200_GRAD_ACCUM, else 1.  Anything
     but an integer >= 1 (``0``, negatives, ``2.5``, ``True``, non-numeric strings) is a ValueError."""
@@ -366,7 +378,8 @@ class Solver:
         ema_decay = args.ema_decay if run_opts.mode == Mode.TRAIN else 0.0
         symm_alloc = None
         if (distributed and not run_opts.optim.gradientClip
-                and args.layer_adaptation == LayerAdaptation.NONE and accum == 1 and ema_decay == 0.0):
+                and args.layer_adaptation == LayerAdaptation.NONE and accum == 1 and ema_decay == 0.0
+                and args.optimizer_state is OptimizerState.FP32):
             from .symm import try_make_allocator
             symm_alloc = try_make_allocator(device, args.world_size)
         from .arena_linear import head_layout_groups
@@ -382,7 +395,8 @@ class Solver:
             for buf in model.buffers():
                 if buf.is_floating_point():
                     buf.data = buf.data.to(torch.bfloat16)
-        optimizer = create_fused_optimizer(arena, run_opts.optim, args.layer_adaptation)
+        opt_state = args.optimizer_state if run_opts.mode == Mode.TRAIN else OptimizerState.FP32
+        optimizer = create_fused_optimizer(arena, run_opts.optim, args.layer_adaptation, opt_state)
         if checkpoint:
             optimizer.load_state_dict(checkpoint.optimizerState)
         ema = None
@@ -441,7 +455,8 @@ class Solver:
             logger.info(
                 "frl_b200 step: precision %s | step issue %s | gradient exchange %s | update %s | "
                 "Linear layers with arena-born gradients %d (%d fused with their ReLU, %d in FP8) | "
-                "other gradients %s | layer adaptation %s | gradient accumulation %s | weight EMA %s",
+                "other gradients %s | layer adaptation %s | gradient accumulation %s | weight EMA %s | "
+                "optimizer state %s",
                 args.precision.value,
                 "CUDA-graph replay after 2 eager steps" if worker.graphed is not None else "eager launches",
                 ("fused NVLS kernel per bucket (K7), %d buckets" % len(pipeline.buckets)) if pipeline.nvls is not None
@@ -462,7 +477,10 @@ class Solver:
                     accum, pipeline.accumulator_bytes / 2 ** 20),
                 "none" if ema is None else
                 "decay %r, one K11 launch per update (%.1f MiB), held-out splits evaluated with it" % (
-                    ema_decay, ema.nbytes / 2 ** 20))
+                    ema_decay, ema.nbytes / 2 ** 20),
+                "8-bit block-wise (K2-q8), %.1f MiB instead of %.1f MiB" % (
+                    optimizer.state_bytes / 2 ** 20, optimizer.fp32_state_bytes / 2 ** 20)
+                if isinstance(optimizer, FusedAdam8bit) else "fp32")
         scheduler = create_lr_scheduler(run_opts, worker.optimizer,
                                         checkpoint.epoch if checkpoint else -1)
         return worker, scheduler, checkpoint
@@ -672,7 +690,8 @@ class Solver:
               precision: Optional[Precision] = None, graph: Optional[bool] = None,
               layer_adaptation: Optional[LayerAdaptation] = None,
               grad_accumulation: Optional[int] = None,
-              ema_decay: Optional[float] = None
+              ema_decay: Optional[float] = None,
+              optimizer_state: Optional[OptimizerState] = None
               ) -> Iterator[PerformanceSummary]:
         """The reference's entry point (solver.py:728-739) plus two keyword-only extensions:
 
@@ -737,13 +756,24 @@ class Solver:
                        parameters (buffers: see INTEGRATION.md; rank 0's are saved).
                        None: FRL_B200_EMA_DECAY (default 0).  Any value but a real number in
                        [0, 1) raises ``ValueError`` before a rank starts.  ``Mode.EVAL`` ignores it.
+        ``optimizer_state``  ``OptimizerState.FP32`` (default) or ``.Q8``: Adam's two moments as
+                       8-bit block-wise codes with one fp32 absmax per 256 elements (K2-q8), about
+                       a quarter of the fp32 state's memory and 16 instead of 28 bytes moved per
+                       parameter in the update; see ``types.OptimizerState``.  Needs
+                       ``OptAlgorithm.ADAM`` without amsgrad and no layer adaptation; any other
+                       combination raises ``ValueError`` before a rank starts.  Checkpoints keep
+                       ``torch.optim.Adam``'s format.  None: FRL_B200_OPTIMIZER_STATE (default
+                       ``fp32``).  ``Mode.EVAL`` ignores it.
         """
         adapt = LayerAdaptation.NONE
         accum = 1
         decay = 0.0
+        opt_state = OptimizerState.FP32
         if run_opts.mode == Mode.TRAIN:
             adapt = resolve_layer_adaptation(layer_adaptation)
             check_layer_adaptation(run_opts.optim, adapt)
+            opt_state = resolve_optimizer_state(optimizer_state)
+            check_optimizer_state(run_opts.optim, adapt, opt_state)
             accum = resolve_grad_accumulation(grad_accumulation)
             decay = resolve_ema_decay(ema_decay)
         n_visible = 0 if run_opts.cpuonly else _cuda_device_count_without_poisoning_fork()
@@ -784,7 +814,8 @@ class Solver:
                 rank=node_idx * device_count + local_rank, local_rank=local_rank,
                 world_size=world_size, group_name=group_name, init_method=init_method,
                 cache=None, precision=prec, save_every=save_every, graph_step=graph,
-                layer_adaptation=adapt, grad_accumulation=accum, ema_decay=decay)
+                layer_adaptation=adapt, grad_accumulation=accum, ema_decay=decay,
+                optimizer_state=opt_state)
             if not run_opts.singleThreaded:
                 parent_conn, child_conn = ctx.Pipe(duplex=False)
                 proc = ctx.Process(target=cls._solver_worker_process,

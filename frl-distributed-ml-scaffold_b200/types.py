@@ -115,6 +115,27 @@ class LayerAdaptation(Enum):
     LAMB = "lamb"
 
 
+class OptimizerState(Enum):
+    """Extension (not in the reference): how Adam's optimizer state is stored, chosen with
+    ``Solver.solve(..., optimizer_state=...)`` or ``FRL_B200_OPTIMIZER_STATE``.
+
+    FP32 - ``exp_avg`` and ``exp_avg_sq`` as fp32 arena-shaped vectors (8 B per parameter).
+    Q8   - 8-bit block-wise dynamic quantization (Dettmers et al., ICLR 2022): per moment one byte
+           per parameter plus one fp32 absmax per block of 256 consecutive elements of a tensor
+           (about 2.03 B per parameter).  ``exp_avg`` is sign + 7-bit index into a 128-entry
+           magnitude table, ``exp_avg_sq`` an 8-bit index into a 256-entry table (the dynamic
+           tree map; ``fused_optim.q8_tables``); values decode to ``table[k] * absmax``.  Every
+           step decodes, applies this package's Adam rule in fp32 (weights and bf16 shadow from
+           the fp32 moments of the step), then re-encodes each block to the nearest table entry
+           (K2-q8, one launch after backward).  Needs ``algo == ADAM``, ``amsgrad == False`` and
+           ``LayerAdaptation.NONE``.  The state dict is ``torch.optim.Adam``'s with decoded fp32
+           moments.  Gradients are all-reduced per bucket and the update runs once after backward:
+           no eager per-bucket update and no fused NVLS step.  ``Mode.EVAL`` ignores the setting.
+    """
+    FP32 = "fp32"
+    Q8 = "8bit"
+
+
 # --- records ---------------------------------------------------------------------------------
 
 class SampleSummary(NamedTuple):

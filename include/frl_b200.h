@@ -188,6 +188,56 @@ int frl_lamb_mt(float* p, float* m, float* v, void* p_lp, const frl_grad_seg* se
                 double grad_scale, const float* grad_scale_dev, const float* dyn, void* stream);
 
 /* ------------------------------------------------------------------------------------------
+ * K2-q8 — Adam with 8-bit block-wise optimizer state (an extension: Dettmers et al., "8-bit
+ * Optimizers via Block-wise Quantization", ICLR 2022).  exp_avg and exp_avg_sq are stored as one
+ * byte per arena element plus one fp32 absmax per block:
+ *   blocks    each segment (parameter tensor) is cut into blocks of FRL_Q8_BLOCK = 256
+ *             consecutive elements starting at its first element; the last may be short; no block
+ *             spans two segments.  Block b of segment s has the global index qbase_dev[s] + b
+ *             (qbase: a prefix sum of ceil(numel / 256) over every arena slot in arena order).
+ *   absmax    per state and block: max |x| over the block, NaN if the block holds a NaN.
+ *   exp_avg   code c = sign bit of the fp32 value << 7 | k, decodes to +-MAG7[k] * absmax.
+ *   exp_avg_sq code k, decodes to MAG8[k] * absmax.
+ *   tables    each entry computed in double and rounded once to fp32, increasing:
+ *             MAG7 = 0, then for i = 0..6, j = 0..2^i - 1: 10^(i-6) * (0.1 + 0.9*(j + 0.5)/2^i)
+ *                    (127 values), the largest of them (0.99296875) replaced by 1.0: 128 entries;
+ *             MAG8 = 0, then for i = 0..6, j = 0..2^(i+1) - 1: 10^(i-6) * (0.1 + 0.9*(j + 0.5)/2^(i+1))
+ *                    (254 values), then 1.0: 256 entries.
+ *   encoding  r = |x| / absmax (IEEE fp32 division; r = 0 if absmax == 0), the code is the index
+ *             of the table entry nearest to r, ties to the smaller index (a NaN r gives index 0).
+ *             Both tables hold 0 and 1, so decoding a block and encoding it again returns the same
+ *             bytes and absmax.
+ *   Code arrays are arena-shaped (one byte per arena element, 16-byte aligned); elements outside
+ *   every segment (padding) are never written.
+ * frl_adam8_mt: arguments of frl_adam_mt (no amsgrad) plus the code and absmax arrays, n_segs,
+ *   qbase_dev (int64 [n_segs]) and seg_flags_dev (int32 [n_segs]; FRL_LW_CLIPPED: grad_scale_dev
+ *   multiplies this segment's gradient, as in K2-lw).  Per element of a listed segment:
+ *   decode m and v; apply frl_adam_mt's fp32 rule exactly (L2-coupled wd, lerp for m, dyn);
+ *   write the master and, with p_lp, the bf16 shadow from this step's fp32 m and v; reduce the
+ *   block's new absmax of m and of v; encode.  A non-finite gradient therefore gives the weights
+ *   frl_adam_mt gives from the same decoded state.  dyn as for frl_adam_mt.  Graph-capturable.
+ * frl_q8_encode_mt / frl_q8_decode_mt: fp32 arena-shaped state x <-> codes and absmax of the
+ *   listed segments, for `state` FRL_Q8_EXP_AVG or FRL_Q8_EXP_AVG_SQ (the segment table's
+ *   gradient pointers are not read).  Decoding writes 0 to the padding of a segment's last
+ *   vector of 4.  Same encoder and decoder as frl_adam8_mt.
+ * frl_q8_tables: host copy of MAG7 (128 floats) and MAG8 (256 floats); either may be NULL.
+ * Every argument check is made before any launch; n_tiles == 0 launches nothing.
+ * ---------------------------------------------------------------------------------------- */
+enum { FRL_Q8_BLOCK = 256, FRL_Q8_EXP_AVG = 0, FRL_Q8_EXP_AVG_SQ = 1 };
+void frl_q8_tables(float* mag7, float* mag8);
+int frl_adam8_mt(float* p, uint8_t* m_q, uint8_t* v_q, float* m_absmax, float* v_absmax, void* p_lp,
+                 const frl_grad_seg* segs_dev, const int64_t* tile_prefix_dev, const int32_t* tile_seg_dev,
+                 int64_t n_tiles, int64_t n_segs, const int64_t* qbase_dev, const int32_t* seg_flags_dev,
+                 double lr, double beta1, double beta2, double eps, double wd, int64_t step,
+                 double grad_scale, const float* grad_scale_dev, const float* dyn, void* stream);
+int frl_q8_encode_mt(const float* x, uint8_t* q, float* absmax, int state, const frl_grad_seg* segs_dev,
+                     const int64_t* tile_prefix_dev, const int32_t* tile_seg_dev, int64_t n_tiles,
+                     int64_t n_segs, const int64_t* qbase_dev, void* stream);
+int frl_q8_decode_mt(const uint8_t* q, const float* absmax, float* x, int state, const frl_grad_seg* segs_dev,
+                     const int64_t* tile_prefix_dev, const int32_t* tile_seg_dev, int64_t n_tiles,
+                     int64_t n_segs, const int64_t* qbase_dev, void* stream);
+
+/* ------------------------------------------------------------------------------------------
  * K10 — gradient accumulation (an extension: the reference has no accumulation).  Several
  * microbatches per optimizer update: after each microbatch's backward, one launch folds every
  * gradient of a K2-mt segment table into an fp32 accumulator.

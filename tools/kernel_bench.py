@@ -1,7 +1,7 @@
 #!/usr/bin/env python
 """Micro-benchmark of every hand-written kernel at the BASELINE shapes (1 GPU).
 
-    python tools/kernel_bench.py [--only k2,k2lw,k3,k5a,...] [--iters 20] [--json out.json]
+    python tools/kernel_bench.py [--only k2,k2lw,k2q8,k3,k5a,...] [--iters 20] [--json out.json]
 
 Each kernel is timed with CUDA events on the launching stream over ROTATING operand sets whose
 total size exceeds the 50 MB L2 (so every launch streams from HBM), after 3 warm-up launches.
@@ -211,6 +211,61 @@ def bench_k2lw(iters):
             print(json.dumps(rec), flush=True)
             out.append(rec)
     return out
+
+
+def bench_k2q8(iters):
+    """K2-q8 (Adam with 8-bit block-wise state) over the headline MLP's 10 tensors (54.7 M
+    parameters), bf16 gradients in the arena, bf16 shadow, timed from a CUDA graph next to K2-mt
+    Adam (``frl_adam_mt``, fp32 state) on the same arena.  The arena is far larger than L2, so every
+    launch streams from HBM.  Bytes from the layout: K2-q8 reads g (2) and reads and writes the
+    master (8), both codes (4) and the shadow (2), plus 2 x 8 bytes of absmax per 256-element block;
+    K2-mt Adam moves 28 bytes per parameter."""
+    from frl_b200.fused_optim import q8_block_bases
+    from frl_b200.multi_tensor import GradSegTable
+
+    class Slot:
+        def __init__(self, index, offset, shape):
+            self.index, self.offset, self.shape = index, offset, shape
+            self.numel = 1
+            for d in shape:
+                self.numel *= d
+            self.is_model = True
+
+    shapes = [(4096, 4096), (4096,)] * 3 + [(1000, 4096), (1000,), (64, 4096), (64,)]
+    slots, off = [], 0
+    for i, sh in enumerate(shapes):
+        slots.append(Slot(i, off, sh))
+        off = (off + slots[-1].numel + 7) // 8 * 8
+    n, n_real = off, sum(s.numel for s in slots)
+    grad = torch.randn(n, device=DEV).bfloat16()
+    table = GradSegTable(slots, DEV)
+    for s in slots:
+        table.point(s, grad.data_ptr() + 2 * s.offset, grad.dtype)
+    table.upload()
+    bases, n_blocks = q8_block_bases(slots)
+    qbase = torch.tensor([bases[s.index] for s in slots], dtype=torch.int64, device=DEV)
+    flags = torch.full((len(slots),), _native.LW_CLIPPED, dtype=torch.int32, device=DEV)
+    p = torch.randn(n, device=DEV) * 0.02
+    lp = torch.empty(n, device=DEV, dtype=torch.bfloat16)
+    m, v = torch.randn(n, device=DEV) * 1e-3, torch.rand(n, device=DEV) * 1e-6
+    mq, vq = torch.zeros(n, dtype=torch.uint8, device=DEV), torch.zeros(n, dtype=torch.uint8, device=DEV)
+    ma, va = torch.zeros(n_blocks, device=DEV), torch.zeros(n_blocks, device=DEV)
+    _native.q8_encode_mt(m, mq, ma, _native.Q8_EXP_AVG, table, qbase)
+    _native.q8_encode_mt(v, vq, va, _native.Q8_EXP_AVG_SQ, table, qbase)
+
+    def q8(i):
+        _native.adam8_mt(p, mq, vq, ma, va, lp, table, qbase, flags, lr=1e-3, beta1=0.9, beta2=0.999, eps=1e-8,
+                         wd=1e-5, step=3)
+
+    def fp32(i):
+        _native.adam_mt(p, m, v, None, lp, table, lr=1e-3, beta1=0.9, beta2=0.999, eps=1e-8, wd=1e-5, step=3)
+
+    q8_bytes = 16 * n_real + 2 * 8 * n_blocks
+    return [timed("K2-q8 adam 8-bit state mlp bf16-grad (%d tensors, %d params, %d blocks)"
+                  % (len(slots), n_real, n_blocks), q8, 1, q8_bytes, iters,
+                  "%.2f B/param" % (q8_bytes / n_real), graph=True),
+            timed("K2-mt adam fp32 state mlp bf16-grad (%d tensors, %d params)" % (len(slots), n_real), fp32, 1,
+                  28 * n_real, iters, "28 B/param", graph=True)]
 
 
 def bench_k10(iters):
@@ -543,7 +598,8 @@ def bench_k9(iters):
 
 BENCHES = {"k2": bench_k2, "k2mt": bench_k2mt, "k2lw": bench_k2lw, "k3": bench_k3, "k4": bench_k4, "k5": bench_k5, "k5a": bench_k5a,
            "k5m": bench_k5m, "k4s": bench_k4s, "k6": bench_k6,
-           "k8": bench_k8, "k8t": bench_k8t, "k9": bench_k9, "k10": bench_k10, "k11": bench_k11}
+           "k8": bench_k8, "k8t": bench_k8t, "k9": bench_k9, "k10": bench_k10, "k11": bench_k11,
+           "k2q8": bench_k2q8}
 
 
 def main():
