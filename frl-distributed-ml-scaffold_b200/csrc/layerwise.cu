@@ -6,10 +6,13 @@
 //   1. stats: per tile, the partial sums of ||w||^2 and of ||g^||^2 (LARS) or ||u||^2 (LAMB).
 //      LAMB also writes its moments here (m, v are needed for u anyway; writing them here and
 //      re-reading them in phase 2 moves 40 B/param with bf16 gradient and shadow, recomputing
-//      them in phase 2 would re-read g, m and v: 42 B/param).  The CTA that finishes the last
-//      tile of a tensor (per-segment atomic ticket) folds that tensor's partials in tile order,
-//      in double, and writes ratio[seg]: deterministic, no float atomics, no host sync.  The
-//      ticket is reset by the folding CTA, so the scratch is zeroed once.
+//      them in phase 2 would re-read g, m and v: 42 B/param).  The squares and every partial sum
+//      are double: an fp32 square overflows once |g| > 1.8e19 and underflows once |g| < 1e-19,
+//      where the trust ratio itself is an ordinary float (LARS is invariant to the gradient's
+//      scale), and an fp32 tile sum overflows once the tile's RMS exceeds 1.4e17.  The CTA that
+//      finishes the last tile of a tensor (per-segment atomic ticket) folds that tensor's
+//      partials in tile order and writes ratio[seg]: deterministic, no float atomics, no host
+//      sync.  The ticket is reset by the folding CTA, so the scratch is zeroed once.
 //   2. apply: reads ratio[seg] and updates master weights, state and the bf16 shadow.
 // Per-step scalars may come from the device (`dyn`) so a captured CUDA graph stays valid.
 #include "frl_common.cuh"
@@ -19,8 +22,8 @@ namespace frl {
 
 constexpr float kLarsTrust = 1e-3f;     // LARS trust coefficient eta (fixed)
 
-// scratch layout: float partial[2 * n_tiles] (16-byte padded), then uint32 ticket[n_segs]
-static inline int64_t partial_bytes(int64_t n_tiles) { return (8 * n_tiles + 15) / 16 * 16; }
+// scratch layout: double partial[2 * n_tiles], then uint32 ticket[n_segs]
+static inline int64_t partial_bytes(int64_t n_tiles) { return 16 * n_tiles; }
 
 struct LarsParams {
     float lr, mu, wd;
@@ -72,9 +75,8 @@ __global__ void __launch_bounds__(kThreads)
 lw_stats_kernel(const float* __restrict__ p_, float* __restrict__ m_, float* __restrict__ v_,
                 const frl_grad_seg* __restrict__ segs, const int64_t* __restrict__ tile_prefix,
                 const int32_t* __restrict__ tile_seg, int64_t n_tiles, const int32_t* __restrict__ flags,
-                float* __restrict__ ratio, float* __restrict__ partial, unsigned int* __restrict__ ticket,
+                float* __restrict__ ratio, double* __restrict__ partial, unsigned int* __restrict__ ticket,
                 P prm, float gscale, const float* __restrict__ gscale_dev, const float* __restrict__ dyn) {
-    __shared__ float fsm[64];
     __shared__ double dsm[64];
     __shared__ bool is_last;
     if (dyn) prm.patch(dyn);
@@ -90,7 +92,7 @@ lw_stats_kernel(const float* __restrict__ p_, float* __restrict__ m_, float* __r
         const int64_t seg_vec = (sv.numel + 3) >> 2;           // arena slices are padded to 8
         const int64_t v0 = sv.t_in * kTileVec + threadIdx.x;
         const int64_t a0 = sv.arena_off >> 2;
-        float sw = 0.f, sd = 0.f;                               // ||w||^2, ||g^||^2 or ||u||^2
+        double sw = 0.0, sd = 0.0;                              // ||w||^2, ||g^||^2 or ||u||^2
         if (LAMB || adapted) {                                  // CTA-uniform
             f32x4 vg[kUnroll], vp[kUnroll], vm[kUnroll], vv[kUnroll];
 #pragma unroll
@@ -113,20 +115,21 @@ lw_stats_kernel(const float* __restrict__ p_, float* __restrict__ m_, float* __r
 #pragma unroll
                 for (int k = 0; k < 4; ++k) {
                     const float g = g4[k] * gs;
-                    sw = fmaf(w4[k], w4[k], sw);
+                    const double w = w4[k];
+                    sw = fma(w, w, sw);
                     if constexpr (LAMB) {
                         m4[k] = fmaf(prm.w1, g - m4[k], m4[k]);             // m.lerp_(g, 1-beta1)
                         q4[k] = fmaf(prm.w2 * g, g, q4[k] * prm.beta2);     // v*beta2 + (1-beta2)*g*g
-                        const float u = prm.dir(m4[k], q4[k], w4[k], lam);
-                        sd = fmaf(u, u, sd);
+                        const double u = prm.dir(m4[k], q4[k], w4[k], lam);
+                        sd = fma(u, u, sd);
                     } else {
-                        sd = fmaf(g, g, sd);
+                        sd = fma(static_cast<double>(g), static_cast<double>(g), sd);
                     }
                 }
                 if (LAMB) { st_stream(m + a0 + e, vm[j]); st_stream(v + a0 + e, vv[j]); }
             }
         }
-        block_sum2(sw, sd, fsm);
+        block_sum2(sw, sd, dsm);
         const int si = sv.seg;
         if (threadIdx.x == 0) {
             partial[2 * tile] = sw;
@@ -143,8 +146,8 @@ lw_stats_kernel(const float* __restrict__ p_, float* __restrict__ m_, float* __r
         const int64_t t0 = __ldg(tile_prefix + si), t1 = __ldg(tile_prefix + si + 1);
         double dw = 0.0, dd = 0.0;
         for (int64_t t = t0 + threadIdx.x; t < t1; t += kThreads) {
-            dw += static_cast<double>(__ldcg(partial + 2 * t));
-            dd += static_cast<double>(__ldcg(partial + 2 * t + 1));
+            dw += __ldcg(partial + 2 * t);
+            dd += __ldcg(partial + 2 * t + 1);
         }
         block_sum2(dw, dd, dsm);
         if (threadIdx.x == 0) {
@@ -238,7 +241,7 @@ static int launch_layerwise(const P& prm, float* p, float* s0, float* s1, void* 
                 "%s: null p/segs/tile_prefix/tile_seg/flags/ratio/scratch", name);
     FRL_REQUIRE(aligned16(p) && aligned16(s0) && aligned16(s1) && aligned16(p_lp) && aligned16(scratch),
                 FRL_E_ALIGN, "%s: arrays must be 16-byte aligned", name);
-    float* partial = static_cast<float*>(scratch);
+    double* partial = static_cast<double*>(scratch);
     unsigned int* ticket = reinterpret_cast<unsigned int*>(static_cast<char*>(scratch) + partial_bytes(n_tiles));
     lw_stats_kernel<LAMB, P><<<grid_for_tiles(lw_stats_kernel<LAMB, P>, n_tiles), kThreads, 0, st>>>(
         p, s0, s1, segs, tile_prefix, tile_seg, n_tiles, flags, ratio, partial, ticket, prm, gscale,

@@ -170,8 +170,9 @@ int frl_rmsprop_mt(float* p, float* sq, float* buf, void* p_lp, const frl_grad_s
  *     ratio = ||w|| / ||u|| if adapted and ||w|| > 0 and ||u|| > 0, else 1 ;  w -= lr*ratio*u
  *     The weight decay is DECOUPLED (part of u), unlike frl_adam's L2-coupled decay.
  * A non-finite gradient yields non-finite weights (a NaN norm takes the ratio-1 branch, which
- * passes the NaN on).  Norms: fp32 per tile, folded per tensor in double in tile order (no float
- * atomics, deterministic).  Two launches: stats (LAMB writes m, v here) and apply.
+ * passes the NaN on).  Norms: squares and per-tile sums in double (no overflow or underflow for
+ * any finite fp32 gradient), folded per tensor in tile order (no float atomics, deterministic).
+ * Two launches: stats (LAMB writes m, v here) and apply.
  *   dyn  LARS: dyn[0] = lr ;  LAMB: dyn[0] = lr, dyn[1] = 1/(1-beta1^t), dyn[2] = sqrt(1-beta2^t).
  * ---------------------------------------------------------------------------------------- */
 enum { FRL_LW_ADAPTED = 1, FRL_LW_CLIPPED = 2 };

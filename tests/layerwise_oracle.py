@@ -115,11 +115,13 @@ class LayerwiseKernelDouble(KernelDouble):
 
 class LayerwiseTorch(torch.optim.Optimizer):
     """Per-parameter LARS / LAMB in stock torch (``mode`` "lars" or "lamb"), one step count per
-    parameter like ``torch.optim.Adam``.  Parameters with 2 or more dimensions are adapted."""
+    parameter like ``torch.optim.Adam``.  Parameters with 2 or more dimensions are adapted.
+    ``last_ratio[p]``: the trust ratio of ``p``'s last update (1.0 where it is not adapted)."""
 
     def __init__(self, params, mode, lr, momentum=0.9, weight_decay=0.0, betas=(0.9, 0.999), eps=1e-8):
         assert mode in ("lars", "lamb")
         self.mode = mode
+        self.last_ratio = {}
         super().__init__(params, dict(lr=lr, momentum=momentum, weight_decay=weight_decay, betas=betas,
                                       eps=eps))
 
@@ -139,7 +141,7 @@ class LayerwiseTorch(torch.optim.Optimizer):
                         ratio = LARS_TRUST * wn / (gn + wd * wn) if wn > 0 and gn > 0 else 1.0
                         d = (g + wd * p) * ratio
                     else:
-                        d = g.clone()
+                        ratio, d = 1.0, g.clone()
                     mu = group["momentum"]
                     if mu != 0:
                         if "momentum_buffer" not in st:
@@ -148,6 +150,7 @@ class LayerwiseTorch(torch.optim.Optimizer):
                             st["momentum_buffer"].mul_(mu).add_(d)
                         d = st["momentum_buffer"]
                     p.add_(d, alpha=-lr)
+                    self.last_ratio[p] = ratio
                 else:
                     b1, b2 = group["betas"]
                     if not st:
@@ -165,3 +168,86 @@ class LayerwiseTorch(torch.optim.Optimizer):
                     wn, un = float(p.norm()), float(u.norm())
                     ratio = wn / un if adapted and wn > 0 and un > 0 else 1.0
                     p.add_(u, alpha=-lr * ratio)
+                    self.last_ratio[p] = ratio
+
+
+# ---- float64 reference of one K2-lw update and its fp32 rounding envelope --------------------------
+# (derivation of the constants: tests/test_gpu_layerwise_paths.py's module docstring)
+
+U, ETA = 2.0 ** -24, 2.0 ** -150
+C_LARS, C_R_LARS = 16, 8            # weights / momentum buffer; trust ratio (relative)
+C_LAMB, C_R_LAMB = 24, 24           # weights, exp_avg, exp_avg_sq; trust ratio (relative, times kappa)
+BETAS, LAMB_EPS = (0.9, 0.999), 1e-6
+
+
+def reference_update(mode, w0, g, s0, *, adapted, lr, mu, wd, step, dtype=torch.float64):
+    """One ``LayerwiseTorch`` step of one tensor in ``dtype`` from the fp32 state ``w0``, ``s0``
+    (LARS: [momentum_buffer] or [], LAMB: [exp_avg, exp_avg_sq]) with effective gradient ``g``;
+    ``step`` is t (LARS: 1 = first step).  Returns (w, states, ratio) as float64 / float."""
+    shape = (1, w0.numel()) if adapted else (w0.numel(),)
+    param = torch.nn.Parameter(w0.to(dtype).reshape(shape).clone())
+    opt = LayerwiseTorch([param], mode, lr=lr, momentum=mu, weight_decay=wd, betas=BETAS, eps=LAMB_EPS)
+    st = opt.state[param]
+    if mode == "lars":
+        names = ("momentum_buffer",) if mu else ()
+        if mu and step > 1:
+            st["momentum_buffer"] = s0[0].to(dtype).reshape(shape).clone()
+    else:
+        names = ("exp_avg", "exp_avg_sq")
+        st["step"] = torch.tensor(float(step - 1))
+        st["exp_avg"], st["exp_avg_sq"] = (s.to(dtype).reshape(shape).clone() for s in s0)
+    param.grad = g.to(dtype).reshape(shape)
+    opt.step()
+    return (param.detach().flatten().double(), [st[n].flatten().double() for n in names],
+            opt.last_ratio[param])
+
+
+def update_envelope(mode, w0, g, s0, ref_w, ref_s, ratio, *, adapted, lr, mu, wd, step):
+    """(bound on the weights, bounds on the states, kappa): c * (U * mag + ETA) per element, and the
+    trust ratio's relative bound is C_R * U * kappa.  kappa = 0 where the rule takes ratio 1
+    (exact), else ||mag(u)|| / ||u|| (1 for LARS)."""
+    w0, g = w0.double(), g.double()
+    s0 = [s.double() for s in s0]
+    if mode == "lars":
+        dn = float(g.norm())
+        kappa = 1.0 if adapted and float(w0.norm()) > 0 and dn > 0 else 0.0
+        mag = ratio * (g.abs() + (wd * w0.abs() if adapted else 0.0))
+        if mu and step > 1:
+            mag = mu * s0[0].abs() + mag
+        c, mags, step_mag = C_LARS, ([mag] if mu else []), lr * mag
+    else:
+        b1, b2 = BETAS
+        lam = wd if adapted else 0.0
+        bc1, bc2 = 1 - b1 ** step, 1 - b2 ** step
+        mag_m = s0[0].abs() + (1 - b1) * (g.abs() + s0[0].abs())
+        mag_v = b2 * s0[1] + (1 - b2) * g * g
+        denom = ref_s[1].sqrt() / math.sqrt(bc2) + LAMB_EPS
+        u = ref_s[0] / bc1 / denom + lam * w0
+        mag_u = mag_m / bc1 / denom + lam * w0.abs()
+        un = float(u.norm())
+        kappa = float(mag_u.norm()) / un if adapted and float(w0.norm()) > 0 and un > 0 else 0.0
+        c, mags, step_mag = C_LAMB, [mag_m, mag_v], lr * ratio * (mag_u + kappa * u.abs())
+    return c * (U * (ref_w.abs() + step_mag) + ETA), [c * (U * m + ETA) for m in mags], kappa
+
+
+def check_update(mode, got_w, got_s, got_ratio, w0, g, s0, *, adapted, lr, mu, wd, step, what,
+                 dtype=torch.float64):
+    """The kernel's update of one tensor (``got_*``, fp32) from (w0, s0) with effective gradient
+    ``g`` against ``reference_update`` in ``dtype`` (fp32 only where fp32 storage itself
+    overflows; both sides then carry their own error, so the bounds double)."""
+    from test_gpu_optim_paths import assert_within
+    ref_w, ref_s, r = reference_update(mode, w0, g, s0, adapted=adapted, lr=lr, mu=mu, wd=wd, step=step,
+                                       dtype=dtype)
+    bw, bs, kappa = update_envelope(mode, w0, g, s0, ref_w, ref_s, r, adapted=adapted, lr=lr, mu=mu, wd=wd,
+                                    step=step)
+    k = 1 if dtype == torch.float64 else 2
+    assert_within(got_w, ref_w, k * bw, what + " weights")
+    for i, (got, ref, b) in enumerate(zip(got_s, ref_s, bs)):
+        assert_within(got, ref, k * b, "%s state %d" % (what, i))
+    if kappa == 0:
+        assert got_ratio == 1.0, "%s: ratio %r, want exactly 1" % (what, got_ratio)
+    else:
+        c_r = C_R_LARS if mode == "lars" else C_R_LAMB
+        assert abs(got_ratio - r) <= k * c_r * U * kappa * abs(r), \
+            "%s: ratio %r, float64 %r (kappa %.3g)" % (what, got_ratio, r, kappa)
+    return r

@@ -1,6 +1,7 @@
-"""K2-lw (LARS, LAMB) on the H100: the kernels against the numpy restatement, determinism, NaN
-containment, and the headline MLP through ``Solver.build_worker`` against stock torch running the
-per-parameter oracle (``tests/layerwise_oracle.py``)."""
+"""K2-lw (LARS, LAMB) on the H100: determinism, NaN containment, and the headline MLP through
+``Solver.build_worker`` against stock torch running the per-parameter oracle
+(``tests/layerwise_oracle.py``).  The kernels against float64 on every instantiation:
+``tests/test_gpu_layerwise_paths.py``."""
 import tempfile
 
 import numpy as np
@@ -14,7 +15,7 @@ from frl_b200.arena import ParamArena
 from frl_b200.multi_tensor import GradSegTable
 from frl_b200.solver import Solver, SolverWorkerArgs
 from frl_b200.types import Device, LayerAdaptation, OptAlgorithm, OptimOpts, Precision
-from layerwise_oracle import LayerwiseTorch, lamb_step, lars_step
+from layerwise_oracle import LayerwiseTorch
 
 pytestmark = pytest.mark.gpu
 
@@ -46,58 +47,6 @@ def _setup(precision, seed=0):
             table.grads.append(ext)
     table.upload()
     return arena, table, grads
-
-
-def _state(opt, name, s):
-    return opt._vec[name][s.offset:s.end].cpu().numpy()
-
-
-@pytest.mark.parametrize("dyn", [False, True])
-@pytest.mark.parametrize("precision", [Precision.FP32, Precision.BF16])
-@pytest.mark.parametrize("mode", ["lars", "lamb"])
-def test_kernels_match_the_restatement(mode, precision, dyn):
-    arena, table, grads = _setup(precision)
-    if mode == "lars":
-        opt = fused_optim.FusedLars(arena, lr=0.1, momentum=0.9, weight_decay=1e-2)
-    else:
-        opt = fused_optim.FusedLamb(arena, lr=0.01, weight_decay=1e-2, eps=1e-6)
-    if dyn:
-        opt.enable_dynamic_scalars()
-    coef = torch.tensor([0.75], device="cuda")
-    w = [arena.master[s.offset:s.end].cpu().numpy().copy() for s in arena.slots]
-    st = {k: [np.zeros(s.numel, np.float32) for s in arena.slots] for k in ("buf", "m", "v")}
-    for step in (1, 2, 3):
-        opt.begin_step()
-        if dyn:
-            # the launch's by-value scalars are wrong on purpose: only the device block is right
-            lr, opt.hyper["lr"] = opt.hyper["lr"], 123.0
-            opt._steps += 7 if mode == "lamb" else 0          # LAMB's by-value bias corrections
-            opt.apply_table(table, grad_scale=0.5, clip_coef_dev=coef)
-            opt.hyper["lr"] = lr
-            opt._steps -= 7 if mode == "lamb" else 0
-        else:
-            opt.apply_table(table, grad_scale=0.5, clip_coef_dev=coef)
-        opt.end_step()
-        ratios = opt.last_ratios(table).cpu().numpy()
-        for i, s in enumerate(arena.slots):
-            gs = 0.5 * (0.75 if s.is_model else 1.0)
-            adapted = len(s.shape) >= 2
-            if mode == "lars":
-                w[i], st["buf"][i], r = lars_step(w[i], grads[i], st["buf"][i], lr=0.1, mu=0.9, wd=1e-2,
-                                                  adapted=adapted, first_step=step == 1, grad_scale=gs)
-                np.testing.assert_allclose(_state(opt, "momentum_buffer", s), st["buf"][i], rtol=1e-5, atol=1e-9)
-            else:
-                w[i], st["m"][i], st["v"][i], r = lamb_step(w[i], grads[i], st["m"][i], st["v"][i], lr=0.01,
-                                                            beta1=0.9, beta2=0.999, eps=1e-6, wd=1e-2, step=step,
-                                                            adapted=adapted, grad_scale=gs)
-                np.testing.assert_allclose(_state(opt, "exp_avg", s), st["m"][i], rtol=1e-5, atol=1e-9)
-                np.testing.assert_allclose(_state(opt, "exp_avg_sq", s), st["v"][i], rtol=1e-5, atol=1e-12)
-            assert abs(ratios[i] - r) <= 1e-5 * abs(r), (step, s.shape, ratios[i], r)
-            got = arena.master[s.offset:s.end].cpu().numpy()
-            np.testing.assert_allclose(got, w[i], rtol=1e-5, atol=1e-7)
-            w[i] = got.copy()          # compare each step from the kernel's own weights
-            if arena.lp is not None and s.is_model:
-                assert torch.equal(arena.lp[s.offset:s.end].cpu(), torch.from_numpy(got).to(torch.bfloat16))
 
 
 @pytest.mark.parametrize("mode", ["lars", "lamb"])
