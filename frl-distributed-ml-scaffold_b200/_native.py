@@ -74,6 +74,10 @@ SIGNATURES = {
                           _i64, _d, _vp, _vp, _vp]),
     "frl_q8_encode_mt": (_i, [_vp, _vp, _vp, _i, _vp, _vp, _vp, _i64, _i64, _vp, _vp]),
     "frl_q8_decode_mt": (_i, [_vp, _vp, _vp, _i, _vp, _vp, _vp, _i64, _i64, _vp, _vp]),
+    "frl_adafactor_plan": (_i64, [_vp, _i64, _vp, _vp]),
+    "frl_adafactor_scratch_bytes": (_i64, [_vp, _i64]),
+    "frl_adafactor_mt": (_i, [_vp, _vp, _vp, _vp, _i64, _vp, _vp, _vp, _vp, _i64, _vp, _vp, _d, _d, _d, _d, _d, _d,
+                              _i64, _d, _vp, _vp, _vp]),
     "frl_grad_accumulate_mt": (_i, [_vp, _vp, _vp, _vp, _i64, _d, _i, _vp, _vp]),
     "frl_weight_ema": (_i, [_vp, _vp, _i64, _d, _vp]),
     "frl_reduce_scratch_bytes": (_i64, []),
@@ -365,6 +369,59 @@ def q8_decode_mt(q, absmax, x, state: int, table, qbase) -> None:
     _check(lib().frl_q8_decode_mt(_ptr(q), _ptr(absmax), _ptr(x), int(state), table.segs_dev_ptr,
                                   table.prefix_dev_ptr, table.tile_seg_dev_ptr, table.n_tiles, table.n_segs,
                                   _ptr(qbase), _stream()), "frl_q8_decode_mt")
+
+
+# ---- K2-af: Adafactor over a segment table ----------------------------------------------------------
+
+def _host_shape(shape: torch.Tensor) -> torch.Tensor:
+    if shape.dtype != torch.int64 or shape.dim() != 2 or shape.shape[1] != 3 or shape.device.type != "cpu":
+        raise NativeLibraryError("Adafactor: shape must be a CPU int64 [n_segs, 3] tensor of (B, R, C)")
+    return shape.contiguous()
+
+
+def adafactor_plan(shape: torch.Tensor):
+    """Band table of the segments' (B, R, C) shapes: (work int64 [n_work, 4], seg_info int64
+    [n_segs, 3]) on the CPU.  See frl_adafactor_plan in include/frl_b200.h."""
+    shape = _host_shape(shape)
+    n_segs = shape.shape[0]
+    n = int(lib().frl_adafactor_plan(_ptr(shape), n_segs, None, None))
+    if n < 0:
+        raise NativeLibraryError("Adafactor: bad segment shape")
+    work = torch.zeros(n, 4, dtype=torch.int64)
+    seg_info = torch.zeros(n_segs, 3, dtype=torch.int64)
+    lib().frl_adafactor_plan(_ptr(shape), n_segs, _ptr(work), _ptr(seg_info))
+    return work, seg_info
+
+
+def adafactor_scratch_bytes(shape: torch.Tensor) -> int:
+    shape = _host_shape(shape)
+    n = int(lib().frl_adafactor_scratch_bytes(_ptr(shape), shape.shape[0]))
+    if n < 0:
+        raise NativeLibraryError("Adafactor: bad segment shape")
+    return n
+
+
+def adafactor_mt(p, state, p_lp, table, plan, *, lr, beta2_decay, eps1, eps2, d, wd, step, grad_scale=1.0,
+                 grad_scale_dev=None, dyn=None) -> None:
+    """K2-af Adafactor over the segments of ``table``.  ``plan``: the device arrays (shape,
+    state_off, seg_flags, work, seg_info, scratch) and the host shape they were built from.  See
+    frl_adafactor_mt in include/frl_b200.h."""
+    shape_dev, state_off, flags, work, seg_info, scratch, shape_host = plan
+    for t in (p, state):
+        if not (t.dtype == torch.float32 and t.is_contiguous()):
+            raise NativeLibraryError("Adafactor: master weights and state must be contiguous fp32")
+    n = table.n_segs
+    if (shape_dev.dtype != torch.int64 or shape_dev.numel() < 3 * n or state_off.dtype != torch.int64
+            or state_off.numel() < n or flags.dtype != torch.int32 or flags.numel() < n
+            or work.dtype != torch.int64 or seg_info.dtype != torch.int64 or seg_info.numel() < 3 * n):
+        raise NativeLibraryError("Adafactor: shape/state_off/work/seg_info must be int64, seg_flags int32, "
+                                 "each covering the table's segments")
+    if n and scratch.numel() * scratch.element_size() < adafactor_scratch_bytes(shape_host):
+        raise NativeLibraryError("Adafactor: scratch too small")
+    _check(lib().frl_adafactor_mt(_ptr(p), _ptr(state), _ptr(p_lp), table.segs_dev_ptr, n, _ptr(shape_dev),
+                                  _ptr(state_off), _ptr(flags), _ptr(work), work.shape[0] if n else 0,
+                                  _ptr(seg_info), _ptr(scratch), lr, beta2_decay, eps1, eps2, d, wd, step,
+                                  grad_scale, _ptr(grad_scale_dev), _ptr(dyn), _stream()), "frl_adafactor_mt")
 
 
 # ---- K10: gradient accumulation over a segment table ----------------------------------------------

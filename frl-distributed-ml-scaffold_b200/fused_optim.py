@@ -8,7 +8,8 @@ torch's per-parameter format so the reference's ``.checkpoint.pth`` files stay i
 ``FusedLars`` / ``FusedLamb`` (an extension, ``types.LayerAdaptation``) keep SGD's / Adam's state
 format and update whole tensors through the K2-lw kernels.  ``FusedAdam8bit`` (an extension,
 ``types.OptimizerState``) keeps Adam's moments as 8-bit block-wise codes (K2-q8) and speaks
-``torch.optim.Adam``'s format in its state dict.
+``torch.optim.Adam``'s format in its state dict.  ``FusedAdafactor`` (an extension, chosen with
+``Solver.solve(..., adafactor=True)``) is ``torch.optim.Adafactor``'s rule and state format (K2-af).
 
 Known limitation: the step count (Adam's bias corrections) is ONE number for the whole arena.
 ``torch.optim`` keeps one per parameter and does not advance it for a parameter whose gradient
@@ -633,6 +634,164 @@ class FusedAdam8bit(_WholeTensorMixin, FusedAdam):
             self._vec = {}
 
 
+# ---- Adafactor (K2-af) -----------------------------------------------------------------------------
+
+def adafactor_shape(shape) -> Tuple[int, int, int]:
+    """(B, R, C) of a parameter under Adafactor: a tensor of 2 or more dimensions is B = prod of
+    the leading dimensions matrices of [R, C] = its last two (factored); any other is
+    (1, 0, numel), kept unfactored.  The kernel's shape array takes (1, 0, 0) for a tensor with no
+    elements (``kernel_shape``): nothing to update."""
+    shape = tuple(int(x) for x in shape)
+    if len(shape) >= 2:
+        return int(np.prod(shape[:-2], dtype=np.int64)), shape[-2], shape[-1]
+    return 1, 0, int(np.prod(shape, dtype=np.int64))
+
+
+def adafactor_kernel_shape(shape) -> Tuple[int, int, int]:
+    return (1, 0, 0) if int(np.prod(tuple(shape), dtype=np.int64)) == 0 else adafactor_shape(shape)
+
+
+def adafactor_state_elems(shape) -> int:
+    b, r, c = adafactor_shape(shape)
+    return b * (r + c) if len(tuple(shape)) >= 2 else c
+
+
+class FusedAdafactor(_WholeTensorMixin, FusedArenaOptimizer):
+    """Adafactor (Shazeer & Stern, ICML 2018) with ``torch.optim.Adafactor``'s rule, defaults and
+    state-dict format: no first moment, the second moment of a 2-D or higher tensor factored into
+    ``row_var`` / ``col_var``, a relative step size and update clipping, decoupled weight decay on
+    every parameter.  The state lives in one compact fp32 buffer (row_var then col_var, or the
+    variance, per slot in arena order), updated by the three K2-af launches over a segment table
+    after backward."""
+
+    def __init__(self, arena, lr=1e-2, beta2_decay=-0.8, eps=(None, 1e-3), d=1.0, weight_decay=0.0):
+        super().__init__(arena, dict(lr=lr, beta2_decay=beta2_decay, eps=tuple(eps), d=d, weight_decay=weight_decay,
+                                     foreach=None, maximize=False))
+        self._off: Dict[int, int] = {}
+        n = 0
+        for s in sorted(arena.slots, key=lambda s: s.offset):
+            self._off[s.index] = n
+            n += adafactor_state_elems(s.shape)
+        self.state_buf = torch.zeros(max(n, 1), dtype=torch.float32, device=arena.device)
+        self._state_elems = n
+
+    @property
+    def state_bytes(self) -> int:
+        """Device bytes of the optimizer state (row / column factors and unfactored variances)."""
+        return 4 * self._state_elems
+
+    @property
+    def fp32_state_bytes(self) -> int:
+        """What ``FusedAdam`` keeps for the same arena: two fp32 arena-shaped vectors."""
+        return 2 * 4 * self.arena.numel
+
+    def _eps1(self) -> float:
+        e = self.hyper["eps"][0]
+        return float(torch.finfo(torch.float32).eps) if e is None else float(e)
+
+    def _dyn_values(self):
+        h = self.hyper
+        t = float(self._steps + 1)
+        lr = float(h["lr"])
+        return (lr, t ** float(h["beta2_decay"]), min(lr, 1.0 / t ** 0.5))
+
+    def _af_plan(self, table):
+        """Per-table device arrays, kept on the table: (B, R, C), state offset, flags
+        (``LW_CLIPPED``: model parameters take the clip coefficient), the band table and the
+        zero-initialised scratch."""
+        plan = getattr(table, "adafactor", None)
+        if plan is None:
+            dev = self.arena.device
+            shape = torch.tensor([adafactor_kernel_shape(s.shape) for s in table.slots] or [(1, 0, 1)],
+                                 dtype=torch.int64)
+            work, seg_info = KERNELS.adafactor_plan(shape)
+            off = torch.tensor([self._off[s.index] for s in table.slots] or [0], dtype=torch.int64)
+            flags = torch.tensor([KERNELS.LW_CLIPPED if s.is_model else 0 for s in table.slots] or [0],
+                                 dtype=torch.int32)
+            nbytes = KERNELS.adafactor_scratch_bytes(shape)
+            scratch = torch.zeros((nbytes + 15) // 16 * 4, dtype=torch.int32, device=dev)
+            plan = table.adafactor = (shape.to(dev), off.to(dev), flags.to(dev), work.to(dev), seg_info.to(dev),
+                                      scratch, shape)
+        return plan
+
+    def apply_table(self, table, *, grad_scale: float = 1.0,
+                    clip_coef_dev: Optional[torch.Tensor] = None) -> None:
+        """Update every slot of ``table`` (K2-af); ``clip_coef_dev`` multiplies the gradients of
+        model parameters only, as in ``apply_range``."""
+        if not table.n_segs:
+            return
+        h = self.hyper
+        KERNELS.adafactor_mt(self.arena.master, self.state_buf, self.arena.lp, table, self._af_plan(table),
+                             lr=float(h["lr"]), beta2_decay=float(h["beta2_decay"]), eps1=self._eps1(),
+                             eps2=float(h["eps"][1]), d=float(h["d"]), wd=float(h["weight_decay"]),
+                             step=self._steps + 1, grad_scale=grad_scale, grad_scale_dev=clip_coef_dev,
+                             dyn=self._dyn)
+
+    def _slot_state(self, s) -> Dict[str, torch.Tensor]:
+        """Views of slot ``s``'s state in torch's shapes."""
+        b, r, c = adafactor_shape(s.shape)
+        o = self._off[s.index]
+        if len(s.shape) < 2:
+            return {"variance": self.state_buf[o:o + c].view(s.shape)}
+        lead = tuple(s.shape[:-2])
+        return {"row_var": self.state_buf[o:o + b * r].view(lead + (r, 1)),
+                "col_var": self.state_buf[o + b * r:o + b * (r + c)].view(lead + (1, c))}
+
+    def state_dict(self) -> Dict[str, Any]:
+        state: Dict[int, Dict[str, Any]] = {}
+        if self._steps > 0:
+            for s in sorted(self.arena.slots, key=lambda s: s.index):
+                entry = {"step": torch.tensor(float(self._steps), dtype=torch.float32)}
+                entry.update({k: v.clone() for k, v in self._slot_state(s).items()})
+                state[s.index] = entry
+        groups = []
+        for g in self.param_groups:
+            packed = {k: v for k, v in g.items() if k != "params"}
+            packed["params"] = list(range(len(g["params"])))
+            groups.append(packed)
+        return {"state": state, "param_groups": groups}
+
+    def load_state_dict(self, state_dict: Dict[str, Any]) -> None:
+        groups = state_dict["param_groups"]
+        if len(groups) != 1 or len(groups[0]["params"]) != len(self.arena.all_params):
+            raise ValueError("loaded state dict has a different number of parameters/groups")
+        for entry in state_dict["state"].values():
+            if "exp_avg" in entry or "exp_avg_sq" in entry or "momentum_buffer" in entry or "square_avg" in entry:
+                raise ValueError("an Adafactor optimizer cannot load another optimizer's state dict "
+                                 "(found %s)" % sorted(k for k in entry if k != "step"))
+        for k, v in groups[0].items():
+            if k != "params":
+                self.param_groups[0][k] = tuple(v) if k == "eps" else v
+        by_index = {s.index: s for s in self.arena.slots}
+        steps = 0
+        for idx, entry in state_dict["state"].items():
+            s = by_index.get(int(idx))
+            if s is None:
+                continue
+            for name, view in self._slot_state(s).items():
+                if name in entry:
+                    view.copy_(entry[name].reshape(view.shape))
+            if "step" in entry:
+                steps = max(steps, int(float(entry["step"])))
+        self._steps = steps
+
+
+def check_adafactor(optim_opts: OptimOpts, layer_adaptation: LayerAdaptation,
+                    optimizer_state: OptimizerState, adafactor: bool) -> None:
+    """Adafactor needs Adam without amsgrad, no layer adaptation and fp32 optimizer state; anything
+    else is a ValueError naming the values."""
+    if not adafactor:
+        return
+    st = OptimizerState(optimizer_state)
+    la = LayerAdaptation(layer_adaptation)
+    if not (optim_opts.algo == OptAlgorithm.ADAM and not optim_opts.amsgrad and la is LayerAdaptation.NONE
+            and st is OptimizerState.FP32):
+        raise ValueError("adafactor cannot be combined with optimizer %r%s, layer adaptation %r and optimizer "
+                         "state %r (adafactor needs adam without amsgrad, layer adaptation none and optimizer "
+                         "state fp32)" % (getattr(optim_opts.algo, "value", optim_opts.algo),
+                                          " with amsgrad" if optim_opts.amsgrad else "", la.value, st.value))
+
+
 def check_optimizer_state(optim_opts: OptimOpts, layer_adaptation: LayerAdaptation,
                           optimizer_state: OptimizerState) -> None:
     """8-bit state needs Adam without amsgrad and without layer adaptation; anything else is a
@@ -662,11 +821,17 @@ def check_layer_adaptation(optim_opts: OptimOpts, layer_adaptation: LayerAdaptat
 
 def create_fused_optimizer(arena: ParamArena, optim_opts: OptimOpts,
                            layer_adaptation: LayerAdaptation = LayerAdaptation.NONE,
-                           optimizer_state: OptimizerState = OptimizerState.FP32) -> FusedArenaOptimizer:
+                           optimizer_state: OptimizerState = OptimizerState.FP32,
+                           adafactor: bool = False) -> FusedArenaOptimizer:
     """Same dispatch and argument mapping as the reference's ``_create_optimizer``; with a layer
-    adaptation, its LARS / LAMB counterpart; with 8-bit optimizer state, ``FusedAdam8bit``."""
+    adaptation, its LARS / LAMB counterpart; with 8-bit optimizer state, ``FusedAdam8bit``; with
+    ``adafactor``, ``FusedAdafactor`` (``lr`` caps the relative step, ``weightDecay`` is its
+    decoupled decay; ``epsilon`` and ``momentum`` are unused)."""
     check_layer_adaptation(optim_opts, layer_adaptation)
     check_optimizer_state(optim_opts, layer_adaptation, optimizer_state)
+    check_adafactor(optim_opts, layer_adaptation, optimizer_state, adafactor)
+    if adafactor:
+        return FusedAdafactor(arena, lr=optim_opts.lr, weight_decay=optim_opts.weightDecay)
     if OptimizerState(optimizer_state) is OptimizerState.Q8:
         return FusedAdam8bit(arena, lr=optim_opts.lr, weight_decay=optim_opts.weightDecay, eps=optim_opts.epsilon)
     if layer_adaptation == LayerAdaptation.LARS:

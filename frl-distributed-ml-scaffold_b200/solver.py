@@ -29,7 +29,7 @@ import torch.nn as nn
 from .arena import ParamArena
 from .criteria import BaseParallelCriterion
 from .ema import EMA_STATE_KEY
-from .fused_optim import (FusedAdam8bit, check_layer_adaptation, check_optimizer_state, create_fused_optimizer,
+from .fused_optim import (FusedAdafactor, FusedAdam8bit, check_adafactor, check_layer_adaptation, check_optimizer_state, create_fused_optimizer,
                           is_adapted)
 from .grad_sync import BufferBroadcaster, GradBucketPipeline
 from .lr_scheduler import DropEpochsScheduler, WarmupMultiStepLR
@@ -48,6 +48,7 @@ PRECISION_ENV = "FRL_B200_PRECISION"      # "fp32" (default, reference parity) |
 GRAD_ACCUM_ENV = "FRL_B200_GRAD_ACCUM"     # microbatches per optimizer update, default 1
 EMA_DECAY_ENV = "FRL_B200_EMA_DECAY"       # weight EMA decay in [0, 1), default 0 (off)
 OPTIMIZER_STATE_ENV = "FRL_B200_OPTIMIZER_STATE"   # "fp32" (default) | "8bit"
+ADAFACTOR_ENV = "FRL_B200_ADAFACTOR"               # "0" (default) | "1"
 EMA_SUFFIX = ".ema"                        # <checkpoint>.ema: the weight EMA next to a checkpoint
 
 
@@ -104,6 +105,8 @@ class SolverWorkerArgs(NamedTuple):
     layer_adaptation: LayerAdaptation = LayerAdaptation.NONE
     # Adam's state storage; placed before ema_decay and grad_accumulation, which stay the last fields
     optimizer_state: OptimizerState = OptimizerState.FP32
+    # Adafactor instead of Adam; placed before ema_decay and grad_accumulation, which stay the last fields
+    adafactor: bool = False
     # weight EMA decay, 0 = off; placed before grad_accumulation, which stays the last field
     ema_decay: float = 0.0
     grad_accumulation: int = 1
@@ -262,6 +265,17 @@ def resolve_optimizer_state(explicit: Optional[OptimizerState] = None) -> Optimi
     return OptimizerState(os.environ.get(OPTIMIZER_STATE_ENV, "fp32").lower())
 
 
+def resolve_adafactor(explicit: Optional[bool] = None) -> bool:
+    """Whether Adam runs as Adafactor: ``explicit``, else FRL_B200_ADAFACTOR (``0``, the default,
+    or ``1``).  Any other value is a ValueError."""
+    if explicit is not None:
+        return bool(explicit)
+    raw = os.environ.get(ADAFACTOR_ENV, "0").strip()
+    if raw not in ("0", "1"):
+        raise ValueError("%s must be 0 or 1, got %r" % (ADAFACTOR_ENV, raw))
+    return raw == "1"
+
+
 def resolve_grad_accumulation(explicit: Optional[int] = None) -> int:
     """Microbatches per optimizer update: ``explicit``, else FRL_B200_GRAD_ACCUM, else 1.  Anything
     but an integer >= 1 (``0``, negatives, ``2.5``, ``True``, non-numeric strings) is a ValueError."""
@@ -379,7 +393,7 @@ class Solver:
         symm_alloc = None
         if (distributed and not run_opts.optim.gradientClip
                 and args.layer_adaptation == LayerAdaptation.NONE and accum == 1 and ema_decay == 0.0
-                and args.optimizer_state is OptimizerState.FP32):
+                and args.optimizer_state is OptimizerState.FP32 and not args.adafactor):
             from .symm import try_make_allocator
             symm_alloc = try_make_allocator(device, args.world_size)
         from .arena_linear import head_layout_groups
@@ -396,7 +410,8 @@ class Solver:
                 if buf.is_floating_point():
                     buf.data = buf.data.to(torch.bfloat16)
         opt_state = args.optimizer_state if run_opts.mode == Mode.TRAIN else OptimizerState.FP32
-        optimizer = create_fused_optimizer(arena, run_opts.optim, args.layer_adaptation, opt_state)
+        adafactor = args.adafactor and run_opts.mode == Mode.TRAIN
+        optimizer = create_fused_optimizer(arena, run_opts.optim, args.layer_adaptation, opt_state, adafactor)
         if checkpoint:
             optimizer.load_state_dict(checkpoint.optimizerState)
         ema = None
@@ -480,7 +495,10 @@ class Solver:
                     ema_decay, ema.nbytes / 2 ** 20),
                 "8-bit block-wise (K2-q8), %.1f MiB instead of %.1f MiB" % (
                     optimizer.state_bytes / 2 ** 20, optimizer.fp32_state_bytes / 2 ** 20)
-                if isinstance(optimizer, FusedAdam8bit) else "fp32")
+                if isinstance(optimizer, FusedAdam8bit) else
+                "adafactor (K2-af), %.1f KiB instead of %.1f MiB" % (
+                    optimizer.state_bytes / 2 ** 10, optimizer.fp32_state_bytes / 2 ** 20)
+                if isinstance(optimizer, FusedAdafactor) else "fp32")
         scheduler = create_lr_scheduler(run_opts, worker.optimizer,
                                         checkpoint.epoch if checkpoint else -1)
         return worker, scheduler, checkpoint
@@ -691,7 +709,8 @@ class Solver:
               layer_adaptation: Optional[LayerAdaptation] = None,
               grad_accumulation: Optional[int] = None,
               ema_decay: Optional[float] = None,
-              optimizer_state: Optional[OptimizerState] = None
+              optimizer_state: Optional[OptimizerState] = None,
+              adafactor: Optional[bool] = None
               ) -> Iterator[PerformanceSummary]:
         """The reference's entry point (solver.py:728-739) plus two keyword-only extensions:
 
@@ -764,16 +783,31 @@ class Solver:
                        combination raises ``ValueError`` before a rank starts.  Checkpoints keep
                        ``torch.optim.Adam``'s format.  None: FRL_B200_OPTIMIZER_STATE (default
                        ``fp32``).  ``Mode.EVAL`` ignores it.
+        ``adafactor``  True: Adafactor (Shazeer & Stern, 2018) with ``torch.optim.Adafactor``'s
+                       rule instead of Adam (K2-af): no first moment, the second moment of a 2-D
+                       or higher weight factored into a row and a column vector, a relative step
+                       size ``min(lr, 1/sqrt(t)) * max(1e-3, RMS(p))`` and update clipping
+                       (d = 1).  ``OptimOpts.lr`` caps the relative step, ``weightDecay`` is the
+                       decoupled decay on every parameter; ``epsilon`` and ``momentum`` are
+                       unused; ``beta2_decay = -0.8`` and ``eps = (None, 1e-3)``.  Needs
+                       ``OptAlgorithm.ADAM`` without amsgrad, no layer adaptation and fp32
+                       optimizer state; any other combination raises ``ValueError`` before a
+                       rank starts.  Checkpoints keep ``torch.optim.Adafactor``'s format.  None:
+                       FRL_B200_ADAFACTOR (``0`` by default, ``1`` to enable).  ``Mode.EVAL``
+                       ignores it.
         """
         adapt = LayerAdaptation.NONE
         accum = 1
         decay = 0.0
         opt_state = OptimizerState.FP32
+        use_adafactor = False
         if run_opts.mode == Mode.TRAIN:
             adapt = resolve_layer_adaptation(layer_adaptation)
             check_layer_adaptation(run_opts.optim, adapt)
             opt_state = resolve_optimizer_state(optimizer_state)
             check_optimizer_state(run_opts.optim, adapt, opt_state)
+            use_adafactor = resolve_adafactor(adafactor)
+            check_adafactor(run_opts.optim, adapt, opt_state, use_adafactor)
             accum = resolve_grad_accumulation(grad_accumulation)
             decay = resolve_ema_decay(ema_decay)
         n_visible = 0 if run_opts.cpuonly else _cuda_device_count_without_poisoning_fork()
@@ -815,7 +849,7 @@ class Solver:
                 world_size=world_size, group_name=group_name, init_method=init_method,
                 cache=None, precision=prec, save_every=save_every, graph_step=graph,
                 layer_adaptation=adapt, grad_accumulation=accum, ema_decay=decay,
-                optimizer_state=opt_state)
+                optimizer_state=opt_state, adafactor=use_adafactor)
             if not run_opts.singleThreaded:
                 parent_conn, child_conn = ctx.Pipe(duplex=False)
                 proc = ctx.Process(target=cls._solver_worker_process,

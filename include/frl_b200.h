@@ -239,6 +239,43 @@ int frl_q8_decode_mt(const uint8_t* q, const float* absmax, float* x, int state,
                      int64_t n_segs, const int64_t* qbase_dev, void* stream);
 
 /* ------------------------------------------------------------------------------------------
+ * K2-af — Adafactor (an extension: Shazeer & Stern, ICML 2018), the rule of
+ * torch.optim.Adafactor with foreach=False and maximize=False.  No first moment; the second
+ * moment of a tensor of 2 or more dimensions, viewed as [B, R, C] (B = product of the leading
+ * dimensions), is factored into row_var [B, R] and col_var [B, C]; a 0-/1-D tensor keeps a full
+ * variance.  Per segment s, fp32, with g^ = g * grad_scale (* *grad_scale_dev if FRL_LW_CLIPPED),
+ * t = step (>= 1) and eps1 passed explicitly (torch's None is the fp32 epsilon 2^-23):
+ *   w_t = t^beta2_decay ; rho = min(lr, 1/sqrt(t))                        (host, double)
+ *   alpha = max(eps2, ||p|| / sqrt(numel)) * rho       (p before the decay; a NaN norm gives eps2)
+ *   factored:   row_var[b,r] = lerp(row_var[b,r], sum_c g^^2 / C, w_t)
+ *               col_var[b,c] = lerp(col_var[b,c], sum_r g^^2 / R, w_t)
+ *               vhat = row_var[b,r] * col_var[b,c] / max(mean_r row_var[b,r], eps1)
+ *   unfactored: variance = lerp(variance, g^^2, w_t) ; vhat = variance
+ *   u = rsqrt(max(vhat, eps1^2)) * g^ ; denom = max(1, ||u|| / (sqrt(numel) * d))  (NaN gives 1)
+ *   p = p * (1 - lr*wd) + (-alpha / denom) * u        (both factors formed in double, rounded once)
+ * lerp is torch's fp32 formula (K11's).  Sums of squares and the norms are double, folded per
+ * tensor in a fixed order: no float atomics, two launches give the same bytes.
+ *   shape_dev      int64 [n_segs][3] = (B, R, C); R = 0 for an unfactored tensor (C = numel)
+ *   state_off_dev  int64 [n_segs]: offset in `state` (one compact fp32 buffer) of the segment's
+ *                  row_var then col_var, or of its variance
+ *   seg_flags_dev  int32 [n_segs]: FRL_LW_CLIPPED as in K2-lw
+ *   work_dev, n_work, seg_info_dev   the band table frl_adafactor_plan builds from the shapes
+ *   scratch        frl_adafactor_scratch_bytes(shape, n_segs) bytes, zero-initialised once
+ *   dyn            dyn[0] = lr, dyn[1] = w_t, dyn[2] = rho (replaces the by-value scalars)
+ * frl_adafactor_plan: host; shape as shape_dev.  Writes work (int64 [n_work][4]) and seg_info
+ *   (int64 [n_segs][3]) when they are not NULL and returns n_work, or -1 on a bad shape.
+ * Three launches (stats, norm, apply); every argument check is made before any launch;
+ * n_work == 0 launches nothing.  Graph-capturable.
+ * ---------------------------------------------------------------------------------------- */
+int64_t frl_adafactor_plan(const int64_t* shape, int64_t n_segs, int64_t* work, int64_t* seg_info);
+int64_t frl_adafactor_scratch_bytes(const int64_t* shape, int64_t n_segs);
+int frl_adafactor_mt(float* p, float* state, void* p_lp, const frl_grad_seg* segs_dev, int64_t n_segs,
+                     const int64_t* shape_dev, const int64_t* state_off_dev, const int32_t* seg_flags_dev,
+                     const int64_t* work_dev, int64_t n_work, const int64_t* seg_info_dev, void* scratch,
+                     double lr, double beta2_decay, double eps1, double eps2, double d, double wd, int64_t step,
+                     double grad_scale, const float* grad_scale_dev, const float* dyn, void* stream);
+
+/* ------------------------------------------------------------------------------------------
  * K10 — gradient accumulation (an extension: the reference has no accumulation).  Several
  * microbatches per optimizer update: after each microbatch's backward, one launch folds every
  * gradient of a K2-mt segment table into an fp32 accumulator.

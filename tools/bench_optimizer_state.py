@@ -1,6 +1,6 @@
 #!/usr/bin/env python
-"""Adam with fp32 optimizer state against Adam with 8-bit block-wise state (K2-q8) on the headline
-workload (1 GPU, BF16, batch 4096, inputs resident, CUDA-graph replay).
+"""Adam with fp32 optimizer state against Adam with 8-bit block-wise state (K2-q8) and against
+Adafactor (K2-af, ``adafactor=True``) on the headline workload (1 GPU, BF16, batch 4096, inputs resident, CUDA-graph replay).
 
     python tools/bench_optimizer_state.py [--batch 4096] [--steps 50] [--warmup 5] [--repeats 5] [--graph 1]
 
@@ -37,8 +37,10 @@ from frl_b200.types import Device, OptimizerState, Precision  # noqa: E402
 HBM_BYTES_PER_S = 3.35e12      # H100 SXM data sheet, not measured
 # bytes the update moves per parameter with bf16 gradients and a bf16 shadow: K2-mt Adam reads g, w,
 # m, v and writes w, m, v, shadow (28); K2-q8 reads g, w and both codes and writes w, both codes and
-# the shadow (16), plus 2 x 8 bytes of absmax per 256-element block (counted from the layout below)
-ARMS = ["fp32", "8bit"]
+# the shadow (16), plus 2 x 8 bytes of absmax per 256-element block (counted from the layout below);
+# K2-af reads g three times and w twice and writes w and the shadow (20; its factored state is not
+# counted)
+ARMS = ["fp32", "8bit", "adafactor"]
 
 
 def card():
@@ -58,7 +60,9 @@ def build(ns, args, arm):
     wargs = SolverWorkerArgs(run_opts=bench.run_opts_for(ns, "adam", args.batch), problem=problem,
                              save_dir=save_dir, run_device=Device.GPU, node_idx=0, node_count=1, rank=0,
                              local_rank=0, world_size=1, group_name=None, init_method="",
-                             precision=Precision.BF16, optimizer_state=OptimizerState(arm))
+                             precision=Precision.BF16,
+                             optimizer_state=OptimizerState.FP32 if arm == "adafactor" else OptimizerState(arm),
+                             adafactor=arm == "adafactor")
     worker, _, _ = Solver.build_worker(wargs)
     worker.model.train()
     worker.criterion.train()
@@ -70,6 +74,8 @@ def update_bytes(worker):
     n = worker.arena.n_trainable
     if getattr(opt, "q8_blocks", None) is not None:
         return 16 * n + 16 * opt.q8_blocks
+    if getattr(opt, "state_buf", None) is not None:
+        return 20 * n
     return 28 * n
 
 

@@ -1,7 +1,7 @@
 #!/usr/bin/env python
 """Micro-benchmark of every hand-written kernel at the BASELINE shapes (1 GPU).
 
-    python tools/kernel_bench.py [--only k2,k2lw,k2q8,k3,k5a,...] [--iters 20] [--json out.json]
+    python tools/kernel_bench.py [--only k2,k2lw,k2q8,k2af,k3,k5a,...] [--iters 20] [--json out.json]
 
 Each kernel is timed with CUDA events on the launching stream over ROTATING operand sets whose
 total size exceeds the 50 MB L2 (so every launch streams from HBM), after 3 warm-up launches.
@@ -266,6 +266,76 @@ def bench_k2q8(iters):
                   "%.2f B/param" % (q8_bytes / n_real), graph=True),
             timed("K2-mt adam fp32 state mlp bf16-grad (%d tensors, %d params)" % (len(slots), n_real), fp32, 1,
                   28 * n_real, iters, "28 B/param", graph=True)]
+
+
+def bench_k2af(iters):
+    """K2-af (Adafactor: stats, norm and apply launches) over the headline MLP's 10 tensors, bf16
+    gradients in the arena, bf16 shadow, timed from a CUDA graph next to K2-mt SGD
+    (``frl_sgd_momentum_mt`` without momentum) on the same arena.  Bytes: g read three times (6),
+    the master read twice and written once (12), the shadow written (2): 20 B/param, SGD's count;
+    the factored state (about 47 K floats) is not counted."""
+    from frl_b200.fused_optim import FusedAdafactor
+    from frl_b200.multi_tensor import GradSegTable
+
+    class Slot:
+        def __init__(self, index, offset, shape):
+            self.index, self.offset, self.shape = index, offset, shape
+            self.numel = 1
+            for d in shape:
+                self.numel *= d
+            self.is_model = True
+
+    class Arena:
+        pass
+
+    shapes = [(4096, 4096), (4096,)] * 3 + [(1000, 4096), (1000,), (64, 4096), (64,)]
+    slots, off = [], 0
+    for i, sh in enumerate(shapes):
+        slots.append(Slot(i, off, sh))
+        off = (off + slots[-1].numel + 7) // 8 * 8
+    n, n_real = off, sum(s.numel for s in slots)
+    grad = torch.randn(n, device=DEV).bfloat16()
+    table = GradSegTable(slots, DEV)
+    for s in slots:
+        table.point(s, grad.data_ptr() + 2 * s.offset, grad.dtype)
+    table.upload()
+    a = Arena()
+    a.slots, a.numel, a.device = slots, n, torch.device(DEV)
+    a.all_params = [torch.nn.Parameter(torch.zeros(1)) for _ in slots]
+    a.master = torch.randn(n, device=DEV) * 0.02
+    a.lp = torch.empty(n, device=DEV, dtype=torch.bfloat16)
+    opt = FusedAdafactor(a, lr=1e-2, weight_decay=1e-5)
+    opt._steps = 2
+
+    def af(i):
+        opt.apply_table(table)
+
+    def sgd(i):
+        _native.sgd_momentum_mt(a.master, None, a.lp, table, lr=1e-3, mu=0.0, dampening=0.0, wd=0.0)
+
+    recs = [timed("K2-af adafactor mlp bf16-grad (%d tensors, %d params, 3 launches)" % (len(slots), n_real), af,
+                  1, 20 * n_real, iters, "20 B/param", graph=True)]
+    # per pass: device time of each kernel under torch.profiler, in a window of its own
+    from torch.profiler import ProfilerActivity, profile
+    with profile(activities=[ProfilerActivity.CUDA]) as prof:
+        for i in range(iters):
+            af(i)
+        torch.cuda.synchronize()
+    passes = {"stats": ("af_stats_kernel", 6), "norm": ("af_update_kernel<false", 2),
+              "apply": ("af_update_kernel<true", 12)}          # name, bytes/param of the pass
+    for ev in prof.key_averages():
+        for pname, (key, bpp) in passes.items():
+            if key in ev.key and ev.count:
+                us = ev.device_time_total / ev.count
+                gbs = bpp * n_real / us / 1e3
+                rec = {"kernel": "K2-af %s pass (%s)" % (pname, ev.key[:60]), "us": round(us, 2),
+                       "bytes": bpp * n_real, "GBps": round(gbs, 1), "frac_of_measured_hbm": round(gbs / peak_gbs(), 3),
+                       "launches": ev.count, "note": "%d B/param, torch.profiler" % bpp}
+                print(json.dumps(rec), flush=True)
+                recs.append(rec)
+    return recs + [
+            timed("K2-mt sgd mlp bf16-grad (%d tensors, %d params)" % (len(slots), n_real), sgd, 1,
+                  10 * n_real, iters, "10 B/param (no momentum)", graph=True)]
 
 
 def bench_k10(iters):
@@ -599,7 +669,7 @@ def bench_k9(iters):
 BENCHES = {"k2": bench_k2, "k2mt": bench_k2mt, "k2lw": bench_k2lw, "k3": bench_k3, "k4": bench_k4, "k5": bench_k5, "k5a": bench_k5a,
            "k5m": bench_k5m, "k4s": bench_k4s, "k6": bench_k6,
            "k8": bench_k8, "k8t": bench_k8t, "k9": bench_k9, "k10": bench_k10, "k11": bench_k11,
-           "k2q8": bench_k2q8}
+           "k2q8": bench_k2q8, "k2af": bench_k2af}
 
 
 def main():
