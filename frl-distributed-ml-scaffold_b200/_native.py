@@ -60,6 +60,8 @@ SIGNATURES = {
     "frl_dw_gemm": (_i, [_vp, _i64, _vp, _i64, _i64, _i64, _i64, _vp, _vp]),
     "frl_dw_gemm_sgd": (_i, [_vp, _i64, _vp, _i64, _i64, _i64, _i64, _vp, _vp, _vp, _vp, _d, _d, _d, _d, _d,
                              _vp, _i, _vp]),
+    "frl_dx_drelu_scratch_bytes": (_i64, [_i64, _i64]),
+    "frl_dx_gemm_drelu": (_i, [_vp, _i64, _vp, _i64, _vp, _i64, _vp, _i64, _vp, _i64, _i64, _i64, _i, _vp, _vp]),
     "frl_mt_tile_elems": (_i64, []),
     "frl_flatten_grads": (_i, [_vp, _vp, _vp, _i64, _vp, _i, _d, _vp]),
     "frl_sgd_momentum_mt": (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _i64, _d, _d, _d, _d, _d, _vp, _vp, _i, _vp]),
@@ -233,6 +235,45 @@ def dw_gemm_sgd(dz, x, gw, p, buf, p_lp, *, lr, mu, dampening, wd, grad_scale=1.
     _check(lib().frl_dw_gemm_sgd(_ptr(dz), dz.stride(0), _ptr(x), x.stride(0), dz.shape[0], dz.shape[1],
                                  x.shape[1], _ptr(gw), _ptr(p), _ptr(buf), _ptr(p_lp), lr, mu, dampening, wd,
                                  grad_scale, _ptr(dyn), int(first_step), _stream()), "frl_dw_gemm_sgd")
+
+
+# ---- K13: data-gradient GEMM with the lower unit's ReLU backward and bias gradient in its epilogue --
+
+def dx_drelu_fits(dz_up, w_up, act, db) -> bool:
+    """Whether K13 can form dZ = [act > 0] * (dz_up w_up) and db from it: bf16 operands with unit
+    column stride and rows 16-byte aligned, a bf16 bias gradient, rows a multiple of 128, columns a
+    multiple of 256 and the contraction width a multiple of 8."""
+    return (dz_up.dim() == 2 and w_up.dim() == 2 and act.dim() == 2 and db.dim() == 1
+            and dz_up.dtype == w_up.dtype == act.dtype == db.dtype == torch.bfloat16
+            and dz_up.stride(1) == 1 and w_up.stride(1) == 1 and act.stride(1) == 1
+            and dz_up.stride(0) % 8 == 0 and w_up.stride(0) % 8 == 0 and act.stride(0) % 8 == 0
+            and dz_up.data_ptr() % 16 == 0 and w_up.data_ptr() % 16 == 0 and act.data_ptr() % 16 == 0
+            and dz_up.shape[1] == w_up.shape[0] and tuple(act.shape) == (dz_up.shape[0], w_up.shape[1])
+            and db.shape[0] == act.shape[1] and db.stride(0) == 1
+            and act.shape[0] % 128 == 0 and act.shape[0] > 0 and act.shape[1] % 256 == 0
+            and dz_up.shape[1] % 8 == 0 and dz_up.shape[1] > 0)
+
+
+_dx_drelu_scratch = {}
+
+#: K13 reads dZ_up in 64-byte rows; when dZ_up's rows start on 128-byte boundaries (a row stride that
+#: is a multiple of 64 bf16) no row straddles a cache line, and at the heads' K = 1064 the GEMM
+#: measured 30 % faster on H100 than with the unpadded stride of 1064
+DX_DRELU_ROW_ALIGN = 64
+
+
+def dx_gemm_drelu(dz_up, w_up, act, dz_out, db_out, accumulate: bool = False) -> None:
+    """dz_out = threshold_backward(bf16(dz_up @ w_up), act, 0); db_out (+)= its column sums (K13)."""
+    rows, cols = act.shape
+    key = (act.device.index, cols)
+    need = int(lib().frl_dx_drelu_scratch_bytes(rows, cols))
+    buf = _dx_drelu_scratch.get(key)
+    if buf is None or buf.numel() * 4 < need:
+        buf = _dx_drelu_scratch[key] = torch.zeros((need + 3) // 4, dtype=torch.int32, device=act.device)
+    _check(lib().frl_dx_gemm_drelu(_ptr(dz_up), dz_up.stride(0), _ptr(w_up), w_up.stride(0), _ptr(act),
+                                   act.stride(0), _ptr(dz_out), dz_out.stride(0), _ptr(db_out), rows,
+                                   dz_up.shape[1], cols, int(accumulate), _ptr(buf), _stream()),
+           "frl_dx_gemm_drelu")
 
 
 # ---- K2-mt / K1: multi-tensor forms (gradients read where autograd left them) ---------------------

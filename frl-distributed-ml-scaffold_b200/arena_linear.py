@@ -43,9 +43,18 @@ Whatever the variant, backward runs one protocol: form dZ (on a ReLU site inside
 overwrites W.  So can the dW GEMM itself: on one GPU with SGD (``GradBucketPipeline.fused_dw_update``)
 a bf16 weight applied once per forward whose shape fits the tile gets its gradient and its update
 from one kernel (``frl_dw_gemm_sgd``, K12).
+
+A fused Linear+ReLU unit (the *producer*) whose output only one Linear site (the *consumer*) reads
+-- the next Linear of the same ``nn.Sequential``, or the fused task heads when the unit ends a
+``MultiTaskModel`` trunk -- is linked to it at patch time (``_link_relu_consumers``; off with
+``FRL_B200_FUSED_DRELU_DX=0``).  In a BF16 step the consumer's dX GEMM is then K13
+(``frl_dx_gemm_drelu``): it writes the producer's dZ = [Y > 0] * dX and the producer's bias
+gradient instead of dX, and the producer's backward skips ``frl_drelu_colsum``.  The dX that K6b
+would re-read is never written.
 """
 import os
 import types
+import weakref
 from collections import Counter
 from typing import List, Optional
 
@@ -182,6 +191,8 @@ class _ArenaLinearFn(torch.autograd.Function):
             saved = (x, weight)
         if relu and saved:
             saved += (y,)
+            if getattr(site, "consumer", None) is not None:
+                site.y_out = weakref.ref(y)
         ctx.save_for_backward(*saved)
         return y
 
@@ -196,7 +207,10 @@ class _ArenaLinearFn(torch.autograd.Function):
         if relu or ctx.fp8:
             dz = dz.contiguous()
         db_written = False
-        if relu:
+        if relu and in_step and site.dz_from_consumer == (pipe.step_id, dz.data_ptr()):
+            site.dz_from_consumer = None             # K13 in the consumer's backward formed dZ and db
+            db_written = True
+        elif relu:
             y2 = saved[-1].reshape(-1, dz.shape[1])
             if in_step:                              # dZ and the bias gradient in one pass
                 dz_relu = torch.empty_like(dz)
@@ -209,7 +223,10 @@ class _ArenaLinearFn(torch.autograd.Function):
         gemms = (_Fp8Gemms if ctx.fp8 else _DenseGemms)(saved, dz, need_dx)
         # dX first: marking the weight's slot ready may launch the bucket's update on the side
         # stream, and that update overwrites the very weight dX = dZ W reads
-        dx = gemms.dx().view(ctx.x_shape) if need_dx else None
+        dx = None
+        if need_dx:
+            dx = _dx_drelu(site.producer, pipe, dz, gemms.weight, gemms.x2) if in_step and not ctx.fp8 else None
+            dx = (dx if dx is not None else gemms.dx()).view(ctx.x_shape)
         if in_step:
             site.weight_grad(pipe, gemms)
             if ctx.has_bias and not db_written and site.bslot is not None:
@@ -246,10 +263,19 @@ class _ArenaMultiHeadFn(torch.autograd.Function):
         (x,) = ctx.saved_tensors
         site = ctx.site
         pipe = site.pipeline
-        dy = torch.cat(dys, dim=1)
-        dx = dy.matmul(site.weight_cat()) if ctx.needs_input_grad[0] else None
+        in_step = pipe is not None and pipe.step_open
+        cols = sum(d.shape[1] for d in dys)
+        # K13 reads dY: give its rows an aligned stride (the pad columns are never read)
+        pad = (-cols) % _native.DX_DRELU_ROW_ALIGN if (in_step and site.producer is not None
+                                                       and ctx.needs_input_grad[0]) else 0
+        dy = torch.cat(dys + ((dys[0].new_empty(dys[0].shape[0], pad),) if pad else ()), dim=1)[:, :cols]
+        dx = None
+        if ctx.needs_input_grad[0]:
+            dx = _dx_drelu(site.producer, pipe, dy, site.weight_cat(), x) if in_step else None
+            if dx is None:
+                dx = dy.matmul(site.weight_cat())
         none = (None,) * (2 * ctx.n_heads)
-        if pipe is not None and pipe.step_open:
+        if in_step:
             gw = site.grad_weight_cat()
             if site.heads[0].wstate.first_touch(pipe.step_id):
                 torch.mm(dy.t(), x, out=gw)
@@ -258,7 +284,7 @@ class _ArenaMultiHeadFn(torch.autograd.Function):
             for h in site.heads[1:]:
                 h.wstate.first_touch(pipe.step_id)
             gb = site.grad_bias_cat()
-            if gb is not None:
+            if gb is not None and dy.is_contiguous():
                 first = site.heads[0].bstate.first_touch(pipe.step_id)
                 for h in site.heads[1:]:
                     h.bstate.first_touch(pipe.step_id)
@@ -296,6 +322,7 @@ class MultiHeadSite:
         b_adjacent = all(h.bslot.end == n.bslot.offset for h, n in zip(heads[:-1], heads[1:]))
         self._b = (heads[0].bslot.offset, heads[-1].bslot.end) if b_adjacent else None
         self._arena = arena
+        self.producer = None          # the Linear+ReLU unit whose output the heads read (K13)
 
     def weight_cat(self) -> torch.Tensor:
         a = self._arena
@@ -376,7 +403,8 @@ class LinearSite:
     site counts its applications in the forward pass (training mode, autograd on) and marks its
     slots ready only when as many backward passes have run; anything left over is marked by
     ``GradBucketPipeline.finish_step`` (after ``backward()`` returned nothing can be missing)."""
-    __slots__ = ("module", "wslot", "bslot", "pipeline", "relu", "wstate", "bstate", "multihead", "fp8")
+    __slots__ = ("module", "wslot", "bslot", "pipeline", "relu", "wstate", "bstate", "multihead", "fp8",
+                 "producer", "consumer", "y_out", "dz_from_consumer")
 
     def __init__(self, module, wslot, bslot, pipeline):
         self.module = module
@@ -386,6 +414,10 @@ class LinearSite:
         self.relu = None              # the nn.ReLU this layer absorbed (FRL_B200_FUSE_RELU)
         self.multihead = None         # on the first head: the MultiHeadSite of its model
         self.fp8 = False              # Precision.FP8 and fp8_site_qualifies: FP8 GEMMs per call
+        self.producer = None          # the Linear+ReLU unit whose output this site reads (K13)
+        self.consumer = None          # on a producer: the one site (or MultiHeadSite) reading its output
+        self.y_out = None             # on a producer: weak reference to the output of its last forward
+        self.dz_from_consumer = None  # on a producer: (step, address) of the dZ K13 formed for it
         states = pipeline.slot_states
         self.wstate = states.setdefault(wslot.index, SlotState())
         self.bstate = states.setdefault(bslot.index, SlotState()) if bslot is not None else None
@@ -434,6 +466,25 @@ class LinearSite:
                 pipe.defer_ready(self.bslot)
 
 
+def _dx_drelu(producer, pipe, dz_up, w_up, x):
+    """The consumer's dX GEMM as K13 (``frl_dx_gemm_drelu``) when it can serve it: returns the
+    producer's dZ, with the producer's bias gradient written, or None (the caller computes dX)."""
+    if producer is None or pipe.arena.precision is not Precision.BF16 or not hasattr(KERNELS, "dx_gemm_drelu"):
+        return None
+    y = producer.y_out() if producer.y_out is not None else None
+    if y is None or y.data_ptr() != x.data_ptr() or y.shape != x.shape or y.stride() != x.stride():
+        return None                      # not the producer's output of this forward
+    act = x.reshape(-1, x.shape[-1])
+    db = pipe.arena.grad_view(producer.bslot)
+    if not _native.dx_drelu_fits(dz_up, w_up, act, db):
+        return None
+    dz = torch.empty_like(act)
+    KERNELS.dx_gemm_drelu(dz_up, w_up, act, dz, db,
+                          accumulate=not producer.bstate.first_touch(pipe.step_id))
+    producer.dz_from_consumer = (pipe.step_id, dz.data_ptr())
+    return dz
+
+
 def _for_backward(*tensors) -> bool:
     return torch.is_grad_enabled() and any(t is not None and t.requires_grad for t in tensors)
 
@@ -478,6 +529,38 @@ def _fuse_relu_pairs(model: nn.Module, sites: List[LinearSite]) -> int:
     return fused
 
 
+def _link_relu_consumers(model: nn.Module, sites: List[LinearSite]) -> int:
+    """Link each fused Linear+ReLU unit to the one site that reads its output: the next Linear of
+    the same ``nn.Sequential`` (adjacent, used once, no hooks), or the fused heads when the unit is
+    the last of a ``MultiTaskModel`` trunk that is an ``nn.Sequential`` used once."""
+    uses = Counter(id(child) for mod in model.modules() for child in mod._modules.values()
+                   if child is not None)
+    by_module = {id(s.module): s for s in sites}
+    heads = next((s.multihead for s in sites if s.multihead is not None), None)
+    linked = 0
+    for seq in model.modules():
+        if type(seq) is not nn.Sequential or _has_hooks(seq):
+            continue
+        kids = list(seq._modules.values())
+        for i, (lin, act) in enumerate(zip(kids, kids[1:])):
+            prod = by_module.get(id(lin))
+            if prod is None or prod.relu is not act or prod.consumer is not None:
+                continue
+            if i + 2 < len(kids):
+                cons = by_module.get(id(kids[i + 2]))
+                if (cons is None or cons.producer is not None or uses[id(cons.module)] != 1
+                        or _has_hooks(cons.module) or cons.multihead is not None):
+                    continue
+            elif (heads is not None and heads.model.model_base is seq and uses[id(seq)] == 1
+                  and heads.producer is None):
+                cons = heads
+            else:
+                continue
+            cons.producer, prod.consumer = prod, cons
+            linked += 1
+    return linked
+
+
 def patch_linears(model: nn.Module, pipeline) -> List[LinearSite]:
     """Route every exact ``nn.Linear`` whose weight lives in the arena through the Function."""
     sites: List[LinearSite] = []
@@ -504,6 +587,8 @@ def patch_linears(model: nn.Module, pipeline) -> List[LinearSite]:
         if site.multihead is not None:              # the fused task heads stay bf16
             for h in site.multihead.heads:
                 h.fp8 = False
+    if os.environ.get("FRL_B200_FUSED_DRELU_DX", "1") != "0":
+        _link_relu_consumers(model, sites)
     repatch_linears(sites)
     return sites
 

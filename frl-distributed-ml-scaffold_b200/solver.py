@@ -470,6 +470,7 @@ class Solver:
             logger.info(
                 "frl_b200 step: precision %s | step issue %s | gradient exchange %s | update %s | "
                 "Linear layers with arena-born gradients %d (%d fused with their ReLU, %d in FP8) | "
+                "ReLU backward %s | "
                 "other gradients %s | layer adaptation %s | gradient accumulation %s | weight EMA %s | "
                 "optimizer state %s",
                 args.precision.value,
@@ -482,6 +483,10 @@ class Solver:
                 if pipeline.fused_dw_update else "one tail launch",
                 len(pipeline.linear_sites), sum(s.relu is not None for s in pipeline.linear_sites),
                 sum(s.fp8 for s in pipeline.linear_sites),
+                ("of %d units in the dX GEMM of the layer above (K13)" % sum(
+                    s.consumer is not None for s in pipeline.linear_sites))
+                if args.precision is Precision.BF16 and any(s.consumer is not None for s in pipeline.linear_sites)
+                else "K6b pass per unit",
                 "read in place through segment tables (K2-mt / one flatten launch per bucket)"
                 if pipeline.mt_enabled else "copied into the arena per tensor",
                 "none" if args.layer_adaptation == LayerAdaptation.NONE else

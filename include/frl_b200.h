@@ -102,6 +102,23 @@ int frl_dw_gemm_sgd(const void* dz, int64_t ld_dz, const void* x, int64_t ld_x, 
                     const float* dyn, int first_step, void* stream);
 
 /* ------------------------------------------------------------------------------------------
+ * K13 — data-gradient GEMM of an upper Linear layer with the lower Linear+ReLU unit's backward in
+ * its epilogue (persistent, TMA + WGMMA):
+ *   dz[r, c]  = act[r, c] <= 0 ? 0 : bf16((dz_up w)[r, c])    (fp32 accumulation, rounded once;
+ *               a NaN activation passes the gradient through, as threshold_backward does)
+ *   db[c]   (+)= sum_r dz[r, c]                                 (fp32 sums, stored as bf16)
+ *   dz_up [rows, k] (ld_dz_up), w [k, cols] (ld_w), act / dz [rows, cols] (ld_act / ld_dz): row-major
+ *   bf16; db [cols] bf16.  rows % 128 == 0, cols % 256 == 0, k % 8 == 0, every pointer except db
+ *   16-byte aligned and every leading dimension a multiple of 8, else FRL_E_ARG.  scratch: at least
+ *   frl_dx_drelu_scratch_bytes(rows, cols) bytes, zeroed before the first launch and left zeroed by
+ *   every launch; launches sharing it must be stream-ordered.  Deterministic: no float atomics.
+ * ---------------------------------------------------------------------------------------- */
+int64_t frl_dx_drelu_scratch_bytes(int64_t rows, int64_t cols);
+int frl_dx_gemm_drelu(const void* dz_up, int64_t ld_dz_up, const void* w, int64_t ld_w, const void* act,
+                      int64_t ld_act, void* dz, int64_t ld_dz, void* db, int64_t rows, int64_t k,
+                      int64_t cols, int accumulate, void* scratch, void* stream);
+
+/* ------------------------------------------------------------------------------------------
  * K2-mt / K1 — multi-tensor forms of the update and the bucket flatten.
  * Replaces the DDP reducer's per-tensor bucket copy-in / copy-out (reference solver.py:287-289 ->
  * torch Reducer) for parameters whose gradients autograd allocates itself (convolutions,

@@ -1,7 +1,7 @@
 #!/usr/bin/env python
 """Micro-benchmark of every hand-written kernel at the BASELINE shapes (1 GPU).
 
-    python tools/kernel_bench.py [--only k2,k2lw,k2q8,k2af,k3,k5a,...] [--iters 20] [--json out.json]
+    python tools/kernel_bench.py [--only k2,k2lw,k2q8,k2af,k3,k5a,k13,...] [--iters 20] [--json out.json]
 
 Each kernel is timed with CUDA events on the launching stream over ROTATING operand sets whose
 total size exceeds the 50 MB L2 (so every launch streams from HBM), after 3 warm-up launches.
@@ -666,10 +666,46 @@ def bench_k9(iters):
     return out
 
 
+def bench_k13(iters):
+    """K13 against what it replaces, torch.mm then K6b, and against torch.mm alone: L2-cold (rotating
+    operand sets), each arm timed from a CUDA graph, the three arms alternated over 3 rounds."""
+    out = []
+    B, N = 4096, 4096
+    for K in (4096, 1064):
+        per = (B * K + K * N + 3 * B * N) * 2
+        ns = sets_for(per)
+        ld = -(-K // _native.DX_DRELU_ROW_ALIGN) * _native.DX_DRELU_ROW_ALIGN   # the step's row stride
+        dz_up = [torch.randn(B, ld, device=DEV).bfloat16()[:, :K] for _ in range(ns)]
+        w = [torch.randn(K, N, device=DEV).bfloat16() for _ in range(ns)]
+        act = [torch.randn(B, N, device=DEV).relu().bfloat16() for _ in range(ns)]
+        dz = [torch.empty(B, N, device=DEV, dtype=torch.bfloat16) for _ in range(ns)]
+        dx = [torch.empty(B, N, device=DEV, dtype=torch.bfloat16) for _ in range(ns)]
+        db = torch.empty(N, device=DEV, dtype=torch.bfloat16)
+
+        def k13(i):
+            _native.dx_gemm_drelu(dz_up[i], w[i], act[i], dz[i], db)
+
+        def mm(i):
+            torch.mm(dz_up[i], w[i], out=dx[i])
+
+        def mm_k6b(i):
+            mm(i)
+            _native.drelu_colsum(dx[i], act[i], dz[i], db)
+
+        shape = "[%d,%d]x[%d,%d]" % (B, K, K, N)
+        for _ in range(3):
+            out.append(timed("K13 dx_gemm_drelu " + shape, k13, ns, per, iters, graph=True))
+            out.append(timed("torch.mm + K6b drelu_colsum " + shape, mm_k6b, ns, per + 4 * B * N, iters,
+                             graph=True))
+            out.append(timed("torch.mm " + shape, mm, ns, per - 2 * B * N, iters, graph=True))
+        del dz_up, w, act, dz, dx
+    return out
+
+
 BENCHES = {"k2": bench_k2, "k2mt": bench_k2mt, "k2lw": bench_k2lw, "k3": bench_k3, "k4": bench_k4, "k5": bench_k5, "k5a": bench_k5a,
            "k5m": bench_k5m, "k4s": bench_k4s, "k6": bench_k6,
            "k8": bench_k8, "k8t": bench_k8t, "k9": bench_k9, "k10": bench_k10, "k11": bench_k11,
-           "k2q8": bench_k2q8, "k2af": bench_k2af}
+           "k2q8": bench_k2q8, "k2af": bench_k2af, "k13": bench_k13}
 
 
 def main():
