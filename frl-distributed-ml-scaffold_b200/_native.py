@@ -80,6 +80,10 @@ SIGNATURES = {
     "frl_adafactor_scratch_bytes": (_i64, [_vp, _i64]),
     "frl_adafactor_mt": (_i, [_vp, _vp, _vp, _vp, _i64, _vp, _vp, _vp, _vp, _i64, _vp, _vp, _d, _d, _d, _d, _d, _d,
                               _i64, _d, _vp, _vp, _vp]),
+    "frl_muon_plan_bytes": (_i64, [_vp, _i64, _vp, _vp]),
+    "frl_muon_plan": (_i, [_vp, _i64, _vp, _vp, _vp]),
+    "frl_muon_mt": (_i, [_vp, _vp, _vp, _vp, _i64, _vp, _vp, _vp, _d, _d, _d, _i, _d, _d, _d, _i, _d, _i, _d, _vp,
+                         _vp, _vp]),
     "frl_grad_accumulate_mt": (_i, [_vp, _vp, _vp, _vp, _i64, _d, _i, _vp, _vp]),
     "frl_weight_ema": (_i, [_vp, _vp, _i64, _d, _vp]),
     "frl_reduce_scratch_bytes": (_i64, []),
@@ -463,6 +467,85 @@ def adafactor_mt(p, state, p_lp, table, plan, *, lr, beta2_decay, eps1, eps2, d,
                                   _ptr(state_off), _ptr(flags), _ptr(work), work.shape[0] if n else 0,
                                   _ptr(seg_info), _ptr(scratch), lr, beta2_decay, eps1, eps2, d, wd, step,
                                   grad_scale, _ptr(grad_scale_dev), _ptr(dyn), _stream()), "frl_adafactor_mt")
+
+
+# ---- K14: Muon over a segment table -----------------------------------------------------------------
+
+class MuonPlan:
+    """K14's plan for one segment table: the host and device copies of the tile tables and tensor
+    maps, its scratch (tickets, norms, partials), the matrices' (segment, arena offset, R, C) rows,
+    and the workspace and exp_avg_sq vector the plan points into."""
+
+    def __init__(self, shape, host, dev, scratch, workspace, state):
+        self.shape, self.host, self.dev, self.scratch = shape, host, dev, scratch
+        self.workspace, self.state = workspace, state
+        self.n_mat = shape.shape[0]
+
+
+def _muon_shape(shape: torch.Tensor) -> torch.Tensor:
+    if shape.dtype != torch.int64 or shape.dim() != 2 or shape.shape[1] != 4 or shape.device.type != "cpu":
+        raise NativeLibraryError("Muon: shape must be a CPU int64 [n_mat, 4] tensor of (segment, arena offset, R, C)")
+    return shape.contiguous()
+
+
+def muon_plan_bytes(shape: torch.Tensor):
+    """(plan bytes, scratch bytes, workspace bytes) of the matrices in ``shape``; host only."""
+    shape = _muon_shape(shape)
+    scratch, ws = C.c_int64(0), C.c_int64(0)
+    n = int(lib().frl_muon_plan_bytes(_ptr(shape), shape.shape[0], C.byref(scratch), C.byref(ws)))
+    if n < 0:
+        raise NativeLibraryError("Muon: bad matrix shape")
+    return n, int(scratch.value), int(ws.value)
+
+
+def muon_plan(shape: torch.Tensor, exp_avg_sq: torch.Tensor, workspace: torch.Tensor) -> MuonPlan:
+    """Plan K14 over the matrices of ``shape`` (see frl_muon_plan in include/frl_b200.h), with the
+    iterates in ``exp_avg_sq`` (fp32, arena-shaped), the Gram buffers in ``workspace`` (which plans
+    over subsets of the same matrices may share) and a fresh zeroed scratch."""
+    shape = _muon_shape(shape)
+    if exp_avg_sq.dtype != torch.float32 or not exp_avg_sq.is_contiguous():
+        raise NativeLibraryError("Muon: exp_avg_sq must be contiguous fp32")
+    nbytes, scratch_bytes, ws_bytes = muon_plan_bytes(shape)
+    if workspace.numel() * workspace.element_size() < ws_bytes or workspace.data_ptr() % 128:
+        raise NativeLibraryError("Muon: workspace needs %d bytes, 128-byte aligned" % ws_bytes)
+    dev = exp_avg_sq.device
+    scratch = torch.zeros((scratch_bytes + 15) // 16 * 4, dtype=torch.int32, device=dev)
+    host = torch.zeros((nbytes + 63) // 64 * 64, dtype=torch.uint8)
+    _check(lib().frl_muon_plan(_ptr(shape), shape.shape[0], _ptr(exp_avg_sq), _ptr(workspace), _ptr(host)),
+           "frl_muon_plan")
+    return MuonPlan(shape, host, host.to(dev), scratch, workspace, exp_avg_sq)
+
+
+def check_muon_hyper(*, lr, wd, momentum, ns_steps, eps, adjust_lr_fn) -> None:
+    """The argument checks of frl_muon_mt, for a caller that must refuse before launching anything."""
+    if not (float(lr) >= 0.0 and float(wd) >= 0.0 and float(momentum) >= 0.0 and float(eps) >= 0.0):
+        raise NativeLibraryError("Muon: lr, weight_decay, momentum and eps must be >= 0")
+    if int(ns_steps) != ns_steps or not 1 <= int(ns_steps) < 100:
+        raise NativeLibraryError("Muon: ns_steps must be an integer in [1, 100), got %r" % (ns_steps,))
+    if adjust_lr_fn not in (None, "original", "match_rms_adamw"):
+        raise NativeLibraryError("Muon: adjust_lr_fn must be None, 'original' or 'match_rms_adamw'")
+
+
+def muon_mt(p, exp_avg, p_lp, table, plan: MuonPlan, *, lr, wd, momentum, nesterov, ns_coefficients, ns_steps, eps,
+            adjust_lr_fn, grad_scale=1.0, grad_scale_dev=None, dyn=None) -> None:
+    """K14 Muon over the matrices of ``plan``, gradients read through ``table`` (the plan's segment
+    indices refer to it).  See frl_muon_mt in include/frl_b200.h."""
+    for t in (p, exp_avg):
+        if not (t.dtype == torch.float32 and t.is_contiguous()):
+            raise NativeLibraryError("Muon: master weights and exp_avg must be contiguous fp32")
+    check_muon_hyper(lr=lr, wd=wd, momentum=momentum, ns_steps=ns_steps, eps=eps, adjust_lr_fn=adjust_lr_fn)
+    if dyn is not None and (dyn.dtype != torch.float32 or dyn.numel() < 3):
+        raise NativeLibraryError("Muon: dyn must be fp32 with at least 3 elements")
+    for seg, _, r, c in plan.shape.tolist():
+        if not (0 <= seg < table.n_segs and table.slots[seg].numel == r * c):
+            raise NativeLibraryError("Muon: the plan's matrix [%d, %d] does not match segment %d of the table"
+                                     % (r, c, seg))
+    a, b, c = (float(x) for x in ns_coefficients)
+    _check(lib().frl_muon_mt(_ptr(p), _ptr(exp_avg), _ptr(p_lp), table.segs_dev_ptr, table.n_segs, _ptr(plan.host),
+                             _ptr(plan.dev), _ptr(plan.scratch), float(lr), float(wd), float(momentum),
+                             int(bool(nesterov)), a, b, c, int(ns_steps), float(eps),
+                             int(adjust_lr_fn == "match_rms_adamw"), float(grad_scale), _ptr(grad_scale_dev),
+                             _ptr(dyn), _stream()), "frl_muon_mt")
 
 
 # ---- K10: gradient accumulation over a segment table ----------------------------------------------

@@ -1,4 +1,5 @@
-// Building blocks of the persistent TMA + WGMMA GEMMs (K12 dw_update.cu, K13 dx_drelu.cu), sm_90a.
+// Building blocks of the persistent TMA + WGMMA GEMMs (K12 dw_update.cu, K13 dx_drelu.cu, K14
+// muon.cu), sm_90a.
 //
 // Both kernels walk 128 x 256 output tiles with one CTA per SM: a TMA producer fills a ring of
 // k-blocks tracked by full/empty mbarriers, two consumer warpgroups run m64n256k16 WGMMAs with fp32
@@ -65,9 +66,9 @@ __device__ __forceinline__ void fence_acc(float* d) {
     for (int i = 0; i < 128; ++i) asm volatile("" : "+f"(d[i]) :: "memory");
 }
 
-// D[64 x 256] (+)= A[64 x 16] B[16 x 256]; B MN-major in shared memory, A MN-major (kTransA = 1)
-// or K-major (kTransA = 0)
-template <int kTransA>
+// D[64 x 256] (+)= A[64 x 16] B[16 x 256]; A MN-major (kTransA = 1) or K-major (kTransA = 0), B
+// MN-major (kTransB = 1) or K-major (kTransB = 0) in shared memory
+template <int kTransA, int kTransB = 1>
 __device__ __forceinline__ void wgmma_m64n256k16(float* d, uint64_t da, uint64_t db, int accumulate) {
     asm volatile(
         "{\n"
@@ -82,7 +83,7 @@ __device__ __forceinline__ void wgmma_m64n256k16(float* d, uint64_t da, uint64_t
         "%80, %81, %82, %83, %84, %85, %86, %87, %88, %89, %90, %91, %92, %93, %94, %95,"
         "%96, %97, %98, %99, %100, %101, %102, %103, %104, %105, %106, %107, %108, %109, %110, %111,"
         "%112, %113, %114, %115, %116, %117, %118, %119, %120, %121, %122, %123, %124, %125, %126, %127"
-        "}, %128, %129, p, 1, 1, %131, 1;\n"
+        "}, %128, %129, p, 1, 1, %131, %132;\n"
         "}\n"
         : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
           "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),
@@ -100,7 +101,7 @@ __device__ __forceinline__ void wgmma_m64n256k16(float* d, uint64_t da, uint64_t
           "+f"(d[104]), "+f"(d[105]), "+f"(d[106]), "+f"(d[107]), "+f"(d[108]), "+f"(d[109]), "+f"(d[110]), "+f"(d[111]),
           "+f"(d[112]), "+f"(d[113]), "+f"(d[114]), "+f"(d[115]), "+f"(d[116]), "+f"(d[117]), "+f"(d[118]), "+f"(d[119]),
           "+f"(d[120]), "+f"(d[121]), "+f"(d[122]), "+f"(d[123]), "+f"(d[124]), "+f"(d[125]), "+f"(d[126]), "+f"(d[127])
-        : "l"(da), "l"(db), "r"(accumulate), "n"(kTransA));
+        : "l"(da), "l"(db), "r"(accumulate), "n"(kTransA), "n"(kTransB));
 }
 
 // output tile `tile` -> first row m0 / column n0: groups of 16 row blocks (all of them if they do

@@ -10,6 +10,8 @@ format and update whole tensors through the K2-lw kernels.  ``FusedAdam8bit`` (a
 ``types.OptimizerState``) keeps Adam's moments as 8-bit block-wise codes (K2-q8) and speaks
 ``torch.optim.Adam``'s format in its state dict.  ``FusedAdafactor`` (an extension, chosen with
 ``Solver.solve(..., adafactor=True)``) is ``torch.optim.Adafactor``'s rule and state format (K2-af).
+``FusedMuon`` (an extension, ``Solver.solve(..., muon=True)``) is ``torch.optim.Muon`` (K14) for the
+model's 2-D weights and this module's Adam (K2-mt) for every other parameter.
 
 Known limitation: the step count (Adam's bias corrections) is ONE number for the whole arena.
 ``torch.optim`` keeps one per parameter and does not advance it for a parameter whose gradient
@@ -792,6 +794,239 @@ def check_adafactor(optim_opts: OptimOpts, layer_adaptation: LayerAdaptation,
                                           " with amsgrad" if optim_opts.amsgrad else "", la.value, st.value))
 
 
+# ---- Muon (K14) for the model's matrices, Adam (K2-mt) for the rest ------------------------------------
+
+MUON_NS_COEFFICIENTS = (3.4445, -4.7750, 2.0315)
+
+
+def is_muon_slot(slot) -> bool:
+    """Muon updates the model parameters with exactly two dimensions (Linear weights, embeddings,
+    task heads); biases, normalisation affine parameters, conv kernels and criterion parameters
+    stay with Adam."""
+    return slot.is_model and len(slot.shape) == 2
+
+
+def _gather_segs(parent, sub, idx: Tuple[torch.Tensor, torch.Tensor]) -> None:
+    """Copy rows ``idx`` (host, device) of ``parent``'s segment table into ``sub``: the host copy, and
+    the device copy on the stream, so a captured CUDA graph re-reads the parent's rows on every
+    replay."""
+    from .multi_tensor import _SEG_BYTES
+    n = sub.n_segs
+    sub._host.view(-1, _SEG_BYTES)[:n] = parent._host.view(-1, _SEG_BYTES)[idx[0]]
+    torch.index_select(parent._dev.view(-1, _SEG_BYTES), 0, idx[1], out=sub._dev.view(-1, _SEG_BYTES)[:n])
+
+
+class FusedMuon(_WholeTensorMixin, FusedAdam):
+    """``torch.optim.Muon`` (group 0: the model's 2-D parameters, ``is_muon_slot``) plus
+    ``FusedAdam``'s rule (group 1: every other parameter), updated once after backward: K14 over
+    the Muon matrices, K2-mt over the rest.  Inside a Muon slot's range ``exp_avg`` holds the
+    momentum buffer and ``exp_avg_sq`` the two bf16 Newton-Schulz iterates, so the state costs
+    what Adam's does; K14's Gram workspace (``workspace_bytes``) comes on top.  ``state_dict()``
+    has the two groups in torch's format; ``split_muon_state_dict`` / ``join_muon_state_dict``
+    convert it to and from a ``torch.optim.Muon`` plus a ``torch.optim.Adam``."""
+
+    STATE_NAMES = (("exp_avg", "exp_avg"), ("exp_avg_sq", "exp_avg_sq"))
+
+    def __init__(self, arena, lr, weight_decay=0.0, momentum=0.95, eps=1e-8, betas=(0.9, 0.999), nesterov=True,
+                 ns_coefficients=MUON_NS_COEFFICIENTS, muon_eps=1e-7, ns_steps=5,
+                 adjust_lr_fn="match_rms_adamw"):
+        super().__init__(arena, lr=lr, betas=betas, eps=eps, weight_decay=weight_decay, amsgrad=False)
+        muon_ids = {id(s.param) for s in arena.slots if is_muon_slot(s)}
+        self.muon_params = [p for p in arena.all_params if id(p) in muon_ids]
+        self.adam_params = [p for p in arena.all_params if id(p) not in muon_ids]
+        adam = dict(self.param_groups[0])
+        adam["params"] = self.adam_params
+        muon = dict(lr=lr, weight_decay=weight_decay, momentum=momentum, nesterov=nesterov,
+                    ns_coefficients=tuple(ns_coefficients), eps=muon_eps, ns_steps=ns_steps,
+                    adjust_lr_fn=adjust_lr_fn, params=self.muon_params)
+        self.param_groups = [muon, adam]
+        self._muon_rows = [(s.offset, s.shape[0], s.shape[1]) for s in arena.slots if is_muon_slot(s)]
+        # one Gram workspace for every table's plan (their launches are stream-ordered): sized for
+        # all the Muon matrices, any subset fits
+        self.workspace_bytes = KERNELS.muon_plan_bytes(torch.tensor(
+            [(0,) + r for r in self._muon_rows], dtype=torch.int64).reshape(-1, 4))[2] if self._muon_rows else 0
+        self._workspace: Optional[torch.Tensor] = None
+
+    @property
+    def hyper(self) -> Dict[str, Any]:
+        return self.param_groups[1]
+
+    @property
+    def muon_group(self) -> Dict[str, Any]:
+        return self.param_groups[0]
+
+    def _dyn_values(self):
+        # dyn[0], dyn[1]: K2-mt's Adam scalars; dyn[2]: K14's lr
+        return super()._dyn_values() + (float(self.muon_group["lr"]),)
+
+    def _split(self, table):
+        """Per-table pieces, kept on the table: K14's plan over its Muon slots and the K2-mt
+        tables of the other slots (all of them; model parameters; criterion parameters) with the
+        rows of ``table`` they take."""
+        split = getattr(table, "muon", None)
+        if split is None:
+            from .multi_tensor import GradSegTable
+            dev = self.arena.device
+            rows = list(enumerate(table.slots))
+            mu = [(i, s) for i, s in rows if is_muon_slot(s)]
+            rest = [(i, s) for i, s in rows if not is_muon_slot(s)]
+            plan = None
+            if mu:
+                shape = torch.tensor([(i, s.offset, s.shape[0], s.shape[1]) for i, s in mu], dtype=torch.int64)
+                if self._workspace is None:
+                    self._workspace = torch.zeros((self.workspace_bytes + 127) // 128 * 32, dtype=torch.int32,
+                                                  device=dev)
+                plan = KERNELS.muon_plan(shape, self._state("exp_avg_sq"), self._workspace)
+            subs = []
+            for keep in (lambda s: True, lambda s: s.is_model, lambda s: not s.is_model):
+                part = [(i, s) for i, s in rest if keep(s)]
+                sub = GradSegTable([s for _, s in part], dev) if part else None
+                rows_of = torch.tensor([i for i, _ in part], dtype=torch.int64)
+                idx = (rows_of, rows_of.to(dev)) if part else None
+                subs.append((sub, idx))
+            split = table.muon = (plan, subs)
+        return split
+
+    def apply_table(self, table, *, grad_scale: float = 1.0,
+                    clip_coef_dev: Optional[torch.Tensor] = None) -> None:
+        """Update every slot of ``table``: one K2-mt launch over the non-Muon slots (two under
+        clipping when the table also holds criterion parameters, which are not clipped), then K14
+        over the Muon slots."""
+        if not table.n_segs:
+            return
+        plan, (every, model, crit) = self._split(table)
+        h, g = self.hyper, self.muon_group
+        if plan is not None:          # refuse before any launch, not after Adam's half of the step
+            KERNELS.check_muon_hyper(lr=g["lr"], wd=g["weight_decay"], momentum=g["momentum"],
+                                     ns_steps=g["ns_steps"], eps=g["eps"], adjust_lr_fn=g["adjust_lr_fn"])
+        launches = [(every, clip_coef_dev)] if clip_coef_dev is None or crit[0] is None else \
+            [(model, clip_coef_dev), (crit, None)]
+        for (sub, idx), coef in launches:
+            if sub is None:
+                continue
+            _gather_segs(table, sub, idx)
+            KERNELS.adam_mt(self.arena.master, self._state("exp_avg"), self._state("exp_avg_sq"), None,
+                            self.arena.lp, sub, lr=float(h["lr"]), beta1=float(h["betas"][0]),
+                            beta2=float(h["betas"][1]), eps=float(h["eps"]), wd=float(h["weight_decay"]),
+                            step=self._steps + 1, grad_scale=grad_scale, grad_scale_dev=coef, dyn=self._dyn)
+        if plan is not None:
+            KERNELS.muon_mt(self.arena.master, self._state("exp_avg"), self.arena.lp, table, plan,
+                            lr=float(g["lr"]), wd=float(g["weight_decay"]), momentum=float(g["momentum"]),
+                            nesterov=bool(g["nesterov"]), ns_coefficients=tuple(g["ns_coefficients"]),
+                            ns_steps=g["ns_steps"], eps=float(g["eps"]), adjust_lr_fn=g["adjust_lr_fn"],
+                            grad_scale=grad_scale, grad_scale_dev=clip_coef_dev, dyn=self._dyn)
+
+    def _positions(self) -> Dict[int, int]:
+        """torch's state-dict index of each parameter: group 0's, then group 1's."""
+        return {id(p): i for i, p in enumerate(self.muon_params + self.adam_params)}
+
+    def state_dict(self) -> Dict[str, Any]:
+        state: Dict[int, Dict[str, Any]] = {}
+        pos = self._positions()
+        if self._steps > 0:
+            for s in sorted(self.arena.slots, key=lambda s: pos[id(s.param)]):
+                view = lambda name: self._state(name)[s.offset:s.end].view(s.shape).clone()
+                if is_muon_slot(s):
+                    state[pos[id(s.param)]] = {"momentum_buffer": view("exp_avg")}
+                else:
+                    state[pos[id(s.param)]] = {"step": torch.tensor(float(self._steps)),
+                                               "exp_avg": view("exp_avg"), "exp_avg_sq": view("exp_avg_sq")}
+        groups, base = [], 0
+        for g in self.param_groups:
+            packed = {k: v for k, v in g.items() if k != "params"}
+            packed["params"] = list(range(base, base + len(g["params"])))
+            base += len(g["params"])
+            groups.append(packed)
+        return {"state": state, "param_groups": groups}
+
+    def load_state_dict(self, state_dict: Dict[str, Any]) -> None:
+        groups = state_dict["param_groups"]
+        if len(groups) != 2:
+            raise ValueError("a Muon optimizer takes a state dict with two param groups (Muon, Adam), got %d; "
+                             "join a torch.optim.Muon and a torch.optim.Adam state dict with join_muon_state_dict"
+                             % len(groups))
+        if len(groups[0]["params"]) != len(self.muon_params) or len(groups[1]["params"]) != len(self.adam_params):
+            raise ValueError("loaded state dict has %d Muon and %d Adam parameters, this optimizer %d and %d"
+                             % (len(groups[0]["params"]), len(groups[1]["params"]), len(self.muon_params),
+                                len(self.adam_params)))
+        for mine, theirs in zip(self.param_groups, groups):
+            for k, v in theirs.items():
+                if k != "params":
+                    mine[k] = tuple(v) if k == "ns_coefficients" else v
+        position = {q: j for j, q in enumerate(list(groups[0]["params"]) + list(groups[1]["params"]))}
+        params = self.muon_params + self.adam_params
+        slots = {id(s.param): s for s in self.arena.slots}
+        steps = 0
+        for key, entry in state_dict["state"].items():
+            if key not in position:
+                continue
+            s = slots.get(id(params[position[key]]))
+            if s is None:
+                continue
+            names = ((("momentum_buffer", "exp_avg"),) if is_muon_slot(s) else
+                     (("exp_avg", "exp_avg"), ("exp_avg_sq", "exp_avg_sq")))
+            for torch_name, vec in names:
+                if entry.get(torch_name) is not None:
+                    self._state(vec)[s.offset:s.end].view(s.shape).copy_(entry[torch_name])
+            if "step" in entry:
+                steps = max(steps, int(float(entry["step"])))
+            elif entry:
+                steps = max(steps, 1)
+        self._steps = steps
+
+
+def split_muon_state_dict(sd: Dict[str, Any]) -> Tuple[Dict[str, Any], Dict[str, Any]]:
+    """A ``FusedMuon`` state dict -> (``torch.optim.Muon`` state dict over group 0's parameters,
+    ``torch.optim.Adam`` state dict over group 1's)."""
+    groups = sd["param_groups"]
+    if len(groups) != 2:
+        raise ValueError("a Muon state dict has two param groups (Muon, Adam), got %d" % len(groups))
+    out = []
+    for g in groups:
+        ids = list(g["params"])
+        state = {j: sd["state"][i] for j, i in enumerate(ids) if i in sd["state"]}
+        packed = dict(g)
+        packed["params"] = list(range(len(ids)))
+        out.append({"state": state, "param_groups": [packed]})
+    return out[0], out[1]
+
+
+def join_muon_state_dict(muon_sd: Dict[str, Any], adam_sd: Dict[str, Any]) -> Dict[str, Any]:
+    """The inverse of ``split_muon_state_dict``: one ``torch.optim.Muon`` and one ``torch.optim.Adam``
+    state dict (one group each) -> a ``FusedMuon`` state dict."""
+    state, groups, base = {}, [], 0
+    for sd in (muon_sd, adam_sd):
+        if len(sd["param_groups"]) != 1:
+            raise ValueError("join_muon_state_dict takes one-group Muon and Adam state dicts")
+        g = sd["param_groups"][0]
+        ids = list(g["params"])
+        for j, i in enumerate(ids):
+            if i in sd["state"]:
+                state[base + j] = sd["state"][i]
+        packed = dict(g)
+        packed["params"] = list(range(base, base + len(ids)))
+        groups.append(packed)
+        base += len(ids)
+    return {"state": state, "param_groups": groups}
+
+
+def check_muon(optim_opts: OptimOpts, layer_adaptation: LayerAdaptation, optimizer_state: OptimizerState,
+               adafactor: bool, muon: bool) -> None:
+    """Muon needs Adam without amsgrad (for the other parameters), no layer adaptation, fp32
+    optimizer state and no Adafactor; anything else is a ValueError naming the values."""
+    if not muon:
+        return
+    st = OptimizerState(optimizer_state)
+    la = LayerAdaptation(layer_adaptation)
+    if not (optim_opts.algo == OptAlgorithm.ADAM and not optim_opts.amsgrad and la is LayerAdaptation.NONE
+            and st is OptimizerState.FP32 and not adafactor):
+        raise ValueError("muon cannot be combined with optimizer %r%s, layer adaptation %r, optimizer state %r%s "
+                         "(muon needs adam without amsgrad, layer adaptation none, optimizer state fp32 and no "
+                         "adafactor)" % (getattr(optim_opts.algo, "value", optim_opts.algo),
+                                         " with amsgrad" if optim_opts.amsgrad else "", la.value, st.value,
+                                         " and adafactor" if adafactor else ""))
+
+
 def check_optimizer_state(optim_opts: OptimOpts, layer_adaptation: LayerAdaptation,
                           optimizer_state: OptimizerState) -> None:
     """8-bit state needs Adam without amsgrad and without layer adaptation; anything else is a
@@ -822,14 +1057,19 @@ def check_layer_adaptation(optim_opts: OptimOpts, layer_adaptation: LayerAdaptat
 def create_fused_optimizer(arena: ParamArena, optim_opts: OptimOpts,
                            layer_adaptation: LayerAdaptation = LayerAdaptation.NONE,
                            optimizer_state: OptimizerState = OptimizerState.FP32,
-                           adafactor: bool = False) -> FusedArenaOptimizer:
+                           adafactor: bool = False, muon: bool = False) -> FusedArenaOptimizer:
     """Same dispatch and argument mapping as the reference's ``_create_optimizer``; with a layer
     adaptation, its LARS / LAMB counterpart; with 8-bit optimizer state, ``FusedAdam8bit``; with
     ``adafactor``, ``FusedAdafactor`` (``lr`` caps the relative step, ``weightDecay`` is its
-    decoupled decay; ``epsilon`` and ``momentum`` are unused)."""
+    decoupled decay; ``epsilon`` and ``momentum`` are unused); with ``muon``, ``FusedMuon`` (one
+    ``lr`` and ``weightDecay`` for both groups, ``momentum`` is Muon's, ``epsilon`` Adam's)."""
     check_layer_adaptation(optim_opts, layer_adaptation)
     check_optimizer_state(optim_opts, layer_adaptation, optimizer_state)
     check_adafactor(optim_opts, layer_adaptation, optimizer_state, adafactor)
+    check_muon(optim_opts, layer_adaptation, optimizer_state, adafactor, muon)
+    if muon:
+        return FusedMuon(arena, lr=optim_opts.lr, weight_decay=optim_opts.weightDecay,
+                         momentum=optim_opts.momentum, eps=optim_opts.epsilon)
     if adafactor:
         return FusedAdafactor(arena, lr=optim_opts.lr, weight_decay=optim_opts.weightDecay)
     if OptimizerState(optimizer_state) is OptimizerState.Q8:

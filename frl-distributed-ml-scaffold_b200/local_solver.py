@@ -24,7 +24,8 @@ class LocalSolver:
               grad_accumulation: Optional[int] = None,
               ema_decay: Optional[float] = None,
               optimizer_state: Optional[OptimizerState] = None,
-              adafactor: Optional[bool] = None) -> PerformanceSummary:
+              adafactor: Optional[bool] = None,
+              muon: Optional[bool] = None) -> PerformanceSummary:
         if save_notebook:
             logger.warning("save_notebook is not supported by frl_b200 (visualisation only)")
         # a stale rendezvous file from a crashed run would poison the file:// store
@@ -38,6 +39,6 @@ class LocalSolver:
                                  init_method="file://" + SYNC_FILE, precision=precision,
                                  graph=graph, layer_adaptation=layer_adaptation,
                                  grad_accumulation=grad_accumulation, ema_decay=ema_decay,
-                                 optimizer_state=optimizer_state, adafactor=adafactor):
+                                 optimizer_state=optimizer_state, adafactor=adafactor, muon=muon):
             pass
         return last

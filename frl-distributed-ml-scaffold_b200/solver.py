@@ -29,7 +29,7 @@ import torch.nn as nn
 from .arena import ParamArena
 from .criteria import BaseParallelCriterion
 from .ema import EMA_STATE_KEY
-from .fused_optim import (FusedAdafactor, FusedAdam8bit, check_adafactor, check_layer_adaptation, check_optimizer_state, create_fused_optimizer,
+from .fused_optim import (FusedAdafactor, FusedAdam8bit, FusedMuon, check_adafactor, check_muon, check_layer_adaptation, check_optimizer_state, create_fused_optimizer,
                           is_adapted)
 from .grad_sync import BufferBroadcaster, GradBucketPipeline
 from .lr_scheduler import DropEpochsScheduler, WarmupMultiStepLR
@@ -49,6 +49,7 @@ GRAD_ACCUM_ENV = "FRL_B200_GRAD_ACCUM"     # microbatches per optimizer update, 
 EMA_DECAY_ENV = "FRL_B200_EMA_DECAY"       # weight EMA decay in [0, 1), default 0 (off)
 OPTIMIZER_STATE_ENV = "FRL_B200_OPTIMIZER_STATE"   # "fp32" (default) | "8bit"
 ADAFACTOR_ENV = "FRL_B200_ADAFACTOR"               # "0" (default) | "1"
+MUON_ENV = "FRL_B200_MUON"                         # "0" (default) | "1"
 EMA_SUFFIX = ".ema"                        # <checkpoint>.ema: the weight EMA next to a checkpoint
 
 
@@ -103,6 +104,9 @@ class SolverWorkerArgs(NamedTuple):
     save_every: int = 1
     graph_step: Optional[bool] = None      # None: FRL_B200_CUDA_GRAPH (default off)
     layer_adaptation: LayerAdaptation = LayerAdaptation.NONE
+    # Muon for the model's 2-D weights, Adam for the rest; placed before optimizer_state, adafactor,
+    # ema_decay and grad_accumulation, which keep their positions at the end
+    muon: bool = False
     # Adam's state storage; placed before ema_decay and grad_accumulation, which stay the last fields
     optimizer_state: OptimizerState = OptimizerState.FP32
     # Adafactor instead of Adam; placed before ema_decay and grad_accumulation, which stay the last fields
@@ -276,6 +280,17 @@ def resolve_adafactor(explicit: Optional[bool] = None) -> bool:
     return raw == "1"
 
 
+def resolve_muon(explicit: Optional[bool] = None) -> bool:
+    """Whether the model's 2-D weights are updated by Muon: ``explicit``, else FRL_B200_MUON (``0``,
+    the default, or ``1``).  Any other value is a ValueError."""
+    if explicit is not None:
+        return bool(explicit)
+    raw = os.environ.get(MUON_ENV, "0").strip()
+    if raw not in ("0", "1"):
+        raise ValueError("%s must be 0 or 1, got %r" % (MUON_ENV, raw))
+    return raw == "1"
+
+
 def resolve_grad_accumulation(explicit: Optional[int] = None) -> int:
     """Microbatches per optimizer update: ``explicit``, else FRL_B200_GRAD_ACCUM, else 1.  Anything
     but an integer >= 1 (``0``, negatives, ``2.5``, ``True``, non-numeric strings) is a ValueError."""
@@ -393,7 +408,7 @@ class Solver:
         symm_alloc = None
         if (distributed and not run_opts.optim.gradientClip
                 and args.layer_adaptation == LayerAdaptation.NONE and accum == 1 and ema_decay == 0.0
-                and args.optimizer_state is OptimizerState.FP32 and not args.adafactor):
+                and args.optimizer_state is OptimizerState.FP32 and not args.adafactor and not args.muon):
             from .symm import try_make_allocator
             symm_alloc = try_make_allocator(device, args.world_size)
         from .arena_linear import head_layout_groups
@@ -411,7 +426,9 @@ class Solver:
                     buf.data = buf.data.to(torch.bfloat16)
         opt_state = args.optimizer_state if run_opts.mode == Mode.TRAIN else OptimizerState.FP32
         adafactor = args.adafactor and run_opts.mode == Mode.TRAIN
-        optimizer = create_fused_optimizer(arena, run_opts.optim, args.layer_adaptation, opt_state, adafactor)
+        muon = args.muon and run_opts.mode == Mode.TRAIN
+        optimizer = create_fused_optimizer(arena, run_opts.optim, args.layer_adaptation, opt_state, adafactor,
+                                           muon)
         if checkpoint:
             optimizer.load_state_dict(checkpoint.optimizerState)
         ema = None
@@ -503,7 +520,11 @@ class Solver:
                 if isinstance(optimizer, FusedAdam8bit) else
                 "adafactor (K2-af), %.1f KiB instead of %.1f MiB" % (
                     optimizer.state_bytes / 2 ** 10, optimizer.fp32_state_bytes / 2 ** 20)
-                if isinstance(optimizer, FusedAdafactor) else "fp32")
+                if isinstance(optimizer, FusedAdafactor) else
+                "muon (K14) on %d of %d tensors (%d params), adam (K2-mt) on the rest, NS workspace %.1f MiB" % (
+                    len(optimizer.muon_params), len(arena.slots),
+                    sum(p.numel() for p in optimizer.muon_params), optimizer.workspace_bytes / 2 ** 20)
+                if isinstance(optimizer, FusedMuon) else "fp32")
         scheduler = create_lr_scheduler(run_opts, worker.optimizer,
                                         checkpoint.epoch if checkpoint else -1)
         return worker, scheduler, checkpoint
@@ -715,7 +736,8 @@ class Solver:
               grad_accumulation: Optional[int] = None,
               ema_decay: Optional[float] = None,
               optimizer_state: Optional[OptimizerState] = None,
-              adafactor: Optional[bool] = None
+              adafactor: Optional[bool] = None,
+              muon: Optional[bool] = None
               ) -> Iterator[PerformanceSummary]:
         """The reference's entry point (solver.py:728-739) plus two keyword-only extensions:
 
@@ -800,12 +822,28 @@ class Solver:
                        rank starts.  Checkpoints keep ``torch.optim.Adafactor``'s format.  None:
                        FRL_B200_ADAFACTOR (``0`` by default, ``1`` to enable).  ``Mode.EVAL``
                        ignores it.
+        ``muon``       True: Muon (``torch.optim.Muon``'s rule, K14) for every model parameter
+                       with exactly two dimensions (Linear weights, embeddings, task heads) and
+                       Adam (K2-mt) for every other parameter.  Muon's momentum buffer is
+                       orthogonalised by 5 Newton-Schulz iterations (coefficients (3.4445,
+                       -4.7750, 2.0315), eps 1e-7, nesterov) on hand-written sm_90a GEMMs; the lr
+                       is scaled by 0.2 * sqrt(max(R, C)) (``adjust_lr_fn="match_rms_adamw"``),
+                       so one ``OptimOpts.lr`` suits both groups and the per-epoch schedule sets
+                       both.  ``weightDecay`` is Muon's decoupled decay and Adam's L2-coupled one;
+                       ``momentum`` is Muon's; ``epsilon`` is Adam's.  Needs ``OptAlgorithm.ADAM``
+                       without amsgrad, no layer adaptation, fp32 optimizer state and no
+                       Adafactor; any other combination raises ``ValueError`` before a rank
+                       starts.  Checkpoints hold two param groups (Muon, Adam) in torch's format;
+                       ``fused_optim.split_muon_state_dict`` / ``join_muon_state_dict`` convert
+                       them to and from a ``torch.optim.Muon`` plus a ``torch.optim.Adam``.  None:
+                       FRL_B200_MUON (``0`` by default, ``1`` to enable).  ``Mode.EVAL`` ignores it.
         """
         adapt = LayerAdaptation.NONE
         accum = 1
         decay = 0.0
         opt_state = OptimizerState.FP32
         use_adafactor = False
+        use_muon = False
         if run_opts.mode == Mode.TRAIN:
             adapt = resolve_layer_adaptation(layer_adaptation)
             check_layer_adaptation(run_opts.optim, adapt)
@@ -813,6 +851,8 @@ class Solver:
             check_optimizer_state(run_opts.optim, adapt, opt_state)
             use_adafactor = resolve_adafactor(adafactor)
             check_adafactor(run_opts.optim, adapt, opt_state, use_adafactor)
+            use_muon = resolve_muon(muon)
+            check_muon(run_opts.optim, adapt, opt_state, use_adafactor, use_muon)
             accum = resolve_grad_accumulation(grad_accumulation)
             decay = resolve_ema_decay(ema_decay)
         n_visible = 0 if run_opts.cpuonly else _cuda_device_count_without_poisoning_fork()
@@ -854,7 +894,7 @@ class Solver:
                 world_size=world_size, group_name=group_name, init_method=init_method,
                 cache=None, precision=prec, save_every=save_every, graph_step=graph,
                 layer_adaptation=adapt, grad_accumulation=accum, ema_decay=decay,
-                optimizer_state=opt_state, adafactor=use_adafactor)
+                optimizer_state=opt_state, adafactor=use_adafactor, muon=use_muon)
             if not run_opts.singleThreaded:
                 parent_conn, child_conn = ctx.Pipe(duplex=False)
                 proc = ctx.Process(target=cls._solver_worker_process,

@@ -293,6 +293,47 @@ int frl_adafactor_mt(float* p, float* state, void* p_lp, const frl_grad_seg* seg
                      double grad_scale, const float* grad_scale_dev, const float* dyn, void* stream);
 
 /* ------------------------------------------------------------------------------------------
+ * K14 — Muon (an extension: Jordan et al. 2024; torch.optim.Muon's rule) for the 2-D weights of
+ * a segment table.  Per matrix p [R, C] (fp32 master), m = min(R, C), n = max(R, C), with
+ * g^ = g * grad_scale (* *grad_scale_dev: every Muon matrix is a model parameter):
+ *   buf = lerp(buf, g^, 1 - momentum)          buf: the matrix's range of exp_avg (fp32)
+ *   u   = nesterov ? lerp(g^, buf, momentum) : buf
+ *   X   = bf16(u) as [m, n] (transposed when R > C); X = bf16(X / max(bf16(||X||_F), bf16(eps)))
+ *   ns_steps times:  A = bf16(X X^T);  B = bf16(b A + c A A);  X = bf16(a X + B X)
+ *     (fp32 accumulation, one bf16 rounding per output element)
+ *   p = p * (1 - lr*wd) - adj * float(O),  O = X transposed back when R > C;  p_lp = bf16(p)
+ *   adj = lr * (adjust_lr ? 0.2 * sqrt(max(R, C)) : sqrt(max(1, R / C)))
+ *     (adjust_lr 1 = "match_rms_adamw", 0 = "original" / None)
+ * The NS iterates ping-pong in the matrix's range of the fp32 exp_avg_sq vector (two bf16
+ * [m, n] matrices in its 4 bytes per element) when n is a multiple of 8, else in the workspace.
+ * The workspace also holds A and B ([m, m] bf16, leading dimension rounded up to 8) per matrix,
+ * laid out from its start in plan order: plans over subsets of the same matrices may share one
+ * workspace sized for all of them, as long as their launches do not overlap.
+ * frl_muon_plan_bytes: host; shape int64 [n_mat][4] = (segment index in the table, arena offset
+ *   (a multiple of 8), R, C).  Returns the plan's size in bytes (-1 on a bad shape) and writes
+ *   the scratch's size (tickets, norms, partials: one per plan) and the workspace's size where
+ *   non-NULL.
+ * frl_muon_plan: host; fills the plan (tensor maps, grouped tile tables) for the given
+ *   exp_avg_sq base and workspace (128-byte aligned).  The caller copies it to the device
+ *   (64-byte aligned) and keeps both copies while the buffers live.
+ * frl_muon_mt: scratch as sized above, 16-byte aligned, zeroed once.  Every planned segment index
+ *   must be < n_segs (FRL_E_ARG otherwise); that segment's numel must be R * C (the table lives on
+ *   the device, so the caller checks this).
+ * frl_muon_mt: prologue (momentum, iterate, per-matrix norm folded in tile order by the last
+ *   CTA of each matrix), normalisation, then 3 * ns_steps persistent TMA + WGMMA launches
+ *   (gram, poly, update) over every matrix at once; Gram and poly compute only tiles on or above
+ *   the diagonal.  The last update writes p and p_lp directly.  No float atomics or split-K:
+ *   repeated launches give the same bytes.  dyn: optional device fp32, dyn[2] = lr (replaces the
+ *   by-value lr).  1 <= ns_steps < 100.  All checks run before the first launch; graph-capturable.
+ * ---------------------------------------------------------------------------------------- */
+int64_t frl_muon_plan_bytes(const int64_t* shape, int64_t n_mat, int64_t* scratch_bytes, int64_t* workspace_bytes);
+int frl_muon_plan(const int64_t* shape, int64_t n_mat, const float* exp_avg_sq, void* workspace, void* plan);
+int frl_muon_mt(float* p, float* exp_avg, void* p_lp, const frl_grad_seg* segs_dev, int64_t n_segs,
+                const void* plan_host, const void* plan_dev, void* scratch, double lr, double wd,
+                double momentum, int nesterov, double a, double b, double c, int ns_steps, double eps,
+                int adjust_lr, double grad_scale, const float* grad_scale_dev, const float* dyn, void* stream);
+
+/* ------------------------------------------------------------------------------------------
  * K10 — gradient accumulation (an extension: the reference has no accumulation).  Several
  * microbatches per optimizer update: after each microbatch's backward, one launch folds every
  * gradient of a K2-mt segment table into an fp32 accumulator.

@@ -1,7 +1,7 @@
 #!/usr/bin/env python
 """Micro-benchmark of every hand-written kernel at the BASELINE shapes (1 GPU).
 
-    python tools/kernel_bench.py [--only k2,k2lw,k2q8,k2af,k3,k5a,k13,...] [--iters 20] [--json out.json]
+    python tools/kernel_bench.py [--only k2,k2lw,k2q8,k2af,k3,k5a,k13,k14,...] [--iters 20] [--json out.json]
 
 Each kernel is timed with CUDA events on the launching stream over ROTATING operand sets whose
 total size exceeds the 50 MB L2 (so every launch streams from HBM), after 3 warm-up launches.
@@ -702,10 +702,99 @@ def bench_k13(iters):
     return out
 
 
+def _muon_case(shapes):
+    """A FusedMuon over 2-D weights of ``shapes`` (plus one bias), bf16 gradients in place."""
+    import torch.nn as nn
+    from frl_b200 import fused_optim
+    from frl_b200.arena import ParamArena
+    from frl_b200.multi_tensor import GradSegTable
+    from frl_b200.types import Precision
+    params = [nn.Parameter(torch.randn(sh) * 0.02) for sh in shapes] + [nn.Parameter(torch.zeros(64))]
+    arena = ParamArena(params, device=DEV, precision=Precision.BF16)
+    opt = fused_optim.FusedMuon(arena, lr=1e-3, weight_decay=1e-5)
+    table = GradSegTable(arena.slots, DEV)
+    grads = [torch.randn(s.shape, device=DEV).bfloat16() for s in arena.slots]
+    for s, g in zip(arena.slots, grads):
+        table.point(s, g.data_ptr(), g.dtype)
+    table.upload()
+    return opt, table, grads
+
+
+def bench_k14(iters):
+    """K14 (Muon) phase by phase at [4096, 4096] and [1000, 4096]: the kernels' device times from
+    torch.profiler over ``iters`` updates captured in a CUDA graph (each update's last NS launch is
+    the weight-writing update), against torch.mm / torch.addmm computing the same bf16 products
+    from a graph.  TFLOP/s counts the full product and, for gram and poly, the tiles K14 computes
+    (on or above the diagonal); the whole update is L2-warm after the first product."""
+    from torch.profiler import ProfilerActivity, profile
+    out = []
+    for R, C in ((4096, 4096), (1000, 4096)):
+        m, n = min(R, C), max(R, C)
+        tm, tn = -(-m // 128), -(-m // 256)
+        frac = sum(max(tn - a // 2, 0) for a in range(tm)) / (tm * tn)
+        flops = {"gram": 2.0 * m * m * n, "poly": 2.0 * m * m * m, "update": 2.0 * m * m * n,
+                 "last update": 2.0 * m * m * n}
+        opt, table, grads = _muon_case([(R, C)])
+        for _ in range(WARMUP):
+            opt.apply_table(table)
+        torch.cuda.synchronize()
+        g = torch.cuda.CUDAGraph()
+        with torch.cuda.graph(g):
+            for _ in range(iters):
+                opt.apply_table(table)
+        g.replay()
+        torch.cuda.synchronize()
+        with profile(activities=[ProfilerActivity.CUDA]) as prof:
+            g.replay()
+            torch.cuda.synchronize()
+        evs = sorted([e for e in prof.events() if e.device_type.name == "CUDA" and "muon" in e.name],
+                     key=lambda e: e.time_range.start)
+        times = {}
+        ns_per_update = 3 * 5
+        per_update = 2 + ns_per_update
+        for i, e in enumerate(evs):
+            j = i % per_update
+            name = ("prologue" if j == 0 else "normalise" if j == 1 else
+                    ("gram", "poly", "update")[(j - 2) % 3])
+            if j == per_update - 1:
+                name = "last update"
+            times.setdefault(name, []).append(e.time_range.elapsed_us())
+        x = torch.randn(m, n, device=DEV).bfloat16()
+        a = torch.randn(m, m, device=DEV).bfloat16()
+        o_mm = torch.empty(m, m, device=DEV, dtype=torch.bfloat16)
+        o_x = torch.empty(m, n, device=DEV, dtype=torch.bfloat16)
+        refs = {"gram": lambda i: torch.mm(x, x.T, out=o_mm),
+                "poly": lambda i: torch.addmm(a, a, a, beta=-4.775, alpha=2.0315, out=o_mm),
+                "update": lambda i: torch.addmm(x, a, x, beta=3.4445, out=o_x)}
+        shape = "[%d,%d]" % (R, C)
+        for name in ("prologue", "normalise", "gram", "poly", "update", "last update"):
+            ts = times.get(name, [])
+            if not ts:
+                continue
+            us = sum(ts) / len(ts)
+            rec = {"kernel": "K14 %s %s" % (name, shape), "us": round(us, 2), "launches": len(ts)}
+            if name in flops:
+                f = flops[name] * (frac if name in ("gram", "poly") else 1.0)
+                rec["TFLOPs_full_product"] = round(flops[name] / us / 1e6, 1)
+                rec["TFLOPs_tiles_computed"] = round(f / us / 1e6, 1)
+            print(json.dumps(rec), flush=True)
+            out.append(rec)
+        for name, fn in refs.items():
+            rec = timed("torch %s %s (bf16, cuBLAS)" % ("mm" if name == "gram" else "addmm", name + " " + shape),
+                        fn, 1, 0, iters, graph=True)
+            rec["TFLOPs"] = round(flops[name] / rec["us"] / 1e6, 1)
+            print(json.dumps({"kernel": rec["kernel"], "TFLOPs": rec["TFLOPs"]}), flush=True)
+            out.append(rec)
+        total = sum(sum(v) for v in times.values()) / iters
+        print(json.dumps({"kernel": "K14 whole update %s" % shape, "us": round(total, 1)}), flush=True)
+        del opt, table, grads, g
+    return out
+
+
 BENCHES = {"k2": bench_k2, "k2mt": bench_k2mt, "k2lw": bench_k2lw, "k3": bench_k3, "k4": bench_k4, "k5": bench_k5, "k5a": bench_k5a,
            "k5m": bench_k5m, "k4s": bench_k4s, "k6": bench_k6,
            "k8": bench_k8, "k8t": bench_k8t, "k9": bench_k9, "k10": bench_k10, "k11": bench_k11,
-           "k2q8": bench_k2q8, "k2af": bench_k2af, "k13": bench_k13}
+           "k2q8": bench_k2q8, "k2af": bench_k2af, "k13": bench_k13, "k14": bench_k14}
 
 
 def main():
