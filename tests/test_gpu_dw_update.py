@@ -4,7 +4,8 @@ the SGD update in its epilogue (``frl_dw_gemm_sgd``).
 * gradient: within cuBLAS's own error of a float64 dZ^T X (the summation order differs, so bit
   equality with cuBLAS is not expected), at the headline 4096^3 and at small, padded shapes;
 * update: bit for bit what K2 (``frl_sgd_momentum``) computes on a copy of the pre-step state from
-  the gradient K12 wrote -- first and later steps, momentum and plain SGD, an lr changed between
+  the gradient K12 wrote, also at the shapes that reach each path of the tile walk
+  (``gemm_sm90_oracle.k12_shapes``) -- first and later steps, momentum and plain SGD, an lr changed between
   CUDA-graph replays through the device-resident scalars, NaN and inf in dZ;
 * wiring: every configuration K12 does not serve (a weight applied twice, FP8, fp32, clipping,
   accumulation, LARS) keeps the tail update and trains to the weights the tail update gives; a 1-GPU
@@ -20,6 +21,7 @@ import frl_b200  # noqa: F401
 from frl_b200 import _native, synthetic
 from frl_b200.solver import Solver, SolverWorkerArgs
 from frl_b200.types import Device, LayerAdaptation, Precision
+import gemm_sm90_oracle as go
 
 pytestmark = pytest.mark.gpu
 SGD = dict(lr=0.01, mu=0.9, dampening=0.0, wd=1e-4)
@@ -61,9 +63,11 @@ def _assert_same_bits(a, b):
 
 @pytest.mark.parametrize("first_step", [True, False])
 @pytest.mark.parametrize("mu", [0.9, 0.0])
-@pytest.mark.parametrize("shape", [(4096, 4096, 4096), (128, 256, 512)])
+@pytest.mark.parametrize("shape", [(4096, 4096, 4096), (128, 256, 512)] + list(go.K12_PATHS))
 def test_update_is_k2_on_the_written_gradient_bit_for_bit(first_step, mu, shape):
-    rows, out, inp = shape
+    # a name: a shape of the tile walk on this device (tests/gemm_sm90_oracle.k12_shapes)
+    sms = torch.cuda.get_device_properties(0).multi_processor_count
+    rows, out, inp = go.k12_shapes(sms)[shape] if isinstance(shape, str) else shape
     dz, x = _operands(rows, out, inp)
     n = out * inp
     p, buf, lp = _state(n)
