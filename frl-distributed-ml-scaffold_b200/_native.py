@@ -56,6 +56,7 @@ SIGNATURES = {
     "frl_device_arch": (_i, []),
     "frl_sgd_momentum": (_i, [_vp, _vp, _vp, _vp, _i64, _d, _d, _d, _d, _d, _vp, _vp, _i, _i, _vp]),
     "frl_adam": (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _i64, _d, _d, _d, _d, _d, _i64, _d, _vp, _vp, _i, _vp]),
+    "frl_adamw": (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _i64, _d, _d, _d, _d, _d, _i64, _d, _vp, _vp, _i, _vp]),
     "frl_rmsprop": (_i, [_vp, _vp, _vp, _vp, _vp, _i64, _d, _d, _d, _d, _d, _d, _vp, _vp, _i, _vp]),
     "frl_dw_gemm": (_i, [_vp, _i64, _vp, _i64, _i64, _i64, _i64, _vp, _vp]),
     "frl_dw_gemm_sgd": (_i, [_vp, _i64, _vp, _i64, _i64, _i64, _i64, _vp, _vp, _vp, _vp, _d, _d, _d, _d, _d,
@@ -66,6 +67,7 @@ SIGNATURES = {
     "frl_flatten_grads": (_i, [_vp, _vp, _vp, _i64, _vp, _i, _d, _vp]),
     "frl_sgd_momentum_mt": (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _i64, _d, _d, _d, _d, _d, _vp, _vp, _i, _vp]),
     "frl_adam_mt": (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _i64, _d, _d, _d, _d, _d, _i64, _d, _vp, _vp, _vp]),
+    "frl_adamw_mt": (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _i64, _d, _d, _d, _d, _d, _i64, _d, _vp, _vp, _vp]),
     "frl_rmsprop_mt": (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _i64, _d, _d, _d, _d, _d, _d, _vp, _vp, _vp]),
     "frl_layerwise_scratch_bytes": (_i64, [_i64, _i64]),
     "frl_lars_mt": (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _i64, _i64, _vp, _vp, _vp, _d, _d, _d, _d, _vp, _vp, _i, _vp]),
@@ -74,6 +76,8 @@ SIGNATURES = {
     "frl_q8_tables": (None, [_vp, _vp]),
     "frl_adam8_mt": (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _i64, _i64, _vp, _vp, _d, _d, _d, _d, _d,
                           _i64, _d, _vp, _vp, _vp]),
+    "frl_adamw8_mt": (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _i64, _i64, _vp, _vp, _d, _d, _d, _d, _d,
+                           _i64, _d, _vp, _vp, _vp]),
     "frl_q8_encode_mt": (_i, [_vp, _vp, _vp, _i, _vp, _vp, _vp, _i64, _i64, _vp, _vp]),
     "frl_q8_decode_mt": (_i, [_vp, _vp, _vp, _i, _vp, _vp, _vp, _i64, _i64, _vp, _vp]),
     "frl_adafactor_plan": (_i64, [_vp, _i64, _vp, _vp]),
@@ -114,6 +118,8 @@ SIGNATURES = {
     "frl_nvls_sgd": (_i, [_vp, _vp, _vp, _vp, _i64, _i, _i, _vp, _i, _vp, _i, _d, _d, _d, _d, _d, _vp, _i, _i, _i, _vp]),
     "frl_nvls_adam": (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _i64, _i, _i, _vp, _i, _vp, _i, _d, _d, _d, _d, _d,
                            _i64, _d, _vp, _i, _i, _vp]),
+    "frl_nvls_adamw": (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _i64, _i, _i, _vp, _i, _vp, _i, _d, _d, _d, _d, _d,
+                            _i64, _d, _vp, _i, _i, _vp]),
     "frl_nvls_rmsprop": (_i, [_vp, _vp, _vp, _vp, _vp, _i64, _i, _i, _vp, _i, _vp, _i, _d, _d, _d, _d, _d, _d,
                               _vp, _i, _i, _vp]),
     "frl_nvls_barrier": (_i, [_vp, _i, _i, _i, _vp]),
@@ -202,6 +208,14 @@ def adam(p, g, m, v, vmax, p_lp, n, *, lr, beta1, beta2, eps, wd, step, grad_sca
     _check(lib().frl_adam(_ptr(p), _ptr(g), _ptr(m), _ptr(v), _ptr(vmax), _ptr(p_lp), n, lr,
                           beta1, beta2, eps, wd, step, grad_scale, _ptr(grad_scale_dev), _ptr(dyn),
                           dtype_code(g.dtype), _stream()), "frl_adam")
+
+
+def adamw(p, g, m, v, vmax, p_lp, n, *, lr, beta1, beta2, eps, wd, step, grad_scale=1.0,
+          grad_scale_dev=None, dyn=None) -> None:
+    """K2 AdamW: ``adam``'s arguments, ``wd`` decoupled (see frl_adamw in include/frl_b200.h)."""
+    _check(lib().frl_adamw(_ptr(p), _ptr(g), _ptr(m), _ptr(v), _ptr(vmax), _ptr(p_lp), n, lr,
+                           beta1, beta2, eps, wd, step, grad_scale, _ptr(grad_scale_dev), _ptr(dyn),
+                           dtype_code(g.dtype), _stream()), "frl_adamw")
 
 
 def rmsprop(p, g, sq, buf, p_lp, n, *, lr, alpha, eps, wd, mu, grad_scale=1.0,
@@ -309,6 +323,14 @@ def adam_mt(p, m, v, vmax, p_lp, table, *, lr, beta1, beta2, eps, wd, step, grad
                              step, grad_scale, _ptr(grad_scale_dev), _ptr(dyn), _stream()), "frl_adam_mt")
 
 
+def adamw_mt(p, m, v, vmax, p_lp, table, *, lr, beta1, beta2, eps, wd, step, grad_scale=1.0,
+             grad_scale_dev=None, dyn=None) -> None:
+    """K2-mt AdamW: ``adam_mt``'s arguments, ``wd`` decoupled."""
+    _check(lib().frl_adamw_mt(_ptr(p), _ptr(m), _ptr(v), _ptr(vmax), _ptr(p_lp), table.segs_dev_ptr,
+                              table.prefix_dev_ptr, table.tile_seg_dev_ptr, table.n_tiles, lr, beta1, beta2, eps, wd,
+                              step, grad_scale, _ptr(grad_scale_dev), _ptr(dyn), _stream()), "frl_adamw_mt")
+
+
 def rmsprop_mt(p, sq, buf, p_lp, table, *, lr, alpha, eps, wd, mu, grad_scale=1.0, grad_scale_dev=None,
                dyn=None) -> None:
     _check(lib().frl_rmsprop_mt(_ptr(p), _ptr(sq), _ptr(buf), _ptr(p_lp), table.segs_dev_ptr,
@@ -396,6 +418,16 @@ def adam8_mt(p, m_q, v_q, m_absmax, v_absmax, p_lp, table, qbase, flags, *, lr, 
                               table.segs_dev_ptr, table.prefix_dev_ptr, table.tile_seg_dev_ptr, table.n_tiles,
                               table.n_segs, _ptr(qbase), _ptr(flags), lr, beta1, beta2, eps, wd, step, grad_scale,
                               _ptr(grad_scale_dev), _ptr(dyn), _stream()), "frl_adam8_mt")
+
+
+def adamw8_mt(p, m_q, v_q, m_absmax, v_absmax, p_lp, table, qbase, flags, *, lr, beta1, beta2, eps, wd, step,
+              grad_scale=1.0, grad_scale_dev=None, dyn=None) -> None:
+    """K2-q8 AdamW: ``adam8_mt``'s arguments, ``wd`` decoupled.  See frl_adamw8_mt in include/frl_b200.h."""
+    _check_q8(table, qbase, flags, codes=(m_q, v_q), absmax=(m_absmax, v_absmax), fp32=(p,))
+    _check(lib().frl_adamw8_mt(_ptr(p), _ptr(m_q), _ptr(v_q), _ptr(m_absmax), _ptr(v_absmax), _ptr(p_lp),
+                               table.segs_dev_ptr, table.prefix_dev_ptr, table.tile_seg_dev_ptr, table.n_tiles,
+                               table.n_segs, _ptr(qbase), _ptr(flags), lr, beta1, beta2, eps, wd, step, grad_scale,
+                               _ptr(grad_scale_dev), _ptr(dyn), _stream()), "frl_adamw8_mt")
 
 
 def q8_encode_mt(x, q, absmax, state: int, table, qbase) -> None:
@@ -744,6 +776,15 @@ def nvls_adam(p, m, v, vmax, mc_g, mc_out, n, link, *, lr, beta1, beta2, eps, wd
                                link.world, link.pads_dev, link.pad_base, _ptr(link.scratch), link.max_blocks, lr, beta1,
                                beta2, eps, wd, step, grad_scale, _ptr(dyn), g_dtype, link.flags, _stream()),
            "frl_nvls_adam")
+
+
+def nvls_adamw(p, m, v, vmax, mc_g, mc_out, n, link, *, lr, beta1, beta2, eps, wd, step, grad_scale,
+               g_dtype, dyn=None) -> None:
+    """K7 AdamW: ``nvls_adam``'s arguments, ``wd`` decoupled."""
+    _check(lib().frl_nvls_adamw(_ptr(p), _ptr(m), _ptr(v), _ptr(vmax), mc_g, mc_out, n, link.rank,
+                                link.world, link.pads_dev, link.pad_base, _ptr(link.scratch), link.max_blocks, lr,
+                                beta1, beta2, eps, wd, step, grad_scale, _ptr(dyn), g_dtype, link.flags, _stream()),
+           "frl_nvls_adamw")
 
 
 def nvls_rmsprop(p, sq, buf, mc_g, mc_out, n, link, *, lr, alpha, eps, wd, mu, grad_scale, g_dtype,

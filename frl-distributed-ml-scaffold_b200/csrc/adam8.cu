@@ -115,13 +115,14 @@ __device__ __forceinline__ void st_code4(uint8_t* q, int64_t e4, uint32_t c) {
 }
 
 // ---- K2-q8 update --------------------------------------------------------------------------------
-template <bool HAS_LP>
+// Rule: AdamRule<false> (frl_adam8_mt) or AdamWRule<false> (frl_adamw8_mt).
+template <typename Rule, bool HAS_LP>
 __global__ void __launch_bounds__(kThreads)
 adam8_mt_kernel(float* __restrict__ p_, uint8_t* __restrict__ mq, uint8_t* __restrict__ vq,
                 float* __restrict__ m_absmax, float* __restrict__ v_absmax, bf16x4* __restrict__ lp,
                 const frl_grad_seg* __restrict__ segs, const int64_t* __restrict__ tile_prefix,
                 const int32_t* __restrict__ tile_seg, int64_t n_tiles, const int64_t* __restrict__ qbase,
-                const int32_t* __restrict__ flags, AdamRule<false> rule, float gscale,
+                const int32_t* __restrict__ flags, Rule rule, float gscale,
                 const float* __restrict__ gscale_dev, const float* __restrict__ dyn) {
     __shared__ float mag7[128], mag8[256];
     __shared__ float red[kUnroll][2 * kThreads / 32];
@@ -288,6 +289,45 @@ extern "C" void frl_q8_tables(float* mag7, float* mag8) {
     for (int i = 0; i < 256; ++i) if (mag8) mag8[i] = kQ8Host.mag8[i];
 }
 
+namespace frl {
+template <typename Rule>
+static int launch_adam8_mt(const Rule& rule, float* p, uint8_t* m_q, uint8_t* v_q, float* m_absmax, float* v_absmax,
+                           void* p_lp, const frl_grad_seg* segs_dev, const int64_t* tile_prefix_dev,
+                           const int32_t* tile_seg_dev, int64_t n_tiles, const int64_t* qbase_dev,
+                           const int32_t* seg_flags_dev, double grad_scale, const float* grad_scale_dev,
+                           const float* dyn, void* stream, const char* name) {
+    const float gs = static_cast<float>(grad_scale);
+    cudaStream_t st = static_cast<cudaStream_t>(stream);
+    bf16x4* lp = static_cast<bf16x4*>(p_lp);
+    if (lp)
+        adam8_mt_kernel<Rule, true><<<grid_for_tiles(adam8_mt_kernel<Rule, true>, n_tiles), kThreads, 0, st>>>(
+            p, m_q, v_q, m_absmax, v_absmax, lp, segs_dev, tile_prefix_dev, tile_seg_dev, n_tiles, qbase_dev,
+            seg_flags_dev, rule, gs, grad_scale_dev, dyn);
+    else
+        adam8_mt_kernel<Rule, false><<<grid_for_tiles(adam8_mt_kernel<Rule, false>, n_tiles), kThreads, 0, st>>>(
+            p, m_q, v_q, m_absmax, v_absmax, lp, segs_dev, tile_prefix_dev, tile_seg_dev, n_tiles, qbase_dev,
+            seg_flags_dev, rule, gs, grad_scale_dev, dyn);
+    return after_launch(name);
+}
+
+// every argument check of frl_adam8_mt / frl_adamw8_mt, before any launch; 1: nothing to launch
+static int check_adam8_args(float* p, uint8_t* m_q, uint8_t* v_q, float* m_absmax, float* v_absmax, void* p_lp,
+                            const frl_grad_seg* segs_dev, const int64_t* tile_prefix_dev,
+                            const int32_t* tile_seg_dev, int64_t n_tiles, int64_t n_segs,
+                            const int64_t* qbase_dev, const int32_t* seg_flags_dev, int64_t step,
+                            const char* name) {
+    int rc = check_table_args(segs_dev, tile_prefix_dev, tile_seg_dev, qbase_dev, n_tiles, n_segs, name);
+    if (rc != 0) return rc;
+    FRL_REQUIRE(step >= 1, FRL_E_ARG, "%s: step must be >= 1", name);
+    if (n_tiles == 0) return 1;
+    FRL_REQUIRE(p && m_q && v_q && m_absmax && v_absmax && seg_flags_dev, FRL_E_ARG,
+                "%s: null p/codes/absmax/seg_flags", name);
+    FRL_REQUIRE(aligned16(p) && aligned16(m_q) && aligned16(v_q) && aligned16(p_lp), FRL_E_ALIGN,
+                "%s: p, codes and p_lp must be 16-byte aligned", name);
+    return 0;
+}
+}  // namespace frl
+
 extern "C" int frl_adam8_mt(float* p, uint8_t* m_q, uint8_t* v_q, float* m_absmax, float* v_absmax, void* p_lp,
                             const frl_grad_seg* segs_dev, const int64_t* tile_prefix_dev,
                             const int32_t* tile_seg_dev, int64_t n_tiles, int64_t n_segs,
@@ -295,27 +335,27 @@ extern "C" int frl_adam8_mt(float* p, uint8_t* m_q, uint8_t* v_q, float* m_absma
                             double beta2, double eps, double wd, int64_t step, double grad_scale,
                             const float* grad_scale_dev, const float* dyn, void* stream) {
     const char* name = "frl_adam8_mt";
-    int rc = check_table_args(segs_dev, tile_prefix_dev, tile_seg_dev, qbase_dev, n_tiles, n_segs, name);
-    if (rc != 0) return rc;
-    FRL_REQUIRE(step >= 1, FRL_E_ARG, "%s: step must be >= 1", name);
-    if (n_tiles == 0) return 0;
-    FRL_REQUIRE(p && m_q && v_q && m_absmax && v_absmax && seg_flags_dev, FRL_E_ARG,
-                "%s: null p/codes/absmax/seg_flags", name);
-    FRL_REQUIRE(aligned16(p) && aligned16(m_q) && aligned16(v_q) && aligned16(p_lp), FRL_E_ALIGN,
-                "%s: p, codes and p_lp must be 16-byte aligned", name);
-    const AdamRule<false> rule = make_adam_rule<false>(lr, beta1, beta2, eps, wd, step);
-    const float gs = static_cast<float>(grad_scale);
-    cudaStream_t st = static_cast<cudaStream_t>(stream);
-    bf16x4* lp = static_cast<bf16x4*>(p_lp);
-    if (lp)
-        adam8_mt_kernel<true><<<grid_for_tiles(adam8_mt_kernel<true>, n_tiles), kThreads, 0, st>>>(
-            p, m_q, v_q, m_absmax, v_absmax, lp, segs_dev, tile_prefix_dev, tile_seg_dev, n_tiles, qbase_dev,
-            seg_flags_dev, rule, gs, grad_scale_dev, dyn);
-    else
-        adam8_mt_kernel<false><<<grid_for_tiles(adam8_mt_kernel<false>, n_tiles), kThreads, 0, st>>>(
-            p, m_q, v_q, m_absmax, v_absmax, lp, segs_dev, tile_prefix_dev, tile_seg_dev, n_tiles, qbase_dev,
-            seg_flags_dev, rule, gs, grad_scale_dev, dyn);
-    return after_launch(name);
+    const int rc = check_adam8_args(p, m_q, v_q, m_absmax, v_absmax, p_lp, segs_dev, tile_prefix_dev, tile_seg_dev,
+                                    n_tiles, n_segs, qbase_dev, seg_flags_dev, step, name);
+    if (rc != 0) return rc > 0 ? 0 : rc;
+    return launch_adam8_mt(make_adam_rule<false>(lr, beta1, beta2, eps, wd, step), p, m_q, v_q, m_absmax, v_absmax,
+                           p_lp, segs_dev, tile_prefix_dev, tile_seg_dev, n_tiles, qbase_dev, seg_flags_dev,
+                           grad_scale, grad_scale_dev, dyn, stream, name);
+}
+
+extern "C" int frl_adamw8_mt(float* p, uint8_t* m_q, uint8_t* v_q, float* m_absmax, float* v_absmax, void* p_lp,
+                             const frl_grad_seg* segs_dev, const int64_t* tile_prefix_dev,
+                             const int32_t* tile_seg_dev, int64_t n_tiles, int64_t n_segs,
+                             const int64_t* qbase_dev, const int32_t* seg_flags_dev, double lr, double beta1,
+                             double beta2, double eps, double wd, int64_t step, double grad_scale,
+                             const float* grad_scale_dev, const float* dyn, void* stream) {
+    const char* name = "frl_adamw8_mt";
+    const int rc = check_adam8_args(p, m_q, v_q, m_absmax, v_absmax, p_lp, segs_dev, tile_prefix_dev, tile_seg_dev,
+                                    n_tiles, n_segs, qbase_dev, seg_flags_dev, step, name);
+    if (rc != 0) return rc > 0 ? 0 : rc;
+    return launch_adam8_mt(make_adamw_rule<false>(lr, beta1, beta2, eps, wd, step), p, m_q, v_q, m_absmax, v_absmax,
+                           p_lp, segs_dev, tile_prefix_dev, tile_seg_dev, n_tiles, qbase_dev, seg_flags_dev,
+                           grad_scale, grad_scale_dev, dyn, stream, name);
 }
 
 extern "C" int frl_q8_encode_mt(const float* x, uint8_t* q, float* absmax, int state,

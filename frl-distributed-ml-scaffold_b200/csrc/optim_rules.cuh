@@ -21,6 +21,22 @@ struct SgdRule {
     }
 };
 
+// Adam's step after any weight decay: moments, amsgrad maximum, bias-corrected parameter update.
+template <bool AMSGRAD>
+__device__ __forceinline__ void adam_moments_and_param(float& p, float g, float& m, float& v, float& vmax,
+                                                       float w1, float beta2, float w2, float eps,
+                                                       float neg_step_size, float bc2_sqrt) {
+    m = fmaf(w1, g - m, m);                       // exp_avg.lerp_(g, 1-beta1), weight < 0.5 branch
+    v = fmaf(w2 * g, g, v * beta2);               // mul_(beta2).addcmul_(g, g, 1-beta2)
+    float vv = v;
+    if (AMSGRAD) {                                // torch.maximum: NaN in either operand wins
+        vmax = (v > vmax || v != v) ? v : vmax;   // (fmaxf would drop it)
+        vv = vmax;
+    }
+    const float denom = sqrtf(vv) / bc2_sqrt + eps;
+    p = fmaf(neg_step_size, m / denom, p);        // addcdiv_(m, denom, -step_size)
+}
+
 template <bool AMSGRAD>
 struct AdamRule {
     float w1;               // 1 - beta1   (lerp weight)
@@ -34,16 +50,33 @@ struct AdamRule {
         bc2_sqrt = __ldg(dyn + 1);
     }
     __device__ __forceinline__ void operator()(float& p, float g, float& m, float& v, float& vmax) const {
-        g = fmaf(wd, p, g);
-        m = fmaf(w1, g - m, m);                       // exp_avg.lerp_(g, 1-beta1), weight < 0.5 branch
-        v = fmaf(w2 * g, g, v * beta2);               // mul_(beta2).addcmul_(g, g, 1-beta2)
-        float vv = v;
-        if (AMSGRAD) {                                // torch.maximum: NaN in either operand wins
-            vmax = (v > vmax || v != v) ? v : vmax;   // (fmaxf would drop it)
-            vv = vmax;
-        }
-        const float denom = sqrtf(vv) / bc2_sqrt + eps;
-        p = fmaf(neg_step_size, m / denom, p);        // addcdiv_(m, denom, -step_size)
+        g = fmaf(wd, p, g);                           // L2-coupled decay (torch Adam)
+        adam_moments_and_param<AMSGRAD>(p, g, m, v, vmax, w1, beta2, w2, eps, neg_step_size, bc2_sqrt);
+    }
+};
+
+// AdamW: torch 2.11's Adam(decoupled_weight_decay=True), i.e. torch.optim.AdamW.  The parameter is
+// first scaled by its own fp32 multiply, p * fp32(1 - lr*wd) (torch: param.mul_(1 - lr*weight_decay)),
+// then Adam's step runs with no decay term in the gradient.  dyn[2] carries the decay factor, so
+// under CUDA-graph replay it follows the scheduled lr as the bias-corrected step size does.
+template <bool AMSGRAD>
+struct AdamWRule {
+    float w1;               // 1 - beta1   (lerp weight)
+    float beta2, w2;        // beta2, 1 - beta2
+    float eps;
+    float neg_step_size;    // -lr / (1 - beta1^t)
+    float bc2_sqrt;         // sqrt(1 - beta2^t)
+    float decay;            // fp32(1 - lr*wd), formed in double
+    static constexpr int kStates = AMSGRAD ? 3 : 2;
+    __device__ __forceinline__ void patch(const float* dyn) {
+        neg_step_size = __ldg(dyn);
+        bc2_sqrt = __ldg(dyn + 1);
+        decay = __ldg(dyn + 2);
+    }
+    __device__ __forceinline__ void operator()(float& p, float g, float& m, float& v, float& vmax) const {
+        p = __fmul_rn(p, decay);                      // param.mul_(1 - lr*wd): its own rounding, never
+                                                      // contracted into the update's FMA
+        adam_moments_and_param<AMSGRAD>(p, g, m, v, vmax, w1, beta2, w2, eps, neg_step_size, bc2_sqrt);
     }
 };
 
@@ -77,6 +110,16 @@ static inline AdamRule<AMS> make_adam_rule(double lr, double beta1, double beta2
     return AdamRule<AMS>{static_cast<float>(1.0 - beta1), static_cast<float>(beta2),
                          static_cast<float>(1.0 - beta2), static_cast<float>(eps), static_cast<float>(wd),
                          static_cast<float>(-(lr / bc1)), static_cast<float>(sqrt(bc2))};
+}
+template <bool AMS>
+static inline AdamWRule<AMS> make_adamw_rule(double lr, double beta1, double beta2, double eps, double wd,
+                                             int64_t step) {
+    const double bc1 = 1.0 - pow(beta1, static_cast<double>(step));
+    const double bc2 = 1.0 - pow(beta2, static_cast<double>(step));
+    return AdamWRule<AMS>{static_cast<float>(1.0 - beta1), static_cast<float>(beta2),
+                          static_cast<float>(1.0 - beta2), static_cast<float>(eps),
+                          static_cast<float>(-(lr / bc1)), static_cast<float>(sqrt(bc2)),
+                          static_cast<float>(1.0 - lr * wd)};
 }
 template <bool MOM>
 static inline RmspropRule<MOM> make_rmsprop_rule(double lr, double alpha, double eps, double wd, double mu) {

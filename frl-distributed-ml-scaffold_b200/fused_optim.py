@@ -11,7 +11,9 @@ format and update whole tensors through the K2-lw kernels.  ``FusedAdam8bit`` (a
 ``torch.optim.Adam``'s format in its state dict.  ``FusedAdafactor`` (an extension, chosen with
 ``Solver.solve(..., adafactor=True)``) is ``torch.optim.Adafactor``'s rule and state format (K2-af).
 ``FusedMuon`` (an extension, ``Solver.solve(..., muon=True)``) is ``torch.optim.Muon`` (K14) for the
-model's 2-D weights and this module's Adam (K2-mt) for every other parameter.
+model's 2-D weights and this module's Adam (K2-mt) for every other parameter.  ``adamw=True`` (an
+extension, ``Solver.solve(..., adamw=True)``) turns the Adam rule of ``FusedAdam``, ``FusedAdam8bit``
+and ``FusedMuon``'s Adam group into ``torch.optim.AdamW``'s decoupled weight decay (``frl_adamw*``).
 
 Known limitation: the step count (Adam's bias corrections) is ONE number for the whole arena.
 ``torch.optim`` keeps one per parameter and does not advance it for a parameter whose gradient
@@ -304,14 +306,26 @@ class FusedSGD(FusedArenaOptimizer):
 
 
 class FusedAdam(FusedArenaOptimizer):
+    """Adam with torch's L2-coupled weight decay, or with ``adamw=True`` torch 2.11's
+    ``Adam(decoupled_weight_decay=True)``, which ``torch.optim.AdamW`` is: each step first scales
+    the parameter by fp32(1 - lr * weight_decay), then takes Adam's step with no decay in the
+    gradient (the ``frl_adamw*`` kernels).  The param group's ``decoupled_weight_decay`` says which,
+    so ``state_dict()`` is ``torch.optim.Adam``'s or ``torch.optim.AdamW``'s format."""
+
     STATE_NAMES = (("exp_avg", "exp_avg"), ("exp_avg_sq", "exp_avg_sq"),
                    ("max_exp_avg_sq", "max_exp_avg_sq"))
 
-    def __init__(self, arena, lr, betas=(0.9, 0.999), eps=1e-8, weight_decay=0.0, amsgrad=False):
+    def __init__(self, arena, lr, betas=(0.9, 0.999), eps=1e-8, weight_decay=0.0, amsgrad=False,
+                 adamw=False):
+        self.adamw = bool(adamw)
         super().__init__(arena, dict(lr=lr, betas=betas, eps=eps, weight_decay=weight_decay,
                                      amsgrad=amsgrad, maximize=False, foreach=None,
                                      capturable=False, differentiable=False, fused=None,
-                                     decoupled_weight_decay=False))
+                                     decoupled_weight_decay=self.adamw))
+
+    def _kernel(self, name: str):
+        """The Adam entry point ``name`` of ``KERNELS``, or its AdamW form (adam -> adamw)."""
+        return getattr(KERNELS, name.replace("adam", "adamw", 1) if self.adamw else name)
 
     def _per_param_extra(self):
         return {"step": torch.tensor(float(self._steps))}
@@ -321,36 +335,47 @@ class FusedAdam(FusedArenaOptimizer):
         step = self._steps + 1
         bc1 = 1.0 - float(h["betas"][0]) ** step
         bc2 = 1.0 - float(h["betas"][1]) ** step
-        return (-(float(h["lr"]) / bc1), bc2 ** 0.5)
+        vals = (-(float(h["lr"]) / bc1), bc2 ** 0.5)
+        if self.adamw:          # dyn[2]: the decay factor, formed in double and rounded once to fp32
+            vals += (float(np.float32(1.0 - float(h["lr"]) * float(h["weight_decay"]))),)
+        return vals
+
+    def load_state_dict(self, state_dict: Dict[str, Any]) -> None:
+        """Moments, step and hyper-parameters as the base class loads them; an AdamW optimizer takes
+        ``torch.optim.Adam`` and ``torch.optim.AdamW`` state dicts alike and keeps reporting the rule
+        it runs (``decoupled_weight_decay=True``)."""
+        super().load_state_dict(state_dict)
+        if self.adamw:
+            self.hyper["decoupled_weight_decay"] = True
 
     def _launch(self, lo, hi, grad_scale, coef):
         h = self.hyper
         p, g, lp = self._slices(lo, hi)
         vmax = self._state("max_exp_avg_sq")[lo:hi] if h["amsgrad"] else None
-        KERNELS.adam(p, g, self._state("exp_avg")[lo:hi], self._state("exp_avg_sq")[lo:hi], vmax,
-                     lp, hi - lo, lr=float(h["lr"]), beta1=float(h["betas"][0]),
-                     beta2=float(h["betas"][1]), eps=float(h["eps"]),
-                     wd=float(h["weight_decay"]), step=self._steps + 1,
-                     grad_scale=grad_scale, grad_scale_dev=coef, dyn=self._dyn)
+        self._kernel("adam")(p, g, self._state("exp_avg")[lo:hi], self._state("exp_avg_sq")[lo:hi], vmax,
+                             lp, hi - lo, lr=float(h["lr"]), beta1=float(h["betas"][0]),
+                             beta2=float(h["betas"][1]), eps=float(h["eps"]),
+                             wd=float(h["weight_decay"]), step=self._steps + 1,
+                             grad_scale=grad_scale, grad_scale_dev=coef, dyn=self._dyn)
 
     def _launch_mt(self, table, grad_scale):
         h = self.hyper
-        KERNELS.adam_mt(self.arena.master, self._state("exp_avg"), self._state("exp_avg_sq"),
-                        self._state("max_exp_avg_sq") if h["amsgrad"] else None, self.arena.lp, table,
-                        lr=float(h["lr"]), beta1=float(h["betas"][0]), beta2=float(h["betas"][1]),
-                        eps=float(h["eps"]), wd=float(h["weight_decay"]), step=self._steps + 1,
-                        grad_scale=grad_scale, dyn=self._dyn)
+        self._kernel("adam_mt")(self.arena.master, self._state("exp_avg"), self._state("exp_avg_sq"),
+                                self._state("max_exp_avg_sq") if h["amsgrad"] else None, self.arena.lp, table,
+                                lr=float(h["lr"]), beta1=float(h["betas"][0]), beta2=float(h["betas"][1]),
+                                eps=float(h["eps"]), wd=float(h["weight_decay"]), step=self._steps + 1,
+                                grad_scale=grad_scale, dyn=self._dyn)
 
     def _launch_nvls(self, lo, hi, grad_scale):
         h = self.hyper
         mc_g, mc_out = self._nvls_ptrs(lo)
         vmax = self._state("max_exp_avg_sq")[lo:hi] if h["amsgrad"] else None
-        KERNELS.nvls_adam(self.arena.master[lo:hi], self._state("exp_avg")[lo:hi],
-                          self._state("exp_avg_sq")[lo:hi], vmax, mc_g, mc_out, hi - lo, self.nvls,
-                          lr=float(h["lr"]), beta1=float(h["betas"][0]), beta2=float(h["betas"][1]),
-                          eps=float(h["eps"]), wd=float(h["weight_decay"]), step=self._steps + 1,
-                          grad_scale=grad_scale, g_dtype=KERNELS.dtype_code(self.arena.grad.dtype),
-                          dyn=self._dyn)
+        self._kernel("nvls_adam")(self.arena.master[lo:hi], self._state("exp_avg")[lo:hi],
+                                  self._state("exp_avg_sq")[lo:hi], vmax, mc_g, mc_out, hi - lo, self.nvls,
+                                  lr=float(h["lr"]), beta1=float(h["betas"][0]), beta2=float(h["betas"][1]),
+                                  eps=float(h["eps"]), wd=float(h["weight_decay"]), step=self._steps + 1,
+                                  grad_scale=grad_scale, g_dtype=KERNELS.dtype_code(self.arena.grad.dtype),
+                                  dyn=self._dyn)
 
 
 class FusedRMSprop(FusedArenaOptimizer):
@@ -545,12 +570,14 @@ class FusedAdam8bit(_WholeTensorMixin, FusedAdam):
     over a segment table after backward.  ``state_dict()`` writes ``torch.optim.Adam``'s format with
     the decoded fp32 moments; ``load_state_dict()`` encodes them, so checkpoints move between
     ``torch.optim.Adam``, ``FusedAdam`` and this optimizer in both directions, and a run resumed
-    from its own checkpoint continues bit for bit (decode-then-encode returns the same codes)."""
+    from its own checkpoint continues bit for bit (decode-then-encode returns the same codes).
+    ``adamw=True``: ``FusedAdam``'s AdamW rule (K2-q8 AdamW) and ``torch.optim.AdamW``'s format."""
 
     STATE_NAMES = (("exp_avg", "exp_avg"), ("exp_avg_sq", "exp_avg_sq"))
 
-    def __init__(self, arena, lr, betas=(0.9, 0.999), eps=1e-8, weight_decay=0.0):
-        super().__init__(arena, lr=lr, betas=betas, eps=eps, weight_decay=weight_decay, amsgrad=False)
+    def __init__(self, arena, lr, betas=(0.9, 0.999), eps=1e-8, weight_decay=0.0, adamw=False):
+        super().__init__(arena, lr=lr, betas=betas, eps=eps, weight_decay=weight_decay, amsgrad=False,
+                         adamw=adamw)
         self._qbase, self.q8_blocks = q8_block_bases(arena.slots)
         dev = arena.device
         self.codes = {n: torch.zeros(arena.numel, dtype=torch.uint8, device=dev) for n, _ in self.STATE_NAMES}
@@ -588,11 +615,11 @@ class FusedAdam8bit(_WholeTensorMixin, FusedAdam):
             return
         h = self.hyper
         qbase, flags = self._q8_buffers(table)
-        KERNELS.adam8_mt(self.arena.master, self.codes["exp_avg"], self.codes["exp_avg_sq"],
-                         self.absmax["exp_avg"], self.absmax["exp_avg_sq"], self.arena.lp, table, qbase, flags,
-                         lr=float(h["lr"]), beta1=float(h["betas"][0]), beta2=float(h["betas"][1]),
-                         eps=float(h["eps"]), wd=float(h["weight_decay"]), step=self._steps + 1,
-                         grad_scale=grad_scale, grad_scale_dev=clip_coef_dev, dyn=self._dyn)
+        self._kernel("adam8_mt")(self.arena.master, self.codes["exp_avg"], self.codes["exp_avg_sq"],
+                                 self.absmax["exp_avg"], self.absmax["exp_avg_sq"], self.arena.lp, table, qbase, flags,
+                                 lr=float(h["lr"]), beta1=float(h["betas"][0]), beta2=float(h["betas"][1]),
+                                 eps=float(h["eps"]), wd=float(h["weight_decay"]), step=self._steps + 1,
+                                 grad_scale=grad_scale, grad_scale_dev=clip_coef_dev, dyn=self._dyn)
 
     def _every_slot(self):
         if self._all_table is None:
@@ -823,14 +850,16 @@ class FusedMuon(_WholeTensorMixin, FusedAdam):
     momentum buffer and ``exp_avg_sq`` the two bf16 Newton-Schulz iterates, so the state costs
     what Adam's does; K14's Gram workspace (``workspace_bytes``) comes on top.  ``state_dict()``
     has the two groups in torch's format; ``split_muon_state_dict`` / ``join_muon_state_dict``
-    convert it to and from a ``torch.optim.Muon`` plus a ``torch.optim.Adam``."""
+    convert it to and from a ``torch.optim.Muon`` plus a ``torch.optim.Adam`` (with ``adamw=True``,
+    a ``torch.optim.AdamW``: group 1 then runs ``FusedAdam``'s AdamW rule)."""
 
     STATE_NAMES = (("exp_avg", "exp_avg"), ("exp_avg_sq", "exp_avg_sq"))
 
     def __init__(self, arena, lr, weight_decay=0.0, momentum=0.95, eps=1e-8, betas=(0.9, 0.999), nesterov=True,
                  ns_coefficients=MUON_NS_COEFFICIENTS, muon_eps=1e-7, ns_steps=5,
-                 adjust_lr_fn="match_rms_adamw"):
-        super().__init__(arena, lr=lr, betas=betas, eps=eps, weight_decay=weight_decay, amsgrad=False)
+                 adjust_lr_fn="match_rms_adamw", adamw=False):
+        super().__init__(arena, lr=lr, betas=betas, eps=eps, weight_decay=weight_decay, amsgrad=False,
+                         adamw=adamw)
         muon_ids = {id(s.param) for s in arena.slots if is_muon_slot(s)}
         self.muon_params = [p for p in arena.all_params if id(p) in muon_ids]
         self.adam_params = [p for p in arena.all_params if id(p) not in muon_ids]
@@ -856,8 +885,16 @@ class FusedMuon(_WholeTensorMixin, FusedAdam):
         return self.param_groups[0]
 
     def _dyn_values(self):
-        # dyn[0], dyn[1]: K2-mt's Adam scalars; dyn[2]: K14's lr
+        # dyn[0], dyn[1]: K2-mt's Adam scalars; then AdamW's decay factor, if any; last: K14's lr,
+        # which K14 reads as its dyn[2] (``_muon_dyn``)
         return super()._dyn_values() + (float(self.muon_group["lr"]),)
+
+    def _muon_dyn(self) -> Optional[torch.Tensor]:
+        """The ``dyn`` K14 is given: the block itself, or with AdamW (whose decay factor takes
+        dyn[2]) the block from its second float, so that K14's dyn[2] is the Muon lr."""
+        if self._dyn is None or not self.adamw:
+            return self._dyn
+        return self._dyn[1:]
 
     def _split(self, table):
         """Per-table pieces, kept on the table: K14's plan over its Muon slots and the K2-mt
@@ -905,16 +942,16 @@ class FusedMuon(_WholeTensorMixin, FusedAdam):
             if sub is None:
                 continue
             _gather_segs(table, sub, idx)
-            KERNELS.adam_mt(self.arena.master, self._state("exp_avg"), self._state("exp_avg_sq"), None,
-                            self.arena.lp, sub, lr=float(h["lr"]), beta1=float(h["betas"][0]),
-                            beta2=float(h["betas"][1]), eps=float(h["eps"]), wd=float(h["weight_decay"]),
-                            step=self._steps + 1, grad_scale=grad_scale, grad_scale_dev=coef, dyn=self._dyn)
+            self._kernel("adam_mt")(self.arena.master, self._state("exp_avg"), self._state("exp_avg_sq"), None,
+                                    self.arena.lp, sub, lr=float(h["lr"]), beta1=float(h["betas"][0]),
+                                    beta2=float(h["betas"][1]), eps=float(h["eps"]), wd=float(h["weight_decay"]),
+                                    step=self._steps + 1, grad_scale=grad_scale, grad_scale_dev=coef, dyn=self._dyn)
         if plan is not None:
             KERNELS.muon_mt(self.arena.master, self._state("exp_avg"), self.arena.lp, table, plan,
                             lr=float(g["lr"]), wd=float(g["weight_decay"]), momentum=float(g["momentum"]),
                             nesterov=bool(g["nesterov"]), ns_coefficients=tuple(g["ns_coefficients"]),
                             ns_steps=g["ns_steps"], eps=float(g["eps"]), adjust_lr_fn=g["adjust_lr_fn"],
-                            grad_scale=grad_scale, grad_scale_dev=clip_coef_dev, dyn=self._dyn)
+                            grad_scale=grad_scale, grad_scale_dev=clip_coef_dev, dyn=self._muon_dyn())
 
     def _positions(self) -> Dict[int, int]:
         """torch's state-dict index of each parameter: group 0's, then group 1's."""
@@ -973,11 +1010,13 @@ class FusedMuon(_WholeTensorMixin, FusedAdam):
             elif entry:
                 steps = max(steps, 1)
         self._steps = steps
+        if self.adamw:
+            self.hyper["decoupled_weight_decay"] = True
 
 
 def split_muon_state_dict(sd: Dict[str, Any]) -> Tuple[Dict[str, Any], Dict[str, Any]]:
     """A ``FusedMuon`` state dict -> (``torch.optim.Muon`` state dict over group 0's parameters,
-    ``torch.optim.Adam`` state dict over group 1's)."""
+    ``torch.optim.Adam`` state dict over group 1's; ``torch.optim.AdamW``'s under AdamW)."""
     groups = sd["param_groups"]
     if len(groups) != 2:
         raise ValueError("a Muon state dict has two param groups (Muon, Adam), got %d" % len(groups))
@@ -993,7 +1032,7 @@ def split_muon_state_dict(sd: Dict[str, Any]) -> Tuple[Dict[str, Any], Dict[str,
 
 def join_muon_state_dict(muon_sd: Dict[str, Any], adam_sd: Dict[str, Any]) -> Dict[str, Any]:
     """The inverse of ``split_muon_state_dict``: one ``torch.optim.Muon`` and one ``torch.optim.Adam``
-    state dict (one group each) -> a ``FusedMuon`` state dict."""
+    or ``torch.optim.AdamW`` state dict (one group each) -> a ``FusedMuon`` state dict."""
     state, groups, base = {}, [], 0
     for sd in (muon_sd, adam_sd):
         if len(sd["param_groups"]) != 1:
@@ -1027,6 +1066,23 @@ def check_muon(optim_opts: OptimOpts, layer_adaptation: LayerAdaptation, optimiz
                                          " and adafactor" if adafactor else ""))
 
 
+def check_adamw(optim_opts: OptimOpts, layer_adaptation: LayerAdaptation, optimizer_state: OptimizerState,
+                adafactor: bool, adamw: bool) -> None:
+    """AdamW is a form of the Adam rule: it needs ``OptAlgorithm.ADAM`` (amsgrad, 8-bit state and
+    Muon as Adam allows them), no layer adaptation (LAMB's decay is already decoupled) and no
+    Adafactor; anything else is a ValueError naming the values."""
+    if not adamw:
+        return
+    st = OptimizerState(optimizer_state)
+    la = LayerAdaptation(layer_adaptation)
+    if not (optim_opts.algo == OptAlgorithm.ADAM and la is LayerAdaptation.NONE and not adafactor):
+        raise ValueError("adamw cannot be combined with optimizer %r%s, layer adaptation %r, optimizer state %r%s "
+                         "(adamw needs adam, layer adaptation none and no adafactor)"
+                         % (getattr(optim_opts.algo, "value", optim_opts.algo),
+                            " with amsgrad" if optim_opts.amsgrad else "", la.value, st.value,
+                            " and adafactor" if adafactor else ""))
+
+
 def check_optimizer_state(optim_opts: OptimOpts, layer_adaptation: LayerAdaptation,
                           optimizer_state: OptimizerState) -> None:
     """8-bit state needs Adam without amsgrad and without layer adaptation; anything else is a
@@ -1057,23 +1113,27 @@ def check_layer_adaptation(optim_opts: OptimOpts, layer_adaptation: LayerAdaptat
 def create_fused_optimizer(arena: ParamArena, optim_opts: OptimOpts,
                            layer_adaptation: LayerAdaptation = LayerAdaptation.NONE,
                            optimizer_state: OptimizerState = OptimizerState.FP32,
-                           adafactor: bool = False, muon: bool = False) -> FusedArenaOptimizer:
+                           adafactor: bool = False, muon: bool = False, adamw: bool = False) -> FusedArenaOptimizer:
     """Same dispatch and argument mapping as the reference's ``_create_optimizer``; with a layer
     adaptation, its LARS / LAMB counterpart; with 8-bit optimizer state, ``FusedAdam8bit``; with
     ``adafactor``, ``FusedAdafactor`` (``lr`` caps the relative step, ``weightDecay`` is its
     decoupled decay; ``epsilon`` and ``momentum`` are unused); with ``muon``, ``FusedMuon`` (one
-    ``lr`` and ``weightDecay`` for both groups, ``momentum`` is Muon's, ``epsilon`` Adam's)."""
+    ``lr`` and ``weightDecay`` for both groups, ``momentum`` is Muon's, ``epsilon`` Adam's); with
+    ``adamw``, the Adam rule of whichever of ``FusedAdam``, ``FusedAdam8bit`` or ``FusedMuon`` is
+    chosen takes decoupled weight decay (``torch.optim.AdamW``)."""
     check_layer_adaptation(optim_opts, layer_adaptation)
     check_optimizer_state(optim_opts, layer_adaptation, optimizer_state)
     check_adafactor(optim_opts, layer_adaptation, optimizer_state, adafactor)
     check_muon(optim_opts, layer_adaptation, optimizer_state, adafactor, muon)
+    check_adamw(optim_opts, layer_adaptation, optimizer_state, adafactor, adamw)
     if muon:
         return FusedMuon(arena, lr=optim_opts.lr, weight_decay=optim_opts.weightDecay,
-                         momentum=optim_opts.momentum, eps=optim_opts.epsilon)
+                         momentum=optim_opts.momentum, eps=optim_opts.epsilon, adamw=adamw)
     if adafactor:
         return FusedAdafactor(arena, lr=optim_opts.lr, weight_decay=optim_opts.weightDecay)
     if OptimizerState(optimizer_state) is OptimizerState.Q8:
-        return FusedAdam8bit(arena, lr=optim_opts.lr, weight_decay=optim_opts.weightDecay, eps=optim_opts.epsilon)
+        return FusedAdam8bit(arena, lr=optim_opts.lr, weight_decay=optim_opts.weightDecay, eps=optim_opts.epsilon,
+                             adamw=adamw)
     if layer_adaptation == LayerAdaptation.LARS:
         return FusedLars(arena, lr=optim_opts.lr, momentum=optim_opts.momentum,
                          weight_decay=optim_opts.weightDecay)
@@ -1088,5 +1148,5 @@ def create_fused_optimizer(arena: ParamArena, optim_opts: OptimOpts,
                         weight_decay=optim_opts.weightDecay)
     if algo == OptAlgorithm.ADAM:
         return FusedAdam(arena, lr=optim_opts.lr, weight_decay=optim_opts.weightDecay,
-                         eps=optim_opts.epsilon, amsgrad=optim_opts.amsgrad)
+                         eps=optim_opts.epsilon, amsgrad=optim_opts.amsgrad, adamw=adamw)
     raise ValueError("Unknown optimization algorithm type")

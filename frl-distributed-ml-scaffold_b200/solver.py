@@ -29,7 +29,7 @@ import torch.nn as nn
 from .arena import ParamArena
 from .criteria import BaseParallelCriterion
 from .ema import EMA_STATE_KEY
-from .fused_optim import (FusedAdafactor, FusedAdam8bit, FusedMuon, check_adafactor, check_muon, check_layer_adaptation, check_optimizer_state, create_fused_optimizer,
+from .fused_optim import (FusedAdafactor, FusedAdam8bit, FusedMuon, check_adafactor, check_adamw, check_muon, check_layer_adaptation, check_optimizer_state, create_fused_optimizer,
                           is_adapted)
 from .grad_sync import BufferBroadcaster, GradBucketPipeline
 from .lr_scheduler import DropEpochsScheduler, WarmupMultiStepLR
@@ -50,6 +50,7 @@ EMA_DECAY_ENV = "FRL_B200_EMA_DECAY"       # weight EMA decay in [0, 1), default
 OPTIMIZER_STATE_ENV = "FRL_B200_OPTIMIZER_STATE"   # "fp32" (default) | "8bit"
 ADAFACTOR_ENV = "FRL_B200_ADAFACTOR"               # "0" (default) | "1"
 MUON_ENV = "FRL_B200_MUON"                         # "0" (default) | "1"
+ADAMW_ENV = "FRL_B200_ADAMW"                       # "0" (default) | "1"
 EMA_SUFFIX = ".ema"                        # <checkpoint>.ema: the weight EMA next to a checkpoint
 
 
@@ -107,6 +108,9 @@ class SolverWorkerArgs(NamedTuple):
     # Muon for the model's 2-D weights, Adam for the rest; placed before optimizer_state, adafactor,
     # ema_decay and grad_accumulation, which keep their positions at the end
     muon: bool = False
+    # AdamW (decoupled weight decay) in every Adam update; placed before optimizer_state, adafactor,
+    # ema_decay and grad_accumulation, which keep their positions at the end
+    adamw: bool = False
     # Adam's state storage; placed before ema_decay and grad_accumulation, which stay the last fields
     optimizer_state: OptimizerState = OptimizerState.FP32
     # Adafactor instead of Adam; placed before ema_decay and grad_accumulation, which stay the last fields
@@ -291,6 +295,17 @@ def resolve_muon(explicit: Optional[bool] = None) -> bool:
     return raw == "1"
 
 
+def resolve_adamw(explicit: Optional[bool] = None) -> bool:
+    """Whether Adam takes decoupled weight decay (AdamW): ``explicit``, else FRL_B200_ADAMW (``0``,
+    the default, or ``1``).  Any other value is a ValueError."""
+    if explicit is not None:
+        return bool(explicit)
+    raw = os.environ.get(ADAMW_ENV, "0").strip()
+    if raw not in ("0", "1"):
+        raise ValueError("%s must be 0 or 1, got %r" % (ADAMW_ENV, raw))
+    return raw == "1"
+
+
 def resolve_grad_accumulation(explicit: Optional[int] = None) -> int:
     """Microbatches per optimizer update: ``explicit``, else FRL_B200_GRAD_ACCUM, else 1.  Anything
     but an integer >= 1 (``0``, negatives, ``2.5``, ``True``, non-numeric strings) is a ValueError."""
@@ -427,8 +442,9 @@ class Solver:
         opt_state = args.optimizer_state if run_opts.mode == Mode.TRAIN else OptimizerState.FP32
         adafactor = args.adafactor and run_opts.mode == Mode.TRAIN
         muon = args.muon and run_opts.mode == Mode.TRAIN
+        adamw = args.adamw and run_opts.mode == Mode.TRAIN
         optimizer = create_fused_optimizer(arena, run_opts.optim, args.layer_adaptation, opt_state, adafactor,
-                                           muon)
+                                           muon, adamw)
         if checkpoint:
             optimizer.load_state_dict(checkpoint.optimizerState)
         ema = None
@@ -489,7 +505,7 @@ class Solver:
                 "Linear layers with arena-born gradients %d (%d fused with their ReLU, %d in FP8) | "
                 "ReLU backward %s | "
                 "other gradients %s | layer adaptation %s | gradient accumulation %s | weight EMA %s | "
-                "optimizer state %s",
+                "optimizer %s | optimizer state %s",
                 args.precision.value,
                 "CUDA-graph replay after 2 eager steps" if worker.graphed is not None else "eager launches",
                 ("fused NVLS kernel per bucket (K7), %d buckets" % len(pipeline.buckets)) if pipeline.nvls is not None
@@ -515,6 +531,13 @@ class Solver:
                 "none" if ema is None else
                 "decay %r, one K11 launch per update (%.1f MiB), held-out splits evaluated with it" % (
                     ema_decay, ema.nbytes / 2 ** 20),
+                ("adamw, decoupled weight decay %r (%s)" % (
+                    run_opts.optim.weightDecay,
+                    "frl_adamw8_mt, K2-q8" if isinstance(optimizer, FusedAdam8bit) else
+                    "frl_adamw_mt, K2-mt, for the non-Muon group" if isinstance(optimizer, FusedMuon) else
+                    "frl_nvls_adamw, K7" if pipeline.nvls is not None else
+                    "frl_adamw / frl_adamw_mt, K2 / K2-mt"))
+                if getattr(optimizer, "adamw", False) else getattr(run_opts.optim.algo, "value", run_opts.optim.algo),
                 "8-bit block-wise (K2-q8), %.1f MiB instead of %.1f MiB" % (
                     optimizer.state_bytes / 2 ** 20, optimizer.fp32_state_bytes / 2 ** 20)
                 if isinstance(optimizer, FusedAdam8bit) else
@@ -737,7 +760,8 @@ class Solver:
               ema_decay: Optional[float] = None,
               optimizer_state: Optional[OptimizerState] = None,
               adafactor: Optional[bool] = None,
-              muon: Optional[bool] = None
+              muon: Optional[bool] = None,
+              adamw: Optional[bool] = None
               ) -> Iterator[PerformanceSummary]:
         """The reference's entry point (solver.py:728-739) plus two keyword-only extensions:
 
@@ -837,6 +861,15 @@ class Solver:
                        ``fused_optim.split_muon_state_dict`` / ``join_muon_state_dict`` convert
                        them to and from a ``torch.optim.Muon`` plus a ``torch.optim.Adam``.  None:
                        FRL_B200_MUON (``0`` by default, ``1`` to enable).  ``Mode.EVAL`` ignores it.
+        ``adamw``      True: AdamW, i.e. torch 2.11's ``Adam(decoupled_weight_decay=True)``, in every
+                       Adam update (K2, K2-mt, K7, K2-q8, and Muon's Adam group): each step first
+                       scales every parameter by fp32(1 - lr * ``weightDecay``), then takes Adam's
+                       step with no decay term in the gradient.  Needs ``OptAlgorithm.ADAM`` (with
+                       or without amsgrad, fp32 or 8-bit state, with or without Muon), no layer
+                       adaptation and no Adafactor; any other combination raises ``ValueError``
+                       before a rank starts.  Checkpoints keep ``torch.optim.AdamW``'s format and
+                       ``torch.optim.Adam`` / ``AdamW`` state dicts resume.  None: FRL_B200_ADAMW
+                       (``0`` by default, ``1`` to enable).  ``Mode.EVAL`` ignores it.
         """
         adapt = LayerAdaptation.NONE
         accum = 1
@@ -844,6 +877,7 @@ class Solver:
         opt_state = OptimizerState.FP32
         use_adafactor = False
         use_muon = False
+        use_adamw = False
         if run_opts.mode == Mode.TRAIN:
             adapt = resolve_layer_adaptation(layer_adaptation)
             check_layer_adaptation(run_opts.optim, adapt)
@@ -853,6 +887,8 @@ class Solver:
             check_adafactor(run_opts.optim, adapt, opt_state, use_adafactor)
             use_muon = resolve_muon(muon)
             check_muon(run_opts.optim, adapt, opt_state, use_adafactor, use_muon)
+            use_adamw = resolve_adamw(adamw)
+            check_adamw(run_opts.optim, adapt, opt_state, use_adafactor, use_adamw)
             accum = resolve_grad_accumulation(grad_accumulation)
             decay = resolve_ema_decay(ema_decay)
         n_visible = 0 if run_opts.cpuonly else _cuda_device_count_without_poisoning_fork()
@@ -894,7 +930,7 @@ class Solver:
                 world_size=world_size, group_name=group_name, init_method=init_method,
                 cache=None, precision=prec, save_every=save_every, graph_step=graph,
                 layer_adaptation=adapt, grad_accumulation=accum, ema_decay=decay,
-                optimizer_state=opt_state, adafactor=use_adafactor, muon=use_muon)
+                optimizer_state=opt_state, adafactor=use_adafactor, muon=use_muon, adamw=use_adamw)
             if not run_opts.singleThreaded:
                 parent_conn, child_conn = ctx.Pipe(duplex=False)
                 proc = ctx.Process(target=cls._solver_worker_process,

@@ -158,7 +158,8 @@ class OptimOpts(NamedTuple):
                   arguments (or the device-resident ``dyn`` block under CUDA-graph replay)
     lr_scheduler  ``drop`` or ``multistep`` closed forms, stepped once per epoch
     weightDecay   L2-COUPLED decay folded into the gradient read, on every parameter (model and
-                  criterion) — this is ``torch.optim``'s ``weight_decay``, not AdamW's
+                  criterion) — this is ``torch.optim``'s ``weight_decay``; for AdamW's decoupled
+                  decay with Adam, pass ``Solver.solve(..., adamw=True)``
     momentum      SGD momentum AND RMSprop momentum (the reference feeds both from this field)
     epsilon       Adam only (RMSprop keeps torch's 1e-8), as in the reference's factory
     amsgrad       Adam: adds the running maximum of the second moment (a third state vector)

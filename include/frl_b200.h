@@ -58,8 +58,10 @@ int          frl_device_arch(void);
  * when it hands Python scalars to fp32 tensor ops.
  *   dyn      optional DEVICE array of per-step scalars that override the by-value arguments,
  *            so a CUDA graph that captured the launch stays valid while they change:
- *            SGD / RMSprop: dyn[0] = lr ;  Adam: dyn[0] = -lr/(1-beta1^t), dyn[1] = sqrt(1-beta2^t).
- * Update rules are torch 2.11's (L2-coupled weight decay: g += wd * p first).
+ *            SGD / RMSprop: dyn[0] = lr ;  Adam: dyn[0] = -lr/(1-beta1^t), dyn[1] = sqrt(1-beta2^t);
+ *            AdamW: Adam's two, then dyn[2] = fp32(1 - lr*wd).
+ * Update rules are torch 2.11's (L2-coupled weight decay: g += wd * p first), except AdamW's
+ * decoupled decay (frl_adamw*).
  * ---------------------------------------------------------------------------------------- */
 
 /* SGD: buf = first_step ? g : mu*buf + (1-dampening)*g ; p -= lr*buf.   mu == 0: buf may be NULL. */
@@ -74,6 +76,23 @@ int frl_adam(float* p, const void* g, float* m, float* v, float* vmax, void* p_l
              double lr, double beta1, double beta2, double eps, double wd, int64_t step,
              double grad_scale, const float* grad_scale_dev, const float* dyn, int g_dtype,
              void* stream);
+
+/* AdamW — torch 2.11's Adam(decoupled_weight_decay=True), which torch.optim.AdamW is.  Four entry
+ * points, each with exactly the arguments of its Adam form: frl_adamw (K2, frl_adam's),
+ * frl_adamw_mt (K2-mt, frl_adam_mt's), frl_adamw8_mt (K2-q8, frl_adam8_mt's) and frl_nvls_adamw
+ * (K7, frl_nvls_adam's).  Per element, with g the scaled gradient:
+ *     p  = p * fp32(1 - lr*wd)             its own fp32 multiply, before anything else
+ *                                         (1 - lr*wd formed in double, rounded once to fp32)
+ *     m  = lerp(m, g, 1-beta1) ; v = beta2*v + (1-beta2)*g^2 ; vmax = max(vmax, v) (amsgrad)
+ *     p += -lr/(1-beta1^t) * m / (sqrt(v or vmax)/sqrt(1-beta2^t) + eps)
+ * The gradient carries no decay term; with wd == 0 the result is frl_adam's, bit for bit.
+ * dyn (may be NULL): dyn[0] = -lr/(1-beta1^t), dyn[1] = sqrt(1-beta2^t), dyn[2] = fp32(1 - lr*wd),
+ * so a captured CUDA graph follows a scheduled lr in the decay as well.  Graph-capturable.  Every
+ * argument check is made before any launch, as in the Adam forms; frl_abi_version() stays 1. */
+int frl_adamw(float* p, const void* g, float* m, float* v, float* vmax, void* p_lp, int64_t n,
+              double lr, double beta1, double beta2, double eps, double wd, int64_t step,
+              double grad_scale, const float* grad_scale_dev, const float* dyn, int g_dtype,
+              void* stream);
 
 /* RMSprop (not centered): sq = alpha*sq + (1-alpha)*g^2 ; avg = sqrt(sq)+eps ;
  * mu > 0: buf = mu*buf + g/avg ; p -= lr*buf     else: p -= lr*g/avg  (buf may be NULL). */
@@ -155,6 +174,12 @@ int frl_adam_mt(float* p, float* m, float* v, float* vmax, void* p_lp, const frl
                 const int64_t* tile_prefix_dev, const int32_t* tile_seg_dev, int64_t n_tiles, double lr, double beta1,
                 double beta2, double eps, double wd, int64_t step, double grad_scale,
                 const float* grad_scale_dev, const float* dyn, void* stream);
+
+/* K2-mt AdamW: frl_adam_mt's arguments, frl_adamw's rule and dyn layout. */
+int frl_adamw_mt(float* p, float* m, float* v, float* vmax, void* p_lp, const frl_grad_seg* segs_dev,
+                 const int64_t* tile_prefix_dev, const int32_t* tile_seg_dev, int64_t n_tiles, double lr, double beta1,
+                 double beta2, double eps, double wd, int64_t step, double grad_scale,
+                 const float* grad_scale_dev, const float* dyn, void* stream);
 
 int frl_rmsprop_mt(float* p, float* sq, float* buf, void* p_lp, const frl_grad_seg* segs_dev,
                    const int64_t* tile_prefix_dev, const int32_t* tile_seg_dev, int64_t n_tiles, double lr, double alpha,
@@ -248,6 +273,13 @@ int frl_adam8_mt(float* p, uint8_t* m_q, uint8_t* v_q, float* m_absmax, float* v
                  int64_t n_tiles, int64_t n_segs, const int64_t* qbase_dev, const int32_t* seg_flags_dev,
                  double lr, double beta1, double beta2, double eps, double wd, int64_t step,
                  double grad_scale, const float* grad_scale_dev, const float* dyn, void* stream);
+/* K2-q8 AdamW: frl_adam8_mt's arguments, encoder and decoder; frl_adamw's rule (no amsgrad) and
+ * dyn layout, applied to the decoded moments. */
+int frl_adamw8_mt(float* p, uint8_t* m_q, uint8_t* v_q, float* m_absmax, float* v_absmax, void* p_lp,
+                  const frl_grad_seg* segs_dev, const int64_t* tile_prefix_dev, const int32_t* tile_seg_dev,
+                  int64_t n_tiles, int64_t n_segs, const int64_t* qbase_dev, const int32_t* seg_flags_dev,
+                  double lr, double beta1, double beta2, double eps, double wd, int64_t step,
+                  double grad_scale, const float* grad_scale_dev, const float* dyn, void* stream);
 int frl_q8_encode_mt(const float* x, uint8_t* q, float* absmax, int state, const frl_grad_seg* segs_dev,
                      const int64_t* tile_prefix_dev, const int32_t* tile_seg_dev, int64_t n_tiles,
                      int64_t n_segs, const int64_t* qbase_dev, void* stream);
@@ -597,6 +629,12 @@ int frl_nvls_adam(float* p, float* m, float* v, float* vmax, const void* mc_g, v
                   void* local_scratch, int max_blocks, double lr, double beta1, double beta2,
                   double eps, double wd,
                   int64_t step, double grad_scale, const float* dyn, int g_dtype, int flags, void* stream);
+/* K7 AdamW: frl_nvls_adam's arguments, frl_adamw's rule and dyn layout. */
+int frl_nvls_adamw(float* p, float* m, float* v, float* vmax, const void* mc_g, void* mc_out,
+                   int64_t n, int rank, int world, void* const* signal_pads_dev, int pad_base,
+                   void* local_scratch, int max_blocks, double lr, double beta1, double beta2,
+                   double eps, double wd,
+                   int64_t step, double grad_scale, const float* dyn, int g_dtype, int flags, void* stream);
 int frl_nvls_rmsprop(float* p, float* sq, float* buf, const void* mc_g, void* mc_out, int64_t n,
                      int rank, int world, void* const* signal_pads_dev, int pad_base,
                      void* local_scratch, int max_blocks, double lr, double alpha, double eps,

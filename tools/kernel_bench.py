@@ -1,7 +1,7 @@
 #!/usr/bin/env python
 """Micro-benchmark of every hand-written kernel at the BASELINE shapes (1 GPU).
 
-    python tools/kernel_bench.py [--only k2,k2lw,k2q8,k2af,k3,k5a,k13,k14,...] [--iters 20] [--json out.json]
+    python tools/kernel_bench.py [--only k2,k2lw,k2q8,k2af,k2w,k3,k5a,k13,k14,...] [--iters 20] [--json out.json]
 
 Each kernel is timed with CUDA events on the launching stream over ROTATING operand sets whose
 total size exceeds the 50 MB L2 (so every launch streams from HBM), after 3 warm-up launches.
@@ -266,6 +266,57 @@ def bench_k2q8(iters):
                   "%.2f B/param" % (q8_bytes / n_real), graph=True),
             timed("K2-mt adam fp32 state mlp bf16-grad (%d tensors, %d params)" % (len(slots), n_real), fp32, 1,
                   28 * n_real, iters, "28 B/param", graph=True)]
+
+
+def bench_k2w(iters):
+    """K2-mt AdamW (``frl_adamw_mt``) beside K2-mt Adam (``frl_adam_mt``) on the headline MLP's arena
+    (10 tensors, 54.7 M parameters), bf16 gradients in the arena, bf16 shadow, fp32 state, each timed
+    from a CUDA graph.  Both rules move 28 bytes per parameter, so the arena (1.5 GB of traffic per
+    launch) is far larger than L2 and every launch streams from HBM.  Five rounds, Adam and AdamW
+    alternating; the last two records are the medians (min-max) and AdamW / Adam."""
+    from frl_b200.multi_tensor import GradSegTable
+
+    class Slot:
+        def __init__(self, index, offset, shape):
+            self.index, self.offset, self.shape = index, offset, shape
+            self.numel = 1
+            for d in shape:
+                self.numel *= d
+            self.is_model = True
+
+    shapes = [(4096, 4096), (4096,)] * 3 + [(1000, 4096), (1000,), (64, 4096), (64,)]
+    slots, off = [], 0
+    for i, sh in enumerate(shapes):
+        slots.append(Slot(i, off, sh))
+        off = (off + slots[-1].numel + 7) // 8 * 8
+    n, n_real = off, sum(s.numel for s in slots)
+    grad = torch.randn(n, device=DEV).bfloat16()
+    table = GradSegTable(slots, DEV)
+    for s in slots:
+        table.point(s, grad.data_ptr() + 2 * s.offset, grad.dtype)
+    table.upload()
+    p = torch.randn(n, device=DEV) * 0.02
+    lp = torch.empty(n, device=DEV, dtype=torch.bfloat16)
+    m, v = torch.randn(n, device=DEV) * 1e-3, torch.rand(n, device=DEV) * 1e-6
+    kw = dict(lr=1e-3, beta1=0.9, beta2=0.999, eps=1e-8, wd=1e-2, step=3)
+    fns = {"adam": lambda i: _native.adam_mt(p, m, v, None, lp, table, **kw),
+           "adamw": lambda i: _native.adamw_mt(p, m, v, None, lp, table, **kw)}
+    out, times = [], {"adam": [], "adamw": []}
+    for r in range(5):
+        for rule in ("adam", "adamw"):
+            rec = timed("K2-mt %s fp32 state mlp bf16-grad (%d tensors, %d params) round %d"
+                        % (rule, len(slots), n_real, r), fns[rule], 1, 28 * n_real, iters, "28 B/param", graph=True)
+            times[rule].append(rec["us"])
+            out.append(rec)
+    med = {k: sorted(t)[len(t) // 2] for k, t in times.items()}
+    summary = {"kernel": "K2-mt adamw vs adam, median of 5 (min-max)",
+               "adam_us": "%.1f (%.1f-%.1f)" % (med["adam"], min(times["adam"]), max(times["adam"])),
+               "adamw_us": "%.1f (%.1f-%.1f)" % (med["adamw"], min(times["adamw"]), max(times["adamw"])),
+               "adamw_over_adam": round(med["adamw"] / med["adam"], 4),
+               "within_5pct": med["adamw"] <= 1.05 * med["adam"]}
+    print(json.dumps(summary), flush=True)
+    out.append(summary)
+    return out
 
 
 def bench_k2af(iters):
@@ -794,7 +845,7 @@ def bench_k14(iters):
 BENCHES = {"k2": bench_k2, "k2mt": bench_k2mt, "k2lw": bench_k2lw, "k3": bench_k3, "k4": bench_k4, "k5": bench_k5, "k5a": bench_k5a,
            "k5m": bench_k5m, "k4s": bench_k4s, "k6": bench_k6,
            "k8": bench_k8, "k8t": bench_k8t, "k9": bench_k9, "k10": bench_k10, "k11": bench_k11,
-           "k2q8": bench_k2q8, "k2af": bench_k2af, "k13": bench_k13, "k14": bench_k14}
+           "k2q8": bench_k2q8, "k2af": bench_k2af, "k13": bench_k13, "k14": bench_k14, "k2w": bench_k2w}
 
 
 def main():
