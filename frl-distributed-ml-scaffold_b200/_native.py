@@ -96,11 +96,16 @@ SIGNATURES = {
     "frl_criteria_forward": (_i, [C.POINTER(TaskDesc), _i, _vp, _vp, _vp, _vp, _vp, _vp, _vp]),
     "frl_criteria_backward": (_i, [C.POINTER(TaskDesc), _i, _vp, _vp, _vp, _vp]),
     "frl_preproc_affine": (_i, [_vp, _i, _vp, _i, _i64, _i64, _i64, _vp, _vp, _vp]),
+    "frl_preproc_affine_nhwc": (_i, [_vp, _i, _vp, _i, _i64, _i, _i64, _vp, _vp, _vp]),
     "frl_cast_scale": (_i, [_vp, _i, _vp, _i, _i64, _f, _vp]),
     "frl_augment_images": (_i, [_vp, _i64, _i, _i, _i, _vp, C.c_uint64, _i, _i, _d, _d, _d, _d, _d, _i, _i,
                                 _vp, _vp, _vp, _i, _i, _i, _vp, _vp]),
     "frl_augment_mix_images": (_i, [_vp, _i64, _i, _i, _i, _vp, C.c_uint64, _i, _i, _d, _d, _d, _d, _d, _i, _i,
                                     _vp, _vp, _vp, _i, _i, _i, _vp, _i, _f, _i, _i, _i, _i, _vp]),
+    "frl_augment_images_nhwc": (_i, [_vp, _i64, _i, _i, _i, _vp, C.c_uint64, _i, _i, _d, _d, _d, _d, _d, _i, _i,
+                                     _vp, _vp, _vp, _i, _i, _i, _vp, _vp]),
+    "frl_augment_mix_images_nhwc": (_i, [_vp, _i64, _i, _i, _i, _vp, C.c_uint64, _i, _i, _d, _d, _d, _d, _d, _i,
+                                         _i, _vp, _vp, _vp, _i, _i, _i, _vp, _i, _f, _i, _i, _i, _i, _vp]),
     "frl_mix_targets": (_i, [_vp, _i, _i64, _i64, _i, _f, _vp, _vp]),
     "frl_colsum_scratch_bytes": (_i64, [_i64, _i64]),
     "frl_colsum": (_i, [_vp, _i, _i64, _i64, _vp, _i, _i, _vp, _vp]),
@@ -654,6 +659,22 @@ def preproc_affine(src, dst, *, inner=1, channels=1, scale=None, bias=None) -> N
                                     _ptr(bias), _stream()), "frl_preproc_affine")
 
 
+def is_nhwc(t) -> bool:
+    """A 4-D tensor stored channels_last whose NCHW order differs (C, H and W not all trivial)."""
+    return t.dim() == 4 and not t.is_contiguous() and t.is_contiguous(memory_format=torch.channels_last)
+
+
+def preproc_affine_nhwc(src, dst, *, scale=None, bias=None) -> None:
+    """K5 into channels_last: ``src`` contiguous [B, C, H, W] (1 <= C <= 4) -> ``dst`` [B, C, H, W]
+    stored channels_last, the values of ``preproc_affine(src, ..., inner=H*W, channels=C)``."""
+    B, Cc, H, W = src.shape
+    assert src.is_contiguous() and dst.shape == src.shape
+    assert dst.is_contiguous(memory_format=torch.channels_last)
+    _check(lib().frl_preproc_affine_nhwc(_ptr(src), dtype_code(src.dtype), _ptr(dst), dtype_code(dst.dtype),
+                                         B, Cc, H * W, _ptr(scale), _ptr(bias), _stream()),
+           "frl_preproc_affine_nhwc")
+
+
 AUG_RRC, AUG_PAD_CROP, AUG_CENTER_RESIZE, AUG_CENTER_CROP = 0, 1, 2, 3
 
 
@@ -663,7 +684,7 @@ MIX_MIXUP, MIX_CUTMIX = 1, 2
 def _augment_args(src, idx, dst, seed, epoch, mode, scale_range, ratio_range, eval_crop, pad, flip, scale, bias,
                   params_out):
     B, Cc, H, W = src.shape
-    assert src.dtype == torch.uint8 and src.is_contiguous() and dst.is_contiguous()
+    assert src.dtype == torch.uint8 and src.is_contiguous() and (dst.is_contiguous() or is_nhwc(dst))
     assert dst.dim() == 4 and tuple(dst.shape[:2]) == (B, Cc)
     assert idx.dtype == torch.int64 and idx.is_contiguous() and idx.numel() == B
     assert params_out is None or (params_out.dtype == torch.int32 and params_out.is_contiguous()
@@ -680,11 +701,13 @@ def augment_images(src, idx, dst, *, seed: int, epoch: int, mode: int, scale_ran
                    flip: bool = True, scale=None, bias=None, params_out=None) -> None:
     """K5a: crop box drawn per (seed, epoch, idx[b]), bilinear resize to ``dst``'s [out_h, out_w],
     optional flip, then ``x * scale[c] + bias[c]``.  ``src`` uint8 [B, C, H, W], ``idx`` device
-    int64 [B], ``dst`` fp32/bf16 [B, C, out_h, out_w], ``params_out`` optional int32 [B, 5]
+    int64 [B], ``dst`` fp32/bf16 [B, C, out_h, out_w] (contiguous, or channels_last: then
+    ``frl_augment_images_nhwc`` writes it), ``params_out`` optional int32 [B, 5]
     (top, left, h, w, flipped).  See frl_augment_images in include/frl_b200.h."""
     args = _augment_args(src, idx, dst, seed, epoch, mode, scale_range, ratio_range, eval_crop, pad, flip, scale,
                          bias, params_out)
-    _check(lib().frl_augment_images(*args, _stream()), "frl_augment_images")
+    name = "frl_augment_images_nhwc" if is_nhwc(dst) else "frl_augment_images"
+    _check(getattr(lib(), name)(*args, _stream()), name)
 
 
 def augment_mix_images(src, idx, dst, *, mix_mode: int, lam: float, box=(0, 0, 0, 0), seed: int, epoch: int,
@@ -697,8 +720,8 @@ def augment_mix_images(src, idx, dst, *, mix_mode: int, lam: float, box=(0, 0, 0
     args = _augment_args(src, idx, dst, seed, epoch, mode, scale_range, ratio_range, eval_crop, pad, flip, scale,
                          bias, params_out)
     y0, y1, x0, x1 = (int(v) for v in box)
-    _check(lib().frl_augment_mix_images(*args, int(mix_mode), float(lam), y0, y1, x0, x1, _stream()),
-           "frl_augment_mix_images")
+    name = "frl_augment_mix_images_nhwc" if is_nhwc(dst) else "frl_augment_mix_images"
+    _check(getattr(lib(), name)(*args, int(mix_mode), float(lam), y0, y1, x0, x1, _stream()), name)
 
 
 def mix_targets(src, dst, lam: float, n_classes: int = 0) -> None:
@@ -719,6 +742,10 @@ def mix_targets(src, dst, lam: float, n_classes: int = 0) -> None:
 
 
 def cast_scale(src, dst, scale: float = 1.0) -> None:
+    """dst = src * scale element by element: both contiguous, or both channels_last (cast as the
+    [B, H, W, C] arrays they store)."""
+    if is_nhwc(src) and is_nhwc(dst):
+        src, dst = src.permute(0, 2, 3, 1), dst.permute(0, 2, 3, 1)
     n = src.numel()
     assert dst.numel() == n and src.is_contiguous() and dst.is_contiguous()
     _check(lib().frl_cast_scale(_ptr(src), dtype_code(src.dtype), _ptr(dst),

@@ -15,6 +15,11 @@ memory directly and one kernel launch over ``[lo, hi)`` updates any contiguous r
 Slices start at multiples of 8 elements (32 B fp32 / 16 B bf16) so every slice is 128-bit
 aligned in both precisions; the padding elements stay zero and are inert under every rule.
 
+``channels_last=True`` lays every trainable 4-D parameter (a Conv2d weight [O, I, kh, kw]) out in
+channels_last element order (O, kh, kw, I), and ``param.data`` is its slice with channels_last
+strides.  Every arena-shaped vector shares that order; ``slot_view`` is the one way to see a slice
+as its parameter.  Exported weights and state dicts are contiguous whatever the layout.
+
 This replaces the per-tensor ``torch.optim`` state and the DDP reducer's bucket copies
 (reference solver.py:162-188, 287-289).
 """
@@ -34,9 +39,10 @@ def _round_up(x: int, a: int) -> int:
 
 
 class ArenaSlot:
-    __slots__ = ("param", "offset", "numel", "shape", "is_model", "uses_lp", "index")
+    __slots__ = ("param", "offset", "numel", "shape", "is_model", "uses_lp", "index", "memory_format")
 
-    def __init__(self, param, offset, numel, shape, is_model, uses_lp, index):
+    def __init__(self, param, offset, numel, shape, is_model, uses_lp, index,
+                 memory_format=torch.contiguous_format):
         self.param = param
         self.offset = offset
         self.numel = numel
@@ -44,6 +50,19 @@ class ArenaSlot:
         self.is_model = is_model
         self.uses_lp = uses_lp
         self.index = index          # position in the optimizer's flat parameter list
+        self.memory_format = memory_format      # element order of the slice
+
+    @property
+    def strides(self) -> Tuple[int, ...]:
+        """Strides of the parameter's view of its slice."""
+        if self.memory_format is torch.channels_last:
+            o, i, kh, kw = self.shape
+            return (kh * kw * i, 1, kw * i, i)
+        st, acc = [], 1
+        for d in reversed(self.shape):
+            st.append(acc)
+            acc *= d
+        return tuple(reversed(st))
 
     @property
     def end(self) -> int:
@@ -54,7 +73,8 @@ class ParamArena:
     def __init__(self, model_params: Iterable[nn.Parameter],
                  criterion_params: Iterable[nn.Parameter] = (),
                  *, device: torch.device, precision: Precision = Precision.FP32,
-                 shared_allocator=None, adjacent: Sequence[Sequence[nn.Parameter]] = ()) -> None:
+                 shared_allocator=None, adjacent: Sequence[Sequence[nn.Parameter]] = (),
+                 channels_last: bool = False) -> None:
         """``shared_allocator(numel, dtype) -> zeroed tensor``: where the vectors other ranks must
         reach (``grad`` and the weights the modules read) come from — symmetric/multicast memory
         for the fused NVLS step; default ``torch.zeros``.
@@ -63,7 +83,9 @@ class ParamArena:
         where the first member would have gone (e.g. the weights of all task heads, so that one
         GEMM can treat them as a single [sum(C_i), K] matrix).  A group is honoured only if every
         member but the last has a multiple of 8 elements (no padding in between); the slot list
-        stays sorted by offset, ``ArenaSlot.index`` keeps the optimizer's parameter position."""
+        stays sorted by offset, ``ArenaSlot.index`` keeps the optimizer's parameter position.
+
+        ``channels_last``: lay every trainable 4-D parameter out in channels_last element order."""
         self.device = torch.device(device)
         self.precision = precision
         self.all_params: List[nn.Parameter] = []
@@ -112,7 +134,8 @@ class ParamArena:
                 if p.dtype != torch.float32:
                     raise TypeError(f"arena expects fp32 parameters at wrap time, got {p.dtype}")
                 uses_lp = is_model and precision.bf16_storage
-                self.slots.append(ArenaSlot(p, off, p.numel(), tuple(p.shape), is_model, uses_lp, idx))
+                fmt = torch.channels_last if channels_last and p.dim() == 4 else torch.contiguous_format
+                self.slots.append(ArenaSlot(p, off, p.numel(), tuple(p.shape), is_model, uses_lp, idx, fmt))
                 off = _round_up(off + p.numel(), ALIGN_ELEMS)
             if is_model:
                 self.model_end = off        # padded end of the model-parameter range
@@ -129,7 +152,7 @@ class ParamArena:
                        if bf16_mode else shared(torch.float32))
         with torch.no_grad():
             for s in self.slots:
-                self.master[s.offset:s.end].copy_(s.param.detach().reshape(-1))
+                self.slot_view(self.master, s).copy_(s.param.detach())
         self.lp: Optional[torch.Tensor] = None
         if bf16_mode:
             self.lp = shared(torch.bfloat16)
@@ -142,19 +165,32 @@ class ParamArena:
     def _storage_for(self, s: ArenaSlot) -> torch.Tensor:
         return self.lp if s.uses_lp else self.master
 
+    @staticmethod
+    def slot_view(vec: torch.Tensor, s: ArenaSlot) -> torch.Tensor:
+        """Slot ``s``'s slice of the arena-shaped vector ``vec`` as a tensor of the parameter's
+        shape, in the slot's element order (channels_last strides for a channels_last slot)."""
+        flat = vec[s.offset:s.end]
+        if s.memory_format is torch.contiguous_format:
+            return flat.view(s.shape)
+        return flat.as_strided(s.shape, s.strides)
+
+    @property
+    def n_channels_last(self) -> int:
+        return sum(s.memory_format is torch.channels_last for s in self.slots)
+
     def _repoint(self) -> None:
         for s in self.slots:
-            s.param.data = self._storage_for(s)[s.offset:s.end].view(s.shape)
+            s.param.data = self.slot_view(self._storage_for(s), s)
             s.param.grad = None
 
     def slot_of(self, p: nn.Parameter) -> ArenaSlot:
         return self._by_id[id(p)]
 
     def grad_view(self, s: ArenaSlot) -> torch.Tensor:
-        return self.grad[s.offset:s.end].view(s.shape)
+        return self.slot_view(self.grad, s)
 
     def master_view(self, s: ArenaSlot) -> torch.Tensor:
-        return self.master[s.offset:s.end].view(s.shape)
+        return self.slot_view(self.master, s)
 
     def new_state(self) -> torch.Tensor:
         return torch.zeros(self.numel, dtype=torch.float32, device=self.device)
@@ -199,7 +235,7 @@ class ParamArena:
                         buf.data = buf.data.float()
             for s in self.slots:
                 saved.append((s.param, s.param.data, s.param.grad))
-                clone = self.master_view(s).detach().clone()
+                clone = self.master_view(s).detach().clone(memory_format=torch.contiguous_format)
                 s.param.data = clone.cpu() if cpu else clone
                 s.param.grad = None
             yield self

@@ -12,6 +12,9 @@
 // frl_augment_mix_images runs the same body over pairs (p, B-1-p) and blends or swaps the two
 // normalised values of every pixel before the one store (Mixup / CutMix); frl_mix_targets mixes
 // the target fields with the same partner and lambda.
+// The _nhwc entry points differ in the store alone (template parameter NHWC): a thread writes the
+// C values of its pixel next to each other, [B, out_h, out_w, C] in memory; the values are the
+// NCHW ones.
 #include <math.h>
 
 #include <algorithm>
@@ -167,7 +170,7 @@ __device__ __forceinline__ void aug_pixel(const AugArgs& a, const uint8_t* img, 
 // MIX_NONE: grid (B, bands), K5a.  MIX_MIXUP / MIX_CUTMIX: grid (ceil(B/2), bands); the CTA of
 // blockIdx.x = p serves the pair (p, B-1-p), forming both samples' normalised values of a pixel
 // and writing both mixed outputs (the middle sample of an odd batch is written as K5a writes it)
-template <typename D, int MIX>
+template <typename D, int MIX, bool NHWC>
 __global__ void __launch_bounds__(kAugThreads)
 augment_kernel(const uint8_t* __restrict__ src, const int64_t* __restrict__ idx, AugArgs a,
                const float* __restrict__ scale, const float* __restrict__ bias, D* __restrict__ dst,
@@ -210,9 +213,11 @@ augment_kernel(const uint8_t* __restrict__ src, const int64_t* __restrict__ idx,
     for (int p = threadIdx.x; p < n; p += kAugThreads) {
         const int oy = y0 + p / a.out_w, ox = p % a.out_w;
         const int64_t od = static_cast<int64_t>(oy) * a.out_w + ox;
+        // element of channel c of this pixel, from the sample's base
+        const auto at = [&](int c) { return NHWC ? od * a.C + c : c * oplane + od; };
         if (MIX == MIX_NONE || !pair) {
             aug_pixel(a, img, box[0], sy, sx, sc, bi, oy, ox,
-                      [&](int c, float v) { out[c * oplane + od] = to_out<D>(v); });
+                      [&](int c, float v) { out[at(c)] = to_out<D>(v); });
             continue;
         }
         float vp[4], vq[4];
@@ -230,8 +235,8 @@ augment_kernel(const uint8_t* __restrict__ src, const int64_t* __restrict__ idx,
                 mp = inside ? vq[c] : vp[c];
                 mq = inside ? vp[c] : vq[c];
             }
-            out[c * oplane + od] = to_out<D>(mp);
-            out_q[c * oplane + od] = to_out<D>(mq);
+            out[at(c)] = to_out<D>(mp);
+            out_q[at(c)] = to_out<D>(mq);
         }
     }
 }
@@ -316,25 +321,25 @@ static AugArgs make_aug_args(int channels, int height, int width, uint64_t seed,
     return a;
 }
 
-template <int MIX>
+template <int MIX, bool NHWC>
 static void launch_augment(const dim3& grid, cudaStream_t st, const void* src, const int64_t* idx, const AugArgs& a,
                            const float* scale, const float* bias, void* dst, int dst_dtype, int32_t* params_out,
                            const MixArgs& mx) {
     const uint8_t* s = static_cast<const uint8_t*>(src);
     if (dst_dtype == FRL_F32)
-        augment_kernel<float, MIX><<<grid, kAugThreads, 0, st>>>(s, idx, a, scale, bias, static_cast<float*>(dst),
-                                                                 params_out, mx);
+        augment_kernel<float, MIX, NHWC><<<grid, kAugThreads, 0, st>>>(s, idx, a, scale, bias,
+                                                                       static_cast<float*>(dst), params_out, mx);
     else
-        augment_kernel<__nv_bfloat16, MIX><<<grid, kAugThreads, 0, st>>>(
+        augment_kernel<__nv_bfloat16, MIX, NHWC><<<grid, kAugThreads, 0, st>>>(
             s, idx, a, scale, bias, static_cast<__nv_bfloat16*>(dst), params_out, mx);
 }
 
-extern "C" int frl_augment_images(const void* src, int64_t batch, int channels, int height, int width,
-                                  const int64_t* idx, uint64_t seed, int epoch, int mode,
-                                  double smin, double smax, double rmin, double rmax, double eval_crop,
-                                  int pad, int flip, const float* scale, const float* bias, void* dst,
-                                  int dst_dtype, int out_h, int out_w, int32_t* params_out, void* stream) {
-    const char* name = "frl_augment_images";
+template <bool NHWC>
+static int augment_images(const char* name, const void* src, int64_t batch, int channels, int height, int width,
+                          const int64_t* idx, uint64_t seed, int epoch, int mode, double smin, double smax,
+                          double rmin, double rmax, double eval_crop, int pad, int flip, const float* scale,
+                          const float* bias, void* dst, int dst_dtype, int out_h, int out_w, int32_t* params_out,
+                          void* stream) {
     const int rc = check_augment_args(name, batch, channels, height, width, epoch, mode, smin, smax, rmin, rmax,
                                       eval_crop, pad, dst_dtype, out_h, out_w);
     if (rc) return rc;
@@ -344,18 +349,18 @@ extern "C" int frl_augment_images(const void* src, int64_t batch, int channels, 
     const AugArgs a = make_aug_args(channels, height, width, seed, epoch, mode, smin, smax, rmin, rmax, eval_crop,
                                     pad, flip, out_h, out_w);
     const dim3 grid(static_cast<unsigned>(batch), static_cast<unsigned>((out_h + kAugRows - 1) / kAugRows));
-    launch_augment<MIX_NONE>(grid, static_cast<cudaStream_t>(stream), src, idx, a, scale, bias, dst, dst_dtype,
-                             params_out, MixArgs{});
+    launch_augment<MIX_NONE, NHWC>(grid, static_cast<cudaStream_t>(stream), src, idx, a, scale, bias, dst,
+                                   dst_dtype, params_out, MixArgs{});
     return after_launch(name);
 }
 
-extern "C" int frl_augment_mix_images(const void* src, int64_t batch, int channels, int height, int width,
-                                      const int64_t* idx, uint64_t seed, int epoch, int mode,
-                                      double smin, double smax, double rmin, double rmax, double eval_crop,
-                                      int pad, int flip, const float* scale, const float* bias, void* dst,
-                                      int dst_dtype, int out_h, int out_w, int32_t* params_out, int mix_mode,
-                                      float lam, int box_y0, int box_y1, int box_x0, int box_x1, void* stream) {
-    const char* name = "frl_augment_mix_images";
+template <bool NHWC>
+static int augment_mix_images(const char* name, const void* src, int64_t batch, int channels, int height,
+                              int width, const int64_t* idx, uint64_t seed, int epoch, int mode, double smin,
+                              double smax, double rmin, double rmax, double eval_crop, int pad, int flip,
+                              const float* scale, const float* bias, void* dst, int dst_dtype, int out_h, int out_w,
+                              int32_t* params_out, int mix_mode, float lam, int box_y0, int box_y1, int box_x0,
+                              int box_x1, void* stream) {
     const int rc = check_augment_args(name, batch, channels, height, width, epoch, mode, smin, smax, rmin, rmax,
                                       eval_crop, pad, dst_dtype, out_h, out_w);
     if (rc) return rc;
@@ -377,11 +382,43 @@ extern "C" int frl_augment_mix_images(const void* src, int64_t batch, int channe
     const dim3 grid(static_cast<unsigned>((batch + 1) / 2), static_cast<unsigned>((out_h + kAugRows - 1) / kAugRows));
     cudaStream_t st = static_cast<cudaStream_t>(stream);
     if (mix_mode == FRL_MIX_MIXUP)
-        launch_augment<MIX_MIXUP>(grid, st, src, idx, a, scale, bias, dst, dst_dtype, params_out, mx);
+        launch_augment<MIX_MIXUP, NHWC>(grid, st, src, idx, a, scale, bias, dst, dst_dtype, params_out, mx);
     else
-        launch_augment<MIX_CUTMIX>(grid, st, src, idx, a, scale, bias, dst, dst_dtype, params_out, mx);
+        launch_augment<MIX_CUTMIX, NHWC>(grid, st, src, idx, a, scale, bias, dst, dst_dtype, params_out, mx);
     return after_launch(name);
 }
+
+#define FRL_AUG_ARGS_DECL                                                                                       \
+    const void *src, int64_t batch, int channels, int height, int width, const int64_t *idx, uint64_t seed,     \
+        int epoch, int mode, double smin, double smax, double rmin, double rmax, double eval_crop, int pad,     \
+        int flip, const float *scale, const float *bias, void *dst, int dst_dtype, int out_h, int out_w,        \
+        int32_t *params_out
+#define FRL_AUG_ARGS                                                                                            \
+    src, batch, channels, height, width, idx, seed, epoch, mode, smin, smax, rmin, rmax, eval_crop, pad, flip,  \
+        scale, bias, dst, dst_dtype, out_h, out_w, params_out
+
+extern "C" int frl_augment_images(FRL_AUG_ARGS_DECL, void* stream) {
+    return augment_images<false>("frl_augment_images", FRL_AUG_ARGS, stream);
+}
+
+extern "C" int frl_augment_images_nhwc(FRL_AUG_ARGS_DECL, void* stream) {
+    return augment_images<true>("frl_augment_images_nhwc", FRL_AUG_ARGS, stream);
+}
+
+extern "C" int frl_augment_mix_images(FRL_AUG_ARGS_DECL, int mix_mode, float lam, int box_y0, int box_y1,
+                                      int box_x0, int box_x1, void* stream) {
+    return augment_mix_images<false>("frl_augment_mix_images", FRL_AUG_ARGS, mix_mode, lam, box_y0, box_y1,
+                                     box_x0, box_x1, stream);
+}
+
+extern "C" int frl_augment_mix_images_nhwc(FRL_AUG_ARGS_DECL, int mix_mode, float lam, int box_y0, int box_y1,
+                                           int box_x0, int box_x1, void* stream) {
+    return augment_mix_images<true>("frl_augment_mix_images_nhwc", FRL_AUG_ARGS, mix_mode, lam, box_y0, box_y1,
+                                    box_x0, box_x1, stream);
+}
+
+#undef FRL_AUG_ARGS
+#undef FRL_AUG_ARGS_DECL
 
 extern "C" int frl_mix_targets(const void* src, int src_dtype, int64_t batch, int64_t inner, int n_classes,
                                float lam, void* dst, void* stream) {

@@ -126,7 +126,7 @@ class WeightEMA:
         names = {id(p): name for name, p in self.module.named_parameters()}
         for s in self.arena.slots:
             if s.is_model:
-                self.ema[s.offset:s.end].copy_(sd[names[id(s.param)]].reshape(-1))
+                ParamArena.slot_view(self.ema, s).copy_(sd[names[id(s.param)]])
         for name, _, e in self.buffers:
             e.copy_(sd[name])
         self.updates = int(blob["updates"])

@@ -223,7 +223,8 @@ class FusedArenaOptimizer(torch.optim.Optimizer):
                 entry = dict(self._per_param_extra())
                 for torch_name, vec_name in self.STATE_NAMES:
                     if vec_name in self._vec:
-                        entry[torch_name] = self._vec[vec_name][s.offset:s.end].view(s.shape).clone()
+                        entry[torch_name] = ParamArena.slot_view(self._vec[vec_name], s).clone(
+                            memory_format=torch.contiguous_format)
                 state[s.index] = entry
         groups = []
         for g in self.param_groups:
@@ -247,7 +248,7 @@ class FusedArenaOptimizer(torch.optim.Optimizer):
                 continue
             for torch_name, vec_name in self.STATE_NAMES:
                 if torch_name in entry and entry[torch_name] is not None:
-                    self._state(vec_name)[s.offset:s.end].view(s.shape).copy_(entry[torch_name])
+                    ParamArena.slot_view(self._state(vec_name), s).copy_(entry[torch_name])
             if "step" in entry:
                 steps = max(steps, int(float(entry["step"])))
             elif entry:
@@ -962,7 +963,8 @@ class FusedMuon(_WholeTensorMixin, FusedAdam):
         pos = self._positions()
         if self._steps > 0:
             for s in sorted(self.arena.slots, key=lambda s: pos[id(s.param)]):
-                view = lambda name: self._state(name)[s.offset:s.end].view(s.shape).clone()
+                view = lambda name: ParamArena.slot_view(self._state(name), s).clone(
+                    memory_format=torch.contiguous_format)
                 if is_muon_slot(s):
                     state[pos[id(s.param)]] = {"momentum_buffer": view("exp_avg")}
                 else:
@@ -1004,7 +1006,7 @@ class FusedMuon(_WholeTensorMixin, FusedAdam):
                      (("exp_avg", "exp_avg"), ("exp_avg_sq", "exp_avg_sq")))
             for torch_name, vec in names:
                 if entry.get(torch_name) is not None:
-                    self._state(vec)[s.offset:s.end].view(s.shape).copy_(entry[torch_name])
+                    ParamArena.slot_view(self._state(vec), s).copy_(entry[torch_name])
             if "step" in entry:
                 steps = max(steps, int(float(entry["step"])))
             elif entry:

@@ -131,7 +131,7 @@ class _Captured:
     def _fill(self, data, target) -> None:
         for dst, src, cast in zip(self.static_in, data, self.cast_in):
             if cast:
-                _native.cast_scale(src.contiguous(), dst, 1.0)
+                _native.cast_scale(src if _native.is_nhwc(src) else src.contiguous(), dst, 1.0)
             else:
                 dst.copy_(src, non_blocking=True)
         for dhead, shead in zip(self.static_tgt, target):

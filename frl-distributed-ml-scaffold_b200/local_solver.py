@@ -26,7 +26,8 @@ class LocalSolver:
               optimizer_state: Optional[OptimizerState] = None,
               adafactor: Optional[bool] = None,
               muon: Optional[bool] = None,
-              adamw: Optional[bool] = None) -> PerformanceSummary:
+              adamw: Optional[bool] = None,
+              channels_last: Optional[bool] = None) -> PerformanceSummary:
         if save_notebook:
             logger.warning("save_notebook is not supported by frl_b200 (visualisation only)")
         # a stale rendezvous file from a crashed run would poison the file:// store
@@ -41,6 +42,6 @@ class LocalSolver:
                                  graph=graph, layer_adaptation=layer_adaptation,
                                  grad_accumulation=grad_accumulation, ema_decay=ema_decay,
                                  optimizer_state=optimizer_state, adafactor=adafactor, muon=muon,
-                                 adamw=adamw):
+                                 adamw=adamw, channels_last=channels_last):
             pass
         return last

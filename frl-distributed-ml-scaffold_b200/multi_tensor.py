@@ -18,12 +18,25 @@ from . import _native
 _SEG_BYTES = C.sizeof(_native.GradSeg)
 
 
+def same_element_order(t: torch.Tensor, slot) -> bool:
+    """Does dense ``t`` (of the slot's shape) list its elements in the slot's arena order?  Strides
+    are compared on the dimensions of size > 1 only: a size-1 dimension's stride is arbitrary (a
+    1x1 convolution's weight, or one with one input channel, has the same element order
+    contiguous and channels_last)."""
+    if slot.memory_format is torch.contiguous_format:
+        return t.is_contiguous()
+    if tuple(t.shape) != tuple(slot.shape):
+        return False
+    return all(a == b for n, a, b in zip(t.shape, t.stride(), slot.strides) if n > 1)
+
+
 def grad_usable_in_place(g: torch.Tensor, slot) -> bool:
-    """Can the kernels read ``g`` where it is?  Dense, in the parameter's own (contiguous)
-    layout, fp32 or bf16, 16-byte aligned — what cuDNN / cuBLAS / the normalisation kernels hand
-    to autograd.  Anything else (channels_last weight gradients, sparse, fp16, odd views) is
-    copied into the arena slice by the caller instead."""
-    return (g.is_cuda and g.layout == torch.strided and g.is_contiguous()
+    """Can the kernels read ``g`` where it is?  Dense, in the slot's element order (contiguous, or
+    channels_last for a channels_last slot: cuDNN's NHWC weight gradients), fp32 or bf16, 16-byte
+    aligned — what cuDNN / cuBLAS / the normalisation kernels hand to autograd.  Anything else
+    (sparse, fp16, odd views, a layout other than the slot's) is copied into the arena slice by
+    the caller instead."""
+    return (g.is_cuda and g.layout == torch.strided and same_element_order(g, slot)
             and g.dtype in (torch.float32, torch.bfloat16) and g.numel() == slot.numel
             and g.data_ptr() % 16 == 0)
 

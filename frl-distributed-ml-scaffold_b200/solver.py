@@ -51,6 +51,7 @@ OPTIMIZER_STATE_ENV = "FRL_B200_OPTIMIZER_STATE"   # "fp32" (default) | "8bit"
 ADAFACTOR_ENV = "FRL_B200_ADAFACTOR"               # "0" (default) | "1"
 MUON_ENV = "FRL_B200_MUON"                         # "0" (default) | "1"
 ADAMW_ENV = "FRL_B200_ADAMW"                       # "0" (default) | "1"
+CHANNELS_LAST_ENV = "FRL_B200_CHANNELS_LAST"       # "0" (default) | "1"
 EMA_SUFFIX = ".ema"                        # <checkpoint>.ema: the weight EMA next to a checkpoint
 
 
@@ -111,6 +112,10 @@ class SolverWorkerArgs(NamedTuple):
     # AdamW (decoupled weight decay) in every Adam update; placed before optimizer_state, adafactor,
     # ema_decay and grad_accumulation, which keep their positions at the end
     adamw: bool = False
+    # channels_last conv weights and NHWC image batches; None: FRL_B200_CHANNELS_LAST (default off).
+    # Placed before optimizer_state, adafactor, ema_decay and grad_accumulation, which keep their
+    # positions at the end
+    channels_last: Optional[bool] = None
     # Adam's state storage; placed before ema_decay and grad_accumulation, which stay the last fields
     optimizer_state: OptimizerState = OptimizerState.FP32
     # Adafactor instead of Adam; placed before ema_decay and grad_accumulation, which stay the last fields
@@ -306,6 +311,25 @@ def resolve_adamw(explicit: Optional[bool] = None) -> bool:
     return raw == "1"
 
 
+def resolve_channels_last(explicit: Optional[bool] = None) -> bool:
+    """Whether conv weights and image batches are channels_last: ``explicit``, else
+    FRL_B200_CHANNELS_LAST (``0``, the default, or ``1``).  Any other value is a ValueError."""
+    if explicit is not None:
+        return bool(explicit)
+    raw = os.environ.get(CHANNELS_LAST_ENV, "0").strip()
+    if raw not in ("0", "1"):
+        raise ValueError("%s must be 0 or 1, got %r" % (CHANNELS_LAST_ENV, raw))
+    return raw == "1"
+
+
+def check_channels_last(channels_last: bool, adafactor: bool) -> None:
+    """Adafactor factors a conv weight's second moment per kh x kw slice of [O*I, kh, kw], which
+    assumes NCHW element order: the two cannot be combined (ValueError)."""
+    if channels_last and adafactor:
+        raise ValueError("adafactor cannot be combined with channels_last: Adafactor's factored second "
+                         "moment assumes NCHW element order of the conv weights")
+
+
 def resolve_grad_accumulation(explicit: Optional[int] = None) -> int:
     """Microbatches per optimizer update: ``explicit``, else FRL_B200_GRAD_ACCUM, else 1.  Anything
     but an integer >= 1 (``0``, negatives, ``2.5``, ``True``, non-numeric strings) is a ValueError."""
@@ -427,9 +451,11 @@ class Solver:
             from .symm import try_make_allocator
             symm_alloc = try_make_allocator(device, args.world_size)
         from .arena_linear import head_layout_groups
+        channels_last = resolve_channels_last(args.channels_last)
+        check_channels_last(channels_last, args.adafactor and run_opts.mode == Mode.TRAIN)
         arena = ParamArena(model.parameters(), criterion.parameters(), device=device,
                            precision=args.precision, shared_allocator=symm_alloc,
-                           adjacent=head_layout_groups(model))
+                           adjacent=head_layout_groups(model), channels_last=channels_last)
         if (args.precision.bf16_storage and any(b.is_floating_point() for b in model.buffers())
                 and not _norm_accepts_fp32_stats(device)):
             # BatchNorm running statistics stay fp32 (what the reference's checkpoints hold: a
@@ -496,7 +522,7 @@ class Solver:
                               serialize_state=(args.local_rank == 0),
                               graph_step=(args.graph_step if args.graph_step is not None
                                           else os.environ.get("FRL_B200_CUDA_GRAPH", "0") == "1"),
-                              ema=ema)
+                              ema=ema, channels_last=channels_last)
         worker.save_every = args.save_every
         if args.rank == 0:
             # one line per run: which of the alternative paths this configuration took
@@ -505,7 +531,7 @@ class Solver:
                 "Linear layers with arena-born gradients %d (%d fused with their ReLU, %d in FP8) | "
                 "ReLU backward %s | "
                 "other gradients %s | layer adaptation %s | gradient accumulation %s | weight EMA %s | "
-                "optimizer %s | optimizer state %s",
+                "optimizer %s | optimizer state %s | memory format %s",
                 args.precision.value,
                 "CUDA-graph replay after 2 eager steps" if worker.graphed is not None else "eager launches",
                 ("fused NVLS kernel per bucket (K7), %d buckets" % len(pipeline.buckets)) if pipeline.nvls is not None
@@ -547,7 +573,14 @@ class Solver:
                 "muon (K14) on %d of %d tensors (%d params), adam (K2-mt) on the rest, NS workspace %.1f MiB" % (
                     len(optimizer.muon_params), len(arena.slots),
                     sum(p.numel() for p in optimizer.muon_params), optimizer.workspace_bytes / 2 ** 20)
-                if isinstance(optimizer, FusedMuon) else "fp32")
+                if isinstance(optimizer, FusedMuon) else "fp32",
+                "contiguous" if not channels_last else
+                "channels_last: %d of %d conv weights (%d params), %s" % (
+                    arena.n_channels_last, sum(len(s.shape) == 4 for s in arena.slots),
+                    sum(s.numel for s in arena.slots if s.memory_format is torch.channels_last),
+                    "batches NHWC from K5/K5a" if all(
+                        getattr(getattr(d, "device_transform", None), "honours_memory_format", False)
+                        for d in problem.datasets) else "converted by the first convolution"))
         scheduler = create_lr_scheduler(run_opts, worker.optimizer,
                                         checkpoint.epoch if checkpoint else -1)
         return worker, scheduler, checkpoint
@@ -761,7 +794,8 @@ class Solver:
               optimizer_state: Optional[OptimizerState] = None,
               adafactor: Optional[bool] = None,
               muon: Optional[bool] = None,
-              adamw: Optional[bool] = None
+              adamw: Optional[bool] = None,
+              channels_last: Optional[bool] = None
               ) -> Iterator[PerformanceSummary]:
         """The reference's entry point (solver.py:728-739) plus two keyword-only extensions:
 
@@ -870,6 +904,20 @@ class Solver:
                        before a rank starts.  Checkpoints keep ``torch.optim.AdamW``'s format and
                        ``torch.optim.Adam`` / ``AdamW`` state dicts resume.  None: FRL_B200_ADAMW
                        (``0`` by default, ``1`` to enable).  ``Mode.EVAL`` ignores it.
+        ``channels_last``  True: every trainable 4-D parameter (Conv2d weights) is laid out in
+                       channels_last element order (O, kh, kw, I) in the arena, and ``param.data``
+                       is its slice with channels_last strides; master and bf16 weights, gradients,
+                       optimizer state, the EMA and the accumulator follow.  cuDNN's NHWC weight
+                       gradients are read in place.  Image batches of ``DeviceImageAugment`` and the
+                       synthetic channel-affine transform come out channels_last (K5 / K5a NHWC);
+                       other inputs are converted by the first convolution.  Checkpoints, state
+                       dicts and ``<stem>.ema`` hold contiguous tensors, so files move between NCHW
+                       and NHWC runs and ``torch.optim`` in every direction.  8-bit state blocks are
+                       256 consecutive arena elements, so they group a conv weight's elements
+                       differently than in an NCHW run; LARS / LAMB norms sum in another order.
+                       Not combinable with Adafactor (``ValueError`` before a rank starts).  Honoured
+                       by ``Mode.EVAL``.  None: FRL_B200_CHANNELS_LAST (``0`` by default, ``1`` to
+                       enable); any other value raises ``ValueError``.
         """
         adapt = LayerAdaptation.NONE
         accum = 1
@@ -891,6 +939,8 @@ class Solver:
             check_adamw(run_opts.optim, adapt, opt_state, use_adafactor, use_adamw)
             accum = resolve_grad_accumulation(grad_accumulation)
             decay = resolve_ema_decay(ema_decay)
+        use_channels_last = resolve_channels_last(channels_last)
+        check_channels_last(use_channels_last, use_adafactor)
         n_visible = 0 if run_opts.cpuonly else _cuda_device_count_without_poisoning_fork()
         if n_visible == 0:
             raise RuntimeError(
@@ -930,7 +980,8 @@ class Solver:
                 world_size=world_size, group_name=group_name, init_method=init_method,
                 cache=None, precision=prec, save_every=save_every, graph_step=graph,
                 layer_adaptation=adapt, grad_accumulation=accum, ema_decay=decay,
-                optimizer_state=opt_state, adafactor=use_adafactor, muon=use_muon, adamw=use_adamw)
+                optimizer_state=opt_state, adafactor=use_adafactor, muon=use_muon, adamw=use_adamw,
+                channels_last=use_channels_last)
             if not run_opts.singleThreaded:
                 parent_conn, child_conn = ctx.Pipe(duplex=False)
                 proc = ctx.Process(target=cls._solver_worker_process,

@@ -309,7 +309,12 @@ class SamplerState:
         does not know ``idx`` (it comes out of a device ``topk``) and the minibatches are separate
         tensors: K8w (``frl_gather_window_rows``) walks a table of their base pointers — one launch,
         only the picked rows move (concatenating the window first was a 0.3 GB device copy per
-        amortisation window at batch 4096 x 4096 bf16, twice: random picks and worst-k)."""
+        amortisation window at batch 4096 x 4096 bf16, twice: random picks and worst-k).
+        channels_last [B, C, H, W] batches are gathered as the [B, H, W, C] rows they store (each
+        sample is contiguous in NHWC too); the rows come back channels_last [k, C, H, W]."""
+        if batches[0].is_cuda and all(_native.is_nhwc(b) for b in batches):
+            rows = _native.gather_window_rows([b.permute(0, 2, 3, 1) for b in batches], idx)
+            return rows.permute(0, 3, 1, 2)
         if batches[0].is_cuda:
             return _native.gather_window_rows([b if b.is_contiguous() else b.contiguous() for b in batches], idx)
         return (batches[0] if len(batches) == 1 else torch.cat(batches)).index_select(0, idx)
@@ -576,7 +581,8 @@ class SolverWorker:
                  pipeline: Optional[GradBucketPipeline] = None,
                  buffers: Optional[BufferBroadcaster] = None,
                  precision: Precision = Precision.FP32,
-                 serialize_state: bool = True, graph_step: bool = False, ema=None) -> None:
+                 serialize_state: bool = True, graph_step: bool = False, ema=None,
+                 channels_last: bool = False) -> None:
         self.model = model
         self.criterion = criterion
         self.optimizer = optimizer
@@ -589,6 +595,7 @@ class SolverWorker:
             self.arena, optimizer, clip_norm=run_opts.optim.gradientClip)
         self.buffers = buffers
         self.ema = ema                 # ema.WeightEMA: held-out splits of a TRAIN run evaluate with it
+        self.channels_last = channels_last       # True: device transforms are asked for NHWC batches
         self.cur_epoch = 0
         self._node_idx = node_idx
         self._node_count = node_count
@@ -812,7 +819,8 @@ class SolverWorker:
         for t in data:
             if t.is_cuda and t.dtype == torch.float32:
                 lp = torch.empty_like(t, dtype=torch.bfloat16)
-                _native.cast_scale(t.contiguous(), lp, 1.0)
+                # in the tensor's own storage order: a channels_last batch stays channels_last
+                _native.cast_scale(t if _native.is_nhwc(t) else t.contiguous(), lp, 1.0)
                 out.append(lp)
             else:
                 out.append(t)
@@ -1001,6 +1009,8 @@ class SolverWorker:
             if self.device.type == "cuda" and supports_device_batches(dataset):
                 # raw dataset in pinned host memory: rows pulled by the GPU, transform on device
                 out_dtype = torch.bfloat16 if self.precision.bf16_storage else torch.float32
+                if self.channels_last:
+                    dataset.device_transform.memory_format = torch.channels_last
                 loaders[split] = DeviceBatchLoader(dataset, batch_size=batchSize, sampler=sampler,
                                                    device=self.device, out_dtype=out_dtype)
                 ld = loaders[split]

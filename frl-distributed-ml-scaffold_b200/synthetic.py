@@ -112,12 +112,15 @@ def _affine_device_transform(shift: float, scale: float, target_fields):
 
 def _channel_affine_device_transform(scale, bias, target_fields):
     """Batched twin of ``ChannelAffineTransform``: raw images [B, C, H, W] (uint8 or float) ->
-    x * scale[c] + bias[c] in ``out_dtype``, one ``frl_preproc_affine`` pass (K5)."""
+    x * scale[c] + bias[c] in ``out_dtype``, one ``frl_preproc_affine`` pass (K5); channels_last
+    images (``memory_format``, 1 to 4 channels) from one ``frl_preproc_affine_nhwc`` pass."""
     import torch
     from . import _native
     from .transform import DeviceBatchTransform
 
     class ChannelAffineDeviceTransform(DeviceBatchTransform):
+        honours_memory_format = True
+
         def __init__(self) -> None:
             self.scale, self.bias = [float(v) for v in scale], [float(v) for v in bias]
             self.target_fields = list(target_fields)
@@ -125,13 +128,18 @@ def _channel_affine_device_transform(scale, bias, target_fields):
 
         def apply(self, raw, split, out_dtype):
             x = raw["x"]
-            out = torch.empty(x.shape, dtype=out_dtype, device=x.device)
+            nhwc = self.memory_format is torch.channels_last and x.dim() == 4 and x.shape[1] <= 4
+            out = torch.empty(x.shape, dtype=out_dtype, device=x.device,
+                              memory_format=torch.channels_last if nhwc else torch.contiguous_format)
             if x.device not in self._coef:
                 self._coef[x.device] = (torch.tensor(self.scale, device=x.device),
                                         torch.tensor(self.bias, device=x.device))
             sc, bi = self._coef[x.device]
-            inner = max(x[0, 0].numel(), 1)
-            _native.preproc_affine(x, out, inner=inner, channels=x.shape[1], scale=sc, bias=bi)
+            if _native.is_nhwc(out):
+                _native.preproc_affine_nhwc(x, out, scale=sc, bias=bi)
+            else:
+                inner = max(x[0, 0].numel(), 1)
+                _native.preproc_affine(x, out, inner=inner, channels=x.shape[1], scale=sc, bias=bi)
             return [out], [(raw[f],) for f in self.target_fields]
 
     return ChannelAffineDeviceTransform()

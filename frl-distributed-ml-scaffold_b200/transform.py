@@ -13,6 +13,7 @@ from abc import ABC, abstractmethod
 from typing import Any, Dict, Generic, List, NamedTuple, Optional, Sequence, Tuple, TypeVar, Union
 
 import numpy as np
+import torch
 from torch import Tensor
 
 from .types import Split
@@ -57,6 +58,13 @@ class DeviceBatchTransform(ABC):
     #: True: ``apply`` is also given ``index=`` (device int64 [B], the dataset row of each sample),
     #: e.g. to key per-sample random draws to the sample rather than to its place in the batch.
     needs_index: bool = False
+
+    #: the layout image batches should come out in; the loop sets ``torch.channels_last`` when the
+    #: run is channels_last (``Solver.solve(..., channels_last=True)``).  A transform that writes
+    #: 4-D image fields in that layout says so with ``honours_memory_format = True``; any other
+    #: keeps returning what it did, and the first convolution converts.
+    memory_format: torch.memory_format = torch.contiguous_format
+    honours_memory_format: bool = False
 
     @abstractmethod
     def apply(self, raw: Dict[str, Tensor], split: Split, out_dtype
@@ -165,9 +173,13 @@ class DeviceImageAugment(DeviceBatchTransform):
     (``frl_augment_mix_images``) and their targets by ``frl_mix_targets``.  Its draws are keyed by
     (``seed``, epoch, rank, the batch's ordinal since ``set_epoch``).  Evaluation splits are not
     mixed and keep their targets as they are.
+    With ``memory_format = torch.channels_last`` the images come out [B, C, out_h, out_w] with
+    channels_last strides (``frl_augment_images_nhwc`` / ``frl_augment_mix_images_nhwc``), the same
+    values as the NCHW output.
     """
 
     needs_index = True
+    honours_memory_format = True
     MODES = ("rrc", "pad_crop")
 
     def __init__(self, image_field: str, target_fields: Sequence[str], *, mode: str = "rrc",
@@ -261,23 +273,26 @@ class DeviceImageAugment(DeviceBatchTransform):
                     ratio_range=self.crop_ratio, eval_crop=self.eval_crop, pad=self.pad, flip=self.flip, scale=sc,
                     bias=bi, params_out=params_out)
 
+    def _out(self, x: Tensor, out_dtype) -> Tensor:
+        return torch.empty((x.shape[0], x.shape[1]) + self.out_size, dtype=out_dtype, device=x.device,
+                           memory_format=self.memory_format)
+
     def augment(self, x: Tensor, index: Tensor, split: Split, out_dtype, params_out=None) -> Tensor:
-        """The normalised, augmented images [B, C, out_h, out_w] of ``out_dtype``."""
-        import torch
+        """The normalised, augmented images [B, C, out_h, out_w] of ``out_dtype``, in
+        ``memory_format``."""
         from . import _native
         sc, bi = self._coefs(x)
-        out = torch.empty((x.shape[0], x.shape[1]) + self.out_size, dtype=out_dtype, device=x.device)
+        out = self._out(x, out_dtype)
         _native.augment_images(x.contiguous(), index, out, **self._native_args(split, sc, bi, params_out))
         return out
 
     def augment_mixed(self, x: Tensor, index: Tensor, out_dtype, mode: int, lam: float, box,
                       params_out=None) -> Tensor:
         """Training images [B, C, out_h, out_w] with sample i mixed with sample B-1-i (``mode``
-        ``BatchMix.MIXUP`` or ``CUTMIX``) in the augmentation pass."""
-        import torch
+        ``BatchMix.MIXUP`` or ``CUTMIX``) in the augmentation pass, in ``memory_format``."""
         from . import _native
         sc, bi = self._coefs(x)
-        out = torch.empty((x.shape[0], x.shape[1]) + self.out_size, dtype=out_dtype, device=x.device)
+        out = self._out(x, out_dtype)
         _native.augment_mix_images(x.contiguous(), index, out, mix_mode=mode, lam=lam, box=box,
                                    **self._native_args(Split.TRAIN, sc, bi, params_out))
         return out

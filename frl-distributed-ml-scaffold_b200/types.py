@@ -131,6 +131,9 @@ class OptimizerState(Enum):
            ``LayerAdaptation.NONE``.  The state dict is ``torch.optim.Adam``'s with decoded fp32
            moments.  Gradients are all-reduced per bucket and the update runs once after backward:
            no eager per-bucket update and no fused NVLS step.  ``Mode.EVAL`` ignores the setting.
+           With ``channels_last=True`` a block is 256 consecutive elements of the conv weight's
+           (O, kh, kw, I) order, so its elements, absmax and codes differ from an NCHW run's; the
+           state dict is still torch's, and loads in either layout re-encode it.
     """
     FP32 = "fp32"
     Q8 = "8bit"

@@ -490,6 +490,14 @@ int frl_preproc_affine(const void* src, int src_dtype, void* dst, int dst_dtype,
                        int64_t inner, int64_t channels, const float* scale, const float* bias,
                        void* stream);
 
+/* K5 into channels_last: src [batch, channels, hw] contiguous (an image batch [B, C, H, W],
+ * hw = H * W, 1 <= channels <= 4; u8 / f32 / bf16) -> dst [batch, hw, channels] in memory (the
+ * NHWC storage of a channels_last [B, C, H, W] tensor; f32 / bf16).  Values are frl_preproc_affine's
+ * with inner = hw bit for bit: dst = fmaf(src, scale[c], bias[c]) (a NULL scale is 1, a NULL bias
+ * 0), or src * 1 when both are NULL.  src and dst 16-byte aligned. */
+int frl_preproc_affine_nhwc(const void* src, int src_dtype, void* dst, int dst_dtype, int64_t batch,
+                            int channels, int64_t hw, const float* scale, const float* bias, void* stream);
+
 /* ------------------------------------------------------------------------------------------
  * K5a — on-device image augmentation: crop box + bilinear resize + horizontal flip + per-channel
  * affine in one pass (an extension: the reference's Problems augment per sample on the host,
@@ -534,6 +542,13 @@ int frl_augment_images(const void* src, int64_t batch, int channels, int height,
                        double smin, double smax, double rmin, double rmax, double eval_crop, int pad,
                        int flip, const float* scale, const float* bias, void* dst, int dst_dtype,
                        int out_h, int out_w, int32_t* params_out, void* stream);
+/* frl_augment_images with dst in [B, out_h, out_w, C] memory order (the NHWC storage of a
+ * channels_last [B, C, out_h, out_w] tensor): the same values, permuted. */
+int frl_augment_images_nhwc(const void* src, int64_t batch, int channels, int height, int width,
+                            const int64_t* idx, uint64_t seed, int epoch, int mode,
+                            double smin, double smax, double rmin, double rmax, double eval_crop, int pad,
+                            int flip, const float* scale, const float* bias, void* dst, int dst_dtype,
+                            int out_h, int out_w, int32_t* params_out, void* stream);
 
 /* K5a with Mixup / CutMix in the same pass (an extension: the usual large-batch ImageNet recipe,
  * Zhang et al. 2018 / Yun et al. 2019).  Arguments as frl_augment_images, plus
@@ -564,6 +579,13 @@ int frl_augment_mix_images(const void* src, int64_t batch, int channels, int hei
                            int flip, const float* scale, const float* bias, void* dst, int dst_dtype,
                            int out_h, int out_w, int32_t* params_out, int mix_mode, float lam,
                            int box_y0, int box_y1, int box_x0, int box_x1, void* stream);
+/* frl_augment_mix_images with dst in [B, out_h, out_w, C] memory order: the same values, permuted. */
+int frl_augment_mix_images_nhwc(const void* src, int64_t batch, int channels, int height, int width,
+                                const int64_t* idx, uint64_t seed, int epoch, int mode,
+                                double smin, double smax, double rmin, double rmax, double eval_crop, int pad,
+                                int flip, const float* scale, const float* bias, void* dst, int dst_dtype,
+                                int out_h, int out_w, int32_t* params_out, int mix_mode, float lam,
+                                int box_y0, int box_y1, int box_x0, int box_x1, void* stream);
 int frl_mix_targets(const void* src, int src_dtype, int64_t batch, int64_t inner, int n_classes, float lam,
                     void* dst, void* stream);
 

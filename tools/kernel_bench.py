@@ -1,7 +1,7 @@
 #!/usr/bin/env python
 """Micro-benchmark of every hand-written kernel at the BASELINE shapes (1 GPU).
 
-    python tools/kernel_bench.py [--only k2,k2lw,k2q8,k2af,k2w,k3,k5a,k13,k14,...] [--iters 20] [--json out.json]
+    python tools/kernel_bench.py [--only k2,k2lw,k2q8,k2af,k2w,k3,k5a,k5nhwc,k13,k14,...] [--iters 20] [--json out.json]
 
 Each kernel is timed with CUDA events on the launching stream over ROTATING operand sets whose
 total size exceeds the 50 MB L2 (so every launch streams from HBM), after 3 warm-up launches.
@@ -842,10 +842,54 @@ def bench_k14(iters):
     return out
 
 
+def bench_k5nhwc(iters):
+    """K5 and K5a into channels_last against their NCHW forms, alternating, same sets: K5 u8 ->
+    bf16 [256, 3, 224, 224] per channel, and K5a RRC u8 [256, 3, 256, 256] -> bf16 [256, 3, 224, 224]
+    (bytes as bench_k5a).  Every form is timed from a CUDA graph over rotating L2-cold sets."""
+    B, Cc, H = 256, 3, 224
+    n = B * Cc * H * H
+    ns = sets_for(n * 3)
+    src = [torch.randint(0, 256, (B, Cc, H, H), device=DEV, dtype=torch.uint8) for _ in range(ns)]
+    fmt = {"NCHW": torch.contiguous_format, "NHWC": torch.channels_last}
+    dst = {k: [torch.empty(B, Cc, H, H, device=DEV, dtype=torch.bfloat16, memory_format=f) for _ in range(ns)]
+           for k, f in fmt.items()}
+    sc, bi = torch.rand(Cc, device=DEV), torch.rand(Cc, device=DEV)
+    k5 = {"NCHW": lambda i: _native.preproc_affine(src[i], dst["NCHW"][i], inner=H * H, channels=Cc, scale=sc, bias=bi),
+          "NHWC": lambda i: _native.preproc_affine_nhwc(src[i], dst["NHWC"][i], scale=sc, bias=bi)}
+    out = []
+    for rep in range(2):
+        for k in ("NCHW", "NHWC"):
+            out.append(timed("K5 preproc_affine%s u8->bf16 [256,3,224,224] per-channel, %s out (round %d)"
+                             % ("_nhwc" if k == "NHWC" else "", k, rep), k5[k], ns, n * 3, iters, graph=True))
+    del src, dst
+    S, O = 256, 224
+    ns = sets_for(B * Cc * (S * S + 2 * O * O))
+    src = [torch.randint(0, 256, (B, Cc, S, S), device=DEV, dtype=torch.uint8) for _ in range(ns)]
+    dst = {k: [torch.empty(B, Cc, O, O, device=DEV, dtype=torch.bfloat16, memory_format=f) for _ in range(ns)]
+           for k, f in fmt.items()}
+    idx = [torch.arange(B, device=DEV, dtype=torch.int64) + i * B for i in range(ns)]
+    params = torch.empty(B, 5, dtype=torch.int32, device=DEV)
+    read = 0
+    for i in range(ns):
+        _native.augment_images(src[i], idx[i], dst["NCHW"][i], seed=0, epoch=1, mode=_native.AUG_RRC, scale=sc,
+                               bias=bi, params_out=params)
+        read += sum(Cc * _taps_touched(int(h), O) * _taps_touched(int(w), O) for h, w in params[:, 2:4].tolist())
+    nbytes = read // ns + B * Cc * O * O * 2
+    kw = dict(seed=0, epoch=1, mode=_native.AUG_RRC, scale=sc, bias=bi)
+    for rep in range(2):
+        for k in ("NCHW", "NHWC"):
+            out.append(timed("K5a augment_images%s RRC u8 [256,3,256,256] -> bf16 [256,3,224,224] %s (round %d)"
+                             % ("_nhwc" if k == "NHWC" else "", k, rep),
+                             lambda i, k=k: _native.augment_images(src[i], idx[i], dst[k][i], **kw), ns, nbytes,
+                             iters, "bytes: touched source lines of the drawn boxes + output", graph=True))
+    return out
+
+
 BENCHES = {"k2": bench_k2, "k2mt": bench_k2mt, "k2lw": bench_k2lw, "k3": bench_k3, "k4": bench_k4, "k5": bench_k5, "k5a": bench_k5a,
            "k5m": bench_k5m, "k4s": bench_k4s, "k6": bench_k6,
            "k8": bench_k8, "k8t": bench_k8t, "k9": bench_k9, "k10": bench_k10, "k11": bench_k11,
-           "k2q8": bench_k2q8, "k2af": bench_k2af, "k13": bench_k13, "k14": bench_k14, "k2w": bench_k2w}
+           "k2q8": bench_k2q8, "k2af": bench_k2af, "k13": bench_k13, "k14": bench_k14, "k2w": bench_k2w,
+           "k5nhwc": bench_k5nhwc}
 
 
 def main():
