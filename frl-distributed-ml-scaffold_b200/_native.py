@@ -47,6 +47,7 @@ class GradSeg(C.Structure):
 
 # name -> (restype, argtypes); every name here must be declared in include/frl_b200.h
 _vp, _i, _i64, _f, _d = C.c_void_p, C.c_int, C.c_int64, C.c_float, C.c_double
+_u64 = C.c_uint64
 SIGNATURES = {
     "frl_abi_version": (_i, []),
     "frl_last_error": (C.c_char_p, []),
@@ -61,6 +62,8 @@ SIGNATURES = {
     "frl_dw_gemm": (_i, [_vp, _i64, _vp, _i64, _i64, _i64, _i64, _vp, _vp]),
     "frl_dw_gemm_sgd": (_i, [_vp, _i64, _vp, _i64, _i64, _i64, _i64, _vp, _vp, _vp, _vp, _d, _d, _d, _d, _d,
                              _vp, _i, _vp]),
+    "frl_dw_gemm_sgd_sr": (_i, [_vp, _i64, _vp, _i64, _i64, _i64, _i64, _vp, _vp, _vp, _i64, _u64, _i64, _d, _d,
+                                _d, _d, _d, _vp, _i, _vp]),
     "frl_dx_drelu_scratch_bytes": (_i64, [_i64, _i64]),
     "frl_dx_gemm_drelu": (_i, [_vp, _i64, _vp, _i64, _vp, _i64, _vp, _i64, _vp, _i64, _i64, _i64, _i, _vp, _vp]),
     "frl_mt_tile_elems": (_i64, []),
@@ -69,6 +72,19 @@ SIGNATURES = {
     "frl_adam_mt": (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _i64, _d, _d, _d, _d, _d, _i64, _d, _vp, _vp, _vp]),
     "frl_adamw_mt": (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _i64, _d, _d, _d, _d, _d, _i64, _d, _vp, _vp, _vp]),
     "frl_rmsprop_mt": (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _i64, _d, _d, _d, _d, _d, _d, _vp, _vp, _vp]),
+    "frl_sgd_momentum_sr": (_i, [_vp, _vp, _vp, _i64, _i64, _u64, _i64, _d, _d, _d, _d, _d, _vp, _vp, _i, _i, _vp]),
+    "frl_adam_sr": (_i, [_vp, _vp, _vp, _vp, _vp, _i64, _i64, _u64, _d, _d, _d, _d, _d, _i64, _d, _vp, _vp, _i, _vp]),
+    "frl_adamw_sr": (_i, [_vp, _vp, _vp, _vp, _vp, _i64, _i64, _u64, _d, _d, _d, _d, _d, _i64, _d, _vp, _vp, _i, _vp]),
+    "frl_rmsprop_sr": (_i, [_vp, _vp, _vp, _vp, _i64, _i64, _u64, _i64, _d, _d, _d, _d, _d, _d, _vp, _vp, _i, _vp]),
+    "frl_sgd_momentum_mt_sr": (_i, [_vp, _vp, _vp, _vp, _vp, _i64, _u64, _i64, _d, _d, _d, _d, _d, _vp, _vp, _i,
+                                    _vp]),
+    "frl_adam_mt_sr": (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _i64, _u64, _d, _d, _d, _d, _d, _i64, _d, _vp, _vp,
+                            _vp]),
+    "frl_adamw_mt_sr": (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _i64, _u64, _d, _d, _d, _d, _d, _i64, _d, _vp, _vp,
+                             _vp]),
+    "frl_rmsprop_mt_sr": (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _i64, _u64, _i64, _d, _d, _d, _d, _d, _d, _vp, _vp,
+                               _vp]),
+    "frl_weight_ema_bf16": (_i, [_vp, _vp, _i64, _d, _vp]),
     "frl_layerwise_scratch_bytes": (_i64, [_i64, _i64]),
     "frl_lars_mt": (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _i64, _i64, _vp, _vp, _vp, _d, _d, _d, _d, _vp, _vp, _i, _vp]),
     "frl_lamb_mt": (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _i64, _i64, _vp, _vp, _vp, _d, _d, _d, _d, _d, _i64,
@@ -260,6 +276,17 @@ def dw_gemm_sgd(dz, x, gw, p, buf, p_lp, *, lr, mu, dampening, wd, grad_scale=1.
                                  grad_scale, _ptr(dyn), int(first_step), _stream()), "frl_dw_gemm_sgd")
 
 
+def dw_gemm_sgd_sr(dz, x, gw, p, buf, *, arena_off, seed, t, lr, mu, dampening, wd, grad_scale=1.0,
+                   first_step=False, dyn=None) -> None:
+    """gw = dz^T x, then ``sgd_momentum_sr``'s update of the bf16 [out, in] weights p (arena elements
+    from ``arena_off``) and buf from it."""
+    if p.dtype != torch.bfloat16:
+        raise NativeLibraryError("dw_gemm_sgd_sr: p must be the bf16 weights, got %s" % p.dtype)
+    _check(lib().frl_dw_gemm_sgd_sr(_ptr(dz), dz.stride(0), _ptr(x), x.stride(0), dz.shape[0], dz.shape[1],
+                                    x.shape[1], _ptr(gw), _ptr(p), _ptr(buf), arena_off, seed, t, lr, mu, dampening,
+                                    wd, grad_scale, _ptr(dyn), int(first_step), _stream()), "frl_dw_gemm_sgd_sr")
+
+
 # ---- K13: data-gradient GEMM with the lower unit's ReLU backward and bias gradient in its epilogue --
 
 def dx_drelu_fits(dz_up, w_up, act, db) -> bool:
@@ -341,6 +368,83 @@ def rmsprop_mt(p, sq, buf, p_lp, table, *, lr, alpha, eps, wd, mu, grad_scale=1.
     _check(lib().frl_rmsprop_mt(_ptr(p), _ptr(sq), _ptr(buf), _ptr(p_lp), table.segs_dev_ptr,
                                 table.prefix_dev_ptr, table.tile_seg_dev_ptr, table.n_tiles, lr, alpha, eps, wd, mu,
                                 grad_scale, _ptr(grad_scale_dev), _ptr(dyn), _stream()), "frl_rmsprop_mt")
+
+
+# ---- K2-sr / K2-mt-sr: updates of bf16 master weights with stochastic rounding --------------------
+
+def _check_sr(p, seed: int) -> None:
+    if p.dtype != torch.bfloat16:
+        raise NativeLibraryError("stochastic-rounding update: p must be the bf16 weights, got %s" % p.dtype)
+    if not 0 <= seed < 1 << 64:
+        raise NativeLibraryError("stochastic-rounding update: seed %r is not a uint64" % (seed,))
+
+
+def sgd_momentum_sr(p, g, buf, n, *, arena_off, seed, t, lr, mu, dampening, wd, grad_scale=1.0,
+                    grad_scale_dev=None, first_step=False, dyn=None) -> None:
+    """K2 SGD on bf16 weights ``p`` (arena elements ``[arena_off, arena_off + n)``), rounded
+    stochastically with the draws of update ``t`` (see frl_sgd_momentum_sr in include/frl_b200.h)."""
+    _check_sr(p, seed)
+    _check(lib().frl_sgd_momentum_sr(_ptr(p), _ptr(g), _ptr(buf), n, arena_off, seed, t, lr, mu, dampening, wd,
+                                     grad_scale, _ptr(grad_scale_dev), _ptr(dyn), int(first_step),
+                                     dtype_code(g.dtype), _stream()), "frl_sgd_momentum_sr")
+
+
+def adam_sr(p, g, m, v, vmax, n, *, arena_off, seed, lr, beta1, beta2, eps, wd, step, grad_scale=1.0,
+            grad_scale_dev=None, dyn=None) -> None:
+    _check_sr(p, seed)
+    _check(lib().frl_adam_sr(_ptr(p), _ptr(g), _ptr(m), _ptr(v), _ptr(vmax), n, arena_off, seed, lr, beta1, beta2,
+                             eps, wd, step, grad_scale, _ptr(grad_scale_dev), _ptr(dyn), dtype_code(g.dtype),
+                             _stream()), "frl_adam_sr")
+
+
+def adamw_sr(p, g, m, v, vmax, n, *, arena_off, seed, lr, beta1, beta2, eps, wd, step, grad_scale=1.0,
+             grad_scale_dev=None, dyn=None) -> None:
+    _check_sr(p, seed)
+    _check(lib().frl_adamw_sr(_ptr(p), _ptr(g), _ptr(m), _ptr(v), _ptr(vmax), n, arena_off, seed, lr, beta1, beta2,
+                              eps, wd, step, grad_scale, _ptr(grad_scale_dev), _ptr(dyn), dtype_code(g.dtype),
+                              _stream()), "frl_adamw_sr")
+
+
+def rmsprop_sr(p, g, sq, buf, n, *, arena_off, seed, t, lr, alpha, eps, wd, mu, grad_scale=1.0,
+               grad_scale_dev=None, dyn=None) -> None:
+    _check_sr(p, seed)
+    _check(lib().frl_rmsprop_sr(_ptr(p), _ptr(g), _ptr(sq), _ptr(buf), n, arena_off, seed, t, lr, alpha, eps, wd,
+                                mu, grad_scale, _ptr(grad_scale_dev), _ptr(dyn), dtype_code(g.dtype), _stream()),
+           "frl_rmsprop_sr")
+
+
+def sgd_momentum_mt_sr(p, buf, table, *, seed, t, lr, mu, dampening, wd, grad_scale=1.0, grad_scale_dev=None,
+                       first_step=False, dyn=None) -> None:
+    """K2-mt SGD on the bf16 weights ``p`` (arena base) over the model slots of ``table``."""
+    _check_sr(p, seed)
+    _check(lib().frl_sgd_momentum_mt_sr(_ptr(p), _ptr(buf), table.segs_dev_ptr, table.prefix_dev_ptr,
+                                        table.tile_seg_dev_ptr, table.n_tiles, seed, t, lr, mu, dampening, wd,
+                                        grad_scale, _ptr(grad_scale_dev), _ptr(dyn), int(first_step), _stream()),
+           "frl_sgd_momentum_mt_sr")
+
+
+def adam_mt_sr(p, m, v, vmax, table, *, seed, lr, beta1, beta2, eps, wd, step, grad_scale=1.0,
+               grad_scale_dev=None, dyn=None) -> None:
+    _check_sr(p, seed)
+    _check(lib().frl_adam_mt_sr(_ptr(p), _ptr(m), _ptr(v), _ptr(vmax), table.segs_dev_ptr, table.prefix_dev_ptr,
+                                table.tile_seg_dev_ptr, table.n_tiles, seed, lr, beta1, beta2, eps, wd, step,
+                                grad_scale, _ptr(grad_scale_dev), _ptr(dyn), _stream()), "frl_adam_mt_sr")
+
+
+def adamw_mt_sr(p, m, v, vmax, table, *, seed, lr, beta1, beta2, eps, wd, step, grad_scale=1.0,
+                grad_scale_dev=None, dyn=None) -> None:
+    _check_sr(p, seed)
+    _check(lib().frl_adamw_mt_sr(_ptr(p), _ptr(m), _ptr(v), _ptr(vmax), table.segs_dev_ptr, table.prefix_dev_ptr,
+                                 table.tile_seg_dev_ptr, table.n_tiles, seed, lr, beta1, beta2, eps, wd, step,
+                                 grad_scale, _ptr(grad_scale_dev), _ptr(dyn), _stream()), "frl_adamw_mt_sr")
+
+
+def rmsprop_mt_sr(p, sq, buf, table, *, seed, t, lr, alpha, eps, wd, mu, grad_scale=1.0, grad_scale_dev=None,
+                  dyn=None) -> None:
+    _check_sr(p, seed)
+    _check(lib().frl_rmsprop_mt_sr(_ptr(p), _ptr(sq), _ptr(buf), table.segs_dev_ptr, table.prefix_dev_ptr,
+                                   table.tile_seg_dev_ptr, table.n_tiles, seed, t, lr, alpha, eps, wd, mu,
+                                   grad_scale, _ptr(grad_scale_dev), _ptr(dyn), _stream()), "frl_rmsprop_mt_sr")
 
 
 # ---- K2-lw: layer-wise adaptive updates (LARS, LAMB) over a segment table -------------------------
@@ -612,6 +716,15 @@ def weight_ema(ema, p, w: float) -> None:
     if p.numel() < ema.numel():
         raise NativeLibraryError("weight EMA: p has %d elements, ema %d" % (p.numel(), ema.numel()))
     _check(lib().frl_weight_ema(_ptr(ema), _ptr(p), ema.numel(), float(w), _stream()), "frl_weight_ema")
+
+
+def weight_ema_bf16(ema, p, w: float) -> None:
+    """``weight_ema`` with ``p`` the contiguous bf16 weights (frl_weight_ema_bf16)."""
+    if ema.dtype != torch.float32 or p.dtype != torch.bfloat16 or not (ema.is_contiguous() and p.is_contiguous()):
+        raise NativeLibraryError("weight EMA (bf16): ema must be contiguous fp32 and p contiguous bf16")
+    if p.numel() < ema.numel():
+        raise NativeLibraryError("weight EMA (bf16): p has %d elements, ema %d" % (p.numel(), ema.numel()))
+    _check(lib().frl_weight_ema_bf16(_ptr(ema), _ptr(p), ema.numel(), float(w), _stream()), "frl_weight_ema_bf16")
 
 
 # ---- K3 -------------------------------------------------------------------------------------

@@ -3,8 +3,11 @@
 Everything the update kernel streams lives in a handful of contiguous fp32 (and bf16) vectors
 with one shared element layout:
 
-    master  fp32 [N]   authoritative weights (what checkpoints store)
-    lp      bf16 [N]   shadow weights the bf16 forward/backward reads (BF16 mode only)
+    master  fp32 [N]   authoritative weights (what checkpoints store); with bf16 master weights
+                       (``types.MasterWeights.BF16``) only the criterion range [model_end, N),
+                       element i at master[i - master_base]
+    lp      bf16 [N]   shadow weights the bf16 forward/backward reads (BF16 mode only); with bf16
+                       master weights the model range of lp IS the weights
     grad    [N]        gradient bucket memory, fp32 or bf16 — what NCCL all-reduces in place
     state_k fp32 [N]   optimizer state (momentum / exp_avg / exp_avg_sq / ...), owned by the
                        optimizer, same layout
@@ -29,7 +32,7 @@ from typing import Dict, Iterable, List, Optional, Sequence, Tuple
 import torch
 import torch.nn as nn
 
-from .types import Precision
+from .types import MasterWeights, Precision
 
 ALIGN_ELEMS = 8
 
@@ -74,7 +77,7 @@ class ParamArena:
                  criterion_params: Iterable[nn.Parameter] = (),
                  *, device: torch.device, precision: Precision = Precision.FP32,
                  shared_allocator=None, adjacent: Sequence[Sequence[nn.Parameter]] = (),
-                 channels_last: bool = False) -> None:
+                 channels_last: bool = False, master_weights: MasterWeights = MasterWeights.FP32) -> None:
         """``shared_allocator(numel, dtype) -> zeroed tensor``: where the vectors other ranks must
         reach (``grad`` and the weights the modules read) come from — symmetric/multicast memory
         for the fused NVLS step; default ``torch.zeros``.
@@ -85,7 +88,11 @@ class ParamArena:
         member but the last has a multiple of 8 elements (no padding in between); the slot list
         stays sorted by offset, ``ArenaSlot.index`` keeps the optimizer's parameter position.
 
-        ``channels_last``: lay every trainable 4-D parameter out in channels_last element order."""
+        ``channels_last``: lay every trainable 4-D parameter out in channels_last element order.
+
+        ``master_weights``: ``MasterWeights.BF16`` allocates no fp32 vector for the model range: the
+        bf16 vector ``lp`` holds the model's weights (rounded to nearest even from the parameters
+        once, here), ``master`` the criterion parameters only.  Needs a bf16-storage precision."""
         self.device = torch.device(device)
         self.precision = precision
         self.all_params: List[nn.Parameter] = []
@@ -148,28 +155,39 @@ class ParamArena:
             return torch.zeros(self.numel, dtype=dtype, device=self.device)
 
         bf16_mode = precision.bf16_storage
-        self.master = (torch.zeros(self.numel, dtype=torch.float32, device=self.device)
+        self.master_weights = MasterWeights(master_weights)
+        self.bf16_master = self.master_weights is MasterWeights.BF16
+        if self.bf16_master and not bf16_mode:
+            raise ValueError("bf16 master weights need a bf16-storage precision, got %s" % precision.value)
+        # arena index of master[0]: the model range has no fp32 copy with bf16 master weights
+        self.master_base = self.model_end if self.bf16_master else 0
+        self.master = (torch.zeros(self.numel - self.master_base, dtype=torch.float32, device=self.device)
                        if bf16_mode else shared(torch.float32))
-        with torch.no_grad():
-            for s in self.slots:
-                self.slot_view(self.master, s).copy_(s.param.detach())
         self.lp: Optional[torch.Tensor] = None
         if bf16_mode:
             self.lp = shared(torch.bfloat16)
+        with torch.no_grad():
+            for s in self.slots:
+                if self.bf16_master and s.uses_lp:
+                    self.slot_view(self.lp, s).copy_(s.param.detach())
+                else:
+                    self.master_view(s).copy_(s.param.detach())
+        if bf16_mode and not self.bf16_master:
             self.lp.copy_(self.master)
         self.grad = shared(self.grad_dtype)
         self._by_id: Dict[int, ArenaSlot] = {id(s.param): s for s in self.slots}
         self._repoint()
 
     # -- views ---------------------------------------------------------------------------------
-    def _storage_for(self, s: ArenaSlot) -> torch.Tensor:
-        return self.lp if s.uses_lp else self.master
+    def _storage_view(self, s: ArenaSlot) -> torch.Tensor:
+        return self.slot_view(self.lp, s) if s.uses_lp else self.master_view(s)
 
     @staticmethod
-    def slot_view(vec: torch.Tensor, s: ArenaSlot) -> torch.Tensor:
+    def slot_view(vec: torch.Tensor, s: ArenaSlot, base: int = 0) -> torch.Tensor:
         """Slot ``s``'s slice of the arena-shaped vector ``vec`` as a tensor of the parameter's
-        shape, in the slot's element order (channels_last strides for a channels_last slot)."""
-        flat = vec[s.offset:s.end]
+        shape, in the slot's element order (channels_last strides for a channels_last slot).
+        ``base``: the arena index of ``vec[0]``."""
+        flat = vec[s.offset - base:s.end - base]
         if s.memory_format is torch.contiguous_format:
             return flat.view(s.shape)
         return flat.as_strided(s.shape, s.strides)
@@ -180,7 +198,7 @@ class ParamArena:
 
     def _repoint(self) -> None:
         for s in self.slots:
-            s.param.data = self.slot_view(self._storage_for(s), s)
+            s.param.data = self._storage_view(s)
             s.param.grad = None
 
     def slot_of(self, p: nn.Parameter) -> ArenaSlot:
@@ -190,7 +208,17 @@ class ParamArena:
         return self.slot_view(self.grad, s)
 
     def master_view(self, s: ArenaSlot) -> torch.Tensor:
-        return self.slot_view(self.master, s)
+        """The slot's fp32 master weights (not for a model slot with bf16 master weights)."""
+        if s.offset < self.master_base:
+            raise ValueError("bf16 master weights: parameter %d has no fp32 master" % s.index)
+        return self.slot_view(self.master, s, self.master_base)
+
+    def weights_fp32(self, s: ArenaSlot) -> torch.Tensor:
+        """The slot's authoritative weights as a fresh contiguous fp32 tensor: its master, or with
+        bf16 master weights its bf16 weights upcast (exactly)."""
+        if s.offset < self.master_base:
+            return self.slot_view(self.lp, s).to(torch.float32, memory_format=torch.contiguous_format)
+        return self.master_view(s).detach().clone(memory_format=torch.contiguous_format)
 
     def new_state(self) -> torch.Tensor:
         return torch.zeros(self.numel, dtype=torch.float32, device=self.device)
@@ -201,8 +229,9 @@ class ParamArena:
 
     # -- bf16 shadow maintenance ---------------------------------------------------------------
     def refresh_shadow(self) -> None:
-        """master -> lp after the master was written from outside the update kernel."""
-        if self.lp is not None:
+        """master -> lp after the master was written from outside the update kernel (nothing to do
+        with bf16 master weights: ``lp`` is the weights)."""
+        if self.lp is not None and not self.bf16_master:
             self.lp.copy_(self.master)
 
     def load_master_from_params(self, tensors: Sequence[Tuple[nn.Parameter, torch.Tensor]]) -> None:
@@ -211,6 +240,8 @@ class ParamArena:
                 s = self._by_id.get(id(p))
                 if s is None:
                     p.data.copy_(value)
+                elif s.offset < self.master_base:
+                    self.slot_view(self.lp, s).copy_(value)     # round to nearest even, once
                 else:
                     self.master_view(s).copy_(value)
         self.refresh_shadow()
@@ -235,7 +266,7 @@ class ParamArena:
                         buf.data = buf.data.float()
             for s in self.slots:
                 saved.append((s.param, s.param.data, s.param.grad))
-                clone = self.master_view(s).detach().clone(memory_format=torch.contiguous_format)
+                clone = self.weights_fp32(s)
                 s.param.data = clone.cpu() if cpu else clone
                 s.param.grad = None
             yield self

@@ -28,21 +28,6 @@ constexpr int kAugRows = 8;
 constexpr int kRrcAttempts = 10;
 constexpr uint32_t kFlipBlock = 10;
 
-struct Philox4 { uint32_t w[4]; };
-
-__device__ __forceinline__ Philox4 philox4x32_10(uint32_t c0, uint32_t c1, uint32_t c2, uint32_t c3,
-                                                 uint32_t k0, uint32_t k1) {
-#pragma unroll
-    for (int r = 0; r < 10; ++r) {
-        const uint32_t lo0 = 0xD2511F53u * c0, hi0 = __umulhi(0xD2511F53u, c0);
-        const uint32_t lo1 = 0xCD9E8D57u * c2, hi1 = __umulhi(0xCD9E8D57u, c2);
-        const uint32_t n0 = hi1 ^ c1 ^ k0, n2 = hi0 ^ c3 ^ k1;
-        c0 = n0; c1 = lo1; c2 = n2; c3 = lo0;
-        k0 += 0x9E3779B9u; k1 += 0xBB67AE85u;
-    }
-    return Philox4{{c0, c1, c2, c3}};
-}
-
 __device__ __forceinline__ double unif(uint32_t w) { return static_cast<double>(w >> 8) * (1.0 / 16777216.0); }
 __device__ __forceinline__ int below(uint32_t w, int n) {
     return static_cast<int>((static_cast<uint64_t>(w) * static_cast<uint64_t>(n)) >> 32);

@@ -23,9 +23,16 @@
 // tensor-core work instead of as a separate memory-bound pass after backward.  What stays exposed
 // is each CTA's last tile, whose update has no main loop left to hide under.
 //
+// frl_dw_gemm_sgd_sr is the same kernel body for bf16 master weights (types.MasterWeights.BF16): the
+// epilogue reads the bf16 weights instead of an fp32 master and stores the SGD result rounded
+// stochastically (sr_bf16, with the draws of the weight's arena index), 14 B per weight -- so it
+// equals frl_dw_gemm followed by frl_sgd_momentum_sr over the slice.
+//
 // Tensor maps are encoded on the host per launch through the driver entry point (libcuda is not
 // linked) and passed as __grid_constant__ parameters; a captured CUDA graph bakes in the
 // operands' addresses, which the step's static activation buffers keep fixed.
+#include <type_traits>
+
 #include "gemm_sm90.cuh"
 #include "optim_rules.cuh"
 
@@ -57,6 +64,28 @@ struct Update {
     const float* dyn;       // device-resident lr (null: the rule's by-value lr)
 };
 
+// bf16 master weights: the slice's bf16 weights are the weights; off = arena index of its element 0
+struct UpdateSr {
+    __nv_bfloat16* w;       // bf16 weights of the slice, [out, in]
+    float* mom;             // momentum buffer of the slice (null: SGD without momentum)
+    SgdRule rule;
+    float gscale;
+    const float* dyn;       // device-resident lr and (dyn[3]) update count (null: by value)
+    int64_t off;
+    uint64_t seed;
+    uint32_t t;
+};
+
+__device__ __forceinline__ void patch(Update& u) {
+    if (u.dyn) u.rule.patch(u.dyn);
+}
+__device__ __forceinline__ void patch(UpdateSr& u) {
+    if (u.dyn) {
+        u.rule.patch(u.dyn);
+        u.t = __float_as_uint(__ldg(u.dyn + 3));
+    }
+}
+
 __device__ __forceinline__ void sgd4(const SgdRule& r, f32x4& p, f32x4& m, float g0, float g1, float g2,
                                      float g3, float gs) {
     float dummy0 = 0.f, dummy1 = 0.f;
@@ -66,13 +95,64 @@ __device__ __forceinline__ void sgd4(const SgdRule& r, f32x4& p, f32x4& m, float
     r(p.w, g3 * gs, m.w, dummy0, dummy1);
 }
 
+// epilogue_rows' access pattern for bf16 master weights: weights read and written as bf16, the SGD
+// result of the bf16 gradient stored with stochastic rounding at the weight's arena index
+__device__ __forceinline__ void epilogue_rows_sr(const uint8_t* staging, __nv_bfloat16* gw, int64_t ld,
+                                                 int64_t m0, int64_t n0, const UpdateSr& u, int e, int n,
+                                                 int lane) {
+    constexpr int kRowsAtOnce = 4;
+    for (int r0 = e; r0 < kBM; r0 += n * kRowsAtOnce) {
+        bf16x4 w[kRowsAtOnce][2], g[kRowsAtOnce][2];
+        f32x4 m[kRowsAtOnce][2];
+#pragma unroll
+        for (int j = 0; j < kRowsAtOnce; ++j) {
+            const int r = r0 + n * j;
+            if (r >= kBM) break;
+            const int64_t row = (m0 + r) * ld + n0;
+#pragma unroll
+            for (int h = 0; h < 2; ++h) {
+                const int col = h * 128 + 4 * lane;
+                g[j][h] = *reinterpret_cast<const bf16x4*>(staging + staging_off(r, col));
+                const bf16x4* wp = reinterpret_cast<const bf16x4*>(u.w + row + col);
+                asm volatile("ld.global.L1::no_allocate.v2.u32 {%0,%1}, [%2];"
+                             : "=r"(w[j][h].a), "=r"(w[j][h].b) : "l"(wp));
+                if (u.mom) m[j][h] = ld_stream(reinterpret_cast<const f32x4*>(u.mom + row + col));
+            }
+        }
+#pragma unroll
+        for (int j = 0; j < kRowsAtOnce; ++j) {
+            const int r = r0 + n * j;
+            if (r >= kBM) break;
+            const int64_t row = (m0 + r) * ld + n0;
+#pragma unroll
+            for (int h = 0; h < 2; ++h) {
+                const int col = h * 128 + 4 * lane;
+                st_stream(reinterpret_cast<bf16x4*>(gw + row + col), g[j][h]);
+                f32x4 q{bf16lo(w[j][h].a), bf16hi(w[j][h].a), bf16lo(w[j][h].b), bf16hi(w[j][h].b)};
+                f32x4 s = u.mom ? m[j][h] : f32x4{0.f, 0.f, 0.f, 0.f};
+                sgd4(u.rule, q, s, bf16lo(g[j][h].a), bf16hi(g[j][h].a), bf16lo(g[j][h].b), bf16hi(g[j][h].b),
+                     u.gscale);
+                const Philox4 d = sr_draws(static_cast<uint64_t>(u.off + row + col) >> 2, u.t, u.seed);
+                st_stream(reinterpret_cast<bf16x4*>(u.w + row + col),
+                          bf16x4{sr_pack(q.x, q.y, d.w[0], d.w[1]), sr_pack(q.z, q.w, d.w[2], d.w[3])});
+                if (u.mom) st_stream(reinterpret_cast<f32x4*>(u.mom + row + col), s);
+            }
+        }
+    }
+}
+
 // Epilogue rows of one tile for worker warp e of n: rows e, e+n, ...; lane l takes the four
 // columns 4l..4l+3 of each 128-column half, so every global access of a warp is one contiguous
 // 512-byte (fp32) or 256-byte (bf16) run of a dW row.  Four rows at a time: 16 loads of 16 bytes
 // in flight per lane.
-template <bool UPDATE>
+template <bool UPDATE, typename U>
 __device__ __forceinline__ void epilogue_rows(const uint8_t* staging, __nv_bfloat16* gw, int64_t ld,
-                                              int64_t m0, int64_t n0, const Update& u, int e, int n, int lane) {
+                                              int64_t m0, int64_t n0, const U& u, int e, int n, int lane) {
+    constexpr bool SR = std::is_same<U, UpdateSr>::value;
+    if constexpr (SR) {
+        epilogue_rows_sr(staging, gw, ld, m0, n0, u, e, n, lane);
+        return;
+    } else {
     constexpr int kRowsAtOnce = 4;
     for (int r0 = e; r0 < kBM; r0 += n * kRowsAtOnce) {
         f32x4 p[kRowsAtOnce][2], m[kRowsAtOnce][2];
@@ -114,12 +194,12 @@ __device__ __forceinline__ void epilogue_rows(const uint8_t* staging, __nv_bfloa
             }
         }
     }
+    }
 }
 
-template <bool UPDATE>
-__global__ void __launch_bounds__(kThreads, 1)
-dw_gemm_kernel(const __grid_constant__ CUtensorMap tm_dz, const __grid_constant__ CUtensorMap tm_x,
-               int M, int N, int K, __nv_bfloat16* __restrict__ gw, Update u) {
+template <bool UPDATE, typename U>
+__device__ __forceinline__ void dw_gemm_body(const CUtensorMap& tm_dz, const CUtensorMap& tm_x, int M, int N,
+                                             int K, __nv_bfloat16* __restrict__ gw, const U& u) {
     extern __shared__ uint8_t smem_raw[];
     uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
     uint8_t* staging = smem + kStages * kStageBytes;
@@ -168,8 +248,8 @@ dw_gemm_kernel(const __grid_constant__ CUtensorMap tm_dz, const __grid_constant_
         return;
     }
     if (warp < 4) {                                   // ---- epilogue warps 1..3
-        Update upd = u;
-        if (UPDATE && upd.dyn) upd.rule.patch(upd.dyn);     // per-step lr (CUDA-graph replays)
+        U upd = u;
+        if (UPDATE) patch(upd);                       // per-step scalars (CUDA-graph replays)
         int it = 0;
         for (int tile = blockIdx.x; tile < n_tiles; tile += gridDim.x, ++it) {
             int m0, n0;
@@ -222,8 +302,8 @@ dw_gemm_kernel(const __grid_constant__ CUtensorMap tm_dz, const __grid_constant_
         // this CTA's last tile: no main loop left to hide its epilogue under, so the consumer warps
         // take 8 of every 11 of its rows (warps 1..3 the other 3)
         const int tile = blockIdx.x + (it - 1) * gridDim.x;
-        Update upd = u;
-        if (UPDATE && upd.dyn) upd.rule.patch(upd.dyn);
+        U upd = u;
+        if (UPDATE) patch(upd);
         mbar_wait(epi_full, (it - 1) & 1);
         int m0, n0;
         tile_origin(tile, tiles_m, tiles_n, m0, n0);
@@ -232,15 +312,29 @@ dw_gemm_kernel(const __grid_constant__ CUtensorMap tm_dz, const __grid_constant_
     }
 }
 
+template <bool UPDATE>
+__global__ void __launch_bounds__(kThreads, 1)
+dw_gemm_kernel(const __grid_constant__ CUtensorMap tm_dz, const __grid_constant__ CUtensorMap tm_x,
+               int M, int N, int K, __nv_bfloat16* __restrict__ gw, Update u) {
+    dw_gemm_body<UPDATE>(tm_dz, tm_x, M, N, K, gw, u);
+}
+
+__global__ void __launch_bounds__(kThreads, 1)
+dw_gemm_sr_kernel(const __grid_constant__ CUtensorMap tm_dz, const __grid_constant__ CUtensorMap tm_x,
+                  int M, int N, int K, __nv_bfloat16* __restrict__ gw, UpdateSr u) {
+    dw_gemm_body<true>(tm_dz, tm_x, M, N, K, gw, u);
+}
+
 // ---- host side ------------------------------------------------------------------------------
 // [rows, cols] row-major bf16 with leading dimension ld (elements), boxes of 64 columns x kBK rows
 static bool encode(CUtensorMap* map, const void* base, int64_t rows, int64_t cols, int64_t ld) {
     return encode_bf16(map, base, rows, cols, ld, 64, kBK, CU_TENSOR_MAP_SWIZZLE_128B);
 }
 
-template <bool UPDATE>
-static int launch(const void* dz, int64_t ld_dz, const void* x, int64_t ld_x, int64_t rows, int64_t out,
-                  int64_t in, void* gw, const Update& u, cudaStream_t st, const char* name) {
+template <typename Kernel, typename U>
+static int launch(Kernel kernel, const void* dz, int64_t ld_dz, const void* x, int64_t ld_x, int64_t rows,
+                  int64_t out, int64_t in, void* gw, const U& u, const void* p, const void* mom, const void* lp,
+                  cudaStream_t st, const char* name) {
     FRL_REQUIRE(dz && x && gw, FRL_E_ARG, "%s: null operand", name);
     FRL_REQUIRE(out % kBM == 0 && in % kBN == 0 && rows % kBK == 0 && rows > 0, FRL_E_ARG,
                 "%s: shape [%lld x %lld] over %lld rows is not a multiple of the %dx%dx%d tile", name,
@@ -249,21 +343,25 @@ static int launch(const void* dz, int64_t ld_dz, const void* x, int64_t ld_x, in
     FRL_REQUIRE(out <= INT32_MAX && in <= INT32_MAX && rows <= INT32_MAX, FRL_E_ARG, "%s: shape too large", name);
     FRL_REQUIRE(ld_dz >= out && ld_x >= in && ld_dz % 8 == 0 && ld_x % 8 == 0, FRL_E_ARG,
                 "%s: leading dimensions must cover the rows and be multiples of 8", name);
-    FRL_REQUIRE(aligned16(dz) && aligned16(x) && aligned16(gw) && aligned16(u.master) && aligned16(u.mom) &&
-                aligned16(u.lp), FRL_E_ALIGN, "%s: arrays must be 16-byte aligned", name);
+    FRL_REQUIRE(aligned16(dz) && aligned16(x) && aligned16(gw) && aligned16(p) && aligned16(mom) &&
+                aligned16(lp), FRL_E_ALIGN, "%s: arrays must be 16-byte aligned", name);
     CUtensorMap tm_dz, tm_x;
     FRL_REQUIRE(encode(&tm_dz, dz, rows, out, ld_dz) && encode(&tm_x, x, rows, in, ld_x), FRL_E_ARG,
                 "%s: cuTensorMapEncodeTiled failed", name);
-    static bool attr_set = false;                  // per instantiation
-    if (!attr_set) {
-        const cudaError_t e = cudaFuncSetAttribute(dw_gemm_kernel<UPDATE>,
-                                                   cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemBytes);
+    // set once per kernel (idempotent, so a repeat for another kernel of the same type costs a call)
+    static const void* attr_set[3] = {nullptr, nullptr, nullptr};
+    const void* key = reinterpret_cast<const void*>(kernel);
+    bool have = false;
+    for (const void* k : attr_set) have = have || k == key;
+    if (!have) {
+        const cudaError_t e = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemBytes);
         FRL_REQUIRE(e == cudaSuccess, static_cast<int>(e), "%s: smem attribute: %s", name, cudaGetErrorString(e));
-        attr_set = true;
+        for (const void*& k : attr_set)
+            if (k == nullptr) { k = key; break; }
     }
     const int n_tiles = static_cast<int>((out / kBM) * (in / kBN));
     const int grid = n_tiles < sm_count() ? n_tiles : sm_count();
-    dw_gemm_kernel<UPDATE><<<grid, kThreads, kSmemBytes, st>>>(
+    kernel<<<grid, kThreads, kSmemBytes, st>>>(
         tm_dz, tm_x, static_cast<int>(out), static_cast<int>(in), static_cast<int>(rows),
         static_cast<__nv_bfloat16*>(gw), u);
     return after_launch(name);
@@ -277,8 +375,8 @@ using namespace frl;
 extern "C" int frl_dw_gemm(const void* dz, int64_t ld_dz, const void* x, int64_t ld_x, int64_t rows,
                            int64_t out, int64_t in, void* gw, void* stream) {
     dw::Update u{};
-    return dw::launch<false>(dz, ld_dz, x, ld_x, rows, out, in, gw, u, static_cast<cudaStream_t>(stream),
-                             "frl_dw_gemm");
+    return dw::launch(dw::dw_gemm_kernel<false>, dz, ld_dz, x, ld_x, rows, out, in, gw, u, nullptr, nullptr, nullptr,
+                      static_cast<cudaStream_t>(stream), "frl_dw_gemm");
 }
 
 extern "C" int frl_dw_gemm_sgd(const void* dz, int64_t ld_dz, const void* x, int64_t ld_x, int64_t rows,
@@ -289,6 +387,23 @@ extern "C" int frl_dw_gemm_sgd(const void* dz, int64_t ld_dz, const void* x, int
     FRL_REQUIRE(mu == 0.0 || buf != nullptr, FRL_E_ARG, "frl_dw_gemm_sgd: momentum needs buf");
     dw::Update u{p, mu != 0.0 ? buf : nullptr, static_cast<__nv_bfloat16*>(p_lp),
                  make_sgd_rule(lr, mu, dampening, wd, first_step), static_cast<float>(grad_scale), dyn};
-    return dw::launch<true>(dz, ld_dz, x, ld_x, rows, out, in, gw, u, static_cast<cudaStream_t>(stream),
-                            "frl_dw_gemm_sgd");
+    return dw::launch(dw::dw_gemm_kernel<true>, dz, ld_dz, x, ld_x, rows, out, in, gw, u, u.master, u.mom, u.lp,
+                      static_cast<cudaStream_t>(stream), "frl_dw_gemm_sgd");
+}
+
+extern "C" int frl_dw_gemm_sgd_sr(const void* dz, int64_t ld_dz, const void* x, int64_t ld_x, int64_t rows,
+                                  int64_t out, int64_t in, void* gw, void* p, float* buf, int64_t arena_off,
+                                  uint64_t seed, int64_t t, double lr, double mu, double dampening, double wd,
+                                  double grad_scale, const float* dyn, int first_step, void* stream) {
+    FRL_REQUIRE(p, FRL_E_ARG, "frl_dw_gemm_sgd_sr: null weights");
+    FRL_REQUIRE(mu == 0.0 || buf != nullptr, FRL_E_ARG, "frl_dw_gemm_sgd_sr: momentum needs buf");
+    FRL_REQUIRE(arena_off >= 0 && arena_off % 4 == 0, FRL_E_ARG,
+                "frl_dw_gemm_sgd_sr: arena offset %lld is not a multiple of 4", static_cast<long long>(arena_off));
+    FRL_REQUIRE(t >= 1 && t <= 0xffffffffll, FRL_E_ARG, "frl_dw_gemm_sgd_sr: update count %lld outside [1, 2^32)",
+                static_cast<long long>(t));
+    dw::UpdateSr u{static_cast<__nv_bfloat16*>(p), mu != 0.0 ? buf : nullptr,
+                   make_sgd_rule(lr, mu, dampening, wd, first_step), static_cast<float>(grad_scale), dyn, arena_off,
+                   seed, static_cast<uint32_t>(t)};
+    return dw::launch(dw::dw_gemm_sr_kernel, dz, ld_dz, x, ld_x, rows, out, in, gw, u, p, u.mom, nullptr,
+                      static_cast<cudaStream_t>(stream), "frl_dw_gemm_sgd_sr");
 }

@@ -79,6 +79,45 @@ __device__ __forceinline__ uint32_t pack_bf16(float lo, float hi) {
 }
 __device__ __forceinline__ float bf16_to_f32(const __nv_bfloat16* p) { return __bfloat162float(*p); }
 
+// ---- Philox4x32-10 (Salmon et al., SC'11): the counter-based generator of the augmentation draws
+// (augment.cu) and of stochastic rounding (sr_bf16 below); restated in numpy by the tests.
+struct Philox4 { uint32_t w[4]; };
+
+__device__ __forceinline__ Philox4 philox4x32_10(uint32_t c0, uint32_t c1, uint32_t c2, uint32_t c3,
+                                                 uint32_t k0, uint32_t k1) {
+#pragma unroll
+    for (int r = 0; r < 10; ++r) {
+        const uint32_t lo0 = 0xD2511F53u * c0, hi0 = __umulhi(0xD2511F53u, c0);
+        const uint32_t lo1 = 0xCD9E8D57u * c2, hi1 = __umulhi(0xCD9E8D57u, c2);
+        const uint32_t n0 = hi1 ^ c1 ^ k0, n2 = hi0 ^ c3 ^ k1;
+        c0 = n0; c1 = lo1; c2 = n2; c3 = lo0;
+        k0 += 0x9E3779B9u; k1 += 0xBB67AE85u;
+    }
+    return Philox4{{c0, c1, c2, c3}};
+}
+
+// ---- stochastic rounding fp32 -> bf16 (include/frl_b200.h, K2-sr) -----------------------------------
+// The four 16-bit draws of arena elements 4q .. 4q+3 at update t: the low halves of the four words of
+// Philox4x32-10 at counter (lo32(q), hi32(q), t, kSrTag), key (lo32(seed), hi32(seed)).
+constexpr uint32_t kSrTag = 0x53520000u;
+
+__device__ __forceinline__ Philox4 sr_draws(uint64_t q, uint32_t t, uint64_t seed) {
+    return philox4x32_10(static_cast<uint32_t>(q), static_cast<uint32_t>(q >> 32), t, kSrTag,
+                         static_cast<uint32_t>(seed), static_cast<uint32_t>(seed >> 32));
+}
+
+// bf16 bits of fp32 x rounded with the 16 random bits r (only the low 16 are used): (bits(x) + r) >> 16
+// rounds the magnitude up with probability (discarded fraction) / 2^16.  NaN stores 0x7FC0 (a carry
+// could otherwise reach the sign bit); +-inf and bf16-exact values carry nothing and stay put.
+__device__ __forceinline__ uint32_t sr_bf16(float x, uint32_t r) {
+    const uint32_t u = __float_as_uint(x);
+    if ((u & 0x7fffffffu) > 0x7f800000u) return 0x7fc0u;
+    return (u + (r & 0xffffu)) >> 16;
+}
+__device__ __forceinline__ uint32_t sr_pack(float lo, float hi, uint32_t r_lo, uint32_t r_hi) {
+    return sr_bf16(lo, r_lo) | (sr_bf16(hi, r_hi) << 16);
+}
+
 // ---- warp / block reductions ----------------------------------------------------------------
 __device__ __forceinline__ float warp_sum(float v) {
 #pragma unroll

@@ -47,7 +47,9 @@ class WeightEMA:
         self.decay = float(decay)
         self.weight = 1.0 - self.decay             # double; the kernel rounds it to fp32
         self.n = arena.model_end
-        self.ema = arena.master[:self.n].clone()   # what a run with 0 updates evaluates with
+        # what a run with 0 updates evaluates with; with bf16 master weights the weights upcast exactly
+        self.bf16 = bool(getattr(arena, "bf16_master", False))
+        self.ema = arena.lp[:self.n].float() if self.bf16 else arena.master[:self.n].clone()
         self.buffers: List[Tuple[str, torch.Tensor, torch.Tensor]] = [
             (name, b, b.detach().clone()) for name, b in module.named_buffers()]
         self.updates = 0
@@ -65,7 +67,10 @@ class WeightEMA:
         first = self.updates == 0
         # the first update is K11 at weight 1, which returns the master weights (torch's lerp at
         # weight 1 is its end point): the same one launch per update, whatever its position
-        KERNELS.weight_ema(self.ema, self.arena.master[:self.n], 1.0 if first else self.weight)
+        if self.bf16:
+            KERNELS.weight_ema_bf16(self.ema, self.arena.lp[:self.n], 1.0 if first else self.weight)
+        else:
+            KERNELS.weight_ema(self.ema, self.arena.master[:self.n], 1.0 if first else self.weight)
         floats = [(e, b) for _, b, e in self.buffers if b.is_floating_point() and not first]
         if floats:
             torch._foreach_lerp_([e for e, _ in floats], [b.detach() for _, b in floats], self.weight)
@@ -75,10 +80,29 @@ class WeightEMA:
         self.updates += 1
 
     @torch.no_grad()
+    def _exchange_bf16(self) -> None:
+        """Bf16 master weights: into the swap, keep the live bf16 weights aside and write the EMA
+        rounded to nearest even in their place; out of it, put the kept bytes back."""
+        lp = self.arena.lp
+        if not self._swapped:
+            self._kept = lp[:self.n].clone()
+            lp[:self.n].copy_(self.ema)
+        else:
+            lp[:self.n].copy_(self._kept)
+            self._kept = None
+        for _, b, e in self.buffers:
+            t = b.detach().clone()
+            b.detach().copy_(e)
+            e.copy_(t)
+
+    @torch.no_grad()
     def _exchange(self) -> None:
         """Swap the averaged and the live values: model range of the master in chunks through one
         transient buffer of at most ``SWAP_CHUNK`` elements, then the bf16 shadow from the master,
         then the buffers.  Pure copies: swapping twice restores every bit."""
+        if self.bf16:
+            self._exchange_bf16()
+            return
         master = self.arena.master
         tmp = torch.empty(min(self.n, SWAP_CHUNK), dtype=torch.float32, device=master.device)
         for lo in range(0, self.n, SWAP_CHUNK):
@@ -117,6 +141,14 @@ class WeightEMA:
         with self.swapped(), self.arena.exported(cpu=True, module=self.module):
             # parameters are private CPU copies inside exported(); buffers are the live tensors
             sd = {k: v.detach().to("cpu", copy=k in buffers) for k, v in self.module.state_dict().items()}
+        if self.bf16:
+            # the swap put the EMA rounded to bf16 in the weights: write the fp32 EMA itself, so a
+            # resumed EMA continues bit for bit
+            names = {id(p): name for name, p in self.module.named_parameters()}
+            for s in self.arena.slots:
+                if s.is_model:
+                    sd[names[id(s.param)]] = ParamArena.slot_view(self.ema, s).to(
+                        "cpu", memory_format=torch.contiguous_format)
         return {"decay": self.decay, "updates": self.updates, "state_dict": sd}
 
     @torch.no_grad()

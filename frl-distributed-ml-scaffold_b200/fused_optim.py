@@ -14,6 +14,9 @@ format and update whole tensors through the K2-lw kernels.  ``FusedAdam8bit`` (a
 model's 2-D weights and this module's Adam (K2-mt) for every other parameter.  ``adamw=True`` (an
 extension, ``Solver.solve(..., adamw=True)``) turns the Adam rule of ``FusedAdam``, ``FusedAdam8bit``
 and ``FusedMuon``'s Adam group into ``torch.optim.AdamW``'s decoupled weight decay (``frl_adamw*``).
+On an arena with bf16 master weights (an extension, ``types.MasterWeights.BF16``) ``FusedSGD``,
+``FusedAdam`` and ``FusedRMSprop`` update the model range through the stochastic-rounding kernels
+(``frl_*_sr``, ``frl_*_mt_sr``) and keep ``sr_seed`` / ``sr_updates`` in their param group.
 
 Known limitation: the step count (Adam's bias corrections) is ONE number for the whole arena.
 ``torch.optim`` keeps one per parameter and does not advance it for a parameter whose gradient
@@ -30,10 +33,26 @@ import torch
 
 from . import _native
 from .arena import ParamArena
-from .types import LayerAdaptation, OptAlgorithm, OptimizerState, OptimOpts
+from .types import LayerAdaptation, MasterWeights, OptAlgorithm, OptimizerState, OptimOpts, Precision
 
 # Kernel entry points; tests exercising host logic on CPU swap this for an oracle-backed double.
 KERNELS = _native
+
+# default key of the stochastic-rounding draws (param group ``sr_seed``, a uint64)
+SR_SEED = 0x5EED_B16F_0000_0001
+
+
+class _ShiftedBase:
+    """``data_ptr()`` of an fp32 vector whose element 0 has arena index ``base``, minus ``base``
+    elements: the arena-base pointer the segment-table kernels add arena offsets to.  Only listed
+    segments are touched, and with bf16 master weights those (criterion parameters) lie at or
+    above ``base``."""
+
+    def __init__(self, vec: torch.Tensor, base: int) -> None:
+        self._ptr = vec.data_ptr() - base * vec.element_size()
+
+    def data_ptr(self) -> int:
+        return self._ptr
 
 
 class FusedArenaOptimizer(torch.optim.Optimizer):
@@ -64,6 +83,15 @@ class FusedArenaOptimizer(torch.optim.Optimizer):
         # fused NVLS step (world > 1): set by the pipeline; each rank then updates only its
         # 1/world shard of every bucket (master + state), the weights arrive by multicast
         self.nvls = None
+        # bf16 master weights: the model range is updated with stochastic rounding
+        self.sr = bool(getattr(arena, "bf16_master", False))
+        if self.sr:
+            self.param_groups[0].setdefault("sr_seed", SR_SEED)
+            self.param_groups[0]["sr_updates"] = 0
+
+    @property
+    def sr_seed(self) -> int:
+        return int(self.hyper["sr_seed"])
 
     # -- device-resident scalars -----------------------------------------------------------------
     def _dyn_values(self) -> Tuple[float, ...]:
@@ -86,6 +114,10 @@ class FusedArenaOptimizer(torch.optim.Optimizer):
         if self._dyn is None:
             return
         vals = self._dyn_values()
+        if self.sr:        # dyn[3]: the update count of the stochastic rounding, as uint32 bits
+            if len(vals) > 3:
+                raise RuntimeError("%s: no dyn slot left for the update count" % type(self).__name__)
+            vals = vals + (0.0,) * (3 - len(vals)) + (self._steps + 1,)
         if vals != self._dyn_last:
             if self._dyn.is_cuda:
                 if getattr(self, "_dyn_host", None) is None:
@@ -95,9 +127,14 @@ class FusedArenaOptimizer(torch.optim.Optimizer):
                 self._dyn_slot += 1
                 for i, v in enumerate(vals):
                     row[i] = v
+                if self.sr:
+                    row.view(torch.int32)[3] = vals[3]
                 self._dyn.copy_(row, non_blocking=True)
             else:
-                self._dyn.copy_(torch.tensor(list(vals) + [0.0] * (4 - len(vals)), dtype=torch.float32))
+                host = torch.tensor(list(vals) + [0.0] * (4 - len(vals)), dtype=torch.float32)
+                if self.sr:
+                    host.view(torch.int32)[3] = vals[3]
+                self._dyn.copy_(host)
             self._dyn_last = vals
 
     # -- state vectors ---------------------------------------------------------------------------
@@ -138,7 +175,7 @@ class FusedArenaOptimizer(torch.optim.Optimizer):
         self._grad_src = grad_src
         try:
             split = self.arena.model_end
-            if clip_coef_dev is not None and lo < split < hi:
+            if (clip_coef_dev is not None or self.sr) and lo < split < hi:
                 self._launch(lo, split, grad_scale, clip_coef_dev)
                 self._launch(split, hi, grad_scale, None)
             else:
@@ -155,11 +192,47 @@ class FusedArenaOptimizer(torch.optim.Optimizer):
         copy is current), reading each gradient where the table says it lies (K2-mt)."""
         if clip_coef_dev is not None:
             raise ValueError("K2-mt takes no clip coefficient: clipped updates go through apply_range")
-        if table.n_segs:
+        if not table.n_segs:
+            return
+        if not self.sr:
             self._launch_mt(table, grad_scale)
+            return
+        model, crit = self._sr_split(table)
+        for (sub, idx), launch in ((model, self._launch_mt_sr), (crit, self._launch_mt)):
+            if sub is not None:
+                _gather_segs(table, sub, idx)
+                launch(sub, grad_scale)
 
     def _launch_mt(self, table, grad_scale: float) -> None:
         raise NotImplementedError
+
+    def _launch_mt_sr(self, table, grad_scale: float) -> None:
+        raise NotImplementedError
+
+    def _sr_split(self, table):
+        """Bf16 master weights: the sub-tables of ``table``'s model slots (K2-mt-sr) and criterion
+        slots (K2-mt on their fp32 master), with the rows of ``table`` they take; kept on the table."""
+        split = getattr(table, "sr_split", None)
+        if split is None:
+            from .multi_tensor import GradSegTable
+            dev = self.arena.device
+            split = []
+            for keep in (lambda s: s.is_model, lambda s: not s.is_model):
+                part = [(i, s) for i, s in enumerate(table.slots) if keep(s)]
+                rows = torch.tensor([i for i, _ in part], dtype=torch.int64)
+                split.append((GradSegTable([s for _, s in part], dev), (rows, rows.to(dev))) if part else (None, None))
+            split = table.sr_split = tuple(split)
+        return split
+
+    def _master_base(self):
+        """What the segment-table kernels take as the fp32 master's arena base pointer."""
+        a = self.arena
+        return a.master if a.master_base == 0 else _ShiftedBase(a.master, a.master_base)
+
+    def _lp_mt(self):
+        """The bf16 shadow the fp32 segment-table kernels write: none with bf16 master weights (their
+        segments are then criterion parameters, which read the fp32 master)."""
+        return None if self.sr else self.arena.lp
 
     # -- fused all-reduce + update + broadcast (K7) ------------------------------------------------
     def apply_range_nvls(self, lo: int, hi: int, *, grad_scale: float) -> None:
@@ -207,10 +280,18 @@ class FusedArenaOptimizer(torch.optim.Optimizer):
 
     # -- views used by the launchers -------------------------------------------------------------
     def _slices(self, lo: int, hi: int):
+        """(weights, gradient, bf16 shadow) of ``[lo, hi)``; with bf16 master weights and ``lo`` in the
+        model range (``_use_sr``) the weights are the bf16 vector and there is no shadow."""
         a = self.arena
-        lp = a.lp[lo:hi] if (a.lp is not None and lo < a.model_end) else None
         g = a.grad if self._grad_src is None else self._grad_src
-        return a.master[lo:hi], g[lo:hi], lp
+        if self._use_sr(lo):
+            return a.lp[lo:hi], g[lo:hi], None
+        lp = a.lp[lo:hi] if (a.lp is not None and lo < a.model_end) else None
+        return a.master[lo - a.master_base:hi - a.master_base], g[lo:hi], lp
+
+    def _use_sr(self, lo: int) -> bool:
+        """Does a launch starting at ``lo`` (never straddling ``model_end``) take the SR kernels?"""
+        return self.sr and lo < self.arena.model_end
 
     # -- torch-format (de)serialisation ----------------------------------------------------------
     def _per_param_extra(self) -> Dict[str, Any]:
@@ -226,6 +307,8 @@ class FusedArenaOptimizer(torch.optim.Optimizer):
                         entry[torch_name] = ParamArena.slot_view(self._vec[vec_name], s).clone(
                             memory_format=torch.contiguous_format)
                 state[s.index] = entry
+        if self.sr:
+            self.hyper["sr_updates"] = self._steps
         groups = []
         for g in self.param_groups:
             packed = {k: v for k, v in g.items() if k != "params"}
@@ -254,6 +337,20 @@ class FusedArenaOptimizer(torch.optim.Optimizer):
             elif entry:
                 steps = max(steps, 1)
         self._steps = steps
+        self._load_sr_keys(groups[0])
+
+    def _load_sr_keys(self, group: Dict[str, Any]) -> None:
+        """Bf16 master weights: the update count comes from ``sr_updates`` where the dict has it (a
+        bf16-master checkpoint), so the stochastic rounding continues with the draws it left off at.
+        An fp32-master optimizer drops the two keys again (its state dict stays torch's)."""
+        h = self.hyper
+        if self.sr:
+            if "sr_updates" in group:
+                self._steps = int(group["sr_updates"])
+            h["sr_seed"] = int(group.get("sr_seed", h.get("sr_seed", SR_SEED)))
+        else:
+            h.pop("sr_seed", None)
+            h.pop("sr_updates", None)
 
 
 class FusedSGD(FusedArenaOptimizer):
@@ -269,6 +366,12 @@ class FusedSGD(FusedArenaOptimizer):
         p, g, lp = self._slices(lo, hi)
         mu = float(h["momentum"])
         buf = self._state("momentum_buffer")[lo:hi] if mu != 0.0 else None
+        if self._use_sr(lo):
+            KERNELS.sgd_momentum_sr(p, g, buf, hi - lo, arena_off=lo, seed=self.sr_seed, t=self._steps + 1,
+                                    lr=float(h["lr"]), mu=mu, dampening=float(h["dampening"]),
+                                    wd=float(h["weight_decay"]), grad_scale=grad_scale, grad_scale_dev=coef,
+                                    first_step=(self._steps == 0), dyn=self._dyn)
+            return
         KERNELS.sgd_momentum(p, g, buf, lp, hi - lo, lr=float(h["lr"]), mu=mu,
                              dampening=float(h["dampening"]), wd=float(h["weight_decay"]),
                              grad_scale=grad_scale, grad_scale_dev=coef,
@@ -281,6 +384,12 @@ class FusedSGD(FusedArenaOptimizer):
         a = self.arena
         mu = float(h["momentum"])
         buf = self._state("momentum_buffer")[slot.offset:slot.end] if mu != 0.0 else None
+        if self._use_sr(slot.offset):
+            KERNELS.dw_gemm_sgd_sr(dz, x, gw, a.lp[slot.offset:slot.end], buf, arena_off=slot.offset,
+                                   seed=self.sr_seed, t=self._steps + 1, lr=float(h["lr"]), mu=mu,
+                                   dampening=float(h["dampening"]), wd=float(h["weight_decay"]),
+                                   grad_scale=grad_scale, first_step=(self._steps == 0), dyn=self._dyn)
+            return
         KERNELS.dw_gemm_sgd(dz, x, gw, a.master[slot.offset:slot.end], buf, a.lp[slot.offset:slot.end],
                             lr=float(h["lr"]), mu=mu, dampening=float(h["dampening"]),
                             wd=float(h["weight_decay"]), grad_scale=grad_scale,
@@ -289,10 +398,18 @@ class FusedSGD(FusedArenaOptimizer):
     def _launch_mt(self, table, grad_scale):
         h = self.hyper
         mu = float(h["momentum"])
-        KERNELS.sgd_momentum_mt(self.arena.master, self._state("momentum_buffer") if mu != 0.0 else None,
-                                self.arena.lp, table, lr=float(h["lr"]), mu=mu,
+        KERNELS.sgd_momentum_mt(self._master_base(), self._state("momentum_buffer") if mu != 0.0 else None,
+                                self._lp_mt(), table, lr=float(h["lr"]), mu=mu,
                                 dampening=float(h["dampening"]), wd=float(h["weight_decay"]),
                                 grad_scale=grad_scale, first_step=(self._steps == 0), dyn=self._dyn)
+
+    def _launch_mt_sr(self, table, grad_scale):
+        h = self.hyper
+        mu = float(h["momentum"])
+        KERNELS.sgd_momentum_mt_sr(self.arena.lp, self._state("momentum_buffer") if mu != 0.0 else None, table,
+                                   seed=self.sr_seed, t=self._steps + 1, lr=float(h["lr"]), mu=mu,
+                                   dampening=float(h["dampening"]), wd=float(h["weight_decay"]),
+                                   grad_scale=grad_scale, first_step=(self._steps == 0), dyn=self._dyn)
 
     def _launch_nvls(self, lo, hi, grad_scale):
         h = self.hyper
@@ -353,6 +470,13 @@ class FusedAdam(FusedArenaOptimizer):
         h = self.hyper
         p, g, lp = self._slices(lo, hi)
         vmax = self._state("max_exp_avg_sq")[lo:hi] if h["amsgrad"] else None
+        if self._use_sr(lo):
+            self._kernel("adam_sr")(p, g, self._state("exp_avg")[lo:hi], self._state("exp_avg_sq")[lo:hi], vmax,
+                                    hi - lo, arena_off=lo, seed=self.sr_seed, lr=float(h["lr"]),
+                                    beta1=float(h["betas"][0]), beta2=float(h["betas"][1]), eps=float(h["eps"]),
+                                    wd=float(h["weight_decay"]), step=self._steps + 1, grad_scale=grad_scale,
+                                    grad_scale_dev=coef, dyn=self._dyn)
+            return
         self._kernel("adam")(p, g, self._state("exp_avg")[lo:hi], self._state("exp_avg_sq")[lo:hi], vmax,
                              lp, hi - lo, lr=float(h["lr"]), beta1=float(h["betas"][0]),
                              beta2=float(h["betas"][1]), eps=float(h["eps"]),
@@ -361,11 +485,19 @@ class FusedAdam(FusedArenaOptimizer):
 
     def _launch_mt(self, table, grad_scale):
         h = self.hyper
-        self._kernel("adam_mt")(self.arena.master, self._state("exp_avg"), self._state("exp_avg_sq"),
-                                self._state("max_exp_avg_sq") if h["amsgrad"] else None, self.arena.lp, table,
+        self._kernel("adam_mt")(self._master_base(), self._state("exp_avg"), self._state("exp_avg_sq"),
+                                self._state("max_exp_avg_sq") if h["amsgrad"] else None, self._lp_mt(), table,
                                 lr=float(h["lr"]), beta1=float(h["betas"][0]), beta2=float(h["betas"][1]),
                                 eps=float(h["eps"]), wd=float(h["weight_decay"]), step=self._steps + 1,
                                 grad_scale=grad_scale, dyn=self._dyn)
+
+    def _launch_mt_sr(self, table, grad_scale):
+        h = self.hyper
+        self._kernel("adam_mt_sr")(self.arena.lp, self._state("exp_avg"), self._state("exp_avg_sq"),
+                                   self._state("max_exp_avg_sq") if h["amsgrad"] else None, table,
+                                   seed=self.sr_seed, lr=float(h["lr"]), beta1=float(h["betas"][0]),
+                                   beta2=float(h["betas"][1]), eps=float(h["eps"]), wd=float(h["weight_decay"]),
+                                   step=self._steps + 1, grad_scale=grad_scale, dyn=self._dyn)
 
     def _launch_nvls(self, lo, hi, grad_scale):
         h = self.hyper
@@ -395,6 +527,12 @@ class FusedRMSprop(FusedArenaOptimizer):
         p, g, lp = self._slices(lo, hi)
         mu = float(h["momentum"])
         buf = self._state("momentum_buffer")[lo:hi] if mu != 0.0 else None
+        if self._use_sr(lo):
+            KERNELS.rmsprop_sr(p, g, self._state("square_avg")[lo:hi], buf, hi - lo, arena_off=lo, seed=self.sr_seed,
+                               t=self._steps + 1, lr=float(h["lr"]), alpha=float(h["alpha"]), eps=float(h["eps"]),
+                               wd=float(h["weight_decay"]), mu=mu, grad_scale=grad_scale, grad_scale_dev=coef,
+                               dyn=self._dyn)
+            return
         KERNELS.rmsprop(p, g, self._state("square_avg")[lo:hi], buf, lp, hi - lo,
                         lr=float(h["lr"]), alpha=float(h["alpha"]), eps=float(h["eps"]),
                         wd=float(h["weight_decay"]), mu=mu, grad_scale=grad_scale,
@@ -403,10 +541,18 @@ class FusedRMSprop(FusedArenaOptimizer):
     def _launch_mt(self, table, grad_scale):
         h = self.hyper
         mu = float(h["momentum"])
-        KERNELS.rmsprop_mt(self.arena.master, self._state("square_avg"),
-                           self._state("momentum_buffer") if mu != 0.0 else None, self.arena.lp, table,
+        KERNELS.rmsprop_mt(self._master_base(), self._state("square_avg"),
+                           self._state("momentum_buffer") if mu != 0.0 else None, self._lp_mt(), table,
                            lr=float(h["lr"]), alpha=float(h["alpha"]), eps=float(h["eps"]),
                            wd=float(h["weight_decay"]), mu=mu, grad_scale=grad_scale, dyn=self._dyn)
+
+    def _launch_mt_sr(self, table, grad_scale):
+        h = self.hyper
+        mu = float(h["momentum"])
+        KERNELS.rmsprop_mt_sr(self.arena.lp, self._state("square_avg"),
+                              self._state("momentum_buffer") if mu != 0.0 else None, table, seed=self.sr_seed,
+                              t=self._steps + 1, lr=float(h["lr"]), alpha=float(h["alpha"]), eps=float(h["eps"]),
+                              wd=float(h["weight_decay"]), mu=mu, grad_scale=grad_scale, dyn=self._dyn)
 
     def _launch_nvls(self, lo, hi, grad_scale):
         h = self.hyper
@@ -1085,6 +1231,28 @@ def check_adamw(optim_opts: OptimOpts, layer_adaptation: LayerAdaptation, optimi
                             " and adafactor" if adafactor else ""))
 
 
+def check_master_weights(master_weights: MasterWeights, precision: Precision, layer_adaptation: LayerAdaptation,
+                         optimizer_state: OptimizerState, adafactor: bool, muon: bool) -> None:
+    """Bf16 master weights need a bf16-storage precision and an update with a stochastic-rounding
+    kernel (SGD, Adam / AdamW, RMSprop); every other combination is a ValueError naming it."""
+    if MasterWeights(master_weights) is not MasterWeights.BF16:
+        return
+    why = None
+    if not Precision(precision).bf16_storage:
+        why = "precision %s (there is no bf16 weight storage to keep)" % Precision(precision).value
+    elif LayerAdaptation(layer_adaptation) is not LayerAdaptation.NONE:
+        why = "layer adaptation %s" % LayerAdaptation(layer_adaptation).value
+    elif adafactor:
+        why = "adafactor"
+    elif muon:
+        why = "muon"
+    elif OptimizerState(optimizer_state) is OptimizerState.Q8:
+        why = "optimizer state %s" % OptimizerState.Q8.value
+    if why is not None:
+        raise ValueError("master_weights=bf16 cannot be combined with %s: stochastic rounding is implemented for "
+                         "the sgd, adam / adamw and rmsprop updates in bf16 and fp8 precision" % why)
+
+
 def check_optimizer_state(optim_opts: OptimOpts, layer_adaptation: LayerAdaptation,
                           optimizer_state: OptimizerState) -> None:
     """8-bit state needs Adam without amsgrad and without layer adaptation; anything else is a
@@ -1128,6 +1296,8 @@ def create_fused_optimizer(arena: ParamArena, optim_opts: OptimOpts,
     check_adafactor(optim_opts, layer_adaptation, optimizer_state, adafactor)
     check_muon(optim_opts, layer_adaptation, optimizer_state, adafactor, muon)
     check_adamw(optim_opts, layer_adaptation, optimizer_state, adafactor, adamw)
+    check_master_weights(getattr(arena, "master_weights", MasterWeights.FP32), arena.precision, layer_adaptation,
+                         optimizer_state, adafactor, muon)
     if muon:
         return FusedMuon(arena, lr=optim_opts.lr, weight_decay=optim_opts.weightDecay,
                          momentum=optim_opts.momentum, eps=optim_opts.epsilon, adamw=adamw)

@@ -630,7 +630,10 @@ class GradBucketPipeline:
         """Replicas start identical to rank ``src`` (DDP does this in its constructor)."""
         if not self.distributed:
             return
-        dist.broadcast(self.arena.master, src=src, group=self.pg)
+        if self.arena.master.numel():
+            dist.broadcast(self.arena.master, src=src, group=self.pg)
+        if getattr(self.arena, "bf16_master", False):
+            dist.broadcast(self.arena.lp, src=src, group=self.pg)       # the model's weights
         self.arena.refresh_shadow()
 
     def sync_sharded_state(self) -> None:

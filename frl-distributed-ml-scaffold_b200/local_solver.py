@@ -9,7 +9,7 @@ from typing import Optional
 
 from .problem import Problem
 from .solver import PerformanceSummary, Solver
-from .types import LayerAdaptation, OptimizerState, Precision, RunOpts
+from .types import LayerAdaptation, MasterWeights, OptimizerState, Precision, RunOpts
 
 logger = logging.getLogger(__name__)
 
@@ -27,7 +27,8 @@ class LocalSolver:
               adafactor: Optional[bool] = None,
               muon: Optional[bool] = None,
               adamw: Optional[bool] = None,
-              channels_last: Optional[bool] = None) -> PerformanceSummary:
+              channels_last: Optional[bool] = None,
+              master_weights: Optional[MasterWeights] = None) -> PerformanceSummary:
         if save_notebook:
             logger.warning("save_notebook is not supported by frl_b200 (visualisation only)")
         # a stale rendezvous file from a crashed run would poison the file:// store
@@ -42,6 +43,6 @@ class LocalSolver:
                                  graph=graph, layer_adaptation=layer_adaptation,
                                  grad_accumulation=grad_accumulation, ema_decay=ema_decay,
                                  optimizer_state=optimizer_state, adafactor=adafactor, muon=muon,
-                                 adamw=adamw, channels_last=channels_last):
+                                 adamw=adamw, channels_last=channels_last, master_weights=master_weights):
             pass
         return last

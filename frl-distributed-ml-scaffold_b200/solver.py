@@ -29,14 +29,14 @@ import torch.nn as nn
 from .arena import ParamArena
 from .criteria import BaseParallelCriterion
 from .ema import EMA_STATE_KEY
-from .fused_optim import (FusedAdafactor, FusedAdam8bit, FusedMuon, check_adafactor, check_adamw, check_muon, check_layer_adaptation, check_optimizer_state, create_fused_optimizer,
+from .fused_optim import (FusedAdafactor, FusedAdam8bit, FusedMuon, check_adafactor, check_adamw, check_muon, check_layer_adaptation, check_master_weights, check_optimizer_state, create_fused_optimizer,
                           is_adapted)
 from .grad_sync import BufferBroadcaster, GradBucketPipeline
 from .lr_scheduler import DropEpochsScheduler, WarmupMultiStepLR
 from .problem import Problem
 from .solver_worker import (FractionalPerformanceSummary, SerializableSampleSummary,
                             SolverWorker)
-from .types import (Device, LayerAdaptation, LRSchedulerAlgorithm, Mode, OptimizerState, Precision, RunOpts,
+from .types import (Device, LayerAdaptation, LRSchedulerAlgorithm, MasterWeights, Mode, OptimizerState, Precision, RunOpts,
                     SampleSummary, Split)
 
 logging.basicConfig(level=logging.INFO, format="%(levelname)s (%(process)d) %(message)s")
@@ -52,6 +52,7 @@ ADAFACTOR_ENV = "FRL_B200_ADAFACTOR"               # "0" (default) | "1"
 MUON_ENV = "FRL_B200_MUON"                         # "0" (default) | "1"
 ADAMW_ENV = "FRL_B200_ADAMW"                       # "0" (default) | "1"
 CHANNELS_LAST_ENV = "FRL_B200_CHANNELS_LAST"       # "0" (default) | "1"
+MASTER_WEIGHTS_ENV = "FRL_B200_MASTER_WEIGHTS"     # "fp32" (default) | "bf16"
 EMA_SUFFIX = ".ema"                        # <checkpoint>.ema: the weight EMA next to a checkpoint
 
 
@@ -116,6 +117,9 @@ class SolverWorkerArgs(NamedTuple):
     # Placed before optimizer_state, adafactor, ema_decay and grad_accumulation, which keep their
     # positions at the end
     channels_last: Optional[bool] = None
+    # fp32 master weights or bf16 weights with stochastic rounding; placed before optimizer_state,
+    # adafactor, ema_decay and grad_accumulation, which keep their positions at the end
+    master_weights: MasterWeights = MasterWeights.FP32
     # Adam's state storage; placed before ema_decay and grad_accumulation, which stay the last fields
     optimizer_state: OptimizerState = OptimizerState.FP32
     # Adafactor instead of Adam; placed before ema_decay and grad_accumulation, which stay the last fields
@@ -322,6 +326,18 @@ def resolve_channels_last(explicit: Optional[bool] = None) -> bool:
     return raw == "1"
 
 
+def resolve_master_weights(explicit: Optional[MasterWeights] = None) -> MasterWeights:
+    """Where the model's authoritative weights live: ``explicit``, else FRL_B200_MASTER_WEIGHTS
+    (``fp32``, the default, or ``bf16``).  Any other value is a ValueError naming the variable."""
+    if explicit is not None:
+        return MasterWeights(explicit)
+    raw = os.environ.get(MASTER_WEIGHTS_ENV, "fp32").strip().lower()
+    try:
+        return MasterWeights(raw)
+    except ValueError:
+        raise ValueError("%s must be fp32 or bf16, got %r" % (MASTER_WEIGHTS_ENV, raw)) from None
+
+
 def check_channels_last(channels_last: bool, adafactor: bool) -> None:
     """Adafactor factors a conv weight's second moment per kh x kw slice of [O*I, kh, kw], which
     assumes NCHW element order: the two cannot be combined (ValueError)."""
@@ -447,15 +463,20 @@ class Solver:
         symm_alloc = None
         if (distributed and not run_opts.optim.gradientClip
                 and args.layer_adaptation == LayerAdaptation.NONE and accum == 1 and ema_decay == 0.0
-                and args.optimizer_state is OptimizerState.FP32 and not args.adafactor and not args.muon):
+                and args.optimizer_state is OptimizerState.FP32 and not args.adafactor and not args.muon
+                and not (MasterWeights(args.master_weights) is MasterWeights.BF16 and run_opts.mode == Mode.TRAIN)):
             from .symm import try_make_allocator
             symm_alloc = try_make_allocator(device, args.world_size)
         from .arena_linear import head_layout_groups
         channels_last = resolve_channels_last(args.channels_last)
         check_channels_last(channels_last, args.adafactor and run_opts.mode == Mode.TRAIN)
+        master_weights = MasterWeights(args.master_weights) if run_opts.mode == Mode.TRAIN else MasterWeights.FP32
+        check_master_weights(master_weights, args.precision, args.layer_adaptation, args.optimizer_state,
+                             args.adafactor, args.muon)
         arena = ParamArena(model.parameters(), criterion.parameters(), device=device,
                            precision=args.precision, shared_allocator=symm_alloc,
-                           adjacent=head_layout_groups(model), channels_last=channels_last)
+                           adjacent=head_layout_groups(model), channels_last=channels_last,
+                           master_weights=master_weights)
         if (args.precision.bf16_storage and any(b.is_floating_point() for b in model.buffers())
                 and not _norm_accepts_fp32_stats(device)):
             # BatchNorm running statistics stay fp32 (what the reference's checkpoints hold: a
@@ -531,7 +552,7 @@ class Solver:
                 "Linear layers with arena-born gradients %d (%d fused with their ReLU, %d in FP8) | "
                 "ReLU backward %s | "
                 "other gradients %s | layer adaptation %s | gradient accumulation %s | weight EMA %s | "
-                "optimizer %s | optimizer state %s | memory format %s",
+                "optimizer %s | optimizer state %s | memory format %s | master weights %s",
                 args.precision.value,
                 "CUDA-graph replay after 2 eager steps" if worker.graphed is not None else "eager launches",
                 ("fused NVLS kernel per bucket (K7), %d buckets" % len(pipeline.buckets)) if pipeline.nvls is not None
@@ -580,7 +601,9 @@ class Solver:
                     sum(s.numel for s in arena.slots if s.memory_format is torch.channels_last),
                     "batches NHWC from K5/K5a" if all(
                         getattr(getattr(d, "device_transform", None), "honours_memory_format", False)
-                        for d in problem.datasets) else "converted by the first convolution"))
+                        for d in problem.datasets) else "converted by the first convolution"),
+                "fp32" if not arena.bf16_master else
+                "bf16 + stochastic rounding, %.1f MiB saved" % (4 * arena.model_end / 2 ** 20))
         scheduler = create_lr_scheduler(run_opts, worker.optimizer,
                                         checkpoint.epoch if checkpoint else -1)
         return worker, scheduler, checkpoint
@@ -795,7 +818,8 @@ class Solver:
               adafactor: Optional[bool] = None,
               muon: Optional[bool] = None,
               adamw: Optional[bool] = None,
-              channels_last: Optional[bool] = None
+              channels_last: Optional[bool] = None,
+              master_weights: Optional[MasterWeights] = None
               ) -> Iterator[PerformanceSummary]:
         """The reference's entry point (solver.py:728-739) plus two keyword-only extensions:
 
@@ -918,6 +942,15 @@ class Solver:
                        Not combinable with Adafactor (``ValueError`` before a rank starts).  Honoured
                        by ``Mode.EVAL``.  None: FRL_B200_CHANNELS_LAST (``0`` by default, ``1`` to
                        enable); any other value raises ``ValueError``.
+        ``master_weights``  ``MasterWeights.FP32`` (default) or ``.BF16``: with BF16 the model's
+                       weights are kept in bf16 only, with no fp32 master (4 B per model parameter
+                       less), and every update rounds stochastically (``types.MasterWeights``).
+                       Needs precision BF16 or FP8 and SGD, Adam / AdamW or RMSprop; refused with
+                       ``ValueError`` before a rank starts with precision FP32, LARS / LAMB, Adafactor,
+                       Muon or 8-bit optimizer state.  Turns off the fused NVLS step (K7); on one GPU
+                       with SGD the dW-GEMM update (K12) runs its SR form.  ``Mode.EVAL`` ignores it.  None:
+                       FRL_B200_MASTER_WEIGHTS (``fp32`` by default, or ``bf16``); any other value
+                       raises ``ValueError``.
         """
         adapt = LayerAdaptation.NONE
         accum = 1
@@ -941,6 +974,10 @@ class Solver:
             decay = resolve_ema_decay(ema_decay)
         use_channels_last = resolve_channels_last(channels_last)
         check_channels_last(use_channels_last, use_adafactor)
+        use_master = MasterWeights.FP32
+        if run_opts.mode == Mode.TRAIN:
+            use_master = resolve_master_weights(master_weights)
+            check_master_weights(use_master, resolve_precision(precision), adapt, opt_state, use_adafactor, use_muon)
         n_visible = 0 if run_opts.cpuonly else _cuda_device_count_without_poisoning_fork()
         if n_visible == 0:
             raise RuntimeError(
@@ -981,7 +1018,7 @@ class Solver:
                 cache=None, precision=prec, save_every=save_every, graph_step=graph,
                 layer_adaptation=adapt, grad_accumulation=accum, ema_decay=decay,
                 optimizer_state=opt_state, adafactor=use_adafactor, muon=use_muon, adamw=use_adamw,
-                channels_last=use_channels_last)
+                channels_last=use_channels_last, master_weights=use_master)
             if not run_opts.singleThreaded:
                 parent_conn, child_conn = ctx.Pipe(duplex=False)
                 proc = ctx.Process(target=cls._solver_worker_process,

@@ -139,6 +139,31 @@ class OptimizerState(Enum):
     Q8 = "8bit"
 
 
+class MasterWeights(Enum):
+    """Extension (not in the reference): where the authoritative copy of the model's weights lives
+    in a BF16 / FP8 run, chosen with ``Solver.solve(..., master_weights=...)`` or
+    ``FRL_B200_MASTER_WEIGHTS``.
+
+    FP32 - an fp32 master vector beside the bf16 weights forward and backward read; every update
+           reads and rewrites the master and writes the bf16 copy (round to nearest even).
+    BF16 - the bf16 weights are the only copy of the model range ``[0, model_end)`` of the arena: 4 B
+           per model parameter less resident memory.  Every update widens the bf16 weight to fp32,
+           applies the unchanged fp32 rule and rounds the result stochastically back to bf16 (K2-sr /
+           K2-mt-sr), so that the expected stored weight equals the fp32 result and updates below half
+           a bf16 ulp are not lost.  The 16 random bits of arena element ``i`` at update ``t`` come
+           from Philox4x32-10 keyed by the optimizer's ``sr_seed`` (include/frl_b200.h, K2-sr); the
+           param group keeps ``sr_seed`` and ``sr_updates``, so a resumed run continues bit for bit.
+           Criterion parameters keep their fp32 master.  Checkpoints keep their fp32 format (the
+           values are bf16-exact) and load in either mode.  Allowed with SGD, Adam / AdamW and RMSprop
+           in ``Precision.BF16`` / ``FP8``; refused with ``Precision.FP32``, layer adaptation, 8-bit
+           optimizer state, Adafactor and Muon.  On one GPU with SGD the dW-GEMM update (K12) runs its
+           stochastic-rounding form; with several GPUs the fused NVLS step (K7) is not used.  The EMA
+           file keeps the fp32 EMA itself.  ``Mode.EVAL`` ignores the setting.
+    """
+    FP32 = "fp32"
+    BF16 = "bf16"
+
+
 # --- records ---------------------------------------------------------------------------------
 
 class SampleSummary(NamedTuple):

@@ -119,6 +119,14 @@ int frl_dw_gemm_sgd(const void* dz, int64_t ld_dz, const void* x, int64_t ld_x, 
                     int64_t out, int64_t in, void* gw, float* p, float* buf, void* p_lp,
                     double lr, double mu, double dampening, double wd, double grad_scale,
                     const float* dyn, int first_step, void* stream);
+/* frl_dw_gemm_sgd_sr: frl_dw_gemm_sgd for bf16 master weights (K2-sr below): p is the slice's bf16
+ * weights (no shadow), arena_off the arena index of p's element 0 (a multiple of 4), seed and t as in
+ * frl_sgd_momentum_sr, dyn[3] = t's bits under replay.  Bit-identical to frl_dw_gemm followed by
+ * frl_sgd_momentum_sr(g_dtype = FRL_BF16) over the slice. */
+int frl_dw_gemm_sgd_sr(const void* dz, int64_t ld_dz, const void* x, int64_t ld_x, int64_t rows,
+                       int64_t out, int64_t in, void* gw, void* p, float* buf, int64_t arena_off, uint64_t seed,
+                       int64_t t, double lr, double mu, double dampening, double wd, double grad_scale,
+                       const float* dyn, int first_step, void* stream);
 
 /* ------------------------------------------------------------------------------------------
  * K13 — data-gradient GEMM of an upper Linear layer with the lower Linear+ReLU unit's backward in
@@ -185,6 +193,54 @@ int frl_rmsprop_mt(float* p, float* sq, float* buf, void* p_lp, const frl_grad_s
                    const int64_t* tile_prefix_dev, const int32_t* tile_seg_dev, int64_t n_tiles, double lr, double alpha,
                    double eps, double wd, double mu, double grad_scale, const float* grad_scale_dev,
                    const float* dyn, void* stream);
+
+/* ------------------------------------------------------------------------------------------
+ * K2-sr / K2-mt-sr — the K2 / K2-mt update on bf16 master weights with stochastic rounding
+ * (an extension, types.MasterWeights.BF16: no fp32 copy of the model's weights exists).
+ * Arguments: those of the fp32 form, except that p is the bf16 weight vector (there is no
+ * separate p_lp), plus arena_off (flat forms: the arena index of p's element 0, a multiple of 4),
+ * seed and t.  The _mt_sr forms take p as the ARENA BASE of the bf16 weights and list model slots.
+ * Per element: widen the bf16 weight to fp32, apply the fp32 form's rule unchanged, store
+ *     bf16 bits = (bits(x) + r) >> 16          (x NaN: 0x7FC0)
+ * where r, the 16 random bits of arena element i at update t (the optimizer's 1-based update
+ * count; the Adam forms use their step), are the low 16 bits of word (i & 3) of
+ *     Philox4x32-10(counter = (lo32(i >> 2), hi32(i >> 2), t, 0x53520000),
+ *                   key     = (lo32(seed), hi32(seed))).
+ * That rounds the magnitude up with probability (discarded fraction) / 2^16, so the expected
+ * stored value is x: +-inf and bf16-exact values never change, a finite value reaches inf only
+ * by carrying out of 0x7F7F.  dyn: the fp32 form's layout, and dyn[3] holds t as a uint32 bit
+ * pattern (it then replaces the t argument).  Graph-capturable.
+ * frl_weight_ema_bf16: frl_weight_ema with p a bf16 vector (10 B per element instead of 12).
+ * ---------------------------------------------------------------------------------------- */
+int frl_sgd_momentum_sr(void* p, const void* g, float* buf, int64_t n, int64_t arena_off, uint64_t seed,
+                        int64_t t, double lr, double mu, double dampening, double wd, double grad_scale,
+                        const float* grad_scale_dev, const float* dyn, int first_step, int g_dtype, void* stream);
+int frl_adam_sr(void* p, const void* g, float* m, float* v, float* vmax, int64_t n, int64_t arena_off,
+                uint64_t seed, double lr, double beta1, double beta2, double eps, double wd, int64_t step,
+                double grad_scale, const float* grad_scale_dev, const float* dyn, int g_dtype, void* stream);
+int frl_adamw_sr(void* p, const void* g, float* m, float* v, float* vmax, int64_t n, int64_t arena_off,
+                 uint64_t seed, double lr, double beta1, double beta2, double eps, double wd, int64_t step,
+                 double grad_scale, const float* grad_scale_dev, const float* dyn, int g_dtype, void* stream);
+int frl_rmsprop_sr(void* p, const void* g, float* sq, float* buf, int64_t n, int64_t arena_off, uint64_t seed,
+                   int64_t t, double lr, double alpha, double eps, double wd, double mu, double grad_scale,
+                   const float* grad_scale_dev, const float* dyn, int g_dtype, void* stream);
+int frl_sgd_momentum_mt_sr(void* p, float* buf, const frl_grad_seg* segs_dev, const int64_t* tile_prefix_dev,
+                           const int32_t* tile_seg_dev, int64_t n_tiles, uint64_t seed, int64_t t, double lr,
+                           double mu, double dampening, double wd, double grad_scale, const float* grad_scale_dev,
+                           const float* dyn, int first_step, void* stream);
+int frl_adam_mt_sr(void* p, float* m, float* v, float* vmax, const frl_grad_seg* segs_dev,
+                   const int64_t* tile_prefix_dev, const int32_t* tile_seg_dev, int64_t n_tiles, uint64_t seed,
+                   double lr, double beta1, double beta2, double eps, double wd, int64_t step, double grad_scale,
+                   const float* grad_scale_dev, const float* dyn, void* stream);
+int frl_adamw_mt_sr(void* p, float* m, float* v, float* vmax, const frl_grad_seg* segs_dev,
+                    const int64_t* tile_prefix_dev, const int32_t* tile_seg_dev, int64_t n_tiles, uint64_t seed,
+                    double lr, double beta1, double beta2, double eps, double wd, int64_t step, double grad_scale,
+                    const float* grad_scale_dev, const float* dyn, void* stream);
+int frl_rmsprop_mt_sr(void* p, float* sq, float* buf, const frl_grad_seg* segs_dev, const int64_t* tile_prefix_dev,
+                      const int32_t* tile_seg_dev, int64_t n_tiles, uint64_t seed, int64_t t, double lr,
+                      double alpha, double eps, double wd, double mu, double grad_scale,
+                      const float* grad_scale_dev, const float* dyn, void* stream);
+int frl_weight_ema_bf16(float* ema, const void* p, int64_t n, double w, void* stream);
 
 /* ------------------------------------------------------------------------------------------
  * K2-lw — layer-wise adaptive updates over a segment table (an extension: the reference offers
