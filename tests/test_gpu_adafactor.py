@@ -89,7 +89,8 @@ def _reference(case, dtype=torch.float64):
     a = case.arena
     params = [torch.nn.Parameter(a.master[s.offset:s.end].view(s.shape).to(dtype).clone()) for s in a.slots]
     h = case.opt.hyper
-    ref = torch.optim.Adafactor(params, lr=h["lr"], weight_decay=h["weight_decay"], eps=EPS, foreach=False)
+    ref = torch.optim.Adafactor(params, lr=h["lr"], beta2_decay=h["beta2_decay"], d=h["d"],
+                                weight_decay=h["weight_decay"], eps=EPS, foreach=False)
     if case.opt._steps:
         sd = case.opt.state_dict()
         sd["param_groups"][0]["eps"] = EPS
@@ -102,12 +103,15 @@ def _check_step(case, gs, coef):
     ref, params = _reference(case)
     before = [p.detach().clone() for p in params]
     for p, g in zip(params, case.g_eff(gs, coef)):
-        p.grad = g.view(p.shape)
+        p.grad = g.view(p.shape) if p.numel() else None      # torch divides by numel
     ref.step()
     coef_dev = torch.tensor([coef], device=DEV) if coef != 1.0 else None
     case.step(gs, coef_dev)
     torch.cuda.synchronize()
     for s, p, p0 in zip(a.slots, params, before):
+        if s.numel == 0:                                     # no band: its state stays zero
+            assert not any(bool(v.any()) for v in case.opt._slot_state(s).values()), s.shape
+            continue
         got = a.master[s.offset:s.end].view(s.shape).double()
         want = p.detach()
         step = (want - p0).abs().max().item()
