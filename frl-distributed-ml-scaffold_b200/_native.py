@@ -58,12 +58,17 @@ SIGNATURES = {
     "frl_sgd_momentum": (_i, [_vp, _vp, _vp, _vp, _i64, _d, _d, _d, _d, _d, _vp, _vp, _i, _i, _vp]),
     "frl_adam": (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _i64, _d, _d, _d, _d, _d, _i64, _d, _vp, _vp, _i, _vp]),
     "frl_adamw": (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _i64, _d, _d, _d, _d, _d, _i64, _d, _vp, _vp, _i, _vp]),
+    "frl_lion": (_i, [_vp, _vp, _vp, _vp, _i64, _d, _d, _d, _d, _d, _vp, _vp, _i, _vp]),
     "frl_rmsprop": (_i, [_vp, _vp, _vp, _vp, _vp, _i64, _d, _d, _d, _d, _d, _d, _vp, _vp, _i, _vp]),
     "frl_dw_gemm": (_i, [_vp, _i64, _vp, _i64, _i64, _i64, _i64, _vp, _vp]),
     "frl_dw_gemm_sgd": (_i, [_vp, _i64, _vp, _i64, _i64, _i64, _i64, _vp, _vp, _vp, _vp, _d, _d, _d, _d, _d,
                              _vp, _i, _vp]),
     "frl_dw_gemm_sgd_sr": (_i, [_vp, _i64, _vp, _i64, _i64, _i64, _i64, _vp, _vp, _vp, _i64, _u64, _i64, _d, _d,
                                 _d, _d, _d, _vp, _i, _vp]),
+    "frl_dw_gemm_lion": (_i, [_vp, _i64, _vp, _i64, _i64, _i64, _i64, _vp, _vp, _vp, _vp, _d, _d, _d, _d, _d,
+                              _vp, _vp]),
+    "frl_dw_gemm_lion_sr": (_i, [_vp, _i64, _vp, _i64, _i64, _i64, _i64, _vp, _vp, _vp, _i64, _u64, _i64, _d, _d,
+                                 _d, _d, _d, _vp, _vp]),
     "frl_dx_drelu_scratch_bytes": (_i64, [_i64, _i64]),
     "frl_dx_gemm_drelu": (_i, [_vp, _i64, _vp, _i64, _vp, _i64, _vp, _i64, _vp, _i64, _i64, _i64, _i, _vp, _vp]),
     "frl_mt_tile_elems": (_i64, []),
@@ -71,10 +76,12 @@ SIGNATURES = {
     "frl_sgd_momentum_mt": (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _i64, _d, _d, _d, _d, _d, _vp, _vp, _i, _vp]),
     "frl_adam_mt": (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _i64, _d, _d, _d, _d, _d, _i64, _d, _vp, _vp, _vp]),
     "frl_adamw_mt": (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _i64, _d, _d, _d, _d, _d, _i64, _d, _vp, _vp, _vp]),
+    "frl_lion_mt": (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _i64, _d, _d, _d, _d, _d, _vp, _vp, _vp]),
     "frl_rmsprop_mt": (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _i64, _d, _d, _d, _d, _d, _d, _vp, _vp, _vp]),
     "frl_sgd_momentum_sr": (_i, [_vp, _vp, _vp, _i64, _i64, _u64, _i64, _d, _d, _d, _d, _d, _vp, _vp, _i, _i, _vp]),
     "frl_adam_sr": (_i, [_vp, _vp, _vp, _vp, _vp, _i64, _i64, _u64, _d, _d, _d, _d, _d, _i64, _d, _vp, _vp, _i, _vp]),
     "frl_adamw_sr": (_i, [_vp, _vp, _vp, _vp, _vp, _i64, _i64, _u64, _d, _d, _d, _d, _d, _i64, _d, _vp, _vp, _i, _vp]),
+    "frl_lion_sr": (_i, [_vp, _vp, _vp, _i64, _i64, _u64, _i64, _d, _d, _d, _d, _d, _vp, _vp, _i, _vp]),
     "frl_rmsprop_sr": (_i, [_vp, _vp, _vp, _vp, _i64, _i64, _u64, _i64, _d, _d, _d, _d, _d, _d, _vp, _vp, _i, _vp]),
     "frl_sgd_momentum_mt_sr": (_i, [_vp, _vp, _vp, _vp, _vp, _i64, _u64, _i64, _d, _d, _d, _d, _d, _vp, _vp, _i,
                                     _vp]),
@@ -82,6 +89,7 @@ SIGNATURES = {
                             _vp]),
     "frl_adamw_mt_sr": (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _i64, _u64, _d, _d, _d, _d, _d, _i64, _d, _vp, _vp,
                              _vp]),
+    "frl_lion_mt_sr": (_i, [_vp, _vp, _vp, _vp, _vp, _i64, _u64, _i64, _d, _d, _d, _d, _d, _vp, _vp, _vp]),
     "frl_rmsprop_mt_sr": (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _i64, _u64, _i64, _d, _d, _d, _d, _d, _d, _vp, _vp,
                                _vp]),
     "frl_weight_ema_bf16": (_i, [_vp, _vp, _i64, _d, _vp]),
@@ -141,6 +149,8 @@ SIGNATURES = {
                            _i64, _d, _vp, _i, _i, _vp]),
     "frl_nvls_adamw": (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _i64, _i, _i, _vp, _i, _vp, _i, _d, _d, _d, _d, _d,
                             _i64, _d, _vp, _i, _i, _vp]),
+    "frl_nvls_lion": (_i, [_vp, _vp, _vp, _vp, _i64, _i, _i, _vp, _i, _vp, _i, _d, _d, _d, _d, _d, _vp, _i, _i,
+                           _vp]),
     "frl_nvls_rmsprop": (_i, [_vp, _vp, _vp, _vp, _vp, _i64, _i, _i, _vp, _i, _vp, _i, _d, _d, _d, _d, _d, _d,
                               _vp, _i, _i, _vp]),
     "frl_nvls_barrier": (_i, [_vp, _i, _i, _i, _vp]),
@@ -239,6 +249,13 @@ def adamw(p, g, m, v, vmax, p_lp, n, *, lr, beta1, beta2, eps, wd, step, grad_sc
                            dtype_code(g.dtype), _stream()), "frl_adamw")
 
 
+def lion(p, g, m, p_lp, n, *, lr, beta1, beta2, wd, grad_scale=1.0, grad_scale_dev=None, dyn=None) -> None:
+    """K2 Lion: ``sgd_momentum``'s arguments with (beta1, beta2) for (mu, dampening), m = exp_avg, ``wd``
+    decoupled (see frl_lion in include/frl_b200.h)."""
+    _check(lib().frl_lion(_ptr(p), _ptr(g), _ptr(m), _ptr(p_lp), n, lr, beta1, beta2, wd, grad_scale,
+                          _ptr(grad_scale_dev), _ptr(dyn), dtype_code(g.dtype), _stream()), "frl_lion")
+
+
 def rmsprop(p, g, sq, buf, p_lp, n, *, lr, alpha, eps, wd, mu, grad_scale=1.0,
             grad_scale_dev=None, dyn=None) -> None:
     _check(lib().frl_rmsprop(_ptr(p), _ptr(g), _ptr(sq), _ptr(buf), _ptr(p_lp), n, lr, alpha,
@@ -285,6 +302,24 @@ def dw_gemm_sgd_sr(dz, x, gw, p, buf, *, arena_off, seed, t, lr, mu, dampening, 
     _check(lib().frl_dw_gemm_sgd_sr(_ptr(dz), dz.stride(0), _ptr(x), x.stride(0), dz.shape[0], dz.shape[1],
                                     x.shape[1], _ptr(gw), _ptr(p), _ptr(buf), arena_off, seed, t, lr, mu, dampening,
                                     wd, grad_scale, _ptr(dyn), int(first_step), _stream()), "frl_dw_gemm_sgd_sr")
+
+
+def dw_gemm_lion(dz, x, gw, p, m, p_lp, *, lr, beta1, beta2, wd, grad_scale=1.0, dyn=None) -> None:
+    """gw = dz^T x, then ``lion``'s update of the [out, in] slices p / m / p_lp from it."""
+    _check(lib().frl_dw_gemm_lion(_ptr(dz), dz.stride(0), _ptr(x), x.stride(0), dz.shape[0], dz.shape[1],
+                                  x.shape[1], _ptr(gw), _ptr(p), _ptr(m), _ptr(p_lp), lr, beta1, beta2, wd,
+                                  grad_scale, _ptr(dyn), _stream()), "frl_dw_gemm_lion")
+
+
+def dw_gemm_lion_sr(dz, x, gw, p, m, *, arena_off, seed, t, lr, beta1, beta2, wd, grad_scale=1.0,
+                    dyn=None) -> None:
+    """gw = dz^T x, then ``lion_sr``'s update of the bf16 [out, in] weights p (arena elements from
+    ``arena_off``) and m from it."""
+    if p.dtype != torch.bfloat16:
+        raise NativeLibraryError("dw_gemm_lion_sr: p must be the bf16 weights, got %s" % p.dtype)
+    _check(lib().frl_dw_gemm_lion_sr(_ptr(dz), dz.stride(0), _ptr(x), x.stride(0), dz.shape[0], dz.shape[1],
+                                     x.shape[1], _ptr(gw), _ptr(p), _ptr(m), arena_off, seed, t, lr, beta1, beta2,
+                                     wd, grad_scale, _ptr(dyn), _stream()), "frl_dw_gemm_lion_sr")
 
 
 # ---- K13: data-gradient GEMM with the lower unit's ReLU backward and bias gradient in its epilogue --
@@ -363,6 +398,13 @@ def adamw_mt(p, m, v, vmax, p_lp, table, *, lr, beta1, beta2, eps, wd, step, gra
                               step, grad_scale, _ptr(grad_scale_dev), _ptr(dyn), _stream()), "frl_adamw_mt")
 
 
+def lion_mt(p, m, p_lp, table, *, lr, beta1, beta2, wd, grad_scale=1.0, grad_scale_dev=None, dyn=None) -> None:
+    """K2-mt Lion: ``lion``'s rule over a segment table (see frl_lion_mt)."""
+    _check(lib().frl_lion_mt(_ptr(p), _ptr(m), _ptr(p_lp), table.segs_dev_ptr, table.prefix_dev_ptr,
+                             table.tile_seg_dev_ptr, table.n_tiles, lr, beta1, beta2, wd, grad_scale,
+                             _ptr(grad_scale_dev), _ptr(dyn), _stream()), "frl_lion_mt")
+
+
 def rmsprop_mt(p, sq, buf, p_lp, table, *, lr, alpha, eps, wd, mu, grad_scale=1.0, grad_scale_dev=None,
                dyn=None) -> None:
     _check(lib().frl_rmsprop_mt(_ptr(p), _ptr(sq), _ptr(buf), _ptr(p_lp), table.segs_dev_ptr,
@@ -405,6 +447,15 @@ def adamw_sr(p, g, m, v, vmax, n, *, arena_off, seed, lr, beta1, beta2, eps, wd,
                               _stream()), "frl_adamw_sr")
 
 
+def lion_sr(p, g, m, n, *, arena_off, seed, t, lr, beta1, beta2, wd, grad_scale=1.0, grad_scale_dev=None,
+            dyn=None) -> None:
+    """K2-sr Lion: ``lion`` on bf16 weights p (arena elements from ``arena_off``), stored rounded
+    stochastically with the draws of update ``t`` (see frl_lion_sr)."""
+    _check_sr(p, seed)
+    _check(lib().frl_lion_sr(_ptr(p), _ptr(g), _ptr(m), n, arena_off, seed, t, lr, beta1, beta2, wd, grad_scale,
+                             _ptr(grad_scale_dev), _ptr(dyn), dtype_code(g.dtype), _stream()), "frl_lion_sr")
+
+
 def rmsprop_sr(p, g, sq, buf, n, *, arena_off, seed, t, lr, alpha, eps, wd, mu, grad_scale=1.0,
                grad_scale_dev=None, dyn=None) -> None:
     _check_sr(p, seed)
@@ -437,6 +488,15 @@ def adamw_mt_sr(p, m, v, vmax, table, *, seed, lr, beta1, beta2, eps, wd, step, 
     _check(lib().frl_adamw_mt_sr(_ptr(p), _ptr(m), _ptr(v), _ptr(vmax), table.segs_dev_ptr, table.prefix_dev_ptr,
                                  table.tile_seg_dev_ptr, table.n_tiles, seed, lr, beta1, beta2, eps, wd, step,
                                  grad_scale, _ptr(grad_scale_dev), _ptr(dyn), _stream()), "frl_adamw_mt_sr")
+
+
+def lion_mt_sr(p, m, table, *, seed, t, lr, beta1, beta2, wd, grad_scale=1.0, grad_scale_dev=None,
+               dyn=None) -> None:
+    """K2-mt-sr Lion: ``lion_mt`` on the bf16 weights' arena base p (see frl_lion_mt_sr)."""
+    _check_sr(p, seed)
+    _check(lib().frl_lion_mt_sr(_ptr(p), _ptr(m), table.segs_dev_ptr, table.prefix_dev_ptr, table.tile_seg_dev_ptr,
+                                table.n_tiles, seed, t, lr, beta1, beta2, wd, grad_scale, _ptr(grad_scale_dev),
+                                _ptr(dyn), _stream()), "frl_lion_mt_sr")
 
 
 def rmsprop_mt_sr(p, sq, buf, table, *, seed, t, lr, alpha, eps, wd, mu, grad_scale=1.0, grad_scale_dev=None,
@@ -925,6 +985,13 @@ def nvls_adamw(p, m, v, vmax, mc_g, mc_out, n, link, *, lr, beta1, beta2, eps, w
                                 link.world, link.pads_dev, link.pad_base, _ptr(link.scratch), link.max_blocks, lr,
                                 beta1, beta2, eps, wd, step, grad_scale, _ptr(dyn), g_dtype, link.flags, _stream()),
            "frl_nvls_adamw")
+
+
+def nvls_lion(p, m, mc_g, mc_out, n, link, *, lr, beta1, beta2, wd, grad_scale, g_dtype, dyn=None) -> None:
+    """K7 Lion: ``nvls_sgd``'s arguments with (beta1, beta2) for (mu, dampening), m = exp_avg."""
+    _check(lib().frl_nvls_lion(_ptr(p), _ptr(m), mc_g, mc_out, n, link.rank, link.world, link.pads_dev,
+                               link.pad_base, _ptr(link.scratch), link.max_blocks, lr, beta1, beta2, wd, grad_scale,
+                               _ptr(dyn), g_dtype, link.flags, _stream()), "frl_nvls_lion")
 
 
 def nvls_rmsprop(p, sq, buf, mc_g, mc_out, n, link, *, lr, alpha, eps, wd, mu, grad_scale, g_dtype,

@@ -1,4 +1,4 @@
-// K12 — weight-gradient GEMM dW = dZ^T X with the SGD update in its epilogue (sm_90a).
+// K12 — weight-gradient GEMM dW = dZ^T X with the SGD or Lion update in its epilogue (sm_90a).
 //
 // dZ is [B, out] and X is [B, in], both row-major bf16, so both WGMMA operands are MN-major
 // (legal for 16-bit types) and dW [out, in] comes out row-major, exactly the weight's slice of
@@ -12,7 +12,7 @@
 //   warps 1..3          epilogue: drain the staging tile row by row while the consumers run the
 //                       next tile's main loop (a CTA's last tile: with the 8 consumer warps).
 //                       Plain mode writes the bf16 gradient.  Update mode writes it too -- every
-//                       reader of the arena's gradient stays correct -- and applies SgdRule to
+//                       reader of the arena's gradient stays correct -- and applies the rule to
 //                       exactly that bf16 value: fp32 master and momentum read and written in
 //                       16-byte row-contiguous accesses, bf16 shadow written.  The rule is K2's,
 //                       with the same device-resident scalars, so the update is bit-identical to
@@ -22,6 +22,9 @@
 // 1.9 TB/s spread over the main loops of a CTA's later tiles, so most of it runs under the
 // tensor-core work instead of as a separate memory-bound pass after backward.  What stays exposed
 // is each CTA's last tile, whose update has no main loop left to hide under.
+//
+// frl_dw_gemm_lion / frl_dw_gemm_lion_sr run LionRule in the same epilogue (exp_avg in the momentum
+// buffer's place, the same 20 B / 14 B per weight): frl_dw_gemm followed by frl_lion / frl_lion_sr.
 //
 // frl_dw_gemm_sgd_sr is the same kernel body for bf16 master weights (types.MasterWeights.BF16): the
 // epilogue reads the bf16 weights instead of an fp32 master and stores the SGD result rounded
@@ -55,39 +58,49 @@ constexpr int kSmemBytes = 1024 + kStages * kStageBytes + kStagingBytes + 256;
 static_assert(kBK % 16 == 0 && kBK <= 256, "k-block must be a multiple of the WGMMA K");
 static_assert(kSmemBytes <= 227 * 1024, "shared memory plan exceeds one CTA per SM");
 
+template <typename Rule>
 struct Update {
     float* master;          // fp32 master weights of the slice, [out, in]
-    float* mom;             // momentum buffer of the slice (null: SGD without momentum)
+    float* mom;             // the rule's state of the slice (null: SGD without momentum)
     __nv_bfloat16* lp;      // bf16 shadow of the slice (null: none)
-    SgdRule rule;
+    Rule rule;
     float gscale;
-    const float* dyn;       // device-resident lr (null: the rule's by-value lr)
+    const float* dyn;       // device-resident per-step scalars (null: the rule's by-value ones)
 };
 
 // bf16 master weights: the slice's bf16 weights are the weights; off = arena index of its element 0
+template <typename Rule>
 struct UpdateSr {
     __nv_bfloat16* w;       // bf16 weights of the slice, [out, in]
-    float* mom;             // momentum buffer of the slice (null: SGD without momentum)
-    SgdRule rule;
+    float* mom;             // the rule's state of the slice (null: SGD without momentum)
+    Rule rule;
     float gscale;
-    const float* dyn;       // device-resident lr and (dyn[3]) update count (null: by value)
+    const float* dyn;       // device-resident scalars and (dyn[3]) update count (null: by value)
     int64_t off;
     uint64_t seed;
     uint32_t t;
 };
 
-__device__ __forceinline__ void patch(Update& u) {
+template <typename U> struct IsSr : std::false_type {};
+template <typename Rule> struct IsSr<UpdateSr<Rule>> : std::true_type {};
+
+template <typename Rule>
+__device__ __forceinline__ void patch(Update<Rule>& u) {
     if (u.dyn) u.rule.patch(u.dyn);
 }
-__device__ __forceinline__ void patch(UpdateSr& u) {
+template <typename Rule>
+__device__ __forceinline__ void patch(UpdateSr<Rule>& u) {
     if (u.dyn) {
         u.rule.patch(u.dyn);
         u.t = __float_as_uint(__ldg(u.dyn + 3));
     }
 }
 
-__device__ __forceinline__ void sgd4(const SgdRule& r, f32x4& p, f32x4& m, float g0, float g1, float g2,
-                                     float g3, float gs) {
+// the rule over 4 elements with one state (SgdRule: the momentum buffer, LionRule: exp_avg)
+template <typename Rule>
+__device__ __forceinline__ void rule4(const Rule& r, f32x4& p, f32x4& m, float g0, float g1, float g2,
+                                      float g3, float gs) {
+    static_assert(Rule::kStates == 1, "the dW epilogue carries one state vector");
     float dummy0 = 0.f, dummy1 = 0.f;
     r(p.x, g0 * gs, m.x, dummy0, dummy1);
     r(p.y, g1 * gs, m.y, dummy0, dummy1);
@@ -95,10 +108,11 @@ __device__ __forceinline__ void sgd4(const SgdRule& r, f32x4& p, f32x4& m, float
     r(p.w, g3 * gs, m.w, dummy0, dummy1);
 }
 
-// epilogue_rows' access pattern for bf16 master weights: weights read and written as bf16, the SGD
+// epilogue_rows' access pattern for bf16 master weights: weights read and written as bf16, the rule's
 // result of the bf16 gradient stored with stochastic rounding at the weight's arena index
+template <typename Rule>
 __device__ __forceinline__ void epilogue_rows_sr(const uint8_t* staging, __nv_bfloat16* gw, int64_t ld,
-                                                 int64_t m0, int64_t n0, const UpdateSr& u, int e, int n,
+                                                 int64_t m0, int64_t n0, const UpdateSr<Rule>& u, int e, int n,
                                                  int lane) {
     constexpr int kRowsAtOnce = 4;
     for (int r0 = e; r0 < kBM; r0 += n * kRowsAtOnce) {
@@ -130,7 +144,7 @@ __device__ __forceinline__ void epilogue_rows_sr(const uint8_t* staging, __nv_bf
                 st_stream(reinterpret_cast<bf16x4*>(gw + row + col), g[j][h]);
                 f32x4 q{bf16lo(w[j][h].a), bf16hi(w[j][h].a), bf16lo(w[j][h].b), bf16hi(w[j][h].b)};
                 f32x4 s = u.mom ? m[j][h] : f32x4{0.f, 0.f, 0.f, 0.f};
-                sgd4(u.rule, q, s, bf16lo(g[j][h].a), bf16hi(g[j][h].a), bf16lo(g[j][h].b), bf16hi(g[j][h].b),
+                rule4(u.rule, q, s, bf16lo(g[j][h].a), bf16hi(g[j][h].a), bf16lo(g[j][h].b), bf16hi(g[j][h].b),
                      u.gscale);
                 const Philox4 d = sr_draws(static_cast<uint64_t>(u.off + row + col) >> 2, u.t, u.seed);
                 st_stream(reinterpret_cast<bf16x4*>(u.w + row + col),
@@ -148,7 +162,7 @@ __device__ __forceinline__ void epilogue_rows_sr(const uint8_t* staging, __nv_bf
 template <bool UPDATE, typename U>
 __device__ __forceinline__ void epilogue_rows(const uint8_t* staging, __nv_bfloat16* gw, int64_t ld,
                                               int64_t m0, int64_t n0, const U& u, int e, int n, int lane) {
-    constexpr bool SR = std::is_same<U, UpdateSr>::value;
+    constexpr bool SR = IsSr<U>::value;
     if constexpr (SR) {
         epilogue_rows_sr(staging, gw, ld, m0, n0, u, e, n, lane);
         return;
@@ -183,7 +197,7 @@ __device__ __forceinline__ void epilogue_rows(const uint8_t* staging, __nv_bfloa
                 st_stream(reinterpret_cast<bf16x4*>(gw + row + col), g[j][h]);
                 if (UPDATE) {
                     f32x4 q = p[j][h], s = u.mom ? m[j][h] : f32x4{0.f, 0.f, 0.f, 0.f};
-                    sgd4(u.rule, q, s, bf16lo(g[j][h].a), bf16hi(g[j][h].a), bf16lo(g[j][h].b),
+                    rule4(u.rule, q, s, bf16lo(g[j][h].a), bf16hi(g[j][h].a), bf16lo(g[j][h].b),
                          bf16hi(g[j][h].b), u.gscale);
                     st_stream(reinterpret_cast<f32x4*>(u.master + row + col), q);
                     if (u.mom) st_stream(reinterpret_cast<f32x4*>(u.mom + row + col), s);
@@ -312,16 +326,17 @@ __device__ __forceinline__ void dw_gemm_body(const CUtensorMap& tm_dz, const CUt
     }
 }
 
-template <bool UPDATE>
+template <bool UPDATE, typename Rule>
 __global__ void __launch_bounds__(kThreads, 1)
 dw_gemm_kernel(const __grid_constant__ CUtensorMap tm_dz, const __grid_constant__ CUtensorMap tm_x,
-               int M, int N, int K, __nv_bfloat16* __restrict__ gw, Update u) {
+               int M, int N, int K, __nv_bfloat16* __restrict__ gw, Update<Rule> u) {
     dw_gemm_body<UPDATE>(tm_dz, tm_x, M, N, K, gw, u);
 }
 
+template <typename Rule>
 __global__ void __launch_bounds__(kThreads, 1)
 dw_gemm_sr_kernel(const __grid_constant__ CUtensorMap tm_dz, const __grid_constant__ CUtensorMap tm_x,
-                  int M, int N, int K, __nv_bfloat16* __restrict__ gw, UpdateSr u) {
+                  int M, int N, int K, __nv_bfloat16* __restrict__ gw, UpdateSr<Rule> u) {
     dw_gemm_body<true>(tm_dz, tm_x, M, N, K, gw, u);
 }
 
@@ -349,7 +364,7 @@ static int launch(Kernel kernel, const void* dz, int64_t ld_dz, const void* x, i
     FRL_REQUIRE(encode(&tm_dz, dz, rows, out, ld_dz) && encode(&tm_x, x, rows, in, ld_x), FRL_E_ARG,
                 "%s: cuTensorMapEncodeTiled failed", name);
     // set once per kernel (idempotent, so a repeat for another kernel of the same type costs a call)
-    static const void* attr_set[3] = {nullptr, nullptr, nullptr};
+    static const void* attr_set[5] = {nullptr, nullptr, nullptr, nullptr, nullptr};
     const void* key = reinterpret_cast<const void*>(kernel);
     bool have = false;
     for (const void* k : attr_set) have = have || k == key;
@@ -374,8 +389,8 @@ using namespace frl;
 
 extern "C" int frl_dw_gemm(const void* dz, int64_t ld_dz, const void* x, int64_t ld_x, int64_t rows,
                            int64_t out, int64_t in, void* gw, void* stream) {
-    dw::Update u{};
-    return dw::launch(dw::dw_gemm_kernel<false>, dz, ld_dz, x, ld_x, rows, out, in, gw, u, nullptr, nullptr, nullptr,
+    dw::Update<SgdRule> u{};
+    return dw::launch(dw::dw_gemm_kernel<false, SgdRule>, dz, ld_dz, x, ld_x, rows, out, in, gw, u, nullptr, nullptr, nullptr,
                       static_cast<cudaStream_t>(stream), "frl_dw_gemm");
 }
 
@@ -385,9 +400,9 @@ extern "C" int frl_dw_gemm_sgd(const void* dz, int64_t ld_dz, const void* x, int
                                const float* dyn, int first_step, void* stream) {
     FRL_REQUIRE(p, FRL_E_ARG, "frl_dw_gemm_sgd: null master");
     FRL_REQUIRE(mu == 0.0 || buf != nullptr, FRL_E_ARG, "frl_dw_gemm_sgd: momentum needs buf");
-    dw::Update u{p, mu != 0.0 ? buf : nullptr, static_cast<__nv_bfloat16*>(p_lp),
+    dw::Update<SgdRule> u{p, mu != 0.0 ? buf : nullptr, static_cast<__nv_bfloat16*>(p_lp),
                  make_sgd_rule(lr, mu, dampening, wd, first_step), static_cast<float>(grad_scale), dyn};
-    return dw::launch(dw::dw_gemm_kernel<true>, dz, ld_dz, x, ld_x, rows, out, in, gw, u, u.master, u.mom, u.lp,
+    return dw::launch(dw::dw_gemm_kernel<true, SgdRule>, dz, ld_dz, x, ld_x, rows, out, in, gw, u, u.master, u.mom, u.lp,
                       static_cast<cudaStream_t>(stream), "frl_dw_gemm_sgd");
 }
 
@@ -401,9 +416,38 @@ extern "C" int frl_dw_gemm_sgd_sr(const void* dz, int64_t ld_dz, const void* x, 
                 "frl_dw_gemm_sgd_sr: arena offset %lld is not a multiple of 4", static_cast<long long>(arena_off));
     FRL_REQUIRE(t >= 1 && t <= 0xffffffffll, FRL_E_ARG, "frl_dw_gemm_sgd_sr: update count %lld outside [1, 2^32)",
                 static_cast<long long>(t));
-    dw::UpdateSr u{static_cast<__nv_bfloat16*>(p), mu != 0.0 ? buf : nullptr,
+    dw::UpdateSr<SgdRule> u{static_cast<__nv_bfloat16*>(p), mu != 0.0 ? buf : nullptr,
                    make_sgd_rule(lr, mu, dampening, wd, first_step), static_cast<float>(grad_scale), dyn, arena_off,
                    seed, static_cast<uint32_t>(t)};
-    return dw::launch(dw::dw_gemm_sr_kernel, dz, ld_dz, x, ld_x, rows, out, in, gw, u, p, u.mom, nullptr,
+    return dw::launch(dw::dw_gemm_sr_kernel<SgdRule>, dz, ld_dz, x, ld_x, rows, out, in, gw, u, p, u.mom, nullptr,
                       static_cast<cudaStream_t>(stream), "frl_dw_gemm_sgd_sr");
+}
+
+// Lion in the epilogue: frl_dw_gemm_sgd's arguments with (beta1, beta2) for (mu, dampening), m = exp_avg
+extern "C" int frl_dw_gemm_lion(const void* dz, int64_t ld_dz, const void* x, int64_t ld_x, int64_t rows,
+                                int64_t out, int64_t in, void* gw, float* p, float* m, void* p_lp, double lr,
+                                double beta1, double beta2, double wd, double grad_scale, const float* dyn,
+                                void* stream) {
+    FRL_REQUIRE(p, FRL_E_ARG, "frl_dw_gemm_lion: null master");
+    FRL_CHECK_LION(beta1, beta2, m, "frl_dw_gemm_lion");
+    dw::Update<LionRule> u{p, m, static_cast<__nv_bfloat16*>(p_lp), make_lion_rule(lr, beta1, beta2, wd),
+                           static_cast<float>(grad_scale), dyn};
+    return dw::launch(dw::dw_gemm_kernel<true, LionRule>, dz, ld_dz, x, ld_x, rows, out, in, gw, u, u.master, u.mom,
+                      u.lp, static_cast<cudaStream_t>(stream), "frl_dw_gemm_lion");
+}
+
+extern "C" int frl_dw_gemm_lion_sr(const void* dz, int64_t ld_dz, const void* x, int64_t ld_x, int64_t rows,
+                                   int64_t out, int64_t in, void* gw, void* p, float* m, int64_t arena_off,
+                                   uint64_t seed, int64_t t, double lr, double beta1, double beta2, double wd,
+                                   double grad_scale, const float* dyn, void* stream) {
+    FRL_REQUIRE(p, FRL_E_ARG, "frl_dw_gemm_lion_sr: null weights");
+    FRL_CHECK_LION(beta1, beta2, m, "frl_dw_gemm_lion_sr");
+    FRL_REQUIRE(arena_off >= 0 && arena_off % 4 == 0, FRL_E_ARG,
+                "frl_dw_gemm_lion_sr: arena offset %lld is not a multiple of 4", static_cast<long long>(arena_off));
+    FRL_REQUIRE(t >= 1 && t <= 0xffffffffll, FRL_E_ARG, "frl_dw_gemm_lion_sr: update count %lld outside [1, 2^32)",
+                static_cast<long long>(t));
+    dw::UpdateSr<LionRule> u{static_cast<__nv_bfloat16*>(p), m, make_lion_rule(lr, beta1, beta2, wd),
+                             static_cast<float>(grad_scale), dyn, arena_off, seed, static_cast<uint32_t>(t)};
+    return dw::launch(dw::dw_gemm_sr_kernel<LionRule>, dz, ld_dz, x, ld_x, rows, out, in, gw, u, p, u.mom, nullptr,
+                      static_cast<cudaStream_t>(stream), "frl_dw_gemm_lion_sr");
 }

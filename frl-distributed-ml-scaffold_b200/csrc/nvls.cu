@@ -303,6 +303,16 @@ extern "C" int frl_nvls_adamw(float* p, float* m, float* v, float* vmax, const v
                                             local_scratch, max_blocks, grad_scale, dyn, g_dtype, flags, stream, "frl_nvls_adamw");
 }
 
+extern "C" int frl_nvls_lion(float* p, float* m, const void* mc_g, void* mc_out, int64_t n, int rank, int world,
+                             void* const* signal_pads_dev, int pad_base, void* local_scratch, int max_blocks,
+                             double lr, double beta1, double beta2, double wd, double grad_scale, const float* dyn,
+                             int g_dtype, int flags, void* stream) {
+    FRL_CHECK_LION(beta1, beta2, m, "frl_nvls_lion");
+    return launch_nvls<LionRule, 1>(make_lion_rule(lr, beta1, beta2, wd), p, m, nullptr, nullptr, mc_g, mc_out, n,
+                                    rank, world, signal_pads_dev, pad_base, local_scratch, max_blocks, grad_scale,
+                                    dyn, g_dtype, flags, stream, "frl_nvls_lion");
+}
+
 extern "C" int frl_nvls_rmsprop(float* p, float* sq, float* buf, const void* mc_g, void* mc_out, int64_t n,
                                 int rank, int world, void* const* signal_pads_dev, int pad_base,
                                 void* local_scratch, int max_blocks, double lr, double alpha, double eps, double wd, double mu,

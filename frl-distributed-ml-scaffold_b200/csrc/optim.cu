@@ -6,7 +6,7 @@
 // clip coefficient) is folded into the gradient read, so the flatten / pre-divide / copy-out
 // passes of the stock DDP reducer do not exist here.
 //
-// HBM-bound: 20 B/param (SGD-momentum), 28 B/param (Adam, AdamW, RMSprop+momentum), 36 B/param
+// HBM-bound: 20 B/param (SGD-momentum, Lion), 28 B/param (Adam, AdamW, RMSprop+momentum), 36 B/param
 // (Adam/AdamW+amsgrad); +2 B with a bf16 shadow, -2 B with a bf16 gradient.
 //
 // Layout: every thread owns 4 consecutive elements per item, so fp32 arrays move as fully
@@ -351,6 +351,17 @@ extern "C" int frl_adamw(float* p, const void* g, float* m, float* v, float* vma
                                               nullptr, p_lp, n, gs, grad_scale_dev, dyn, g_dtype, st, "frl_adamw");
 }
 
+// Lion: frl_sgd_momentum's arguments with (beta1, beta2) for (mu, dampening) and no first_step;
+// m = exp_avg, wd the decoupled coefficient (LionRule)
+extern "C" int frl_lion(float* p, const void* g, float* m, void* p_lp, int64_t n, double lr, double beta1,
+                        double beta2, double wd, double grad_scale, const float* grad_scale_dev, const float* dyn,
+                        int g_dtype, void* stream) {
+    FRL_CHECK_LION(beta1, beta2, m, "frl_lion");
+    return launch_update<LionRule, 1>(make_lion_rule(lr, beta1, beta2, wd), p, g, m, nullptr, nullptr, p_lp, n,
+                                      static_cast<float>(grad_scale), grad_scale_dev, dyn, g_dtype,
+                                      static_cast<cudaStream_t>(stream), "frl_lion");
+}
+
 extern "C" int frl_rmsprop(float* p, const void* g, float* sq, float* buf, void* p_lp, int64_t n,
                            double lr, double alpha, double eps, double wd, double mu,
                            double grad_scale, const float* grad_scale_dev, const float* dyn,
@@ -442,6 +453,17 @@ extern "C" int frl_adamw_mt(float* p, float* m, float* v, float* vmax, void* p_l
     return launch_update_mt<AdamWRule<false>, 2>(make_adamw_rule<false>(lr, beta1, beta2, eps, wd, step), p, m, v,
                                                  nullptr, p_lp, segs_dev, tile_prefix_dev, tile_seg_dev, n_tiles, gs,
                                                  grad_scale_dev, dyn, st, "frl_adamw_mt");
+}
+
+extern "C" int frl_lion_mt(float* p, float* m, void* p_lp, const frl_grad_seg* segs_dev,
+                           const int64_t* tile_prefix_dev, const int32_t* tile_seg_dev, int64_t n_tiles, double lr,
+                           double beta1, double beta2, double wd, double grad_scale, const float* grad_scale_dev,
+                           const float* dyn, void* stream) {
+    FRL_CHECK_LION(beta1, beta2, m, "frl_lion_mt");
+    return launch_update_mt<LionRule, 1>(make_lion_rule(lr, beta1, beta2, wd), p, m, nullptr, nullptr, p_lp,
+                                         segs_dev, tile_prefix_dev, tile_seg_dev, n_tiles,
+                                         static_cast<float>(grad_scale), grad_scale_dev, dyn,
+                                         static_cast<cudaStream_t>(stream), "frl_lion_mt");
 }
 
 extern "C" int frl_rmsprop_mt(float* p, float* sq, float* buf, void* p_lp, const frl_grad_seg* segs_dev,

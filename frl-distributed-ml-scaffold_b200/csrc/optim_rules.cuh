@@ -80,6 +80,30 @@ struct AdamWRule {
     }
 };
 
+// Lion (Chen et al. 2023, Algorithm 2) with decoupled weight decay: one state, m = exp_avg.
+//   p = p * fp32(1 - lr*wd)            its own multiply, as AdamWRule's
+//   c = lerp(m, g, 1 - beta1)          the update direction's interpolation
+//   p = p - lr * sign(c)               sign(NaN) is NaN, so a non-finite gradient reaches the weight
+//   m = lerp(m, g, 1 - beta2)
+// dyn[0] is lr and dyn[1] the decay factor, so a replayed graph follows the scheduled lr in both.
+struct LionRule {
+    float w1, w2;           // 1 - beta1, 1 - beta2   (lerp weights)
+    float neg_lr;
+    float decay;            // fp32(1 - lr*wd), formed in double
+    static constexpr int kStates = 1;
+    __device__ __forceinline__ void patch(const float* dyn) {
+        neg_lr = -__ldg(dyn);
+        decay = __ldg(dyn + 1);
+    }
+    __device__ __forceinline__ void operator()(float& p, float g, float& m, float&, float&) const {
+        p = __fmul_rn(p, decay);
+        const float c = fmaf(w1, g - m, m);
+        const float s = c > 0.f ? 1.f : c < 0.f ? -1.f : c == 0.f ? 0.f : c;     // NaN stays NaN
+        p = fmaf(neg_lr, s, p);
+        m = fmaf(w2, g - m, m);
+    }
+};
+
 template <bool MOMENTUM>
 struct RmspropRule {
     float alpha, one_minus_alpha, eps, wd, mu, neg_lr;
@@ -120,6 +144,17 @@ static inline AdamWRule<AMS> make_adamw_rule(double lr, double beta1, double bet
                           static_cast<float>(1.0 - beta2), static_cast<float>(eps),
                           static_cast<float>(-(lr / bc1)), static_cast<float>(sqrt(bc2)),
                           static_cast<float>(1.0 - lr * wd)};
+}
+// the argument checks every Lion entry point makes before any launch (inside a function returning int)
+#define FRL_CHECK_LION(beta1, beta2, m, name)                                                            \
+    do {                                                                                                 \
+        FRL_REQUIRE((m) != nullptr, FRL_E_ARG, "%s: null exp_avg", name);                                \
+        FRL_REQUIRE((beta1) >= 0.0 && (beta1) < 1.0 && (beta2) >= 0.0 && (beta2) < 1.0, FRL_E_ARG,        \
+                    "%s: betas (%g, %g) outside [0, 1)", name, (beta1), (beta2));                        \
+    } while (0)
+static inline LionRule make_lion_rule(double lr, double beta1, double beta2, double wd) {
+    return LionRule{static_cast<float>(1.0 - beta1), static_cast<float>(1.0 - beta2), static_cast<float>(-lr),
+                    static_cast<float>(1.0 - lr * wd)};
 }
 template <bool MOM>
 static inline RmspropRule<MOM> make_rmsprop_rule(double lr, double alpha, double eps, double wd, double mu) {

@@ -6,7 +6,7 @@
 // The draws depend on the element's global arena index and the update count t only, so every rank,
 // bucketing and launch split rounds an element the same way.
 //
-// HBM-bound: 14 B/param (SGD-momentum), 22 B/param (Adam, AdamW, RMSprop+momentum), 30 B/param
+// HBM-bound: 14 B/param (SGD-momentum, Lion), 22 B/param (Adam, AdamW, RMSprop+momentum), 30 B/param
 // (Adam/AdamW+amsgrad) with an fp32 gradient, -2 B with a bf16 one: the fp32 master's 8 B of
 // read + write and the shadow's 2 B become 4 B of bf16 read + write.  One Philox4x32-10 call per
 // 4 elements (~40 integer multiplies) runs under that traffic.
@@ -313,6 +313,15 @@ extern "C" int frl_adamw_sr(void* p, const void* g, float* m, float* v, float* v
                                      dyn, g_dtype, stream, "frl_adamw_sr");
 }
 
+extern "C" int frl_lion_sr(void* p, const void* g, float* m, int64_t n, int64_t arena_off, uint64_t seed,
+                           int64_t t, double lr, double beta1, double beta2, double wd, double grad_scale,
+                           const float* grad_scale_dev, const float* dyn, int g_dtype, void* stream) {
+    FRL_CHECK_LION(beta1, beta2, m, "frl_lion_sr");
+    return launch_update_sr<LionRule, 1>(make_lion_rule(lr, beta1, beta2, wd), p, g, m, nullptr, nullptr, n,
+                                         arena_off, seed, t, static_cast<float>(grad_scale), grad_scale_dev, dyn,
+                                         g_dtype, static_cast<cudaStream_t>(stream), "frl_lion_sr");
+}
+
 extern "C" int frl_rmsprop_sr(void* p, const void* g, float* sq, float* buf, int64_t n, int64_t arena_off,
                               uint64_t seed, int64_t t, double lr, double alpha, double eps, double wd, double mu,
                               double grad_scale, const float* grad_scale_dev, const float* dyn, int g_dtype,
@@ -382,6 +391,17 @@ extern "C" int frl_adamw_mt_sr(void* p, float* m, float* v, float* vmax, const f
     auto make = [&](auto ams) { return make_adamw_rule<decltype(ams)::value>(lr, beta1, beta2, eps, wd, step); };
     return adam_family_mt_sr<AdamWRule>(make, p, m, v, vmax, segs_dev, tile_prefix_dev, tile_seg_dev, n_tiles, seed,
                                         step, grad_scale, grad_scale_dev, dyn, stream, "frl_adamw_mt_sr");
+}
+
+extern "C" int frl_lion_mt_sr(void* p, float* m, const frl_grad_seg* segs_dev, const int64_t* tile_prefix_dev,
+                              const int32_t* tile_seg_dev, int64_t n_tiles, uint64_t seed, int64_t t, double lr,
+                              double beta1, double beta2, double wd, double grad_scale, const float* grad_scale_dev,
+                              const float* dyn, void* stream) {
+    FRL_CHECK_LION(beta1, beta2, m, "frl_lion_mt_sr");
+    return launch_update_mt_sr<LionRule, 1>(make_lion_rule(lr, beta1, beta2, wd), p, m, nullptr, nullptr, segs_dev,
+                                            tile_prefix_dev, tile_seg_dev, n_tiles, seed, t,
+                                            static_cast<float>(grad_scale), grad_scale_dev, dyn,
+                                            static_cast<cudaStream_t>(stream), "frl_lion_mt_sr");
 }
 
 extern "C" int frl_rmsprop_mt_sr(void* p, float* sq, float* buf, const frl_grad_seg* segs_dev,

@@ -15,8 +15,10 @@ model's 2-D weights and this module's Adam (K2-mt) for every other parameter.  `
 extension, ``Solver.solve(..., adamw=True)``) turns the Adam rule of ``FusedAdam``, ``FusedAdam8bit``
 and ``FusedMuon``'s Adam group into ``torch.optim.AdamW``'s decoupled weight decay (``frl_adamw*``).
 On an arena with bf16 master weights (an extension, ``types.MasterWeights.BF16``) ``FusedSGD``,
-``FusedAdam`` and ``FusedRMSprop`` update the model range through the stochastic-rounding kernels
+``FusedAdam``, ``FusedRMSprop`` and ``FusedLion`` update the model range through the stochastic-rounding kernels
 (``frl_*_sr``, ``frl_*_mt_sr``) and keep ``sr_seed`` / ``sr_updates`` in their param group.
+``FusedLion`` (an extension, ``Solver.solve(..., lion=True)``) is Lion's sign-momentum rule with
+decoupled weight decay on SGD's state shape (``frl_lion*``); it too has SR forms.
 
 Known limitation: the step count (Adam's bias corrections) is ONE number for the whole arena.
 ``torch.optim`` keeps one per parameter and does not advance it for a parameter whose gradient
@@ -564,6 +566,86 @@ class FusedRMSprop(FusedArenaOptimizer):
                              eps=float(h["eps"]), wd=float(h["weight_decay"]), mu=mu,
                              grad_scale=grad_scale,
                              g_dtype=KERNELS.dtype_code(self.arena.grad.dtype), dyn=self._dyn)
+
+
+class FusedLion(FusedArenaOptimizer):
+    """Lion (Chen et al. 2023, *Symbolic Discovery of Optimization Algorithms*, Algorithm 2) with
+    decoupled weight decay on every parameter the optimizer owns: per element,
+    ``p *= fp32(1 - lr*wd)``, ``p -= lr * sign(lerp(exp_avg, g, 1 - beta1))``, then
+    ``exp_avg = lerp(exp_avg, g, 1 - beta2)``.  One state vector, so SGD-with-momentum's state size
+    and bytes per update; the ``frl_lion*`` kernels on every path SGD has, K12 included.
+    ``state_dict()`` is the layout of the published Lion implementations (lion-pytorch, timm): group
+    ``lr``, ``betas``, ``weight_decay`` and per-parameter ``exp_avg``.  Lion wants a 3-10x smaller lr
+    than AdamW; nothing here rescales it."""
+
+    STATE_NAMES = (("exp_avg", "exp_avg"),)
+
+    def __init__(self, arena, lr, betas=(0.9, 0.99), weight_decay=0.0):
+        super().__init__(arena, dict(lr=lr, betas=tuple(betas), weight_decay=weight_decay))
+
+    def _dyn_values(self):
+        h = self.hyper
+        lr = float(h["lr"])       # dyn[1]: the decay factor, formed in double and rounded once to fp32
+        return (lr, float(np.float32(1.0 - lr * float(h["weight_decay"]))))
+
+    def _hyper(self) -> Dict[str, float]:
+        h = self.hyper
+        return dict(lr=float(h["lr"]), beta1=float(h["betas"][0]), beta2=float(h["betas"][1]),
+                    wd=float(h["weight_decay"]))
+
+    def load_state_dict(self, state_dict: Dict[str, Any]) -> None:
+        """A Lion state dict only: one holding another optimizer's state (SGD's ``momentum_buffer``,
+        Adam's ``exp_avg_sq``, ...) or another optimizer's param group (no ``betas``, or SGD's
+        ``momentum``; also before its first step, when the state is empty) is refused with a
+        ValueError naming the keys."""
+        for entry in state_dict["state"].values():
+            foreign = sorted(k for k in entry if k not in ("exp_avg", "step"))
+            if foreign:
+                raise ValueError("a Lion optimizer cannot load another optimizer's state dict (found %s; Lion "
+                                 "keeps exp_avg only)" % foreign)
+        for g in state_dict["param_groups"]:
+            if "betas" not in g or "momentum" in g:
+                raise ValueError("a Lion optimizer cannot load another optimizer's state dict (param group keys %s; "
+                                 "Lion's group has betas and no momentum)" % sorted(k for k in g if k != "params"))
+        super().load_state_dict(state_dict)
+        self.hyper["betas"] = tuple(self.hyper["betas"])
+
+    def _launch(self, lo, hi, grad_scale, coef):
+        p, g, lp = self._slices(lo, hi)
+        m = self._state("exp_avg")[lo:hi]
+        if self._use_sr(lo):
+            KERNELS.lion_sr(p, g, m, hi - lo, arena_off=lo, seed=self.sr_seed, t=self._steps + 1, **self._hyper(),
+                            grad_scale=grad_scale, grad_scale_dev=coef, dyn=self._dyn)
+            return
+        KERNELS.lion(p, g, m, lp, hi - lo, **self._hyper(), grad_scale=grad_scale, grad_scale_dev=coef,
+                     dyn=self._dyn)
+
+    def update_in_dw_gemm(self, slot, dz, x, gw, *, grad_scale: float = 1.0) -> None:
+        """K12: the weight gradient gw = dz^T x of ``slot`` and, in the same kernel, this step's Lion
+        update of the slot from exactly that bf16 gradient (what ``_launch`` over the slot does)."""
+        a = self.arena
+        m = self._state("exp_avg")[slot.offset:slot.end]
+        if self._use_sr(slot.offset):
+            KERNELS.dw_gemm_lion_sr(dz, x, gw, a.lp[slot.offset:slot.end], m, arena_off=slot.offset,
+                                    seed=self.sr_seed, t=self._steps + 1, **self._hyper(), grad_scale=grad_scale,
+                                    dyn=self._dyn)
+            return
+        KERNELS.dw_gemm_lion(dz, x, gw, a.master[slot.offset:slot.end], m, a.lp[slot.offset:slot.end],
+                             **self._hyper(), grad_scale=grad_scale, dyn=self._dyn)
+
+    def _launch_mt(self, table, grad_scale):
+        KERNELS.lion_mt(self._master_base(), self._state("exp_avg"), self._lp_mt(), table, **self._hyper(),
+                        grad_scale=grad_scale, dyn=self._dyn)
+
+    def _launch_mt_sr(self, table, grad_scale):
+        KERNELS.lion_mt_sr(self.arena.lp, self._state("exp_avg"), table, seed=self.sr_seed, t=self._steps + 1,
+                           **self._hyper(), grad_scale=grad_scale, dyn=self._dyn)
+
+    def _launch_nvls(self, lo, hi, grad_scale):
+        mc_g, mc_out = self._nvls_ptrs(lo)
+        KERNELS.nvls_lion(self.arena.master[lo:hi], self._state("exp_avg")[lo:hi], mc_g, mc_out, hi - lo, self.nvls,
+                          **self._hyper(), grad_scale=grad_scale, g_dtype=KERNELS.dtype_code(self.arena.grad.dtype),
+                          dyn=self._dyn)
 
 
 def is_adapted(slot) -> bool:
@@ -1231,6 +1313,19 @@ def check_adamw(optim_opts: OptimOpts, layer_adaptation: LayerAdaptation, optimi
                             " and adafactor" if adafactor else ""))
 
 
+def check_lion(optim_opts: OptimOpts, layer_adaptation: LayerAdaptation, lion: bool) -> None:
+    """Lion replaces SGD-with-momentum's rule and keeps its state shape: it needs ``OptAlgorithm.SGD``
+    and no layer adaptation; anything else is a ValueError naming the values.  (Adafactor, Muon,
+    AdamW and 8-bit state need Adam, so their own checks refuse them next to Lion.)"""
+    if not lion:
+        return
+    la = LayerAdaptation(layer_adaptation)
+    if not (optim_opts.algo == OptAlgorithm.SGD and la is LayerAdaptation.NONE):
+        raise ValueError("lion cannot be combined with optimizer %r and layer adaptation %r (lion needs sgd, "
+                         "whose momentum is its beta1, and layer adaptation none)"
+                         % (getattr(optim_opts.algo, "value", optim_opts.algo), la.value))
+
+
 def check_master_weights(master_weights: MasterWeights, precision: Precision, layer_adaptation: LayerAdaptation,
                          optimizer_state: OptimizerState, adafactor: bool, muon: bool) -> None:
     """Bf16 master weights need a bf16-storage precision and an update with a stochastic-rounding
@@ -1283,19 +1378,22 @@ def check_layer_adaptation(optim_opts: OptimOpts, layer_adaptation: LayerAdaptat
 def create_fused_optimizer(arena: ParamArena, optim_opts: OptimOpts,
                            layer_adaptation: LayerAdaptation = LayerAdaptation.NONE,
                            optimizer_state: OptimizerState = OptimizerState.FP32,
-                           adafactor: bool = False, muon: bool = False, adamw: bool = False) -> FusedArenaOptimizer:
+                           adafactor: bool = False, muon: bool = False, adamw: bool = False,
+                           lion: bool = False) -> FusedArenaOptimizer:
     """Same dispatch and argument mapping as the reference's ``_create_optimizer``; with a layer
     adaptation, its LARS / LAMB counterpart; with 8-bit optimizer state, ``FusedAdam8bit``; with
     ``adafactor``, ``FusedAdafactor`` (``lr`` caps the relative step, ``weightDecay`` is its
     decoupled decay; ``epsilon`` and ``momentum`` are unused); with ``muon``, ``FusedMuon`` (one
     ``lr`` and ``weightDecay`` for both groups, ``momentum`` is Muon's, ``epsilon`` Adam's); with
     ``adamw``, the Adam rule of whichever of ``FusedAdam``, ``FusedAdam8bit`` or ``FusedMuon`` is
-    chosen takes decoupled weight decay (``torch.optim.AdamW``)."""
+    chosen takes decoupled weight decay (``torch.optim.AdamW``); with ``lion``, ``FusedLion`` (``momentum``
+    is beta1, beta2 is 0.99, ``weightDecay`` its decoupled decay)."""
     check_layer_adaptation(optim_opts, layer_adaptation)
     check_optimizer_state(optim_opts, layer_adaptation, optimizer_state)
     check_adafactor(optim_opts, layer_adaptation, optimizer_state, adafactor)
     check_muon(optim_opts, layer_adaptation, optimizer_state, adafactor, muon)
     check_adamw(optim_opts, layer_adaptation, optimizer_state, adafactor, adamw)
+    check_lion(optim_opts, layer_adaptation, lion)
     check_master_weights(getattr(arena, "master_weights", MasterWeights.FP32), arena.precision, layer_adaptation,
                          optimizer_state, adafactor, muon)
     if muon:
@@ -1315,6 +1413,9 @@ def create_fused_optimizer(arena: ParamArena, optim_opts: OptimOpts,
     if algo == OptAlgorithm.RMSPROP:
         return FusedRMSprop(arena, lr=optim_opts.lr, momentum=optim_opts.momentum,
                             weight_decay=optim_opts.weightDecay)
+    if algo == OptAlgorithm.SGD and lion:
+        return FusedLion(arena, lr=optim_opts.lr, betas=(optim_opts.momentum, 0.99),
+                         weight_decay=optim_opts.weightDecay)
     if algo == OptAlgorithm.SGD:
         return FusedSGD(arena, lr=optim_opts.lr, momentum=optim_opts.momentum,
                         weight_decay=optim_opts.weightDecay)

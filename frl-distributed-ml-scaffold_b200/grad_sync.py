@@ -38,7 +38,7 @@ import torch.nn as nn
 
 from . import _native
 from .arena import ParamArena
-from .fused_optim import FusedArenaOptimizer, FusedSGD
+from .fused_optim import FusedArenaOptimizer, FusedLion, FusedSGD
 from .types import Precision
 
 KERNELS = _native     # swapped by CPU tests of the host logic
@@ -251,11 +251,12 @@ class GradBucketPipeline:
         self._acc_seen = set()         # slots that got a gradient in some microbatch of the open group
         self.last_ready: frozenset = frozenset()
         # K12: one GPU, one tail update (eager per-bucket updates would race the GEMM for the same
-        # weights' state), no global norm, no accumulator, plain SGD on bf16 shadow weights
+        # weights' state), no global norm, no accumulator, plain SGD or Lion on bf16 shadow weights
         self.fused_dw_update = (
             not self.distributed and not self.eager and self.clip_norm == 0.0 and self.accumulation == 1
-            and type(optimizer) is FusedSGD and arena.precision is Precision.BF16
-            and hasattr(KERNELS, "dw_gemm_sgd") and (self.on_cuda or KERNELS is not _native)
+            and type(optimizer) in (FusedSGD, FusedLion) and arena.precision is Precision.BF16
+            and hasattr(KERNELS, "dw_gemm_lion" if type(optimizer) is FusedLion else "dw_gemm_sgd")
+            and (self.on_cuda or KERNELS is not _native)
             and os.environ.get("FRL_B200_FUSED_DW_UPDATE", "1") != "0")
         self.dw_updated: set = set()      # slot indices K12 updated in this step
 

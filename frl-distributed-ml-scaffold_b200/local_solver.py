@@ -28,7 +28,8 @@ class LocalSolver:
               muon: Optional[bool] = None,
               adamw: Optional[bool] = None,
               channels_last: Optional[bool] = None,
-              master_weights: Optional[MasterWeights] = None) -> PerformanceSummary:
+              master_weights: Optional[MasterWeights] = None,
+              lion: Optional[bool] = None) -> PerformanceSummary:
         if save_notebook:
             logger.warning("save_notebook is not supported by frl_b200 (visualisation only)")
         # a stale rendezvous file from a crashed run would poison the file:// store
@@ -43,6 +44,7 @@ class LocalSolver:
                                  graph=graph, layer_adaptation=layer_adaptation,
                                  grad_accumulation=grad_accumulation, ema_decay=ema_decay,
                                  optimizer_state=optimizer_state, adafactor=adafactor, muon=muon,
-                                 adamw=adamw, channels_last=channels_last, master_weights=master_weights):
+                                 adamw=adamw, channels_last=channels_last, master_weights=master_weights,
+                                 lion=lion):
             pass
         return last

@@ -29,7 +29,7 @@ import torch.nn as nn
 from .arena import ParamArena
 from .criteria import BaseParallelCriterion
 from .ema import EMA_STATE_KEY
-from .fused_optim import (FusedAdafactor, FusedAdam8bit, FusedMuon, check_adafactor, check_adamw, check_muon, check_layer_adaptation, check_master_weights, check_optimizer_state, create_fused_optimizer,
+from .fused_optim import (FusedAdafactor, FusedAdam8bit, FusedLion, FusedMuon, check_adafactor, check_adamw, check_lion, check_muon, check_layer_adaptation, check_master_weights, check_optimizer_state, create_fused_optimizer,
                           is_adapted)
 from .grad_sync import BufferBroadcaster, GradBucketPipeline
 from .lr_scheduler import DropEpochsScheduler, WarmupMultiStepLR
@@ -51,6 +51,7 @@ OPTIMIZER_STATE_ENV = "FRL_B200_OPTIMIZER_STATE"   # "fp32" (default) | "8bit"
 ADAFACTOR_ENV = "FRL_B200_ADAFACTOR"               # "0" (default) | "1"
 MUON_ENV = "FRL_B200_MUON"                         # "0" (default) | "1"
 ADAMW_ENV = "FRL_B200_ADAMW"                       # "0" (default) | "1"
+LION_ENV = "FRL_B200_LION"                         # "0" (default) | "1"
 CHANNELS_LAST_ENV = "FRL_B200_CHANNELS_LAST"       # "0" (default) | "1"
 MASTER_WEIGHTS_ENV = "FRL_B200_MASTER_WEIGHTS"     # "fp32" (default) | "bf16"
 EMA_SUFFIX = ".ema"                        # <checkpoint>.ema: the weight EMA next to a checkpoint
@@ -107,6 +108,9 @@ class SolverWorkerArgs(NamedTuple):
     save_every: int = 1
     graph_step: Optional[bool] = None      # None: FRL_B200_CUDA_GRAPH (default off)
     layer_adaptation: LayerAdaptation = LayerAdaptation.NONE
+    # Lion in place of SGD-with-momentum's rule; placed before muon, so every field from muon to the
+    # end keeps its position counted from the end of the tuple
+    lion: bool = False
     # Muon for the model's 2-D weights, Adam for the rest; placed before optimizer_state, adafactor,
     # ema_decay and grad_accumulation, which keep their positions at the end
     muon: bool = False
@@ -315,6 +319,17 @@ def resolve_adamw(explicit: Optional[bool] = None) -> bool:
     return raw == "1"
 
 
+def resolve_lion(explicit: Optional[bool] = None) -> bool:
+    """Whether SGD's rule is replaced by Lion: ``explicit``, else FRL_B200_LION (``0``, the default,
+    or ``1``).  Any other value is a ValueError."""
+    if explicit is not None:
+        return bool(explicit)
+    raw = os.environ.get(LION_ENV, "0").strip()
+    if raw not in ("0", "1"):
+        raise ValueError("%s must be 0 or 1, got %r" % (LION_ENV, raw))
+    return raw == "1"
+
+
 def resolve_channels_last(explicit: Optional[bool] = None) -> bool:
     """Whether conv weights and image batches are channels_last: ``explicit``, else
     FRL_B200_CHANNELS_LAST (``0``, the default, or ``1``).  Any other value is a ValueError."""
@@ -490,8 +505,9 @@ class Solver:
         adafactor = args.adafactor and run_opts.mode == Mode.TRAIN
         muon = args.muon and run_opts.mode == Mode.TRAIN
         adamw = args.adamw and run_opts.mode == Mode.TRAIN
+        lion = args.lion and run_opts.mode == Mode.TRAIN
         optimizer = create_fused_optimizer(arena, run_opts.optim, args.layer_adaptation, opt_state, adafactor,
-                                           muon, adamw)
+                                           muon, adamw, lion)
         if checkpoint:
             optimizer.load_state_dict(checkpoint.optimizerState)
         ema = None
@@ -584,7 +600,16 @@ class Solver:
                     "frl_adamw_mt, K2-mt, for the non-Muon group" if isinstance(optimizer, FusedMuon) else
                     "frl_nvls_adamw, K7" if pipeline.nvls is not None else
                     "frl_adamw / frl_adamw_mt, K2 / K2-mt"))
-                if getattr(optimizer, "adamw", False) else getattr(run_opts.optim.algo, "value", run_opts.optim.algo),
+                if getattr(optimizer, "adamw", False) else
+                "lion, betas (%r, %r), decoupled weight decay %r (%s)" % (
+                    optimizer.hyper["betas"][0], optimizer.hyper["betas"][1], optimizer.hyper["weight_decay"],
+                    "frl_nvls_lion, K7" if pipeline.nvls is not None else
+                    ("frl_dw_gemm_lion%s, K12, for the trunk's weights, %s for the rest" % (
+                        "_sr" if optimizer.sr else "",
+                        "frl_lion_sr / frl_lion_mt_sr, K2-sr" if optimizer.sr else "frl_lion / frl_lion_mt, K2 / K2-mt"))
+                    if pipeline.fused_dw_update else
+                    "frl_lion_sr / frl_lion_mt_sr, K2-sr" if optimizer.sr else "frl_lion / frl_lion_mt, K2 / K2-mt")
+                if isinstance(optimizer, FusedLion) else getattr(run_opts.optim.algo, "value", run_opts.optim.algo),
                 "8-bit block-wise (K2-q8), %.1f MiB instead of %.1f MiB" % (
                     optimizer.state_bytes / 2 ** 20, optimizer.fp32_state_bytes / 2 ** 20)
                 if isinstance(optimizer, FusedAdam8bit) else
@@ -819,7 +844,8 @@ class Solver:
               muon: Optional[bool] = None,
               adamw: Optional[bool] = None,
               channels_last: Optional[bool] = None,
-              master_weights: Optional[MasterWeights] = None
+              master_weights: Optional[MasterWeights] = None,
+              lion: Optional[bool] = None
               ) -> Iterator[PerformanceSummary]:
         """The reference's entry point (solver.py:728-739) plus two keyword-only extensions:
 
@@ -951,6 +977,18 @@ class Solver:
                        with SGD the dW-GEMM update (K12) runs its SR form.  ``Mode.EVAL`` ignores it.  None:
                        FRL_B200_MASTER_WEIGHTS (``fp32`` by default, or ``bf16``); any other value
                        raises ``ValueError``.
+        ``lion``       True: Lion (Chen et al. 2023, Algorithm 2) in place of SGD-with-momentum's rule,
+                       on every update path SGD has (K2, K2-mt, K2-sr, K7, and K12 on one GPU): each
+                       step scales every parameter by fp32(1 - lr * ``weightDecay``), then moves it
+                       by -lr * sign(lerp(exp_avg, g, 1 - beta1)) and updates exp_avg =
+                       lerp(exp_avg, g, 1 - beta2).  ``momentum`` is beta1 (0 allowed), beta2 is
+                       0.99, ``lr`` is Lion's lr, unscaled: Lion wants a 3-10x smaller lr than
+                       AdamW.  One state vector (``exp_avg``), so SGD's state size.  Needs
+                       ``OptAlgorithm.SGD`` and no layer adaptation; Adam, RMSprop, LARS (and
+                       Adafactor, Muon, AdamW, 8-bit state, which need Adam) raise ``ValueError``
+                       before a rank starts.  Checkpoints hold ``lr``, ``betas``, ``weight_decay``
+                       and ``exp_avg``, the layout of lion-pytorch and timm.  None: FRL_B200_LION
+                       (``0`` by default, ``1`` to enable).  ``Mode.EVAL`` ignores it.
         """
         adapt = LayerAdaptation.NONE
         accum = 1
@@ -959,6 +997,7 @@ class Solver:
         use_adafactor = False
         use_muon = False
         use_adamw = False
+        use_lion = False
         if run_opts.mode == Mode.TRAIN:
             adapt = resolve_layer_adaptation(layer_adaptation)
             check_layer_adaptation(run_opts.optim, adapt)
@@ -970,6 +1009,8 @@ class Solver:
             check_muon(run_opts.optim, adapt, opt_state, use_adafactor, use_muon)
             use_adamw = resolve_adamw(adamw)
             check_adamw(run_opts.optim, adapt, opt_state, use_adafactor, use_adamw)
+            use_lion = resolve_lion(lion)
+            check_lion(run_opts.optim, adapt, use_lion)
             accum = resolve_grad_accumulation(grad_accumulation)
             decay = resolve_ema_decay(ema_decay)
         use_channels_last = resolve_channels_last(channels_last)
@@ -1018,7 +1059,7 @@ class Solver:
                 cache=None, precision=prec, save_every=save_every, graph_step=graph,
                 layer_adaptation=adapt, grad_accumulation=accum, ema_decay=decay,
                 optimizer_state=opt_state, adafactor=use_adafactor, muon=use_muon, adamw=use_adamw,
-                channels_last=use_channels_last, master_weights=use_master)
+                channels_last=use_channels_last, master_weights=use_master, lion=use_lion)
             if not run_opts.singleThreaded:
                 parent_conn, child_conn = ctx.Pipe(duplex=False)
                 proc = ctx.Process(target=cls._solver_worker_process,

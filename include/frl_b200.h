@@ -59,7 +59,7 @@ int          frl_device_arch(void);
  *   dyn      optional DEVICE array of per-step scalars that override the by-value arguments,
  *            so a CUDA graph that captured the launch stays valid while they change:
  *            SGD / RMSprop: dyn[0] = lr ;  Adam: dyn[0] = -lr/(1-beta1^t), dyn[1] = sqrt(1-beta2^t);
- *            AdamW: Adam's two, then dyn[2] = fp32(1 - lr*wd).
+ *            AdamW: Adam's two, then dyn[2] = fp32(1 - lr*wd);  Lion: dyn[0] = lr, dyn[1] = fp32(1 - lr*wd).
  * Update rules are torch 2.11's (L2-coupled weight decay: g += wd * p first), except AdamW's
  * decoupled decay (frl_adamw*).
  * ---------------------------------------------------------------------------------------- */
@@ -94,6 +94,24 @@ int frl_adamw(float* p, const void* g, float* m, float* v, float* vmax, void* p_
               double grad_scale, const float* grad_scale_dev, const float* dyn, int g_dtype,
               void* stream);
 
+/* Lion (Chen et al. 2023, Symbolic Discovery of Optimization Algorithms, Algorithm 2), with one
+ * state m = exp_avg (non-NULL; it starts at zero and there is no first-step special case).  Seven
+ * entry points, each with its SGD form's arguments with (beta1, beta2) in place of (mu, dampening)
+ * and no first_step: frl_lion (K2), frl_lion_mt (K2-mt), frl_lion_sr / frl_lion_mt_sr (K2-sr),
+ * frl_nvls_lion (K7), frl_dw_gemm_lion / frl_dw_gemm_lion_sr (K12).  Per element, in fp32, with g
+ * the scaled gradient:
+ *     p = p * fp32(1 - lr*wd)              its own fp32 multiply (1 - lr*wd formed in double,
+ *                                          rounded once), as AdamW's
+ *     c = fmaf(1-beta1, g - m, m)          lerp(m, g, 1-beta1)
+ *     p = fmaf(-lr, sign(c), p)            sign: +1 / -1 / 0, and NaN for a NaN c
+ *     m = fmaf(1-beta2, g - m, m)          lerp(m, g, 1-beta2)
+ * 20 B per parameter with an fp32 gradient and no shadow, as SGD with momentum.  beta1 and beta2
+ * must lie in [0, 1) (FRL_E_ARG).  dyn (may be NULL): dyn[0] = lr, dyn[1] = fp32(1 - lr*wd), and
+ * for the _sr forms dyn[3] = t.  Every argument check is made before any launch; graph-capturable. */
+int frl_lion(float* p, const void* g, float* m, void* p_lp, int64_t n, double lr, double beta1, double beta2,
+             double wd, double grad_scale, const float* grad_scale_dev, const float* dyn, int g_dtype,
+             void* stream);
+
 /* RMSprop (not centered): sq = alpha*sq + (1-alpha)*g^2 ; avg = sqrt(sq)+eps ;
  * mu > 0: buf = mu*buf + g/avg ; p -= lr*buf     else: p -= lr*g/avg  (buf may be NULL). */
 int frl_rmsprop(float* p, const void* g, float* sq, float* buf, void* p_lp, int64_t n,
@@ -103,7 +121,7 @@ int frl_rmsprop(float* p, const void* g, float* sq, float* buf, void* p_lp, int6
 
 /* ------------------------------------------------------------------------------------------
  * K12 — weight-gradient GEMM gw = dz^T x on the tensor cores (persistent, TMA + WGMMA), with
- * an optional SGD update of the same weights in its epilogue.
+ * an optional SGD or Lion update of the same weights in its epilogue.
  *   dz [rows, out] (leading dimension ld_dz), x [rows, in] (ld_x): row-major bf16;
  *   gw [out, in]: contiguous bf16, written in both forms (fp32 accumulation, rounded once).
  *   out % 128 == 0, in % 256 == 0, rows % 64 == 0 (FRL_E_ARG); every pointer 16-byte aligned
@@ -127,6 +145,17 @@ int frl_dw_gemm_sgd_sr(const void* dz, int64_t ld_dz, const void* x, int64_t ld_
                        int64_t out, int64_t in, void* gw, void* p, float* buf, int64_t arena_off, uint64_t seed,
                        int64_t t, double lr, double mu, double dampening, double wd, double grad_scale,
                        const float* dyn, int first_step, void* stream);
+
+/* frl_dw_gemm_lion / frl_dw_gemm_lion_sr: frl_dw_gemm_sgd / frl_dw_gemm_sgd_sr with frl_lion's rule
+ * (m = exp_avg of the slice, non-NULL): bit-identical to frl_dw_gemm followed by frl_lion /
+ * frl_lion_sr (g_dtype = FRL_BF16) over the slice. */
+int frl_dw_gemm_lion(const void* dz, int64_t ld_dz, const void* x, int64_t ld_x, int64_t rows,
+                     int64_t out, int64_t in, void* gw, float* p, float* m, void* p_lp, double lr, double beta1,
+                     double beta2, double wd, double grad_scale, const float* dyn, void* stream);
+int frl_dw_gemm_lion_sr(const void* dz, int64_t ld_dz, const void* x, int64_t ld_x, int64_t rows,
+                        int64_t out, int64_t in, void* gw, void* p, float* m, int64_t arena_off, uint64_t seed,
+                        int64_t t, double lr, double beta1, double beta2, double wd, double grad_scale,
+                        const float* dyn, void* stream);
 
 /* ------------------------------------------------------------------------------------------
  * K13 — data-gradient GEMM of an upper Linear layer with the lower Linear+ReLU unit's backward in
@@ -189,6 +218,11 @@ int frl_adamw_mt(float* p, float* m, float* v, float* vmax, void* p_lp, const fr
                  double beta2, double eps, double wd, int64_t step, double grad_scale,
                  const float* grad_scale_dev, const float* dyn, void* stream);
 
+/* K2-mt Lion: frl_sgd_momentum_mt's arguments, frl_lion's rule and dyn layout. */
+int frl_lion_mt(float* p, float* m, void* p_lp, const frl_grad_seg* segs_dev, const int64_t* tile_prefix_dev,
+                const int32_t* tile_seg_dev, int64_t n_tiles, double lr, double beta1, double beta2, double wd,
+                double grad_scale, const float* grad_scale_dev, const float* dyn, void* stream);
+
 int frl_rmsprop_mt(float* p, float* sq, float* buf, void* p_lp, const frl_grad_seg* segs_dev,
                    const int64_t* tile_prefix_dev, const int32_t* tile_seg_dev, int64_t n_tiles, double lr, double alpha,
                    double eps, double wd, double mu, double grad_scale, const float* grad_scale_dev,
@@ -221,6 +255,9 @@ int frl_adam_sr(void* p, const void* g, float* m, float* v, float* vmax, int64_t
 int frl_adamw_sr(void* p, const void* g, float* m, float* v, float* vmax, int64_t n, int64_t arena_off,
                  uint64_t seed, double lr, double beta1, double beta2, double eps, double wd, int64_t step,
                  double grad_scale, const float* grad_scale_dev, const float* dyn, int g_dtype, void* stream);
+int frl_lion_sr(void* p, const void* g, float* m, int64_t n, int64_t arena_off, uint64_t seed, int64_t t,
+                double lr, double beta1, double beta2, double wd, double grad_scale, const float* grad_scale_dev,
+                const float* dyn, int g_dtype, void* stream);
 int frl_rmsprop_sr(void* p, const void* g, float* sq, float* buf, int64_t n, int64_t arena_off, uint64_t seed,
                    int64_t t, double lr, double alpha, double eps, double wd, double mu, double grad_scale,
                    const float* grad_scale_dev, const float* dyn, int g_dtype, void* stream);
@@ -236,6 +273,10 @@ int frl_adamw_mt_sr(void* p, float* m, float* v, float* vmax, const frl_grad_seg
                     const int64_t* tile_prefix_dev, const int32_t* tile_seg_dev, int64_t n_tiles, uint64_t seed,
                     double lr, double beta1, double beta2, double eps, double wd, int64_t step, double grad_scale,
                     const float* grad_scale_dev, const float* dyn, void* stream);
+int frl_lion_mt_sr(void* p, float* m, const frl_grad_seg* segs_dev, const int64_t* tile_prefix_dev,
+                   const int32_t* tile_seg_dev, int64_t n_tiles, uint64_t seed, int64_t t, double lr, double beta1,
+                   double beta2, double wd, double grad_scale, const float* grad_scale_dev, const float* dyn,
+                   void* stream);
 int frl_rmsprop_mt_sr(void* p, float* sq, float* buf, const frl_grad_seg* segs_dev, const int64_t* tile_prefix_dev,
                       const int32_t* tile_seg_dev, int64_t n_tiles, uint64_t seed, int64_t t, double lr,
                       double alpha, double eps, double wd, double mu, double grad_scale,
@@ -713,6 +754,11 @@ int frl_nvls_adamw(float* p, float* m, float* v, float* vmax, const void* mc_g, 
                    void* local_scratch, int max_blocks, double lr, double beta1, double beta2,
                    double eps, double wd,
                    int64_t step, double grad_scale, const float* dyn, int g_dtype, int flags, void* stream);
+/* K7 Lion: frl_nvls_sgd's arguments with (beta1, beta2) for (mu, dampening); frl_lion's rule and dyn. */
+int frl_nvls_lion(float* p, float* m, const void* mc_g, void* mc_out, int64_t n, int rank, int world,
+                  void* const* signal_pads_dev, int pad_base, void* local_scratch, int max_blocks, double lr,
+                  double beta1, double beta2, double wd, double grad_scale, const float* dyn, int g_dtype, int flags,
+                  void* stream);
 int frl_nvls_rmsprop(float* p, float* sq, float* buf, const void* mc_g, void* mc_out, int64_t n,
                      int rank, int world, void* const* signal_pads_dev, int pad_base,
                      void* local_scratch, int max_blocks, double lr, double alpha, double eps,

@@ -1,7 +1,7 @@
 #!/usr/bin/env python
 """Micro-benchmark of every hand-written kernel at the BASELINE shapes (1 GPU).
 
-    python tools/kernel_bench.py [--only k2,k2lw,k2q8,k2af,k2w,k3,k5a,k5nhwc,k13,k14,...] [--iters 20] [--json out.json]
+    python tools/kernel_bench.py [--only k2,k2lw,k2q8,k2af,k2w,k2lion,k3,k5a,k5nhwc,k13,k14,...] [--iters 20] [--json out.json]
 
 Each kernel is timed with CUDA events on the launching stream over ROTATING operand sets whose
 total size exceeds the 50 MB L2 (so every launch streams from HBM), after 3 warm-up launches.
@@ -314,6 +314,59 @@ def bench_k2w(iters):
                "adamw_us": "%.1f (%.1f-%.1f)" % (med["adamw"], min(times["adamw"]), max(times["adamw"])),
                "adamw_over_adam": round(med["adamw"] / med["adam"], 4),
                "within_5pct": med["adamw"] <= 1.05 * med["adam"]}
+    print(json.dumps(summary), flush=True)
+    out.append(summary)
+    return out
+
+
+def bench_k2lion(iters):
+    """K2-mt Lion (``frl_lion_mt``) beside K2-mt SGD with momentum (``frl_sgd_momentum_mt``) on the
+    headline MLP's arena (10 tensors, 54.7 M parameters), bf16 gradients in the arena, bf16 shadow, one
+    fp32 state vector, each timed from a CUDA graph.  Both rules move 20 bytes per parameter (1.1 GB
+    per launch, far larger than L2).  Five rounds, SGD and Lion alternating; the last record holds the
+    medians (min-max), Lion / SGD and Lion's share of the data-sheet 3.35 TB/s."""
+    from frl_b200.multi_tensor import GradSegTable
+
+    class Slot:
+        def __init__(self, index, offset, shape):
+            self.index, self.offset, self.shape = index, offset, shape
+            self.numel = 1
+            for d in shape:
+                self.numel *= d
+            self.is_model = True
+
+    shapes = [(4096, 4096), (4096,)] * 3 + [(1000, 4096), (1000,), (64, 4096), (64,)]
+    slots, off = [], 0
+    for i, sh in enumerate(shapes):
+        slots.append(Slot(i, off, sh))
+        off = (off + slots[-1].numel + 7) // 8 * 8
+    n, n_real = off, sum(s.numel for s in slots)
+    grad = torch.randn(n, device=DEV).bfloat16()
+    table = GradSegTable(slots, DEV)
+    for s in slots:
+        table.point(s, grad.data_ptr() + 2 * s.offset, grad.dtype)
+    table.upload()
+    p = torch.randn(n, device=DEV) * 0.02
+    lp = torch.empty(n, device=DEV, dtype=torch.bfloat16)
+    m = torch.randn(n, device=DEV) * 1e-3
+    fns = {"sgd": lambda i: _native.sgd_momentum_mt(p, m, lp, table, lr=1e-2, mu=0.9, dampening=0.0, wd=1e-5),
+           "lion": lambda i: _native.lion_mt(p, m, lp, table, lr=1e-4, beta1=0.9, beta2=0.99, wd=1e-5)}
+    out, times = [], {"sgd": [], "lion": []}
+    for r in range(5):
+        for rule in ("sgd", "lion"):
+            rec = timed("K2-mt %s mlp bf16-grad (%d tensors, %d params) round %d" % (rule, len(slots), n_real, r),
+                        fns[rule], 1, 20 * n_real, iters, "20 B/param", graph=True)
+            times[rule].append(rec["us"])
+            out.append(rec)
+    med = {k: sorted(t)[len(t) // 2] for k, t in times.items()}
+    lion_tbs = 20 * n_real / med["lion"] / 1e6
+    summary = {"kernel": "K2-mt lion vs sgd momentum, median of 5 (min-max)",
+               "sgd_us": "%.1f (%.1f-%.1f)" % (med["sgd"], min(times["sgd"]), max(times["sgd"])),
+               "lion_us": "%.1f (%.1f-%.1f)" % (med["lion"], min(times["lion"]), max(times["lion"])),
+               "lion_over_sgd": round(med["lion"] / med["sgd"], 4),
+               "within_3pct": med["lion"] <= 1.03 * med["sgd"],
+               "lion_TBps": round(lion_tbs, 3), "lion_frac_of_3.35TBps": round(lion_tbs / 3.35, 3),
+               "at_least_0.83": lion_tbs / 3.35 >= 0.83}
     print(json.dumps(summary), flush=True)
     out.append(summary)
     return out
@@ -889,7 +942,7 @@ BENCHES = {"k2": bench_k2, "k2mt": bench_k2mt, "k2lw": bench_k2lw, "k3": bench_k
            "k5m": bench_k5m, "k4s": bench_k4s, "k6": bench_k6,
            "k8": bench_k8, "k8t": bench_k8t, "k9": bench_k9, "k10": bench_k10, "k11": bench_k11,
            "k2q8": bench_k2q8, "k2af": bench_k2af, "k13": bench_k13, "k14": bench_k14, "k2w": bench_k2w,
-           "k5nhwc": bench_k5nhwc}
+           "k5nhwc": bench_k5nhwc, "k2lion": bench_k2lion}
 
 
 def main():
