@@ -131,6 +131,14 @@ SIGNATURES = {
     "frl_augment_mix_images_nhwc": (_i, [_vp, _i64, _i, _i, _i, _vp, C.c_uint64, _i, _i, _d, _d, _d, _d, _d, _i,
                                          _i, _vp, _vp, _vp, _i, _i, _i, _vp, _i, _f, _i, _i, _i, _i, _vp]),
     "frl_mix_targets": (_i, [_vp, _i, _i64, _i64, _i, _f, _vp, _vp]),
+    "frl_augment_policy_images": (_i, [_vp, _i64, _i, _i, _i, _vp, C.c_uint64, _i, _i, _d, _d, _d, _d, _i, _i, _i,
+                                       _i, _i, _i, _vp, _d, _d, _d, _d, _d, _i, _vp, _vp, _vp, _vp, _i, _i, _i,
+                                       _vp, _vp, _vp]),
+    "frl_augment_policy_images_nhwc": (_i, [_vp, _i64, _i, _i, _i, _vp, C.c_uint64, _i, _i, _d, _d, _d, _d, _i, _i,
+                                            _i, _i, _i, _i, _vp, _d, _d, _d, _d, _d, _i, _vp, _vp, _vp, _vp, _i, _i,
+                                            _i, _vp, _vp, _vp]),
+    "frl_mix_images": (_i, [_vp, _i, _i64, _i, _i, _i, _i, _f, _i, _i, _i, _i, _vp]),
+    "frl_mix_images_nhwc": (_i, [_vp, _i, _i64, _i, _i, _i, _i, _f, _i, _i, _i, _i, _vp]),
     "frl_colsum_scratch_bytes": (_i64, [_i64, _i64]),
     "frl_colsum": (_i, [_vp, _i, _i64, _i64, _vp, _i, _i, _vp, _vp]),
     "frl_drelu_colsum": (_i, [_vp, _vp, _vp, _i, _i64, _i64, _vp, _i, _i, _vp, _vp]),
@@ -912,6 +920,58 @@ def mix_targets(src, dst, lam: float, n_classes: int = 0) -> None:
         inner = src[0].numel() if B else 1
     _check(lib().frl_mix_targets(_ptr(src), dtype_code(src.dtype), B, inner, int(n_classes), float(lam), _ptr(dst),
                                  _stream()), "frl_mix_targets")
+
+
+POLICY_NONE, POLICY_TRIVIAL_AUGMENT, POLICY_RAND_AUGMENT = 0, 1, 2
+#: bytes of shared memory K5p stages a sample's uint8 crop in (FRL_AUGMENT_POLICY_SMEM_BYTES)
+POLICY_SMEM_BYTES = 224256
+
+
+def augment_policy_images(src, idx, dst, *, seed: int, epoch: int, mode: int, scale_range=(0.08, 1.0),
+                          ratio_range=(3.0 / 4.0, 4.0 / 3.0), pad: int = 0, flip: bool = True,
+                          policy: int = POLICY_NONE, num_ops: int = 1, magnitude: int = 0, mags=None,
+                          erase_p: float = 0.0, erase_scale=(0.02, 0.33), erase_ratio=(0.3, 3.3),
+                          erase_random: bool = False, erase_value=None, scale=None, bias=None, params_out=None,
+                          policy_out=None) -> None:
+    """K5p: K5a's training crop and flip, then the policy (``POLICY_TRIVIAL_AUGMENT`` /
+    ``POLICY_RAND_AUGMENT``, magnitude table ``mags`` device fp32 [14, num_bins]), the affine and
+    random erasing (``erase_p`` > 0; ``erase_random`` or ``erase_value`` device fp32 [C]).
+    ``policy_out`` optional int32 [B, 3*num_ops + 5] (num_ops 0 without a policy).  Other
+    arguments as ``augment_images``.  See frl_augment_policy_images in include/frl_b200.h."""
+    B, Cc, H, W = src.shape
+    assert src.dtype == torch.uint8 and src.is_contiguous() and (dst.is_contiguous() or is_nhwc(dst))
+    assert dst.dim() == 4 and tuple(dst.shape[:2]) == (B, Cc)
+    assert idx.dtype == torch.int64 and idx.is_contiguous() and idx.numel() == B
+    assert params_out is None or (params_out.dtype == torch.int32 and params_out.is_contiguous()
+                                  and tuple(params_out.shape) == (B, 5))
+    n_ops = num_ops if policy != POLICY_NONE else 0
+    assert policy_out is None or (policy_out.dtype == torch.int32 and policy_out.is_contiguous()
+                                  and tuple(policy_out.shape) == (B, 3 * n_ops + 5))
+    num_bins = 0
+    if mags is not None:
+        assert mags.dtype == torch.float32 and mags.is_contiguous() and mags.dim() == 2 and mags.shape[0] == 14
+        num_bins = mags.shape[1]
+    assert erase_value is None or (erase_value.dtype == torch.float32 and erase_value.numel() == Cc)
+    name = "frl_augment_policy_images_nhwc" if is_nhwc(dst) else "frl_augment_policy_images"
+    _check(getattr(lib(), name)(
+        _ptr(src), B, Cc, H, W, _ptr(idx), int(seed) & (2 ** 64 - 1), int(epoch), int(mode),
+        float(scale_range[0]), float(scale_range[1]), float(ratio_range[0]), float(ratio_range[1]), int(pad),
+        int(bool(flip)), int(policy), int(num_ops), int(magnitude), int(num_bins), _ptr(mags), float(erase_p),
+        float(erase_scale[0]), float(erase_scale[1]), float(erase_ratio[0]), float(erase_ratio[1]),
+        int(bool(erase_random)), _ptr(erase_value), _ptr(scale), _ptr(bias), _ptr(dst), dtype_code(dst.dtype),
+        dst.shape[2], dst.shape[3], _ptr(params_out), _ptr(policy_out), _stream()), name)
+
+
+def mix_images(dst, *, mix_mode: int, lam: float, box=(0, 0, 0, 0)) -> None:
+    """Mixup (``MIX_MIXUP``) or CutMix (``MIX_CUTMIX``, ``box`` = (y0, y1, x0, x1)) of the finished
+    images ``dst`` [B, C, H, W] (contiguous or channels_last, fp32 / bf16) in place, sample p with
+    B-1-p.  See frl_mix_images in include/frl_b200.h."""
+    assert dst.dim() == 4 and (dst.is_contiguous() or is_nhwc(dst))
+    B, Cc, H, W = dst.shape
+    y0, y1, x0, x1 = (int(v) for v in box)
+    name = "frl_mix_images_nhwc" if is_nhwc(dst) else "frl_mix_images"
+    _check(getattr(lib(), name)(_ptr(dst), dtype_code(dst.dtype), B, Cc, H, W, int(mix_mode), float(lam), y0, y1,
+                                x0, x1, _stream()), name)
 
 
 def cast_scale(src, dst, scale: float = 1.0) -> None:

@@ -469,7 +469,8 @@ def make_resnet_problem(ns, save_dir: str, config: str = "resnet18", image: int 
                         n_train: int = 64, n_test: int = 0, pinned: bool = False,
                         uint8: bool = False, augment: Optional[str] = None,
                         stored_image: Optional[int] = None, mixup_alpha: float = 0.0,
-                        cutmix_alpha: float = 0.0, label_smoothing: float = 0.0):
+                        cutmix_alpha: float = 0.0, label_smoothing: float = 0.0,
+                        policy: Optional[str] = None, random_erasing: float = 0.0):
     """Configs 4/5: a torchvision ResNet trunk (its ``fc`` removed) behind
     ``ListSelect`` and one ``nn.Linear`` head per task; x ~ N(0,1) of shape [3, image, image], or
     (``uint8``) raw 8-bit images normalised per channel by the transform (150 kB/sample over
@@ -482,7 +483,10 @@ def make_resnet_problem(ns, save_dir: str, config: str = "resnet18", image: int 
     then pinned; their per-sample transform serves the evaluation splits only.
     ``mixup_alpha`` / ``cutmix_alpha`` (need ``augment``): Mixup / CutMix of the training batches
     (``transform.BatchMix`` over every head's target field) in the augmentation pass.
-    ``label_smoothing``: the classification heads' ``CrossEntropyLoss(label_smoothing=...)``."""
+    ``label_smoothing``: the classification heads' ``CrossEntropyLoss(label_smoothing=...)``.
+    ``policy`` (needs ``augment``): ``"ta_wide"`` (``TrivialAugmentWide()``) or ``"ra"``
+    (``RandAugment()``) on the training crops; ``random_erasing``: ``RandomErasing(p=...)`` of the
+    training images when > 0 (K5p)."""
     import torchvision
     stored = image if stored_image is None else int(stored_image)
     if augment is None and stored != image:
@@ -490,6 +494,8 @@ def make_resnet_problem(ns, save_dir: str, config: str = "resnet18", image: int 
     arch, heads = RESNET_CONFIGS[config]
     aug = None
     mix = None
+    if (policy is not None or random_erasing) and augment is None:
+        raise ValueError("policy / random_erasing run on the device augmentation path: pass augment=...")
     if mixup_alpha or cutmix_alpha:
         from .transform import BatchMix
         if augment is None:
@@ -502,8 +508,15 @@ def make_resnet_problem(ns, save_dir: str, config: str = "resnet18", image: int 
             raise ValueError("augment works on raw uint8 images: pass uint8=True")
         if augment not in DeviceImageAugment.MODES:
             raise ValueError(f"augment must be None or one of {DeviceImageAugment.MODES}, got {augment!r}")
+        from .transform import RandAugment, RandomErasing, TrivialAugmentWide
+        policies = {None: None, "ta_wide": TrivialAugmentWide, "ra": RandAugment}
+        if policy not in policies:
+            raise ValueError(f"policy must be None, 'ta_wide' or 'ra', got {policy!r}")
+        pol = None if policy is None else policies[policy]()
+        erasing = RandomErasing(p=random_erasing) if random_erasing else None
         aug = DeviceImageAugment("x", [field for _, _, field, _ in heads], mode=augment, out_size=image, pad=4,
-                                 scale=U8_CHANNEL_AFFINE[0], bias=U8_CHANNEL_AFFINE[1], mix=mix)
+                                 scale=U8_CHANNEL_AFFINE[0], bias=U8_CHANNEL_AFFINE[1], mix=mix, policy=pol,
+                                 erasing=erasing)
         aug.check_image(3, stored, stored)
     feat = {"resnet18": 512, "resnet50": 2048}[arch]
     Reg, Cls = _task_classes(ns)

@@ -150,6 +150,114 @@ class BatchMix:
         return self.CUTMIX, lam, (y0, y1, x0, x1)
 
 
+#: torchvision's ``_AUGMENTATION_SPACE`` order; K5p's op ids are the positions in it
+POLICY_OPS = ("Identity", "ShearX", "ShearY", "TranslateX", "TranslateY", "Rotate", "Brightness", "Color",
+              "Contrast", "Sharpness", "Posterize", "Solarize", "AutoContrast", "Equalize")
+
+
+def _int_arg(name: str, value, lo: int, hi: Optional[int] = None) -> int:
+    if isinstance(value, bool) or not isinstance(value, (int, np.integer)) or value < lo or (hi is not None
+                                                                                          and value > hi):
+        rng = f"[{lo}, {hi}]" if hi is not None else f">= {lo}"
+        raise ValueError(f"{name} must be an integer {rng}, got {value!r}")
+    return int(value)
+
+
+class TrivialAugmentWide:
+    """TrivialAugmentWide (Müller & Hutter 2021) for ``DeviceImageAugment(..., policy=...)``: one op
+    per training sample, a random magnitude bin and sign, as torchvision's
+    ``TrivialAugmentWide(num_magnitude_bins)`` with NEAREST interpolation and fill 0."""
+
+    native = 1
+    num_ops = 1
+    magnitude = 0
+
+    def __init__(self, num_magnitude_bins: int = 31) -> None:
+        self.num_magnitude_bins = _int_arg("num_magnitude_bins", num_magnitude_bins, 2)
+
+    def magnitudes(self, height: int, width: int) -> Tensor:
+        """fp32 [14, num_magnitude_bins]: torchvision's unsigned magnitude table (0 for the ops
+        without a magnitude)."""
+        nb = self.num_magnitude_bins
+        lin = lambda hi: torch.linspace(0.0, hi, nb)  # noqa: E731
+        rows = [None, lin(0.99), lin(0.99), lin(32.0), lin(32.0), lin(135.0), lin(0.99), lin(0.99), lin(0.99),
+                lin(0.99), (8 - (torch.arange(nb) / ((nb - 1) / 6))).round().int(), torch.linspace(1.0, 0.0, nb),
+                None, None]
+        return torch.stack([torch.zeros(nb) if r is None else r.float() for r in rows])
+
+    def __repr__(self) -> str:
+        return f"TrivialAugmentWide(num_magnitude_bins={self.num_magnitude_bins})"
+
+
+class RandAugment:
+    """RandAugment (Cubuk et al. 2020) for ``DeviceImageAugment(..., policy=...)``: ``num_ops``
+    (1 to 4) random ops per training sample at the fixed ``magnitude`` bin with a random sign, as
+    torchvision's ``RandAugment`` with NEAREST interpolation and fill 0."""
+
+    native = 2
+
+    def __init__(self, num_ops: int = 2, magnitude: int = 9, num_magnitude_bins: int = 31) -> None:
+        self.num_ops = _int_arg("num_ops", num_ops, 1, 4)
+        self.num_magnitude_bins = _int_arg("num_magnitude_bins", num_magnitude_bins, 2)
+        self.magnitude = _int_arg("magnitude", magnitude, 0, self.num_magnitude_bins - 1)
+
+    def magnitudes(self, height: int, width: int) -> Tensor:
+        """fp32 [14, num_magnitude_bins]; TranslateX / TranslateY scale with ``width`` / ``height``."""
+        nb = self.num_magnitude_bins
+        lin = lambda hi: torch.linspace(0.0, hi, nb)  # noqa: E731
+        rows = [None, lin(0.3), lin(0.3), lin(150.0 / 331.0 * width), lin(150.0 / 331.0 * height), lin(30.0),
+                lin(0.9), lin(0.9), lin(0.9), lin(0.9), (8 - (torch.arange(nb) / ((nb - 1) / 4))).round().int(),
+                torch.linspace(1.0, 0.0, nb), None, None]
+        return torch.stack([torch.zeros(nb) if r is None else r.float() for r in rows])
+
+    def __repr__(self) -> str:
+        return (f"RandAugment(num_ops={self.num_ops}, magnitude={self.magnitude}, "
+                f"num_magnitude_bins={self.num_magnitude_bins})")
+
+
+class RandomErasing:
+    """Random erasing (Zhong et al. 2020) of the normalised training images, as torchvision's
+    ``RandomErasing(p, scale, ratio, value)``: ``value`` a number, one number per channel, or
+    ``"random"`` (standard normal values from the device's counter-based generator, not torch's
+    stream)."""
+
+    def __init__(self, p: float = 0.5, scale=(0.02, 0.33), ratio=(0.3, 3.3), value=0.0) -> None:
+        if not (isinstance(p, (int, float)) and not isinstance(p, bool) and 0.0 <= p <= 1.0):
+            raise ValueError(f"p must be in [0, 1], got {p!r}")
+        try:
+            lo, hi = (float(v) for v in scale)
+        except (TypeError, ValueError):
+            raise ValueError(f"scale must be a pair of numbers, got {scale!r}") from None
+        if not 0.0 <= lo <= hi <= 1.0:
+            raise ValueError(f"scale must satisfy 0 <= scale[0] <= scale[1] <= 1, got {scale!r}")
+        self.p = float(p)
+        self.scale = (lo, hi)
+        self.ratio = _pair("ratio", ratio)
+        if isinstance(value, str):
+            if value != "random":
+                raise ValueError(f"value must be a number, a sequence of numbers or 'random', got {value!r}")
+            self.value: Optional[List[float]] = None
+        else:
+            vals = [value] if isinstance(value, (int, float)) else list(value)
+            if not 1 <= len(vals) <= 4 or not all(isinstance(v, (int, float)) and math.isfinite(v) for v in vals):
+                raise ValueError(f"value must be a finite number or 1 to 4 of them, got {value!r}")
+            self.value = [float(v) for v in vals]
+
+    @property
+    def random(self) -> bool:
+        return self.value is None
+
+    def values(self, channels: int) -> List[float]:
+        """The erasing value of every channel (``value`` is not "random")."""
+        if len(self.value) not in (1, channels):
+            raise ValueError(f"RandomErasing value has {len(self.value)} entries for {channels}-channel images")
+        return self.value * channels if len(self.value) == 1 else list(self.value)
+
+    def __repr__(self) -> str:
+        v = "random" if self.value is None else self.value
+        return f"RandomErasing(p={self.p}, scale={self.scale}, ratio={self.ratio}, value={v!r})"
+
+
 def _dist_rank() -> int:
     import torch.distributed as dist
     return dist.get_rank() if dist.is_available() and dist.is_initialized() else 0
@@ -173,6 +281,12 @@ class DeviceImageAugment(DeviceBatchTransform):
     (``frl_augment_mix_images``) and their targets by ``frl_mix_targets``.  Its draws are keyed by
     (``seed``, epoch, rank, the batch's ordinal since ``set_epoch``).  Evaluation splits are not
     mixed and keep their targets as they are.
+    ``policy``: a ``TrivialAugmentWide`` or ``RandAugment``; ``erasing``: a ``RandomErasing``.
+    With either, training images go through K5p (``frl_augment_policy_images``): the same crop and
+    flip, then the policy on the uint8 crop, the normalisation and the erasing, as torchvision v2
+    does them; a mixed batch is then mixed over the finished images (``frl_mix_images``).  Their
+    draws are keyed as the crop's.  Images need 1 or 3 channels with a policy, and a
+    C x out_h x out_w crop of at most ``_native.POLICY_SMEM_BYTES`` bytes.
     With ``memory_format = torch.channels_last`` the images come out [B, C, out_h, out_w] with
     channels_last strides (``frl_augment_images_nhwc`` / ``frl_augment_mix_images_nhwc``), the same
     values as the NCHW output.
@@ -187,7 +301,9 @@ class DeviceImageAugment(DeviceBatchTransform):
                  mean: Optional[Sequence[float]] = None, std: Optional[Sequence[float]] = None,
                  scale: Optional[Sequence[float]] = None, bias: Optional[Sequence[float]] = None,
                  seed: int = 0, eval_crop: float = 0.875, flip: bool = True,
-                 mix: Optional[BatchMix] = None) -> None:
+                 mix: Optional[BatchMix] = None,
+                 policy: Optional[Union[TrivialAugmentWide, RandAugment]] = None,
+                 erasing: Optional[RandomErasing] = None) -> None:
         if mode not in self.MODES:
             raise ValueError(f"mode must be one of {self.MODES}, got {mode!r}")
         oh, ow = (out_size, out_size) if isinstance(out_size, int) else tuple(out_size)
@@ -230,6 +346,13 @@ class DeviceImageAugment(DeviceBatchTransform):
         if mix is not None and not isinstance(mix, BatchMix):
             raise ValueError(f"mix must be a BatchMix or None, got {mix!r}")
         self.mix = mix
+        if policy is not None and not isinstance(policy, (TrivialAugmentWide, RandAugment)):
+            raise ValueError(f"policy must be a TrivialAugmentWide, a RandAugment or None, got {policy!r}")
+        if erasing is not None and not isinstance(erasing, RandomErasing):
+            raise ValueError(f"erasing must be a RandomErasing or None, got {erasing!r}")
+        self.policy = policy
+        self.erasing = erasing
+        self._policy_tabs: Dict[Any, Tuple[Optional[Tensor], Optional[Tensor]]] = {}
         self.epoch = 0
         self.ordinal = 0          # training batches served since set_epoch (keys the mix draws)
         self._targets_checked = False
@@ -251,6 +374,19 @@ class DeviceImageAugment(DeviceBatchTransform):
             raise ValueError(f"out_size {self.out_size} does not fit {height}x{width} images padded by {self.pad}")
         if self.mode == "rrc" and (round(height * self.eval_crop) < 1 or round(width * self.eval_crop) < 1):
             raise ValueError(f"eval_crop {self.eval_crop} leaves no pixel of {height}x{width} images")
+        if self.policy is not None or self.erasing is not None:
+            from . import _native
+            if self.policy is not None and channels not in (1, 3):
+                raise ValueError(f"{self.policy!r} needs 1- or 3-channel images (torchvision's colour ops), "
+                                 f"got {channels}")
+            if channels > 3:
+                raise ValueError(f"RandomErasing on the device serves 1 to 3 channels, got {channels}")
+            if channels * oh * ow > _native.POLICY_SMEM_BYTES:
+                raise ValueError(f"a {channels}x{oh}x{ow} crop ({channels * oh * ow} bytes) does not fit one CTA's "
+                                 f"shared memory ({_native.POLICY_SMEM_BYTES} bytes): out_size too large for "
+                                 f"policy / erasing")
+            if self.erasing is not None and not self.erasing.random:
+                self.erasing.values(channels)
 
     def native_mode(self, split: Split) -> int:
         from . import _native
@@ -284,6 +420,35 @@ class DeviceImageAugment(DeviceBatchTransform):
         sc, bi = self._coefs(x)
         out = self._out(x, out_dtype)
         _native.augment_images(x.contiguous(), index, out, **self._native_args(split, sc, bi, params_out))
+        return out
+
+    def _policy_tables(self, x: Tensor):
+        """(magnitude table, erasing values) on ``x``'s device, built once per device."""
+        if x.device not in self._policy_tabs:
+            oh, ow = self.out_size
+            mags = None if self.policy is None else self.policy.magnitudes(oh, ow).to(x.device).contiguous()
+            ev = None
+            if self.erasing is not None and not self.erasing.random:
+                ev = torch.tensor(self.erasing.values(x.shape[1]), dtype=torch.float32, device=x.device)
+            self._policy_tabs[x.device] = (mags, ev)
+        return self._policy_tabs[x.device]
+
+    def augment_policy(self, x: Tensor, index: Tensor, out_dtype, params_out=None, policy_out=None) -> Tensor:
+        """Training images [B, C, out_h, out_w] of ``out_dtype`` in ``memory_format``: K5a's crop and
+        flip, then ``policy``, the affine and ``erasing`` (K5p, ``frl_augment_policy_images``)."""
+        from . import _native
+        sc, bi = self._coefs(x)
+        mags, ev = self._policy_tables(x)
+        out = self._out(x, out_dtype)
+        pol, er = self.policy, self.erasing
+        _native.augment_policy_images(
+            x.contiguous(), index, out, seed=self.seed, epoch=self.epoch, mode=self.native_mode(Split.TRAIN),
+            scale_range=self.crop_scale, ratio_range=self.crop_ratio, pad=self.pad, flip=self.flip,
+            policy=_native.POLICY_NONE if pol is None else pol.native, num_ops=1 if pol is None else pol.num_ops,
+            magnitude=0 if pol is None else pol.magnitude, mags=mags, erase_p=0.0 if er is None else er.p,
+            erase_scale=(0.02, 0.33) if er is None else er.scale, erase_ratio=(0.3, 3.3) if er is None else er.ratio,
+            erase_random=er is not None and er.random, erase_value=ev, scale=sc, bias=bi, params_out=params_out,
+            policy_out=policy_out)
         return out
 
     def augment_mixed(self, x: Tensor, index: Tensor, out_dtype, mode: int, lam: float, box,
@@ -330,12 +495,23 @@ class DeviceImageAugment(DeviceBatchTransform):
     def apply(self, raw, split, out_dtype, index=None):
         if index is None:
             raise ValueError("DeviceImageAugment.apply needs index= (the dataset row of every sample)")
+        per_sample = (self.policy is not None or self.erasing is not None) and split == Split.TRAIN
         if self.mix is None or split != Split.TRAIN:
-            out = self.augment(raw[self.image_field], index, split, out_dtype)
+            if per_sample:
+                out = self.augment_policy(raw[self.image_field], index, out_dtype)
+            else:
+                out = self.augment(raw[self.image_field], index, split, out_dtype)
             return [out], [(raw[f],) for f in self.target_fields]
         mode, lam, box = self.mix.draw(self.seed, self.epoch, _dist_rank(), self.ordinal, *self.out_size)
         self.ordinal += 1
         x = raw[self.image_field]
+        if per_sample:
+            # Mixup / CutMix over the finished images (frl_mix_images): a bf16 Mixup rounds twice
+            from . import _native
+            out = self.augment_policy(x, index, out_dtype)
+            if mode != BatchMix.NONE:
+                _native.mix_images(out, mix_mode=mode, lam=lam, box=box)
+            return [out], self.mix_targets(raw, lam)
         if mode == BatchMix.NONE:
             out = self.augment(x, index, split, out_dtype)
         else:

@@ -686,6 +686,86 @@ int frl_augment_mix_images_nhwc(const void* src, int64_t batch, int channels, in
 int frl_mix_targets(const void* src, int src_dtype, int64_t batch, int64_t inner, int n_classes, float lam,
                     void* dst, void* stream);
 
+/* ------------------------------------------------------------------------------------------
+ * K5p — K5a's training crop and flip, then an automatic augmentation policy (TrivialAugmentWide,
+ * Müller & Hutter 2021, or RandAugment, Cubuk et al. 2020), then the affine, then random erasing
+ * (Zhong et al. 2020), as torchvision v2 does them on a uint8 image.  One CTA per sample stages its
+ * crop in shared memory.
+ *   src, idx, seed, epoch, smin..rmax, pad, flip, scale, bias, dst, out_h, out_w, params_out:
+ *              as frl_augment_images; mode FRL_AUG_RRC or FRL_AUG_PAD_CROP only
+ *   policy     FRL_POLICY_NONE (erasing alone), FRL_POLICY_TRIVIAL_AUGMENT (num_ops must be 1) or
+ *              FRL_POLICY_RAND_AUGMENT (num_ops in [1, 4], magnitude in [0, num_bins)); a policy
+ *              needs channels 1 or 3, K5p serves at most 3
+ *   mags       device fp32 [14, num_bins], num_bins >= 2: the magnitude of op o at bin k (the
+ *              unsigned table torchvision builds for the output size; Posterize's bits as floats;
+ *              0 for the three ops without a magnitude)
+ *   erase_p    probability of erasing, in [0, 1]; 0 turns erasing off.  erase_smin/smax: area share
+ *              in [0, 1]; erase_rmin/rmax > 0: aspect range.  erase_random != 0: N(0, 1) values;
+ *              else erase_value (device fp32 [C], NULL = 0), in the normalised domain
+ *   policy_out optional int32 [B, 3*num_ops + 5] (num_ops 0 without a policy): (op, bin, sign) per
+ *              op, then (erased, top, left, h, w)
+ * channels * out_h * out_w must be at most FRL_AUGMENT_POLICY_SMEM_BYTES (FRL_E_ARG).
+ *
+ * Draws (Philox4x32-10 with K5a's key and counter (lo32(i), hi32(i), epoch, block); u(w) and
+ * int(w, n) as K5a's; K5a's blocks 0..10 keep their meaning, so the box and flip do not depend on
+ * the policy or erasing):
+ *   op k (k < num_ops): block 11 + k: op = int(w0, 14) in torchvision's _AUGMENTATION_SPACE order
+ *     (Identity, ShearX, ShearY, TranslateX, TranslateY, Rotate, Brightness, Color, Contrast,
+ *     Sharpness, Posterize, Solarize, AutoContrast, Equalize); bin = int(w1, num_bins) for
+ *     TrivialAugmentWide, `magnitude` for RandAugment; sign = -1 if w2 >> 31 for the nine signed
+ *     ops (ShearX .. Sharpness), else +1.  Ops without a magnitude record bin 0.
+ *     magnitude = sign * mags[op, bin].
+ *   erasing: block 15: erase if u(w0) < erase_p.  Attempt t = 0..9 uses block 16 + t, in double:
+ *     area = out_h*out_w * (smin + u(w0)*(smax - smin)); aspect = exp(log rmin + u(w1)*(log rmax -
+ *     log rmin)); h = rint(sqrt(area*aspect)), w = rint(sqrt(area/aspect)) (h takes the product,
+ *     the reverse of RRC); accepted if h < out_h and w < out_w: top = int(w2, out_h-h+1),
+ *     left = int(w3, out_w-w+1).  No attempt accepted: nothing is erased.
+ *   random values: element e = (c*h + y)*w + x of the box uses block 32 + e/4, pair j = (e/2) % 2:
+ *     u1 = ((w_{2j} >> 8) + 1) * 2^-24, u2 = (w_{2j+1} >> 8) * 2^-24, r = sqrt(-2 ln u1),
+ *     value = r cos(2 pi u2) for even e, r sin(2 pi u2) for odd e (fp32; not torch's stream).
+ * Pixels:
+ *   1. the crop: K5a's bilinear value v before the affine, rounded half to even to uint8
+ *      (F.resized_crop(x.float(), antialias=False).round_()); flipped samples mirrored.
+ *   2. each op on the uint8 image, uint8 after every op, as TrivialAugmentWide.
+ *      _apply_image_or_video_transform does it: geometric ops with NEAREST and fill 0, their
+ *      inverse matrix from torchvision's formula in double, the grid in fp32; colour ops in fp32
+ *      with torch's roundings, then clamped to [0, 255] and truncated.
+ *   3. dst = fmaf(v, scale[c], bias[c]) as K5a; inside the erased box the erasing value instead.
+ * dst is also the CTA's scratch: it stages index-map op results in its own sample's region.
+ * Graph-capturable: no host reads, no allocation.  Every argument check comes before any launch.
+ * ---------------------------------------------------------------------------------------- */
+enum { FRL_POLICY_NONE = 0, FRL_POLICY_TRIVIAL_AUGMENT = 1, FRL_POLICY_RAND_AUGMENT = 2 };
+enum { FRL_AUGMENT_POLICY_SMEM_BYTES = 224256 };
+int frl_augment_policy_images(const void* src, int64_t batch, int channels, int height, int width,
+                              const int64_t* idx, uint64_t seed, int epoch, int mode,
+                              double smin, double smax, double rmin, double rmax, int pad, int flip,
+                              int policy, int num_ops, int magnitude, int num_bins, const float* mags,
+                              double erase_p, double erase_smin, double erase_smax, double erase_rmin,
+                              double erase_rmax, int erase_random, const float* erase_value,
+                              const float* scale, const float* bias, void* dst, int dst_dtype,
+                              int out_h, int out_w, int32_t* params_out, int32_t* policy_out, void* stream);
+/* frl_augment_policy_images with dst in [B, out_h, out_w, C] memory order: the same values. */
+int frl_augment_policy_images_nhwc(const void* src, int64_t batch, int channels, int height, int width,
+                                   const int64_t* idx, uint64_t seed, int epoch, int mode,
+                                   double smin, double smax, double rmin, double rmax, int pad, int flip,
+                                   int policy, int num_ops, int magnitude, int num_bins, const float* mags,
+                                   double erase_p, double erase_smin, double erase_smax, double erase_rmin,
+                                   double erase_rmax, int erase_random, const float* erase_value,
+                                   const float* scale, const float* bias, void* dst, int dst_dtype,
+                                   int out_h, int out_w, int32_t* params_out, int32_t* policy_out,
+                                   void* stream);
+
+/* Mixup / CutMix of finished images in place: dst [B, C, out_h, out_w] (fp32 / bf16; the _nhwc
+ * form: [B, out_h, out_w, C] in memory), sample p with sample j = B-1-p, p < B/2:
+ *   Mixup:  out_p = round(__fadd_rn(__fmul_rn(lam, a_p), __fmul_rn(lam1, a_j))), lam1 as
+ *           frl_augment_mix_images.  a_p is the stored value, so bf16 images round twice.
+ *   CutMix: a_p and a_j swap inside [box_y0, box_y1) x [box_x0, box_x1) (exact).
+ * The middle sample of an odd batch is left as it is.  Every argument check comes before any launch. */
+int frl_mix_images(void* dst, int dst_dtype, int64_t batch, int channels, int out_h, int out_w, int mix_mode,
+                   float lam, int box_y0, int box_y1, int box_x0, int box_x1, void* stream);
+int frl_mix_images_nhwc(void* dst, int dst_dtype, int64_t batch, int channels, int out_h, int out_w,
+                        int mix_mode, float lam, int box_y0, int box_y1, int box_x0, int box_x1, void* stream);
+
 /* dtype conversion / scaled copy used by the arena (master -> shadow refresh after a
  * checkpoint load, gradient flatten for modules the arena cannot write into directly):
  * dst = src * scale. */
