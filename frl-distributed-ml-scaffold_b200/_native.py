@@ -93,6 +93,24 @@ SIGNATURES = {
     "frl_rmsprop_mt_sr": (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _i64, _u64, _i64, _d, _d, _d, _d, _d, _d, _vp, _vp,
                                _vp]),
     "frl_weight_ema_bf16": (_i, [_vp, _vp, _i64, _d, _vp]),
+    "frl_sgd_momentum_mt_grouped": (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _i64, _vp, _vp, _vp, _i, _d, _d, _d, _vp, _i,
+                                         _vp]),
+    "frl_adam_mt_grouped": (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _i64, _vp, _vp, _vp, _i, _d, _d, _d, _d, _vp,
+                                 _vp]),
+    "frl_adamw_mt_grouped": (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _i64, _vp, _vp, _vp, _i, _d, _d, _d, _d,
+                                  _vp, _vp]),
+    "frl_lion_mt_grouped": (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _i64, _vp, _vp, _vp, _i, _d, _d, _d, _vp, _vp]),
+    "frl_rmsprop_mt_grouped": (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _i64, _vp, _vp, _vp, _i, _d, _d, _d, _d, _vp,
+                                    _vp]),
+    "frl_sgd_momentum_mt_grouped_sr": (_i, [_vp, _vp, _vp, _vp, _vp, _i64, _vp, _vp, _vp, _i, _u64, _d, _d, _d, _vp,
+                                            _i, _vp]),
+    "frl_adam_mt_grouped_sr": (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _i64, _vp, _vp, _vp, _i, _u64, _d, _d, _d, _d,
+                                    _vp, _vp]),
+    "frl_adamw_mt_grouped_sr": (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _i64, _vp, _vp, _vp, _i, _u64, _d, _d, _d,
+                                     _d, _vp, _vp]),
+    "frl_lion_mt_grouped_sr": (_i, [_vp, _vp, _vp, _vp, _vp, _i64, _vp, _vp, _vp, _i, _u64, _d, _d, _d, _vp, _vp]),
+    "frl_rmsprop_mt_grouped_sr": (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _i64, _vp, _vp, _vp, _i, _u64, _d, _d, _d, _d,
+                                       _vp, _vp]),
     "frl_layerwise_scratch_bytes": (_i64, [_i64, _i64]),
     "frl_lars_mt": (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _i64, _i64, _vp, _vp, _vp, _d, _d, _d, _d, _vp, _vp, _i, _vp]),
     "frl_lamb_mt": (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _i64, _i64, _vp, _vp, _vp, _d, _d, _d, _d, _d, _i64,
@@ -513,6 +531,118 @@ def rmsprop_mt_sr(p, sq, buf, table, *, seed, t, lr, alpha, eps, wd, mu, grad_sc
     _check(lib().frl_rmsprop_mt_sr(_ptr(p), _ptr(sq), _ptr(buf), table.segs_dev_ptr, table.prefix_dev_ptr,
                                    table.tile_seg_dev_ptr, table.n_tiles, seed, t, lr, alpha, eps, wd, mu,
                                    grad_scale, _ptr(grad_scale_dev), _ptr(dyn), _stream()), "frl_rmsprop_mt_sr")
+
+
+# ---- K2-mt grouped / K2-mt-sr grouped: parameter groups over a segment table --------------------
+
+GROUP_DYN_COLS = 8       # FRL_GROUP_DYN_COLS: floats per row of the group_dyn table
+
+
+class SegGroups:
+    """The group arrays of one segment table (see frl_*_mt_grouped in include/frl_b200.h): the
+    device int32 ``seg_group`` / ``seg_flags`` of its segments and the fp32 ``[n_groups, 8]`` row
+    table ``group_dyn`` (shared, not owned: the optimizer rewrites its rows).  The group indices are
+    validated here, on the host, because the kernels do not read them back before launching."""
+
+    def __init__(self, seg_group: Sequence[int], seg_flags: Sequence[int], group_dyn: torch.Tensor) -> None:
+        if group_dyn.dtype != torch.float32 or group_dyn.dim() != 2 or group_dyn.shape[1] != GROUP_DYN_COLS \
+                or not group_dyn.is_contiguous() or group_dyn.shape[0] < 1:
+            raise NativeLibraryError("grouped update: group_dyn must be contiguous fp32 [n_groups >= 1, %d], got %s %s"
+                                     % (GROUP_DYN_COLS, group_dyn.dtype, tuple(group_dyn.shape)))
+        n_groups = group_dyn.shape[0]
+        if len(seg_group) != len(seg_flags):
+            raise NativeLibraryError("grouped update: %d segment groups for %d segment flags"
+                                     % (len(seg_group), len(seg_flags)))
+        bad = [g for g in seg_group if not 0 <= int(g) < n_groups]
+        if bad:
+            raise NativeLibraryError("grouped update: group indices %s outside [0, %d)" % (sorted(set(bad)), n_groups))
+        dev = group_dyn.device
+        self.n_segs = len(seg_group)
+        self.n_groups = n_groups
+        self.seg_group = torch.tensor([int(g) for g in seg_group] or [0], dtype=torch.int32).to(dev)
+        self.seg_flags = torch.tensor([int(f) for f in seg_flags] or [0], dtype=torch.int32).to(dev)
+        self.group_dyn = group_dyn
+
+
+def _grouped(table, groups: "SegGroups"):
+    if groups.n_segs != table.n_segs:
+        raise NativeLibraryError("grouped update: group arrays of %d segments for a table of %d"
+                                 % (groups.n_segs, table.n_segs))
+    return (table.segs_dev_ptr, table.prefix_dev_ptr, table.tile_seg_dev_ptr, table.n_tiles,
+            _ptr(groups.seg_group), _ptr(groups.seg_flags), _ptr(groups.group_dyn), groups.n_groups)
+
+
+def sgd_momentum_mt_grouped(p, buf, p_lp, table, groups, *, mu, dampening, grad_scale=1.0, grad_scale_dev=None,
+                            first_step=False) -> None:
+    """K2-mt SGD with each segment's lr / wd from its group's row (see frl_sgd_momentum_mt_grouped)."""
+    _check(lib().frl_sgd_momentum_mt_grouped(_ptr(p), _ptr(buf), _ptr(p_lp), *_grouped(table, groups), mu, dampening,
+                                             grad_scale, _ptr(grad_scale_dev), int(first_step), _stream()),
+           "frl_sgd_momentum_mt_grouped")
+
+
+def adam_mt_grouped(p, m, v, vmax, p_lp, table, groups, *, beta1, beta2, eps, grad_scale=1.0,
+                    grad_scale_dev=None) -> None:
+    _check(lib().frl_adam_mt_grouped(_ptr(p), _ptr(m), _ptr(v), _ptr(vmax), _ptr(p_lp), *_grouped(table, groups),
+                                     beta1, beta2, eps, grad_scale, _ptr(grad_scale_dev), _stream()),
+           "frl_adam_mt_grouped")
+
+
+def adamw_mt_grouped(p, m, v, vmax, p_lp, table, groups, *, beta1, beta2, eps, grad_scale=1.0,
+                     grad_scale_dev=None) -> None:
+    _check(lib().frl_adamw_mt_grouped(_ptr(p), _ptr(m), _ptr(v), _ptr(vmax), _ptr(p_lp), *_grouped(table, groups),
+                                      beta1, beta2, eps, grad_scale, _ptr(grad_scale_dev), _stream()),
+           "frl_adamw_mt_grouped")
+
+
+def lion_mt_grouped(p, m, p_lp, table, groups, *, beta1, beta2, grad_scale=1.0, grad_scale_dev=None) -> None:
+    _check(lib().frl_lion_mt_grouped(_ptr(p), _ptr(m), _ptr(p_lp), *_grouped(table, groups), beta1, beta2,
+                                     grad_scale, _ptr(grad_scale_dev), _stream()), "frl_lion_mt_grouped")
+
+
+def rmsprop_mt_grouped(p, sq, buf, p_lp, table, groups, *, alpha, eps, mu, grad_scale=1.0,
+                       grad_scale_dev=None) -> None:
+    _check(lib().frl_rmsprop_mt_grouped(_ptr(p), _ptr(sq), _ptr(buf), _ptr(p_lp), *_grouped(table, groups), alpha,
+                                        eps, mu, grad_scale, _ptr(grad_scale_dev), _stream()),
+           "frl_rmsprop_mt_grouped")
+
+
+def sgd_momentum_mt_grouped_sr(p, buf, table, groups, *, seed, mu, dampening, grad_scale=1.0, grad_scale_dev=None,
+                               first_step=False) -> None:
+    """K2-mt-sr SGD with each segment's lr / wd and the update count from its group's row."""
+    _check_sr(p, seed)
+    _check(lib().frl_sgd_momentum_mt_grouped_sr(_ptr(p), _ptr(buf), *_grouped(table, groups), seed, mu, dampening,
+                                                grad_scale, _ptr(grad_scale_dev), int(first_step), _stream()),
+           "frl_sgd_momentum_mt_grouped_sr")
+
+
+def adam_mt_grouped_sr(p, m, v, vmax, table, groups, *, seed, beta1, beta2, eps, grad_scale=1.0,
+                       grad_scale_dev=None) -> None:
+    _check_sr(p, seed)
+    _check(lib().frl_adam_mt_grouped_sr(_ptr(p), _ptr(m), _ptr(v), _ptr(vmax), *_grouped(table, groups), seed, beta1,
+                                        beta2, eps, grad_scale, _ptr(grad_scale_dev), _stream()),
+           "frl_adam_mt_grouped_sr")
+
+
+def adamw_mt_grouped_sr(p, m, v, vmax, table, groups, *, seed, beta1, beta2, eps, grad_scale=1.0,
+                        grad_scale_dev=None) -> None:
+    _check_sr(p, seed)
+    _check(lib().frl_adamw_mt_grouped_sr(_ptr(p), _ptr(m), _ptr(v), _ptr(vmax), *_grouped(table, groups), seed,
+                                         beta1, beta2, eps, grad_scale, _ptr(grad_scale_dev), _stream()),
+           "frl_adamw_mt_grouped_sr")
+
+
+def lion_mt_grouped_sr(p, m, table, groups, *, seed, beta1, beta2, grad_scale=1.0, grad_scale_dev=None) -> None:
+    _check_sr(p, seed)
+    _check(lib().frl_lion_mt_grouped_sr(_ptr(p), _ptr(m), *_grouped(table, groups), seed, beta1, beta2, grad_scale,
+                                        _ptr(grad_scale_dev), _stream()), "frl_lion_mt_grouped_sr")
+
+
+def rmsprop_mt_grouped_sr(p, sq, buf, table, groups, *, seed, alpha, eps, mu, grad_scale=1.0,
+                          grad_scale_dev=None) -> None:
+    _check_sr(p, seed)
+    _check(lib().frl_rmsprop_mt_grouped_sr(_ptr(p), _ptr(sq), _ptr(buf), *_grouped(table, groups), seed, alpha, eps,
+                                           mu, grad_scale, _ptr(grad_scale_dev), _stream()),
+           "frl_rmsprop_mt_grouped_sr")
 
 
 # ---- K2-lw: layer-wise adaptive updates (LARS, LAMB) over a segment table -------------------------

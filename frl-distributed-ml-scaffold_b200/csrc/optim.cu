@@ -185,6 +185,70 @@ __device__ __forceinline__ void mt_full_tile(const Rule& rule, float gs, f32x4* 
     }
 }
 
+// one tile of a segment: interior tiles run the flat kernel's body, the last tile of a segment (or
+// a small tensor) is bounds-checked, element-wise at the very end
+template <typename Rule, int NS, bool HAS_LP>
+__device__ __forceinline__ void mt_tile(const Rule& rule, float gs, f32x4* p, f32x4* s0, f32x4* s1, f32x4* s2,
+                                        bf16x4* lp, const SegView& sv) {
+    const f32x4 zero{0.f, 0.f, 0.f, 0.f};
+    const int64_t v0 = sv.t_in * kTileVec + threadIdx.x;      // vec4 index inside the segment
+    const int64_t a0 = sv.arena_off >> 2;                     // vec4 index of the segment in the arena
+    if ((sv.t_in + 1) * kTileVec <= (sv.numel >> 2)) {        // CTA-uniform: interior tile
+        if (sv.g_dtype == FRL_F32)
+            mt_full_tile<Rule, f32x4, NS, HAS_LP>(rule, gs, p, s0, s1, s2, lp, static_cast<const f32x4*>(sv.g), a0, v0);
+        else
+            mt_full_tile<Rule, bf16x4, NS, HAS_LP>(rule, gs, p, s0, s1, s2, lp, static_cast<const bf16x4*>(sv.g), a0, v0);
+        return;
+    }
+    const int64_t seg_vec = (sv.numel + 3) >> 2;              // arena slices are padded to 8
+#pragma unroll 1
+    for (int j = 0; j < kUnroll; ++j) {
+        const int64_t v = v0 + j * kThreads;
+        if (v >= seg_vec) break;
+        const int64_t i = a0 + v;
+        f32x4 qg = seg_load4(sv, v << 2), qp = ld_stream(p + i);
+        f32x4 q0 = NS > 0 ? ld_stream(s0 + i) : zero;
+        f32x4 q1 = NS > 1 ? ld_stream(s1 + i) : zero;
+        f32x4 q2 = NS > 2 ? ld_stream(s2 + i) : zero;
+        apply4(rule, qp, qg, gs, q0, q1, q2);
+        st_stream(p + i, qp);
+        if (NS > 0) st_stream(s0 + i, q0);
+        if (NS > 1) st_stream(s1 + i, q1);
+        if (NS > 2) st_stream(s2 + i, q2);
+        if (HAS_LP) st_stream(lp + i, bf16x4{pack_bf16(qp.x, qp.y), pack_bf16(qp.z, qp.w)});
+    }
+}
+
+// GROUPED (the _mt_grouped forms): per tile, the segment's group row patches a register copy of the
+// rule (one L1/L2-resident read of a few floats per 16 KB+ tile) and the segment's FRL_LW_CLIPPED
+// flag decides whether the device clip coefficient applies; dyn is unused.
+template <typename Rule, int NS, bool HAS_LP, bool GROUPED>
+__device__ __forceinline__ void update_mt_body(float* __restrict__ p_, float* __restrict__ s0_, float* __restrict__ s1_,
+                                               float* __restrict__ s2_, bf16x4* __restrict__ lp,
+                                               const frl_grad_seg* __restrict__ segs,
+                                               const int64_t* __restrict__ tile_prefix,
+                                               const int32_t* __restrict__ tile_seg, int64_t n_tiles, Rule rule,
+                                               float gscale, const float* __restrict__ gscale_dev,
+                                               const float* __restrict__ dyn, const GroupTable& grp) {
+    if (dyn) rule.patch(dyn);
+    f32x4* p = reinterpret_cast<f32x4*>(p_);
+    f32x4* s0 = reinterpret_cast<f32x4*>(s0_);
+    f32x4* s1 = reinterpret_cast<f32x4*>(s1_);
+    f32x4* s2 = reinterpret_cast<f32x4*>(s2_);
+    const float gs = gscale_dev ? gscale * __ldg(gscale_dev) : gscale;
+    for (int64_t tile = blockIdx.x; tile < n_tiles; tile += gridDim.x) {
+        const SegView sv = find_segment(segs, tile_prefix, tile_seg, tile);
+        if constexpr (GROUPED) {
+            Rule r = rule;
+            r.patch_group(grp.rows + FRL_GROUP_DYN_COLS * __ldg(grp.seg_group + sv.seg));
+            mt_tile<Rule, NS, HAS_LP>(r, seg_scale(__ldg(grp.seg_flags + sv.seg), gscale, gscale_dev),
+                                      p, s0, s1, s2, lp, sv);
+        } else {
+            mt_tile<Rule, NS, HAS_LP>(rule, gs, p, s0, s1, s2, lp, sv);
+        }
+    }
+}
+
 template <typename Rule, int NS, bool HAS_LP>
 __global__ void __launch_bounds__(kThreads)
 update_mt_kernel(float* __restrict__ p_, float* __restrict__ s0_, float* __restrict__ s1_,
@@ -192,45 +256,19 @@ update_mt_kernel(float* __restrict__ p_, float* __restrict__ s0_, float* __restr
                  const frl_grad_seg* __restrict__ segs, const int64_t* __restrict__ tile_prefix,
                  const int32_t* __restrict__ tile_seg, int64_t n_tiles, Rule rule, float gscale,
                  const float* __restrict__ gscale_dev, const float* __restrict__ dyn) {
-    if (dyn) rule.patch(dyn);
-    f32x4* p = reinterpret_cast<f32x4*>(p_);
-    f32x4* s0 = reinterpret_cast<f32x4*>(s0_);
-    f32x4* s1 = reinterpret_cast<f32x4*>(s1_);
-    f32x4* s2 = reinterpret_cast<f32x4*>(s2_);
-    const float gs = gscale_dev ? gscale * __ldg(gscale_dev) : gscale;
-    const f32x4 zero{0.f, 0.f, 0.f, 0.f};
-    for (int64_t tile = blockIdx.x; tile < n_tiles; tile += gridDim.x) {
-        const SegView sv = find_segment(segs, tile_prefix, tile_seg, tile);
-        const int64_t v0 = sv.t_in * kTileVec + threadIdx.x;      // vec4 index inside the segment
-        const int64_t a0 = sv.arena_off >> 2;                     // vec4 index of the segment in the arena
-        if ((sv.t_in + 1) * kTileVec <= (sv.numel >> 2)) {        // CTA-uniform: interior tile
-            if (sv.g_dtype == FRL_F32)
-                mt_full_tile<Rule, f32x4, NS, HAS_LP>(rule, gs, p, s0, s1, s2, lp,
-                                                      static_cast<const f32x4*>(sv.g), a0, v0);
-            else
-                mt_full_tile<Rule, bf16x4, NS, HAS_LP>(rule, gs, p, s0, s1, s2, lp,
-                                                       static_cast<const bf16x4*>(sv.g), a0, v0);
-            continue;
-        }
-        // last tile of a segment (or a small tensor): bounds-checked, element-wise at the very end
-        const int64_t seg_vec = (sv.numel + 3) >> 2;              // arena slices are padded to 8
-#pragma unroll 1
-        for (int j = 0; j < kUnroll; ++j) {
-            const int64_t v = v0 + j * kThreads;
-            if (v >= seg_vec) break;
-            const int64_t i = a0 + v;
-            f32x4 qg = seg_load4(sv, v << 2), qp = ld_stream(p + i);
-            f32x4 q0 = NS > 0 ? ld_stream(s0 + i) : zero;
-            f32x4 q1 = NS > 1 ? ld_stream(s1 + i) : zero;
-            f32x4 q2 = NS > 2 ? ld_stream(s2 + i) : zero;
-            apply4(rule, qp, qg, gs, q0, q1, q2);
-            st_stream(p + i, qp);
-            if (NS > 0) st_stream(s0 + i, q0);
-            if (NS > 1) st_stream(s1 + i, q1);
-            if (NS > 2) st_stream(s2 + i, q2);
-            if (HAS_LP) st_stream(lp + i, bf16x4{pack_bf16(qp.x, qp.y), pack_bf16(qp.z, qp.w)});
-        }
-    }
+    update_mt_body<Rule, NS, HAS_LP, false>(p_, s0_, s1_, s2_, lp, segs, tile_prefix, tile_seg, n_tiles, rule, gscale,
+                                            gscale_dev, dyn, GroupTable{});
+}
+
+template <typename Rule, int NS, bool HAS_LP>
+__global__ void __launch_bounds__(kThreads)
+update_mt_grouped_kernel(float* __restrict__ p_, float* __restrict__ s0_, float* __restrict__ s1_,
+                         float* __restrict__ s2_, bf16x4* __restrict__ lp,
+                         const frl_grad_seg* __restrict__ segs, const int64_t* __restrict__ tile_prefix,
+                         const int32_t* __restrict__ tile_seg, int64_t n_tiles, Rule rule, float gscale,
+                         const float* __restrict__ gscale_dev, GroupTable grp) {
+    update_mt_body<Rule, NS, HAS_LP, true>(p_, s0_, s1_, s2_, lp, segs, tile_prefix, tile_seg, n_tiles, rule, gscale,
+                                           gscale_dev, nullptr, grp);
 }
 
 template <typename DVec>
@@ -269,17 +307,29 @@ flatten_kernel(DVec* __restrict__ dst, const frl_grad_seg* __restrict__ segs,
     }
 }
 
-template <typename Rule, int NS>
+template <typename Rule, int NS, bool G = false>
 static int launch_update_mt(const Rule& rule, float* p, float* s0, float* s1, float* s2, void* p_lp,
                             const frl_grad_seg* segs, const int64_t* tile_prefix, const int32_t* tile_seg,
                             int64_t n_tiles, float gscale, const float* gscale_dev, const float* dyn,
-                            cudaStream_t st, const char* name) {
+                            cudaStream_t st, const char* name, GroupTable grp = {}, int n_groups = 0) {
     FRL_REQUIRE(n_tiles >= 0, FRL_E_ARG, "%s: negative tile count", name);
     if (n_tiles == 0) return 0;
     FRL_REQUIRE(p && segs && tile_prefix && tile_seg, FRL_E_ARG, "%s: null p/segs/tile_prefix/tile_seg", name);
     FRL_REQUIRE(aligned16(p) && aligned16(s0) && aligned16(s1) && aligned16(s2) && aligned16(p_lp),
                 FRL_E_ALIGN, "%s: arrays must be 16-byte aligned", name);
     bf16x4* lp = static_cast<bf16x4*>(p_lp);
+    if constexpr (G) {
+        FRL_CHECK_GROUPS(grp, n_groups, name);
+        if (lp)
+            update_mt_grouped_kernel<Rule, NS, true><<<grid_for_tiles(update_mt_grouped_kernel<Rule, NS, true>, n_tiles),
+                                                       kThreads, 0, st>>>(
+                p, s0, s1, s2, lp, segs, tile_prefix, tile_seg, n_tiles, rule, gscale, gscale_dev, grp);
+        else
+            update_mt_grouped_kernel<Rule, NS, false><<<grid_for_tiles(update_mt_grouped_kernel<Rule, NS, false>, n_tiles),
+                                                        kThreads, 0, st>>>(
+                p, s0, s1, s2, lp, segs, tile_prefix, tile_seg, n_tiles, rule, gscale, gscale_dev, grp);
+        return after_launch(name);
+    }
     if (lp)
         update_mt_kernel<Rule, NS, true><<<grid_for_tiles(update_mt_kernel<Rule, NS, true>, n_tiles), kThreads, 0, st>>>(
             p, s0, s1, s2, lp, segs, tile_prefix, tile_seg, n_tiles, rule, gscale, gscale_dev, dyn);
@@ -481,4 +531,101 @@ extern "C" int frl_rmsprop_mt(float* p, float* sq, float* buf, void* p_lp, const
     return launch_update_mt<RmspropRule<false>, 1>(make_rmsprop_rule<false>(lr, alpha, eps, wd, mu), p, sq, nullptr, nullptr,
                                                    p_lp, segs_dev, tile_prefix_dev, tile_seg_dev, n_tiles, gs,
                                                    grad_scale_dev, dyn, st, "frl_rmsprop_mt");
+}
+
+// ---- parameter-group (K2-mt grouped) entry points --------------------------------------------------
+// The ungrouped form's arguments without lr / wd / dyn (each segment's group row supplies them) and
+// with the group table after n_tiles; see include/frl_b200.h.
+
+extern "C" int frl_sgd_momentum_mt_grouped(float* p, float* buf, void* p_lp, const frl_grad_seg* segs_dev,
+                                           const int64_t* tile_prefix_dev, const int32_t* tile_seg_dev,
+                                           int64_t n_tiles, const int32_t* seg_group_dev, const int32_t* seg_flags_dev,
+                                           const float* group_dyn, int n_groups, double mu, double dampening,
+                                           double grad_scale, const float* grad_scale_dev, int first_step,
+                                           void* stream) {
+    const char* name = "frl_sgd_momentum_mt_grouped";
+    FRL_REQUIRE(mu == 0.0 || buf != nullptr, FRL_E_ARG, "%s: momentum needs buf", name);
+    const SgdRule r = make_sgd_rule(0.0, mu, dampening, 0.0, first_step);
+    const GroupTable grp{seg_group_dev, seg_flags_dev, group_dyn};
+    cudaStream_t st = static_cast<cudaStream_t>(stream);
+    const float gs = static_cast<float>(grad_scale);
+    if (mu != 0.0)
+        return launch_update_mt<SgdRule, 1, true>(r, p, buf, nullptr, nullptr, p_lp, segs_dev, tile_prefix_dev,
+                                                  tile_seg_dev, n_tiles, gs, grad_scale_dev, nullptr, st, name, grp,
+                                                  n_groups);
+    return launch_update_mt<SgdRule, 0, true>(r, p, nullptr, nullptr, nullptr, p_lp, segs_dev, tile_prefix_dev,
+                                              tile_seg_dev, n_tiles, gs, grad_scale_dev, nullptr, st, name, grp,
+                                              n_groups);
+}
+
+template <template <bool> class R, typename Make>
+static int adam_family_mt_grouped(Make make, float* p, float* m, float* v, float* vmax, void* p_lp,
+                                  const frl_grad_seg* segs, const int64_t* prefix, const int32_t* tseg,
+                                  int64_t n_tiles, GroupTable grp, int n_groups, double grad_scale,
+                                  const float* gsd, void* stream, const char* name) {
+    FRL_REQUIRE(m && v, FRL_E_ARG, "%s: null state", name);
+    const float gs = static_cast<float>(grad_scale);
+    cudaStream_t st = static_cast<cudaStream_t>(stream);
+    if (vmax)
+        return launch_update_mt<R<true>, 3, true>(make(std::true_type{}), p, m, v, vmax, p_lp, segs, prefix, tseg,
+                                                  n_tiles, gs, gsd, nullptr, st, name, grp, n_groups);
+    return launch_update_mt<R<false>, 2, true>(make(std::false_type{}), p, m, v, nullptr, p_lp, segs, prefix, tseg,
+                                               n_tiles, gs, gsd, nullptr, st, name, grp, n_groups);
+}
+
+extern "C" int frl_adam_mt_grouped(float* p, float* m, float* v, float* vmax, void* p_lp, const frl_grad_seg* segs_dev,
+                                   const int64_t* tile_prefix_dev, const int32_t* tile_seg_dev, int64_t n_tiles,
+                                   const int32_t* seg_group_dev, const int32_t* seg_flags_dev, const float* group_dyn,
+                                   int n_groups, double beta1, double beta2, double eps, double grad_scale,
+                                   const float* grad_scale_dev, void* stream) {
+    auto make = [&](auto ams) { return make_adam_rule<decltype(ams)::value>(0.0, beta1, beta2, eps, 0.0, 1); };
+    return adam_family_mt_grouped<AdamRule>(make, p, m, v, vmax, p_lp, segs_dev, tile_prefix_dev, tile_seg_dev,
+                                            n_tiles, GroupTable{seg_group_dev, seg_flags_dev, group_dyn}, n_groups,
+                                            grad_scale, grad_scale_dev, stream, "frl_adam_mt_grouped");
+}
+
+extern "C" int frl_adamw_mt_grouped(float* p, float* m, float* v, float* vmax, void* p_lp, const frl_grad_seg* segs_dev,
+                                    const int64_t* tile_prefix_dev, const int32_t* tile_seg_dev, int64_t n_tiles,
+                                    const int32_t* seg_group_dev, const int32_t* seg_flags_dev, const float* group_dyn,
+                                    int n_groups, double beta1, double beta2, double eps, double grad_scale,
+                                    const float* grad_scale_dev, void* stream) {
+    auto make = [&](auto ams) { return make_adamw_rule<decltype(ams)::value>(0.0, beta1, beta2, eps, 0.0, 1); };
+    return adam_family_mt_grouped<AdamWRule>(make, p, m, v, vmax, p_lp, segs_dev, tile_prefix_dev, tile_seg_dev,
+                                             n_tiles, GroupTable{seg_group_dev, seg_flags_dev, group_dyn}, n_groups,
+                                             grad_scale, grad_scale_dev, stream, "frl_adamw_mt_grouped");
+}
+
+extern "C" int frl_lion_mt_grouped(float* p, float* m, void* p_lp, const frl_grad_seg* segs_dev,
+                                   const int64_t* tile_prefix_dev, const int32_t* tile_seg_dev, int64_t n_tiles,
+                                   const int32_t* seg_group_dev, const int32_t* seg_flags_dev, const float* group_dyn,
+                                   int n_groups, double beta1, double beta2, double grad_scale,
+                                   const float* grad_scale_dev, void* stream) {
+    FRL_CHECK_LION(beta1, beta2, m, "frl_lion_mt_grouped");
+    return launch_update_mt<LionRule, 1, true>(make_lion_rule(0.0, beta1, beta2, 0.0), p, m, nullptr, nullptr, p_lp,
+                                               segs_dev, tile_prefix_dev, tile_seg_dev, n_tiles,
+                                               static_cast<float>(grad_scale), grad_scale_dev, nullptr,
+                                               static_cast<cudaStream_t>(stream), "frl_lion_mt_grouped",
+                                               GroupTable{seg_group_dev, seg_flags_dev, group_dyn}, n_groups);
+}
+
+extern "C" int frl_rmsprop_mt_grouped(float* p, float* sq, float* buf, void* p_lp, const frl_grad_seg* segs_dev,
+                                      const int64_t* tile_prefix_dev, const int32_t* tile_seg_dev, int64_t n_tiles,
+                                      const int32_t* seg_group_dev, const int32_t* seg_flags_dev,
+                                      const float* group_dyn, int n_groups, double alpha, double eps, double mu,
+                                      double grad_scale, const float* grad_scale_dev, void* stream) {
+    const char* name = "frl_rmsprop_mt_grouped";
+    FRL_REQUIRE(sq, FRL_E_ARG, "%s: null sq", name);
+    FRL_REQUIRE(mu == 0.0 || buf != nullptr, FRL_E_ARG, "%s: momentum needs buf", name);
+    const GroupTable grp{seg_group_dev, seg_flags_dev, group_dyn};
+    cudaStream_t st = static_cast<cudaStream_t>(stream);
+    const float gs = static_cast<float>(grad_scale);
+    if (mu != 0.0)
+        return launch_update_mt<RmspropRule<true>, 2, true>(make_rmsprop_rule<true>(0.0, alpha, eps, 0.0, mu), p, sq,
+                                                            buf, nullptr, p_lp, segs_dev, tile_prefix_dev,
+                                                            tile_seg_dev, n_tiles, gs, grad_scale_dev, nullptr, st,
+                                                            name, grp, n_groups);
+    return launch_update_mt<RmspropRule<false>, 1, true>(make_rmsprop_rule<false>(0.0, alpha, eps, 0.0, mu), p, sq,
+                                                         nullptr, nullptr, p_lp, segs_dev, tile_prefix_dev,
+                                                         tile_seg_dev, n_tiles, gs, grad_scale_dev, nullptr, st, name,
+                                                         grp, n_groups);
 }

@@ -6,11 +6,15 @@
 namespace frl {
 
 // ---- update rules (scalar, fp32) ------------------------------------------------------------
+// patch(dyn): the per-step scalars of the rule's dyn layout.  patch_group(row): the same from one
+// row of a parameter-group table (FRL_GROUP_DYN_COLS floats: columns 0-3 the dyn layout for that
+// group's lr / wd, column 4 the group's L2-coupled decay, read by the rules that have one).
 struct SgdRule {
     float neg_lr, mu, one_minus_damp, wd;
     int first_step, has_buf;
     static constexpr int kStates = 1;
     __device__ __forceinline__ void patch(const float* dyn) { neg_lr = -__ldg(dyn); }
+    __device__ __forceinline__ void patch_group(const float* row) { patch(row); wd = __ldg(row + 4); }
     __device__ __forceinline__ void operator()(float& p, float g, float& buf, float&, float&) const {
         g = fmaf(wd, p, g);
         if (has_buf) {
@@ -49,6 +53,7 @@ struct AdamRule {
         neg_step_size = __ldg(dyn);
         bc2_sqrt = __ldg(dyn + 1);
     }
+    __device__ __forceinline__ void patch_group(const float* row) { patch(row); wd = __ldg(row + 4); }
     __device__ __forceinline__ void operator()(float& p, float g, float& m, float& v, float& vmax) const {
         g = fmaf(wd, p, g);                           // L2-coupled decay (torch Adam)
         adam_moments_and_param<AMSGRAD>(p, g, m, v, vmax, w1, beta2, w2, eps, neg_step_size, bc2_sqrt);
@@ -73,6 +78,7 @@ struct AdamWRule {
         bc2_sqrt = __ldg(dyn + 1);
         decay = __ldg(dyn + 2);
     }
+    __device__ __forceinline__ void patch_group(const float* row) { patch(row); }
     __device__ __forceinline__ void operator()(float& p, float g, float& m, float& v, float& vmax) const {
         p = __fmul_rn(p, decay);                      // param.mul_(1 - lr*wd): its own rounding, never
                                                       // contracted into the update's FMA
@@ -95,6 +101,7 @@ struct LionRule {
         neg_lr = -__ldg(dyn);
         decay = __ldg(dyn + 1);
     }
+    __device__ __forceinline__ void patch_group(const float* row) { patch(row); }
     __device__ __forceinline__ void operator()(float& p, float g, float& m, float&, float&) const {
         p = __fmul_rn(p, decay);
         const float c = fmaf(w1, g - m, m);
@@ -109,6 +116,7 @@ struct RmspropRule {
     float alpha, one_minus_alpha, eps, wd, mu, neg_lr;
     static constexpr int kStates = MOMENTUM ? 2 : 1;
     __device__ __forceinline__ void patch(const float* dyn) { neg_lr = -__ldg(dyn); }
+    __device__ __forceinline__ void patch_group(const float* row) { patch(row); wd = __ldg(row + 4); }
     __device__ __forceinline__ void operator()(float& p, float g, float& sq, float& buf, float&) const {
         g = fmaf(wd, p, g);
         sq = fmaf(one_minus_alpha * g, g, sq * alpha);
@@ -119,6 +127,25 @@ struct RmspropRule {
     }
 };
 
+
+// Parameter groups of a segment-table update (the _mt_grouped forms): per segment its group and
+// its FRL_LW_CLIPPED flag, per group one row of FRL_GROUP_DYN_COLS floats.  Zero in the ungrouped
+// instantiations, which never read it.
+struct GroupTable {
+    const int32_t* seg_group;
+    const int32_t* seg_flags;
+    const float* rows;
+};
+
+// the argument checks of a grouped launch (inside a function returning int); the group index of each
+// segment is validated on the host when the table is built
+#define FRL_CHECK_GROUPS(grp, n_groups, name)                                                            \
+    do {                                                                                                 \
+        FRL_REQUIRE((n_groups) >= 1, FRL_E_ARG, "%s: n_groups %d < 1", name, (n_groups));                 \
+        FRL_REQUIRE((grp).seg_group && (grp).seg_flags && (grp).rows, FRL_E_ARG,                         \
+                    "%s: null seg_group / seg_flags / group_dyn", name);                                 \
+        FRL_REQUIRE(aligned16((grp).rows), FRL_E_ALIGN, "%s: group_dyn must be 16-byte aligned", name);  \
+    } while (0)
 
 // ---- host-side construction from the double-precision hyper-parameters -----------------------
 static inline SgdRule make_sgd_rule(double lr, double mu, double dampening, double wd, int first_step) {

@@ -194,6 +194,70 @@ __device__ __forceinline__ void mt_full_tile_sr(const Rule& rule, float gs, bf16
     }
 }
 
+// one tile of a segment: interior tiles unchecked, the last tile of a segment bounds-checked; the
+// padding up to the slice's multiple of 8 takes a zero gradient and, from zero weights and state,
+// stays zero under every rule
+template <typename Rule, int NS>
+__device__ __forceinline__ void mt_tile_sr(const Rule& rule, float gs, bf16x4* p, f32x4* s0, f32x4* s1, f32x4* s2,
+                                           const SegView& sv, uint32_t t, uint64_t seed) {
+    const f32x4 zero{0.f, 0.f, 0.f, 0.f};
+    const int64_t v0 = sv.t_in * kTileVec + threadIdx.x;
+    const int64_t a0 = sv.arena_off >> 2;
+    if ((sv.t_in + 1) * kTileVec <= (sv.numel >> 2)) {        // CTA-uniform: interior tile
+        if (sv.g_dtype == FRL_F32)
+            mt_full_tile_sr<Rule, f32x4, NS>(rule, gs, p, s0, s1, s2, static_cast<const f32x4*>(sv.g), a0, v0,
+                                             t, seed);
+        else
+            mt_full_tile_sr<Rule, bf16x4, NS>(rule, gs, p, s0, s1, s2, static_cast<const bf16x4*>(sv.g), a0,
+                                              v0, t, seed);
+        return;
+    }
+    const int64_t seg_vec = (sv.numel + 3) >> 2;
+#pragma unroll 1
+    for (int j = 0; j < kUnroll; ++j) {
+        const int64_t v = v0 + j * kThreads;
+        if (v >= seg_vec) break;
+        const int64_t i = a0 + v;
+        f32x4 q0 = NS > 0 ? ld_stream(s0 + i) : zero;
+        f32x4 q1 = NS > 1 ? ld_stream(s1 + i) : zero;
+        f32x4 q2 = NS > 2 ? ld_stream(s2 + i) : zero;
+        st_stream(p + i, apply4_sr(rule, ld_stream_rw(p + i), seg_load4(sv, v << 2), gs, q0, q1, q2,
+                                   static_cast<uint64_t>(i), t, seed));
+        if (NS > 0) st_stream(s0 + i, q0);
+        if (NS > 1) st_stream(s1 + i, q1);
+        if (NS > 2) st_stream(s2 + i, q2);
+    }
+}
+
+// GROUPED: as update_mt_body's (optim.cu); the update count t is the row's column 3
+template <typename Rule, int NS, bool GROUPED>
+__device__ __forceinline__ void update_mt_sr_body(bf16x4* __restrict__ p, float* __restrict__ s0_,
+                                                  float* __restrict__ s1_, float* __restrict__ s2_,
+                                                  const frl_grad_seg* __restrict__ segs,
+                                                  const int64_t* __restrict__ tile_prefix,
+                                                  const int32_t* __restrict__ tile_seg, int64_t n_tiles, uint64_t seed,
+                                                  uint32_t t, Rule rule, float gscale,
+                                                  const float* __restrict__ gscale_dev, const float* __restrict__ dyn,
+                                                  const GroupTable& grp) {
+    patch_sr(rule, t, dyn);
+    f32x4* s0 = reinterpret_cast<f32x4*>(s0_);
+    f32x4* s1 = reinterpret_cast<f32x4*>(s1_);
+    f32x4* s2 = reinterpret_cast<f32x4*>(s2_);
+    const float gs = gscale_dev ? gscale * __ldg(gscale_dev) : gscale;
+    for (int64_t tile = blockIdx.x; tile < n_tiles; tile += gridDim.x) {
+        const SegView sv = find_segment(segs, tile_prefix, tile_seg, tile);
+        if constexpr (GROUPED) {
+            const float* row = grp.rows + FRL_GROUP_DYN_COLS * __ldg(grp.seg_group + sv.seg);
+            Rule r = rule;
+            r.patch_group(row);
+            mt_tile_sr<Rule, NS>(r, seg_scale(__ldg(grp.seg_flags + sv.seg), gscale, gscale_dev), p, s0, s1, s2, sv,
+                                 __float_as_uint(__ldg(row + 3)), seed);
+        } else {
+            mt_tile_sr<Rule, NS>(rule, gs, p, s0, s1, s2, sv, t, seed);
+        }
+    }
+}
+
 template <typename Rule, int NS>
 __global__ void __launch_bounds__(kThreads)
 update_mt_sr_kernel(bf16x4* __restrict__ p, float* __restrict__ s0_, float* __restrict__ s1_,
@@ -201,50 +265,27 @@ update_mt_sr_kernel(bf16x4* __restrict__ p, float* __restrict__ s0_, float* __re
                     const int64_t* __restrict__ tile_prefix, const int32_t* __restrict__ tile_seg,
                     int64_t n_tiles, uint64_t seed, uint32_t t, Rule rule, float gscale,
                     const float* __restrict__ gscale_dev, const float* __restrict__ dyn) {
-    patch_sr(rule, t, dyn);
-    f32x4* s0 = reinterpret_cast<f32x4*>(s0_);
-    f32x4* s1 = reinterpret_cast<f32x4*>(s1_);
-    f32x4* s2 = reinterpret_cast<f32x4*>(s2_);
-    const float gs = gscale_dev ? gscale * __ldg(gscale_dev) : gscale;
-    const f32x4 zero{0.f, 0.f, 0.f, 0.f};
-    for (int64_t tile = blockIdx.x; tile < n_tiles; tile += gridDim.x) {
-        const SegView sv = find_segment(segs, tile_prefix, tile_seg, tile);
-        const int64_t v0 = sv.t_in * kTileVec + threadIdx.x;
-        const int64_t a0 = sv.arena_off >> 2;
-        if ((sv.t_in + 1) * kTileVec <= (sv.numel >> 2)) {        // CTA-uniform: interior tile
-            if (sv.g_dtype == FRL_F32)
-                mt_full_tile_sr<Rule, f32x4, NS>(rule, gs, p, s0, s1, s2, static_cast<const f32x4*>(sv.g), a0, v0,
-                                                 t, seed);
-            else
-                mt_full_tile_sr<Rule, bf16x4, NS>(rule, gs, p, s0, s1, s2, static_cast<const bf16x4*>(sv.g), a0,
-                                                  v0, t, seed);
-            continue;
-        }
-        // last tile of a segment: bounds-checked; the padding up to the slice's multiple of 8 takes a
-        // zero gradient and, from zero weights and state, stays zero under every rule
-        const int64_t seg_vec = (sv.numel + 3) >> 2;
-#pragma unroll 1
-        for (int j = 0; j < kUnroll; ++j) {
-            const int64_t v = v0 + j * kThreads;
-            if (v >= seg_vec) break;
-            const int64_t i = a0 + v;
-            f32x4 q0 = NS > 0 ? ld_stream(s0 + i) : zero;
-            f32x4 q1 = NS > 1 ? ld_stream(s1 + i) : zero;
-            f32x4 q2 = NS > 2 ? ld_stream(s2 + i) : zero;
-            st_stream(p + i, apply4_sr(rule, ld_stream_rw(p + i), seg_load4(sv, v << 2), gs, q0, q1, q2,
-                                       static_cast<uint64_t>(i), t, seed));
-            if (NS > 0) st_stream(s0 + i, q0);
-            if (NS > 1) st_stream(s1 + i, q1);
-            if (NS > 2) st_stream(s2 + i, q2);
-        }
-    }
+    update_mt_sr_body<Rule, NS, false>(p, s0_, s1_, s2_, segs, tile_prefix, tile_seg, n_tiles, seed, t, rule, gscale,
+                                       gscale_dev, dyn, GroupTable{});
 }
 
 template <typename Rule, int NS>
+__global__ void __launch_bounds__(kThreads)
+update_mt_grouped_sr_kernel(bf16x4* __restrict__ p, float* __restrict__ s0_, float* __restrict__ s1_,
+                            float* __restrict__ s2_, const frl_grad_seg* __restrict__ segs,
+                            const int64_t* __restrict__ tile_prefix, const int32_t* __restrict__ tile_seg,
+                            int64_t n_tiles, uint64_t seed, Rule rule, float gscale,
+                            const float* __restrict__ gscale_dev, GroupTable grp) {
+    update_mt_sr_body<Rule, NS, true>(p, s0_, s1_, s2_, segs, tile_prefix, tile_seg, n_tiles, seed, 1u, rule, gscale,
+                                      gscale_dev, nullptr, grp);
+}
+
+template <typename Rule, int NS, bool G = false>
 static int launch_update_mt_sr(const Rule& rule, void* p, float* s0, float* s1, float* s2,
                                const frl_grad_seg* segs, const int64_t* tile_prefix, const int32_t* tile_seg,
                                int64_t n_tiles, uint64_t seed, int64_t t, float gscale, const float* gscale_dev,
-                               const float* dyn, cudaStream_t st, const char* name) {
+                               const float* dyn, cudaStream_t st, const char* name, GroupTable grp = {},
+                               int n_groups = 0) {
     FRL_REQUIRE(n_tiles >= 0, FRL_E_ARG, "%s: negative tile count", name);
     if (n_tiles == 0) return 0;
     FRL_REQUIRE(p && segs && tile_prefix && tile_seg, FRL_E_ARG, "%s: null p/segs/tile_prefix/tile_seg", name);
@@ -252,6 +293,14 @@ static int launch_update_mt_sr(const Rule& rule, void* p, float* s0, float* s1, 
                 static_cast<long long>(t));
     FRL_REQUIRE(aligned16(p) && aligned16(s0) && aligned16(s1) && aligned16(s2), FRL_E_ALIGN,
                 "%s: arrays must be 16-byte aligned", name);
+    if constexpr (G) {
+        FRL_CHECK_GROUPS(grp, n_groups, name);
+        update_mt_grouped_sr_kernel<Rule, NS><<<grid_sr<update_mt_grouped_sr_kernel<Rule, NS>>(n_tiles * kTileElems),
+                                                kThreads, 0, st>>>(
+            static_cast<bf16x4*>(p), s0, s1, s2, segs, tile_prefix, tile_seg, n_tiles, seed, rule, gscale,
+            gscale_dev, grp);
+        return after_launch(name);
+    }
     update_mt_sr_kernel<Rule, NS><<<grid_sr<update_mt_sr_kernel<Rule, NS>>(n_tiles * kTileElems), kThreads, 0, st>>>(
         static_cast<bf16x4*>(p), s0, s1, s2, segs, tile_prefix, tile_seg, n_tiles, seed,
         static_cast<uint32_t>(t), rule, gscale, gscale_dev, dyn);
@@ -420,4 +469,103 @@ extern "C" int frl_rmsprop_mt_sr(void* p, float* sq, float* buf, const frl_grad_
                                                       nullptr, nullptr, segs_dev, tile_prefix_dev, tile_seg_dev,
                                                       n_tiles, seed, t, gs, grad_scale_dev, dyn, st,
                                                       "frl_rmsprop_mt_sr");
+}
+
+// ---- parameter-group (K2-mt-sr grouped) entry points -----------------------------------------------
+// The _mt_sr form's arguments without t / step, lr / wd and dyn (each segment's group row supplies
+// them, the update count in its column 3) and with the group table after n_tiles.
+
+extern "C" int frl_sgd_momentum_mt_grouped_sr(void* p, float* buf, const frl_grad_seg* segs_dev,
+                                              const int64_t* tile_prefix_dev, const int32_t* tile_seg_dev,
+                                              int64_t n_tiles, const int32_t* seg_group_dev,
+                                              const int32_t* seg_flags_dev, const float* group_dyn, int n_groups,
+                                              uint64_t seed, double mu, double dampening, double grad_scale,
+                                              const float* grad_scale_dev, int first_step, void* stream) {
+    const char* name = "frl_sgd_momentum_mt_grouped_sr";
+    FRL_REQUIRE(mu == 0.0 || buf != nullptr, FRL_E_ARG, "%s: momentum needs buf", name);
+    const SgdRule r = make_sgd_rule(0.0, mu, dampening, 0.0, first_step);
+    const GroupTable grp{seg_group_dev, seg_flags_dev, group_dyn};
+    cudaStream_t st = static_cast<cudaStream_t>(stream);
+    const float gs = static_cast<float>(grad_scale);
+    if (mu != 0.0)
+        return launch_update_mt_sr<SgdRule, 1, true>(r, p, buf, nullptr, nullptr, segs_dev, tile_prefix_dev,
+                                                     tile_seg_dev, n_tiles, seed, 1, gs, grad_scale_dev, nullptr, st,
+                                                     name, grp, n_groups);
+    return launch_update_mt_sr<SgdRule, 0, true>(r, p, nullptr, nullptr, nullptr, segs_dev, tile_prefix_dev,
+                                                 tile_seg_dev, n_tiles, seed, 1, gs, grad_scale_dev, nullptr, st,
+                                                 name, grp, n_groups);
+}
+
+template <template <bool> class R, typename Make>
+static int adam_family_mt_grouped_sr(Make make, void* p, float* m, float* v, float* vmax, const frl_grad_seg* segs,
+                                     const int64_t* prefix, const int32_t* tseg, int64_t n_tiles, GroupTable grp,
+                                     int n_groups, uint64_t seed, double grad_scale, const float* gsd, void* stream,
+                                     const char* name) {
+    FRL_REQUIRE(m && v, FRL_E_ARG, "%s: null state", name);
+    const float gs = static_cast<float>(grad_scale);
+    cudaStream_t st = static_cast<cudaStream_t>(stream);
+    if (vmax)
+        return launch_update_mt_sr<R<true>, 3, true>(make(std::true_type{}), p, m, v, vmax, segs, prefix, tseg,
+                                                     n_tiles, seed, 1, gs, gsd, nullptr, st, name, grp, n_groups);
+    return launch_update_mt_sr<R<false>, 2, true>(make(std::false_type{}), p, m, v, nullptr, segs, prefix, tseg,
+                                                  n_tiles, seed, 1, gs, gsd, nullptr, st, name, grp, n_groups);
+}
+
+extern "C" int frl_adam_mt_grouped_sr(void* p, float* m, float* v, float* vmax, const frl_grad_seg* segs_dev,
+                                      const int64_t* tile_prefix_dev, const int32_t* tile_seg_dev, int64_t n_tiles,
+                                      const int32_t* seg_group_dev, const int32_t* seg_flags_dev,
+                                      const float* group_dyn, int n_groups, uint64_t seed, double beta1, double beta2,
+                                      double eps, double grad_scale, const float* grad_scale_dev, void* stream) {
+    auto make = [&](auto ams) { return make_adam_rule<decltype(ams)::value>(0.0, beta1, beta2, eps, 0.0, 1); };
+    return adam_family_mt_grouped_sr<AdamRule>(make, p, m, v, vmax, segs_dev, tile_prefix_dev, tile_seg_dev, n_tiles,
+                                               GroupTable{seg_group_dev, seg_flags_dev, group_dyn}, n_groups, seed,
+                                               grad_scale, grad_scale_dev, stream, "frl_adam_mt_grouped_sr");
+}
+
+extern "C" int frl_adamw_mt_grouped_sr(void* p, float* m, float* v, float* vmax, const frl_grad_seg* segs_dev,
+                                       const int64_t* tile_prefix_dev, const int32_t* tile_seg_dev, int64_t n_tiles,
+                                       const int32_t* seg_group_dev, const int32_t* seg_flags_dev,
+                                       const float* group_dyn, int n_groups, uint64_t seed, double beta1,
+                                       double beta2, double eps, double grad_scale, const float* grad_scale_dev,
+                                       void* stream) {
+    auto make = [&](auto ams) { return make_adamw_rule<decltype(ams)::value>(0.0, beta1, beta2, eps, 0.0, 1); };
+    return adam_family_mt_grouped_sr<AdamWRule>(make, p, m, v, vmax, segs_dev, tile_prefix_dev, tile_seg_dev, n_tiles,
+                                                GroupTable{seg_group_dev, seg_flags_dev, group_dyn}, n_groups, seed,
+                                                grad_scale, grad_scale_dev, stream, "frl_adamw_mt_grouped_sr");
+}
+
+extern "C" int frl_lion_mt_grouped_sr(void* p, float* m, const frl_grad_seg* segs_dev, const int64_t* tile_prefix_dev,
+                                      const int32_t* tile_seg_dev, int64_t n_tiles, const int32_t* seg_group_dev,
+                                      const int32_t* seg_flags_dev, const float* group_dyn, int n_groups,
+                                      uint64_t seed, double beta1, double beta2, double grad_scale,
+                                      const float* grad_scale_dev, void* stream) {
+    FRL_CHECK_LION(beta1, beta2, m, "frl_lion_mt_grouped_sr");
+    return launch_update_mt_sr<LionRule, 1, true>(make_lion_rule(0.0, beta1, beta2, 0.0), p, m, nullptr, nullptr,
+                                                  segs_dev, tile_prefix_dev, tile_seg_dev, n_tiles, seed, 1,
+                                                  static_cast<float>(grad_scale), grad_scale_dev, nullptr,
+                                                  static_cast<cudaStream_t>(stream), "frl_lion_mt_grouped_sr",
+                                                  GroupTable{seg_group_dev, seg_flags_dev, group_dyn}, n_groups);
+}
+
+extern "C" int frl_rmsprop_mt_grouped_sr(void* p, float* sq, float* buf, const frl_grad_seg* segs_dev,
+                                         const int64_t* tile_prefix_dev, const int32_t* tile_seg_dev, int64_t n_tiles,
+                                         const int32_t* seg_group_dev, const int32_t* seg_flags_dev,
+                                         const float* group_dyn, int n_groups, uint64_t seed, double alpha,
+                                         double eps, double mu, double grad_scale, const float* grad_scale_dev,
+                                         void* stream) {
+    const char* name = "frl_rmsprop_mt_grouped_sr";
+    FRL_REQUIRE(sq, FRL_E_ARG, "%s: null sq", name);
+    FRL_REQUIRE(mu == 0.0 || buf != nullptr, FRL_E_ARG, "%s: momentum needs buf", name);
+    const GroupTable grp{seg_group_dev, seg_flags_dev, group_dyn};
+    cudaStream_t st = static_cast<cudaStream_t>(stream);
+    const float gs = static_cast<float>(grad_scale);
+    if (mu != 0.0)
+        return launch_update_mt_sr<RmspropRule<true>, 2, true>(make_rmsprop_rule<true>(0.0, alpha, eps, 0.0, mu), p,
+                                                               sq, buf, nullptr, segs_dev, tile_prefix_dev,
+                                                               tile_seg_dev, n_tiles, seed, 1, gs, grad_scale_dev,
+                                                               nullptr, st, name, grp, n_groups);
+    return launch_update_mt_sr<RmspropRule<false>, 1, true>(make_rmsprop_rule<false>(0.0, alpha, eps, 0.0, mu), p, sq,
+                                                            nullptr, nullptr, segs_dev, tile_prefix_dev, tile_seg_dev,
+                                                            n_tiles, seed, 1, gs, grad_scale_dev, nullptr, st, name,
+                                                            grp, n_groups);
 }

@@ -64,16 +64,28 @@ class FusedArenaOptimizer(torch.optim.Optimizer):
 
     @property
     def needs_whole_tensors(self) -> bool:
-        """True if an update needs every gradient of a tensor at once (per-tensor norms): the
+        """True if an update needs every gradient of a tensor at once (per-tensor norms), or if the
+        optimizer has several param groups (one grouped segment-table update, K2-mt grouped): the
         pipeline then updates once after backward, never per bucket or per shard."""
-        return False
+        return self.grouped
 
-    def __init__(self, arena: ParamArena, defaults: Dict[str, Any]) -> None:
+    def __init__(self, arena: ParamArena, defaults: Dict[str, Any],
+                 param_groups: Optional[List[Dict[str, Any]]] = None) -> None:
         self.arena = arena
         params = arena.all_params
         if not params:
             raise ValueError("optimizer got an empty parameter list")
-        super().__init__(params, defaults)
+        super().__init__(params if param_groups is None else param_groups, defaults)
+        # state-dict position of each parameter: consecutive group by group (torch's numbering)
+        self._pos: Dict[int, int] = {}
+        self._group_of: Dict[int, int] = {}
+        for gi, g in enumerate(self.param_groups):
+            for p in g["params"]:
+                self._group_of[id(p)] = gi
+                self._pos[id(p)] = len(self._pos)
+        if param_groups is not None and set(self._pos) != {id(p) for p in params}:
+            raise ValueError("the param groups must hold exactly the arena's parameters")
+        self.grouped = len(self.param_groups) > 1
         self._vec: Dict[str, torch.Tensor] = {}
         self._steps = 0                # completed optimizer steps
         self._in_step = False
@@ -90,6 +102,11 @@ class FusedArenaOptimizer(torch.optim.Optimizer):
         if self.sr:
             self.param_groups[0].setdefault("sr_seed", SR_SEED)
             self.param_groups[0]["sr_updates"] = 0
+        if self.grouped:
+            # one dyn row per group, read by every grouped launch (eager or replayed), so there are no
+            # by-value lr / wd arguments a captured graph would freeze
+            self._dyn = torch.zeros(len(self.param_groups), KERNELS.GROUP_DYN_COLS, dtype=torch.float32,
+                                    device=arena.device)
 
     @property
     def sr_seed(self) -> int:
@@ -98,13 +115,37 @@ class FusedArenaOptimizer(torch.optim.Optimizer):
     # -- device-resident scalars -----------------------------------------------------------------
     def _dyn_values(self) -> Tuple[float, ...]:
         """Scalars of the NEXT step (``_steps + 1``) in the layout the kernel's ``dyn`` expects."""
-        return (float(self.hyper["lr"]),)
+        return self._dyn_row(self.hyper)
+
+    def _dyn_row(self, h: Dict[str, Any]) -> Tuple[float, ...]:
+        """``_dyn_values`` for the lr / weight decay of param group ``h``."""
+        return (float(h["lr"]),)
+
+    def _group_rows(self) -> np.ndarray:
+        """The grouped ``dyn`` table of the next step: per group, columns 0-2 its ``_dyn_row``, column
+        3 the update count (uint32 bits), column 4 its weight decay (the L2-coupled rules' wd)."""
+        rows = np.zeros((len(self.param_groups), KERNELS.GROUP_DYN_COLS), dtype=np.float32)
+        for gi, h in enumerate(self.param_groups):
+            vals = self._dyn_row(h)
+            rows[gi, :len(vals)] = vals
+            rows[gi, 4] = float(h["weight_decay"])
+        rows.view(np.uint32)[:, 3] = self._steps + 1
+        return rows
 
     def enable_dynamic_scalars(self) -> None:
         if self._dyn is None:
             self._dyn = torch.zeros(4, dtype=torch.float32, device=self.arena.device)
             self._dyn_last = None
         self.refresh_dynamic_scalars()
+
+    def disable_dynamic_scalars(self) -> None:
+        """Back to by-value scalars (a failed CUDA-graph capture continues with eager launches).  With
+        several param groups the rows stay: every grouped launch and K12 read them, eager or not, and
+        the segment tables point at them; the next step uploads them afresh."""
+        if self.grouped:
+            self._dyn_last = None
+        else:
+            self._dyn = None
 
     _DYN_RING = 16        # pinned staging rows; the host never runs this many steps ahead
 
@@ -114,6 +155,9 @@ class FusedArenaOptimizer(torch.optim.Optimizer):
         which serialises the host's work for step k+1 with the device's work for step k; Adam's
         bias corrections change every step)."""
         if self._dyn is None:
+            return
+        if self.grouped:
+            self._refresh_group_rows()
             return
         vals = self._dyn_values()
         if self.sr:        # dyn[3]: the update count of the stochastic rounding, as uint32 bits
@@ -138,6 +182,40 @@ class FusedArenaOptimizer(torch.optim.Optimizer):
                     host.view(torch.int32)[3] = vals[3]
                 self._dyn.copy_(host)
             self._dyn_last = vals
+
+    def _refresh_group_rows(self) -> None:
+        rows = self._group_rows()
+        if self._dyn_last is not None and np.array_equal(rows.view(np.uint32), self._dyn_last):
+            return
+        if self._dyn.is_cuda:
+            if getattr(self, "_dyn_host", None) is None:
+                self._dyn_host = torch.zeros((self._DYN_RING,) + rows.shape, dtype=torch.float32, pin_memory=True)
+                self._dyn_slot = 0
+            row = self._dyn_host[self._dyn_slot % self._DYN_RING]
+            self._dyn_slot += 1
+            row.copy_(torch.from_numpy(rows))
+            self._dyn.copy_(row, non_blocking=True)
+        else:
+            self._dyn.copy_(torch.from_numpy(rows))
+        self._dyn_last = rows.view(np.uint32).copy()
+
+    def _slot_hyper(self, slot) -> Tuple[Dict[str, Any], Optional[torch.Tensor]]:
+        """The param group of ``slot`` and the ``dyn`` its single-slot launches read (K12): its
+        group's row with several groups, which columns 0-3 make a valid ``dyn`` of the rule."""
+        if not self.grouped:
+            return self.hyper, self._dyn
+        gi = self._group_of[id(slot.param)]
+        return self.param_groups[gi], self._dyn[gi]
+
+    def _seg_groups(self, table):
+        """The group arrays of ``table`` (``_native.SegGroups``), built on first use and kept on the
+        table: each slot's group, FRL_LW_CLIPPED on model slots, and the shared ``dyn`` rows."""
+        groups = getattr(table, "param_groups", None)
+        if groups is None:
+            groups = table.param_groups = KERNELS.SegGroups(
+                [self._group_of[id(s.param)] for s in table.slots],
+                [KERNELS.LW_CLIPPED if s.is_model else 0 for s in table.slots], self._dyn)
+        return groups
 
     # -- state vectors ---------------------------------------------------------------------------
     def _state(self, name: str) -> torch.Tensor:
@@ -171,8 +249,14 @@ class FusedArenaOptimizer(torch.optim.Optimizer):
         the norm kernel) multiplies model-parameter gradients only — the reference clips
         ``model.parameters()`` and leaves criterion parameters alone
         (reference solver_worker.py:588-591).  ``grad_src``: an arena-shaped gradient vector read
-        instead of ``arena.grad`` (the fp32 gradient accumulator)."""
+        instead of ``arena.grad`` (the fp32 gradient accumulator).  With several param groups: the
+        whole slots inside ``[lo, hi)`` through the grouped segment-table update."""
         if hi <= lo:
+            return
+        if self.grouped:
+            if grad_src is not None:
+                raise ValueError("a grouped update reads its gradients through a segment table, not grad_src")
+            _WholeTensorMixin.apply_range(self, lo, hi, grad_scale=grad_scale, clip_coef_dev=clip_coef_dev)
             return
         self._grad_src = grad_src
         try:
@@ -191,7 +275,12 @@ class FusedArenaOptimizer(torch.optim.Optimizer):
     def apply_table(self, table, *, grad_scale: float = 1.0,
                     clip_coef_dev: Optional[torch.Tensor] = None) -> None:
         """Update every arena slot listed in ``table`` (a ``multi_tensor.GradSegTable`` whose device
-        copy is current), reading each gradient where the table says it lies (K2-mt)."""
+        copy is current), reading each gradient where the table says it lies (K2-mt).  With several
+        param groups: the grouped forms (K2-mt grouped, K2-mt-sr grouped), each slot with its group's
+        lr / weight decay; ``clip_coef_dev`` then multiplies the gradients of model parameters only."""
+        if self.grouped:
+            self._apply_grouped(table, grad_scale, clip_coef_dev)
+            return
         if clip_coef_dev is not None:
             raise ValueError("K2-mt takes no clip coefficient: clipped updates go through apply_range")
         if not table.n_segs:
@@ -209,6 +298,24 @@ class FusedArenaOptimizer(torch.optim.Optimizer):
         raise NotImplementedError
 
     def _launch_mt_sr(self, table, grad_scale: float) -> None:
+        raise NotImplementedError
+
+    def _apply_grouped(self, table, grad_scale: float, coef) -> None:
+        if not table.n_segs:
+            return
+        if not self.sr:
+            self._launch_mt_grouped(table, self._seg_groups(table), grad_scale, coef)
+            return
+        model, crit = self._sr_split(table)
+        for (sub, idx), launch in ((model, self._launch_mt_grouped_sr), (crit, self._launch_mt_grouped)):
+            if sub is not None:
+                _gather_segs(table, sub, idx)
+                launch(sub, self._seg_groups(sub), grad_scale, coef)
+
+    def _launch_mt_grouped(self, table, groups, grad_scale: float, coef) -> None:
+        raise NotImplementedError
+
+    def _launch_mt_grouped_sr(self, table, groups, grad_scale: float, coef) -> None:
         raise NotImplementedError
 
     def _sr_split(self, table):
@@ -302,30 +409,35 @@ class FusedArenaOptimizer(torch.optim.Optimizer):
     def state_dict(self) -> Dict[str, Any]:
         state: Dict[int, Dict[str, Any]] = {}
         if self._steps > 0:
-            for s in sorted(self.arena.slots, key=lambda s: s.index):     # torch's key order
+            for s in sorted(self.arena.slots, key=lambda s: self._pos[id(s.param)]):     # torch's key order
                 entry = dict(self._per_param_extra())
                 for torch_name, vec_name in self.STATE_NAMES:
                     if vec_name in self._vec:
                         entry[torch_name] = ParamArena.slot_view(self._vec[vec_name], s).clone(
                             memory_format=torch.contiguous_format)
-                state[s.index] = entry
+                state[self._pos[id(s.param)]] = entry
         if self.sr:
             self.hyper["sr_updates"] = self._steps
-        groups = []
+        groups, first = [], 0
         for g in self.param_groups:
             packed = {k: v for k, v in g.items() if k != "params"}
-            packed["params"] = list(range(len(g["params"])))
+            packed["params"] = list(range(first, first + len(g["params"])))
+            first += len(g["params"])
             groups.append(packed)
         return {"state": state, "param_groups": groups}
 
     def load_state_dict(self, state_dict: Dict[str, Any]) -> None:
         groups = state_dict["param_groups"]
-        if len(groups) != 1 or len(groups[0]["params"]) != len(self.arena.all_params):
-            raise ValueError("loaded state dict has a different number of parameters/groups")
-        for k, v in groups[0].items():
-            if k != "params":
-                self.param_groups[0][k] = v
-        by_index = {s.index: s for s in self.arena.slots}
+        mine = [len(g["params"]) for g in self.param_groups]
+        theirs = [len(g["params"]) for g in groups]
+        if mine != theirs:
+            raise ValueError("loaded state dict has a different number of parameters/groups: %d param groups of %s "
+                             "params; this optimizer has %d of %s" % (len(theirs), theirs, len(mine), mine))
+        for mine_g, theirs_g in zip(self.param_groups, groups):
+            for k, v in theirs_g.items():
+                if k != "params":
+                    mine_g[k] = v
+        by_index = {self._pos[id(s.param)]: s for s in self.arena.slots}
         steps = 0
         for idx, entry in state_dict["state"].items():
             s = by_index.get(int(idx))
@@ -358,10 +470,10 @@ class FusedArenaOptimizer(torch.optim.Optimizer):
 class FusedSGD(FusedArenaOptimizer):
     STATE_NAMES = (("momentum_buffer", "momentum_buffer"),)
 
-    def __init__(self, arena, lr, momentum=0.0, dampening=0.0, weight_decay=0.0):
+    def __init__(self, arena, lr, momentum=0.0, dampening=0.0, weight_decay=0.0, param_groups=None):
         super().__init__(arena, dict(lr=lr, momentum=momentum, dampening=dampening,
                                      weight_decay=weight_decay, nesterov=False, maximize=False,
-                                     foreach=None, differentiable=False, fused=None))
+                                     foreach=None, differentiable=False, fused=None), param_groups)
 
     def _launch(self, lo, hi, grad_scale, coef):
         h = self.hyper
@@ -381,8 +493,9 @@ class FusedSGD(FusedArenaOptimizer):
 
     def update_in_dw_gemm(self, slot, dz, x, gw, *, grad_scale: float = 1.0) -> None:
         """K12: the weight gradient gw = dz^T x of ``slot`` and, in the same kernel, this step's
-        update of the slot from exactly that bf16 gradient (what ``_launch`` over the slot does)."""
-        h = self.hyper
+        update of the slot from exactly that bf16 gradient (what ``_launch`` over the slot does); with
+        several param groups, the slot's group's lr / weight decay and ``dyn`` row."""
+        h, dyn = self._slot_hyper(slot)
         a = self.arena
         mu = float(h["momentum"])
         buf = self._state("momentum_buffer")[slot.offset:slot.end] if mu != 0.0 else None
@@ -390,12 +503,12 @@ class FusedSGD(FusedArenaOptimizer):
             KERNELS.dw_gemm_sgd_sr(dz, x, gw, a.lp[slot.offset:slot.end], buf, arena_off=slot.offset,
                                    seed=self.sr_seed, t=self._steps + 1, lr=float(h["lr"]), mu=mu,
                                    dampening=float(h["dampening"]), wd=float(h["weight_decay"]),
-                                   grad_scale=grad_scale, first_step=(self._steps == 0), dyn=self._dyn)
+                                   grad_scale=grad_scale, first_step=(self._steps == 0), dyn=dyn)
             return
         KERNELS.dw_gemm_sgd(dz, x, gw, a.master[slot.offset:slot.end], buf, a.lp[slot.offset:slot.end],
                             lr=float(h["lr"]), mu=mu, dampening=float(h["dampening"]),
                             wd=float(h["weight_decay"]), grad_scale=grad_scale,
-                            first_step=(self._steps == 0), dyn=self._dyn)
+                            first_step=(self._steps == 0), dyn=dyn)
 
     def _launch_mt(self, table, grad_scale):
         h = self.hyper
@@ -412,6 +525,21 @@ class FusedSGD(FusedArenaOptimizer):
                                    seed=self.sr_seed, t=self._steps + 1, lr=float(h["lr"]), mu=mu,
                                    dampening=float(h["dampening"]), wd=float(h["weight_decay"]),
                                    grad_scale=grad_scale, first_step=(self._steps == 0), dyn=self._dyn)
+
+    def _launch_mt_grouped(self, table, groups, grad_scale, coef):
+        h = self.hyper
+        mu = float(h["momentum"])
+        KERNELS.sgd_momentum_mt_grouped(self._master_base(), self._state("momentum_buffer") if mu != 0.0 else None,
+                                        self._lp_mt(), table, groups, mu=mu, dampening=float(h["dampening"]),
+                                        grad_scale=grad_scale, grad_scale_dev=coef, first_step=(self._steps == 0))
+
+    def _launch_mt_grouped_sr(self, table, groups, grad_scale, coef):
+        h = self.hyper
+        mu = float(h["momentum"])
+        KERNELS.sgd_momentum_mt_grouped_sr(self.arena.lp, self._state("momentum_buffer") if mu != 0.0 else None,
+                                           table, groups, seed=self.sr_seed, mu=mu, dampening=float(h["dampening"]),
+                                           grad_scale=grad_scale, grad_scale_dev=coef,
+                                           first_step=(self._steps == 0))
 
     def _launch_nvls(self, lo, hi, grad_scale):
         h = self.hyper
@@ -436,12 +564,12 @@ class FusedAdam(FusedArenaOptimizer):
                    ("max_exp_avg_sq", "max_exp_avg_sq"))
 
     def __init__(self, arena, lr, betas=(0.9, 0.999), eps=1e-8, weight_decay=0.0, amsgrad=False,
-                 adamw=False):
+                 adamw=False, param_groups=None):
         self.adamw = bool(adamw)
         super().__init__(arena, dict(lr=lr, betas=betas, eps=eps, weight_decay=weight_decay,
                                      amsgrad=amsgrad, maximize=False, foreach=None,
                                      capturable=False, differentiable=False, fused=None,
-                                     decoupled_weight_decay=self.adamw))
+                                     decoupled_weight_decay=self.adamw), param_groups)
 
     def _kernel(self, name: str):
         """The Adam entry point ``name`` of ``KERNELS``, or its AdamW form (adam -> adamw)."""
@@ -450,8 +578,7 @@ class FusedAdam(FusedArenaOptimizer):
     def _per_param_extra(self):
         return {"step": torch.tensor(float(self._steps))}
 
-    def _dyn_values(self):
-        h = self.hyper
+    def _dyn_row(self, h):
         step = self._steps + 1
         bc1 = 1.0 - float(h["betas"][0]) ** step
         bc2 = 1.0 - float(h["betas"][1]) ** step
@@ -466,7 +593,8 @@ class FusedAdam(FusedArenaOptimizer):
         it runs (``decoupled_weight_decay=True``)."""
         super().load_state_dict(state_dict)
         if self.adamw:
-            self.hyper["decoupled_weight_decay"] = True
+            for g in self.param_groups:
+                g["decoupled_weight_decay"] = True
 
     def _launch(self, lo, hi, grad_scale, coef):
         h = self.hyper
@@ -501,6 +629,21 @@ class FusedAdam(FusedArenaOptimizer):
                                    beta2=float(h["betas"][1]), eps=float(h["eps"]), wd=float(h["weight_decay"]),
                                    step=self._steps + 1, grad_scale=grad_scale, dyn=self._dyn)
 
+    def _launch_mt_grouped(self, table, groups, grad_scale, coef):
+        h = self.hyper
+        self._kernel("adam_mt_grouped")(self._master_base(), self._state("exp_avg"), self._state("exp_avg_sq"),
+                                        self._state("max_exp_avg_sq") if h["amsgrad"] else None, self._lp_mt(),
+                                        table, groups, beta1=float(h["betas"][0]), beta2=float(h["betas"][1]),
+                                        eps=float(h["eps"]), grad_scale=grad_scale, grad_scale_dev=coef)
+
+    def _launch_mt_grouped_sr(self, table, groups, grad_scale, coef):
+        h = self.hyper
+        self._kernel("adam_mt_grouped_sr")(self.arena.lp, self._state("exp_avg"), self._state("exp_avg_sq"),
+                                           self._state("max_exp_avg_sq") if h["amsgrad"] else None, table, groups,
+                                           seed=self.sr_seed, beta1=float(h["betas"][0]),
+                                           beta2=float(h["betas"][1]), eps=float(h["eps"]), grad_scale=grad_scale,
+                                           grad_scale_dev=coef)
+
     def _launch_nvls(self, lo, hi, grad_scale):
         h = self.hyper
         mc_g, mc_out = self._nvls_ptrs(lo)
@@ -516,10 +659,10 @@ class FusedAdam(FusedArenaOptimizer):
 class FusedRMSprop(FusedArenaOptimizer):
     STATE_NAMES = (("square_avg", "square_avg"), ("momentum_buffer", "momentum_buffer"))
 
-    def __init__(self, arena, lr, alpha=0.99, eps=1e-8, weight_decay=0.0, momentum=0.0):
+    def __init__(self, arena, lr, alpha=0.99, eps=1e-8, weight_decay=0.0, momentum=0.0, param_groups=None):
         super().__init__(arena, dict(lr=lr, momentum=momentum, alpha=alpha, eps=eps,
                                      centered=False, weight_decay=weight_decay, capturable=False,
-                                     foreach=None, maximize=False, differentiable=False))
+                                     foreach=None, maximize=False, differentiable=False), param_groups)
 
     def _per_param_extra(self):
         return {"step": torch.tensor(float(self._steps))}
@@ -556,6 +699,22 @@ class FusedRMSprop(FusedArenaOptimizer):
                               t=self._steps + 1, lr=float(h["lr"]), alpha=float(h["alpha"]), eps=float(h["eps"]),
                               wd=float(h["weight_decay"]), mu=mu, grad_scale=grad_scale, dyn=self._dyn)
 
+    def _launch_mt_grouped(self, table, groups, grad_scale, coef):
+        h = self.hyper
+        mu = float(h["momentum"])
+        KERNELS.rmsprop_mt_grouped(self._master_base(), self._state("square_avg"),
+                                   self._state("momentum_buffer") if mu != 0.0 else None, self._lp_mt(), table, groups,
+                                   alpha=float(h["alpha"]), eps=float(h["eps"]), mu=mu, grad_scale=grad_scale,
+                                   grad_scale_dev=coef)
+
+    def _launch_mt_grouped_sr(self, table, groups, grad_scale, coef):
+        h = self.hyper
+        mu = float(h["momentum"])
+        KERNELS.rmsprop_mt_grouped_sr(self.arena.lp, self._state("square_avg"),
+                                      self._state("momentum_buffer") if mu != 0.0 else None, table, groups,
+                                      seed=self.sr_seed, alpha=float(h["alpha"]), eps=float(h["eps"]), mu=mu,
+                                      grad_scale=grad_scale, grad_scale_dev=coef)
+
     def _launch_nvls(self, lo, hi, grad_scale):
         h = self.hyper
         mu = float(h["momentum"])
@@ -580,16 +739,15 @@ class FusedLion(FusedArenaOptimizer):
 
     STATE_NAMES = (("exp_avg", "exp_avg"),)
 
-    def __init__(self, arena, lr, betas=(0.9, 0.99), weight_decay=0.0):
-        super().__init__(arena, dict(lr=lr, betas=tuple(betas), weight_decay=weight_decay))
+    def __init__(self, arena, lr, betas=(0.9, 0.99), weight_decay=0.0, param_groups=None):
+        super().__init__(arena, dict(lr=lr, betas=tuple(betas), weight_decay=weight_decay), param_groups)
 
-    def _dyn_values(self):
-        h = self.hyper
+    def _dyn_row(self, h):
         lr = float(h["lr"])       # dyn[1]: the decay factor, formed in double and rounded once to fp32
         return (lr, float(np.float32(1.0 - lr * float(h["weight_decay"]))))
 
-    def _hyper(self) -> Dict[str, float]:
-        h = self.hyper
+    def _hyper(self, h: Optional[Dict[str, Any]] = None) -> Dict[str, float]:
+        h = self.hyper if h is None else h
         return dict(lr=float(h["lr"]), beta1=float(h["betas"][0]), beta2=float(h["betas"][1]),
                     wd=float(h["weight_decay"]))
 
@@ -608,7 +766,8 @@ class FusedLion(FusedArenaOptimizer):
                 raise ValueError("a Lion optimizer cannot load another optimizer's state dict (param group keys %s; "
                                  "Lion's group has betas and no momentum)" % sorted(k for k in g if k != "params"))
         super().load_state_dict(state_dict)
-        self.hyper["betas"] = tuple(self.hyper["betas"])
+        for g in self.param_groups:
+            g["betas"] = tuple(g["betas"])
 
     def _launch(self, lo, hi, grad_scale, coef):
         p, g, lp = self._slices(lo, hi)
@@ -622,16 +781,18 @@ class FusedLion(FusedArenaOptimizer):
 
     def update_in_dw_gemm(self, slot, dz, x, gw, *, grad_scale: float = 1.0) -> None:
         """K12: the weight gradient gw = dz^T x of ``slot`` and, in the same kernel, this step's Lion
-        update of the slot from exactly that bf16 gradient (what ``_launch`` over the slot does)."""
+        update of the slot from exactly that bf16 gradient (what ``_launch`` over the slot does); with
+        several param groups, the slot's group's lr / weight decay and ``dyn`` row."""
         a = self.arena
+        h, dyn = self._slot_hyper(slot)
         m = self._state("exp_avg")[slot.offset:slot.end]
         if self._use_sr(slot.offset):
             KERNELS.dw_gemm_lion_sr(dz, x, gw, a.lp[slot.offset:slot.end], m, arena_off=slot.offset,
-                                    seed=self.sr_seed, t=self._steps + 1, **self._hyper(), grad_scale=grad_scale,
-                                    dyn=self._dyn)
+                                    seed=self.sr_seed, t=self._steps + 1, **self._hyper(h), grad_scale=grad_scale,
+                                    dyn=dyn)
             return
         KERNELS.dw_gemm_lion(dz, x, gw, a.master[slot.offset:slot.end], m, a.lp[slot.offset:slot.end],
-                             **self._hyper(), grad_scale=grad_scale, dyn=self._dyn)
+                             **self._hyper(h), grad_scale=grad_scale, dyn=dyn)
 
     def _launch_mt(self, table, grad_scale):
         KERNELS.lion_mt(self._master_base(), self._state("exp_avg"), self._lp_mt(), table, **self._hyper(),
@@ -640,6 +801,18 @@ class FusedLion(FusedArenaOptimizer):
     def _launch_mt_sr(self, table, grad_scale):
         KERNELS.lion_mt_sr(self.arena.lp, self._state("exp_avg"), table, seed=self.sr_seed, t=self._steps + 1,
                            **self._hyper(), grad_scale=grad_scale, dyn=self._dyn)
+
+    def _launch_mt_grouped(self, table, groups, grad_scale, coef):
+        h = self.hyper
+        KERNELS.lion_mt_grouped(self._master_base(), self._state("exp_avg"), self._lp_mt(), table, groups,
+                                beta1=float(h["betas"][0]), beta2=float(h["betas"][1]), grad_scale=grad_scale,
+                                grad_scale_dev=coef)
+
+    def _launch_mt_grouped_sr(self, table, groups, grad_scale, coef):
+        h = self.hyper
+        KERNELS.lion_mt_grouped_sr(self.arena.lp, self._state("exp_avg"), table, groups, seed=self.sr_seed,
+                                   beta1=float(h["betas"][0]), beta2=float(h["betas"][1]), grad_scale=grad_scale,
+                                   grad_scale_dev=coef)
 
     def _launch_nvls(self, lo, hi, grad_scale):
         mc_g, mc_out = self._nvls_ptrs(lo)
@@ -1362,6 +1535,86 @@ def check_optimizer_state(optim_opts: OptimOpts, layer_adaptation: LayerAdaptati
                             " with amsgrad" if optim_opts.amsgrad else "", la.value))
 
 
+GROUP_KEYS = ("params", "lr", "weight_decay")
+
+
+def no_decay_1d_groups(model) -> List[Dict[str, Any]]:
+    """The param groups of the ``no_decay_1d`` switch: every model parameter with ``ndim <= 1``
+    (biases, normalisation parameters) in one group with ``weight_decay = 0``; none if there is no
+    such parameter."""
+    flat = [p for p in model.parameters() if p.ndim <= 1]
+    return [{"params": flat, "weight_decay": 0.0}] if flat else []
+
+
+def resolve_param_groups(model, criterion_params, hook_groups) -> Optional[List[Dict[str, Any]]]:
+    """The canonical param groups of an optimizer from the groups a Problem's ``get_param_groups``
+    hook (or the ``no_decay_1d`` switch) returned; None if there are none (``hook_groups`` None).
+
+    Canonical order, which numbers the params of the state dict: the hook's groups in the order
+    returned, then one default group (``OptimOpts``' lr / weightDecay, no keys of its own) with every
+    remaining model parameter in ``model.parameters()`` order followed by the criterion parameters;
+    the default group is omitted if empty.  A group is a dict with ``params`` (model parameters) and
+    optionally ``lr`` / ``weight_decay`` (absolute values, torch's meaning).  Any other key, an empty
+    group, a parameter listed twice, one that is not in ``model.parameters()`` and a criterion
+    parameter are each a ValueError."""
+    if hook_groups is None:
+        return None
+    model_params = list(model.parameters())
+    model_ids = {id(p) for p in model_params}
+    crit = list(criterion_params)
+    crit_ids = {id(p) for p in crit}
+    seen = set()
+    out: List[Dict[str, Any]] = []
+    for gi, g in enumerate(hook_groups):
+        if not isinstance(g, dict) or "params" not in g:
+            raise ValueError("param group %d must be a dict with a 'params' key, got %r" % (gi, type(g).__name__))
+        extra = sorted(str(k) for k in g if k not in GROUP_KEYS)
+        if extra:
+            raise ValueError("param group %d has key %s: a group may set only 'lr' and 'weight_decay' (momentum, "
+                             "betas, eps and the rest are per optimizer)" % (gi, ", ".join(repr(k) for k in extra)))
+        params = [g["params"]] if isinstance(g["params"], torch.Tensor) else list(g["params"])
+        if not params:
+            raise ValueError("param group %d is empty" % gi)
+        for p in params:
+            if id(p) in crit_ids:
+                raise ValueError("param group %d lists a criterion parameter: groups hold model parameters only" % gi)
+            if id(p) not in model_ids:
+                raise ValueError("param group %d lists a parameter that is not in model.parameters()" % gi)
+            if id(p) in seen:
+                raise ValueError("param group %d lists a parameter that an earlier group already holds" % gi)
+            seen.add(id(p))
+        group: Dict[str, Any] = {"params": params}
+        for k in ("lr", "weight_decay"):
+            if k in g:
+                group[k] = float(g[k])
+        out.append(group)
+    rest = [p for p in model_params if id(p) not in seen] + [p for p in crit if id(p) not in model_ids]
+    if rest:
+        out.append({"params": rest})
+    return out
+
+
+def check_param_groups(layer_adaptation: LayerAdaptation, optimizer_state: OptimizerState, adafactor: bool,
+                       muon: bool, grouped: bool) -> None:
+    """Param groups (a Problem's ``get_param_groups`` hook or ``no_decay_1d``) need SGD, Adam / AdamW,
+    RMSprop or Lion; LARS / LAMB (their decay exclusion is built in), 8-bit state, Adafactor and Muon
+    are a ValueError naming the combination."""
+    if not grouped:
+        return
+    why = None
+    if LayerAdaptation(layer_adaptation) is not LayerAdaptation.NONE:
+        why = "layer adaptation %s" % LayerAdaptation(layer_adaptation).value
+    elif OptimizerState(optimizer_state) is OptimizerState.Q8:
+        why = "optimizer state %s" % OptimizerState.Q8.value
+    elif adafactor:
+        why = "adafactor"
+    elif muon:
+        why = "muon"
+    if why is not None:
+        raise ValueError("param groups (get_param_groups / no_decay_1d) cannot be combined with %s: per-group lr and "
+                         "weight decay are implemented for sgd, adam / adamw, rmsprop and lion" % why)
+
+
 def check_layer_adaptation(optim_opts: OptimOpts, layer_adaptation: LayerAdaptation) -> None:
     """LARS needs the SGD rule, LAMB the Adam rule without amsgrad; anything else is a ValueError."""
     la = LayerAdaptation(layer_adaptation)
@@ -1379,7 +1632,8 @@ def create_fused_optimizer(arena: ParamArena, optim_opts: OptimOpts,
                            layer_adaptation: LayerAdaptation = LayerAdaptation.NONE,
                            optimizer_state: OptimizerState = OptimizerState.FP32,
                            adafactor: bool = False, muon: bool = False, adamw: bool = False,
-                           lion: bool = False) -> FusedArenaOptimizer:
+                           lion: bool = False, param_groups: Optional[List[Dict[str, Any]]] = None
+                           ) -> FusedArenaOptimizer:
     """Same dispatch and argument mapping as the reference's ``_create_optimizer``; with a layer
     adaptation, its LARS / LAMB counterpart; with 8-bit optimizer state, ``FusedAdam8bit``; with
     ``adafactor``, ``FusedAdafactor`` (``lr`` caps the relative step, ``weightDecay`` is its
@@ -1387,13 +1641,15 @@ def create_fused_optimizer(arena: ParamArena, optim_opts: OptimOpts,
     ``lr`` and ``weightDecay`` for both groups, ``momentum`` is Muon's, ``epsilon`` Adam's); with
     ``adamw``, the Adam rule of whichever of ``FusedAdam``, ``FusedAdam8bit`` or ``FusedMuon`` is
     chosen takes decoupled weight decay (``torch.optim.AdamW``); with ``lion``, ``FusedLion`` (``momentum``
-    is beta1, beta2 is 0.99, ``weightDecay`` its decoupled decay)."""
+    is beta1, beta2 is 0.99, ``weightDecay`` its decoupled decay).  ``param_groups``: the canonical groups
+    of ``resolve_param_groups`` (SGD, Adam / AdamW, RMSprop and Lion only)."""
     check_layer_adaptation(optim_opts, layer_adaptation)
     check_optimizer_state(optim_opts, layer_adaptation, optimizer_state)
     check_adafactor(optim_opts, layer_adaptation, optimizer_state, adafactor)
     check_muon(optim_opts, layer_adaptation, optimizer_state, adafactor, muon)
     check_adamw(optim_opts, layer_adaptation, optimizer_state, adafactor, adamw)
     check_lion(optim_opts, layer_adaptation, lion)
+    check_param_groups(layer_adaptation, optimizer_state, adafactor, muon, param_groups is not None)
     check_master_weights(getattr(arena, "master_weights", MasterWeights.FP32), arena.precision, layer_adaptation,
                          optimizer_state, adafactor, muon)
     if muon:
@@ -1412,14 +1668,15 @@ def create_fused_optimizer(arena: ParamArena, optim_opts: OptimOpts,
     algo = optim_opts.algo
     if algo == OptAlgorithm.RMSPROP:
         return FusedRMSprop(arena, lr=optim_opts.lr, momentum=optim_opts.momentum,
-                            weight_decay=optim_opts.weightDecay)
+                            weight_decay=optim_opts.weightDecay, param_groups=param_groups)
     if algo == OptAlgorithm.SGD and lion:
         return FusedLion(arena, lr=optim_opts.lr, betas=(optim_opts.momentum, 0.99),
-                         weight_decay=optim_opts.weightDecay)
+                         weight_decay=optim_opts.weightDecay, param_groups=param_groups)
     if algo == OptAlgorithm.SGD:
         return FusedSGD(arena, lr=optim_opts.lr, momentum=optim_opts.momentum,
-                        weight_decay=optim_opts.weightDecay)
+                        weight_decay=optim_opts.weightDecay, param_groups=param_groups)
     if algo == OptAlgorithm.ADAM:
         return FusedAdam(arena, lr=optim_opts.lr, weight_decay=optim_opts.weightDecay,
-                         eps=optim_opts.epsilon, amsgrad=optim_opts.amsgrad, adamw=adamw)
+                         eps=optim_opts.epsilon, amsgrad=optim_opts.amsgrad, adamw=adamw,
+                         param_groups=param_groups)
     raise ValueError("Unknown optimization algorithm type")

@@ -73,7 +73,7 @@ class GraphedTrainStep:
             w = self.worker
             w.pipeline._step_open = False
             w.optimizer._in_step = False
-            w.optimizer._dyn = None
+            w.optimizer.disable_dynamic_scalars()
             torch.cuda.synchronize()
             return None
         self._graphs[sig] = cap

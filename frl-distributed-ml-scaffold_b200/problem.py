@@ -67,6 +67,14 @@ class Problem(ABC, Generic[BatchMetaT, AnnoParamT]):
     def get_criterion(self) -> BaseParallelCriterion:
         """Criterion matching ``get_model``'s outputs; called once in every rank process."""
 
+    def get_param_groups(self, model: torch.nn.Module) -> Optional[List[Dict[str, Any]]]:
+        """Optional optimizer param groups over ``model``'s parameters (called in every rank with the
+        model ``get_model`` built): dicts with ``params`` and optionally ``lr`` / ``weight_decay``,
+        absolute values that override ``OptimOpts`` for the group, as in ``torch.optim``.  Parameters
+        no group lists form a default group after them (see ``fused_optim.resolve_param_groups``).
+        None (the default): one group, ``OptimOpts`` for every parameter."""
+        return None
+
     @staticmethod
     def get_solver_buck_target() -> Optional[str]:
         return None

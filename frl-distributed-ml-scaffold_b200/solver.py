@@ -29,8 +29,8 @@ import torch.nn as nn
 from .arena import ParamArena
 from .criteria import BaseParallelCriterion
 from .ema import EMA_STATE_KEY
-from .fused_optim import (FusedAdafactor, FusedAdam8bit, FusedLion, FusedMuon, check_adafactor, check_adamw, check_lion, check_muon, check_layer_adaptation, check_master_weights, check_optimizer_state, create_fused_optimizer,
-                          is_adapted)
+from .fused_optim import (FusedAdafactor, FusedAdam8bit, FusedLion, FusedMuon, check_adafactor, check_adamw, check_lion, check_muon, check_layer_adaptation, check_master_weights, check_optimizer_state, check_param_groups,
+                          create_fused_optimizer, is_adapted, no_decay_1d_groups, resolve_param_groups)
 from .grad_sync import BufferBroadcaster, GradBucketPipeline
 from .lr_scheduler import DropEpochsScheduler, WarmupMultiStepLR
 from .problem import Problem
@@ -52,6 +52,7 @@ ADAFACTOR_ENV = "FRL_B200_ADAFACTOR"               # "0" (default) | "1"
 MUON_ENV = "FRL_B200_MUON"                         # "0" (default) | "1"
 ADAMW_ENV = "FRL_B200_ADAMW"                       # "0" (default) | "1"
 LION_ENV = "FRL_B200_LION"                         # "0" (default) | "1"
+NO_DECAY_1D_ENV = "FRL_B200_NO_DECAY_1D"           # "0" (default) | "1"
 CHANNELS_LAST_ENV = "FRL_B200_CHANNELS_LAST"       # "0" (default) | "1"
 MASTER_WEIGHTS_ENV = "FRL_B200_MASTER_WEIGHTS"     # "fp32" (default) | "bf16"
 EMA_SUFFIX = ".ema"                        # <checkpoint>.ema: the weight EMA next to a checkpoint
@@ -108,6 +109,10 @@ class SolverWorkerArgs(NamedTuple):
     save_every: int = 1
     graph_step: Optional[bool] = None      # None: FRL_B200_CUDA_GRAPH (default off)
     layer_adaptation: LayerAdaptation = LayerAdaptation.NONE
+    # no weight decay on parameters with ndim <= 1; None: FRL_B200_NO_DECAY_1D, read when the worker is
+    # built.  Placed before lion, so every field from lion to the end keeps its order and its position
+    # counted from the end of the tuple
+    no_decay_1d: Optional[bool] = None
     # Lion in place of SGD-with-momentum's rule; placed before muon, so every field from muon to the
     # end keeps its position counted from the end of the tuple
     lion: bool = False
@@ -330,6 +335,68 @@ def resolve_lion(explicit: Optional[bool] = None) -> bool:
     return raw == "1"
 
 
+def resolve_no_decay_1d(explicit: Optional[bool] = None) -> bool:
+    """Whether every model parameter with ndim <= 1 goes in a group with weight_decay 0: ``explicit``,
+    else FRL_B200_NO_DECAY_1D (``0``, the default, or ``1``).  Any other value is a ValueError."""
+    if explicit is not None:
+        return bool(explicit)
+    raw = os.environ.get(NO_DECAY_1D_ENV, "0").strip()
+    if raw not in ("0", "1"):
+        raise ValueError("%s must be 0 or 1, got %r" % (NO_DECAY_1D_ENV, raw))
+    return raw == "1"
+
+
+def has_param_group_hook(problem) -> bool:
+    """True if ``problem`` defines ``get_param_groups`` other than the base class's (which returns None);
+    a reference Problem subclass has none."""
+    hook = getattr(type(problem), "get_param_groups", None)
+    return callable(hook) and hook is not Problem.get_param_groups
+
+
+def problem_param_groups(problem, model: nn.Module, criterion: nn.Module,
+                         no_decay_1d: bool) -> Optional[List[Dict[str, Any]]]:
+    """The canonical param groups of a training run (``fused_optim.resolve_param_groups``) from the
+    Problem's ``get_param_groups`` hook or, with ``no_decay_1d``, from the switch's own hook
+    (``fused_optim.no_decay_1d_groups``); None if neither gives groups.  Both at once is a ValueError."""
+    hooked = problem.get_param_groups(model) if has_param_group_hook(problem) else None
+    if no_decay_1d:
+        if hooked is not None:
+            raise ValueError("no_decay_1d cannot be combined with a Problem whose get_param_groups returns groups: "
+                             "put the no-decay group in the hook")
+        hooked = no_decay_1d_groups(model)
+    return resolve_param_groups(model, criterion.parameters(), hooked)
+
+
+def validate_param_groups(problem, no_decay_1d: bool, layer_adaptation: LayerAdaptation,
+                          optimizer_state: OptimizerState, adafactor: bool, muon: bool) -> None:
+    """The param-group checks of ``Solver.solve``, before a rank starts: the hook's groups are resolved
+    against a model and criterion built here, with the host RNG states put back afterwards so the
+    ranks build the same model as without the check.  Only a run with the switch on or a Problem that
+    defines ``get_param_groups`` pays for it: one more ``get_model()`` / ``get_criterion()`` in the parent
+    (for resnet50x4 a few hundred MB of host memory, freed again).  A ``get_model`` that touches CUDA
+    makes the parent unsafe to fork, and the ranks are then spawned, so the Problem must pickle."""
+    if not (no_decay_1d or has_param_group_hook(problem)):
+        return
+    import random
+    py_state, np_state = random.getstate(), np.random.get_state()
+    try:
+        with torch.random.fork_rng(devices=[]):
+            groups = problem_param_groups(problem, problem.get_model(), problem.get_criterion(), no_decay_1d)
+    finally:
+        random.setstate(py_state)
+        np.random.set_state(np_state)
+    check_param_groups(layer_adaptation, optimizer_state, adafactor, muon, groups is not None)
+
+
+def describe_param_groups(optimizer) -> str:
+    """The INFO line's param-group field: per group its tensors, lr and weight decay, or ``none`` when
+    the optimizer has one group (the ungrouped update paths)."""
+    if not getattr(optimizer, "grouped", False):
+        return "none"
+    return "%d: %s (grouped K2-mt)" % (len(optimizer.param_groups), ", ".join(
+        "%d tensors, lr %r, wd %r" % (len(g["params"]), g["lr"], g["weight_decay"]) for g in optimizer.param_groups))
+
+
 def resolve_channels_last(explicit: Optional[bool] = None) -> bool:
     """Whether conv weights and image batches are channels_last: ``explicit``, else
     FRL_B200_CHANNELS_LAST (``0``, the default, or ``1``).  Any other value is a ValueError."""
@@ -506,8 +573,11 @@ class Solver:
         muon = args.muon and run_opts.mode == Mode.TRAIN
         adamw = args.adamw and run_opts.mode == Mode.TRAIN
         lion = args.lion and run_opts.mode == Mode.TRAIN
+        param_groups = None
+        if run_opts.mode == Mode.TRAIN:
+            param_groups = problem_param_groups(problem, model, criterion, resolve_no_decay_1d(args.no_decay_1d))
         optimizer = create_fused_optimizer(arena, run_opts.optim, args.layer_adaptation, opt_state, adafactor,
-                                           muon, adamw, lion)
+                                           muon, adamw, lion, param_groups)
         if checkpoint:
             optimizer.load_state_dict(checkpoint.optimizerState)
         ema = None
@@ -568,7 +638,7 @@ class Solver:
                 "Linear layers with arena-born gradients %d (%d fused with their ReLU, %d in FP8) | "
                 "ReLU backward %s | "
                 "other gradients %s | layer adaptation %s | gradient accumulation %s | weight EMA %s | "
-                "optimizer %s | optimizer state %s | memory format %s | master weights %s",
+                "optimizer %s | optimizer state %s | memory format %s | master weights %s | param groups %s",
                 args.precision.value,
                 "CUDA-graph replay after 2 eager steps" if worker.graphed is not None else "eager launches",
                 ("fused NVLS kernel per bucket (K7), %d buckets" % len(pipeline.buckets)) if pipeline.nvls is not None
@@ -628,7 +698,8 @@ class Solver:
                         getattr(getattr(d, "device_transform", None), "honours_memory_format", False)
                         for d in problem.datasets) else "converted by the first convolution"),
                 "fp32" if not arena.bf16_master else
-                "bf16 + stochastic rounding, %.1f MiB saved" % (4 * arena.model_end / 2 ** 20))
+                "bf16 + stochastic rounding, %.1f MiB saved" % (4 * arena.model_end / 2 ** 20),
+                describe_param_groups(optimizer))
         scheduler = create_lr_scheduler(run_opts, worker.optimizer,
                                         checkpoint.epoch if checkpoint else -1)
         return worker, scheduler, checkpoint
@@ -845,7 +916,8 @@ class Solver:
               adamw: Optional[bool] = None,
               channels_last: Optional[bool] = None,
               master_weights: Optional[MasterWeights] = None,
-              lion: Optional[bool] = None
+              lion: Optional[bool] = None,
+              no_decay_1d: Optional[bool] = None
               ) -> Iterator[PerformanceSummary]:
         """The reference's entry point (solver.py:728-739) plus two keyword-only extensions:
 
@@ -989,6 +1061,29 @@ class Solver:
                        before a rank starts.  Checkpoints hold ``lr``, ``betas``, ``weight_decay``
                        and ``exp_avg``, the layout of lion-pytorch and timm.  None: FRL_B200_LION
                        (``0`` by default, ``1`` to enable).  ``Mode.EVAL`` ignores it.
+        ``no_decay_1d``  True: every model parameter with ``ndim <= 1`` (biases, normalisation
+                       parameters) goes in a param group with ``weight_decay = 0``, exactly what a
+                       Problem ``get_param_groups`` hook returning ``[{"params": [p for p in
+                       model.parameters() if p.ndim <= 1], "weight_decay": 0.0}]`` does (the group is
+                       omitted if empty).  Param groups in general come from the Problem's optional
+                       ``get_param_groups(model)``: dicts with ``params`` (model parameters) and
+                       optionally ``lr`` / ``weight_decay``, absolute values overriding ``OptimOpts``
+                       for the group.  Canonical group order, which numbers the params of the state
+                       dict: the hook's groups in the order returned, then one default group
+                       (``OptimOpts``' lr / weightDecay) with every remaining model parameter in
+                       ``model.parameters()`` order followed by the criterion parameters, omitted if
+                       empty.  Checkpoints are ``torch.optim.<X>(groups)``'s state dict; the per-epoch
+                       schedule scales each group from its own lr.  With more than one group the update
+                       is one grouped segment-table launch after backward (K2-mt grouped; K12 stays on
+                       one GPU), with no per-bucket eager update and no fused NVLS step (K7).  Needs SGD,
+                       Adam / AdamW, RMSprop or Lion; LARS / LAMB, 8-bit state, Adafactor and Muon, any
+                       key but ``params`` / ``lr`` / ``weight_decay``, an empty group, a parameter listed
+                       twice or not in ``model.parameters()``, a criterion parameter, and the switch
+                       together with a hook that returns groups raise ``ValueError`` before a rank
+                       starts; to check them the parent builds the model and criterion once more
+                       (host RNG state restored), and a ``get_model`` that touches CUDA there makes the
+                       ranks spawn rather than fork.  None: FRL_B200_NO_DECAY_1D (``0`` by default, ``1`` to enable); any
+                       other value raises ``ValueError``.  ``Mode.EVAL`` ignores groups.
         """
         adapt = LayerAdaptation.NONE
         accum = 1
@@ -998,6 +1093,7 @@ class Solver:
         use_muon = False
         use_adamw = False
         use_lion = False
+        use_no_decay_1d = False
         if run_opts.mode == Mode.TRAIN:
             adapt = resolve_layer_adaptation(layer_adaptation)
             check_layer_adaptation(run_opts.optim, adapt)
@@ -1011,6 +1107,8 @@ class Solver:
             check_adamw(run_opts.optim, adapt, opt_state, use_adafactor, use_adamw)
             use_lion = resolve_lion(lion)
             check_lion(run_opts.optim, adapt, use_lion)
+            use_no_decay_1d = resolve_no_decay_1d(no_decay_1d)
+            validate_param_groups(problem, use_no_decay_1d, adapt, opt_state, use_adafactor, use_muon)
             accum = resolve_grad_accumulation(grad_accumulation)
             decay = resolve_ema_decay(ema_decay)
         use_channels_last = resolve_channels_last(channels_last)
@@ -1059,7 +1157,8 @@ class Solver:
                 cache=None, precision=prec, save_every=save_every, graph_step=graph,
                 layer_adaptation=adapt, grad_accumulation=accum, ema_decay=decay,
                 optimizer_state=opt_state, adafactor=use_adafactor, muon=use_muon, adamw=use_adamw,
-                channels_last=use_channels_last, master_weights=use_master, lion=use_lion)
+                channels_last=use_channels_last, master_weights=use_master, lion=use_lion,
+                no_decay_1d=use_no_decay_1d)
             if not run_opts.singleThreaded:
                 parent_conn, child_conn = ctx.Pipe(duplex=False)
                 proc = ctx.Process(target=cls._solver_worker_process,

@@ -284,6 +284,86 @@ int frl_rmsprop_mt_sr(void* p, float* sq, float* buf, const frl_grad_seg* segs_d
 int frl_weight_ema_bf16(float* ema, const void* p, int64_t n, double w, void* stream);
 
 /* ------------------------------------------------------------------------------------------
+ * K2-mt grouped / K2-mt-sr grouped — parameter groups (torch.optim's param_groups): a learning
+ * rate and a weight decay per group, in the segment-table update of SGD (with or without
+ * momentum), Adam, AdamW, RMSprop and Lion.  Arguments: those of the frl_*_mt / frl_*_mt_sr form
+ * without lr, wd, dyn and t / step, and after n_tiles
+ *   seg_group_dev  int32 [n_segs]: the group of each segment, in [0, n_groups) (the caller
+ *                  validates it when it builds the table: the kernel does not read it back first)
+ *   seg_flags_dev  int32 [n_segs]: FRL_LW_CLIPPED = grad_scale_dev multiplies this segment's
+ *                  gradient (model parameters under clipping), as in K2-lw; other bits ignored
+ *   group_dyn      fp32 [n_groups][FRL_GROUP_DYN_COLS], 16-byte aligned, read at every launch
+ *                  (eager or replayed from a CUDA graph), one row per group g with lr_g, wd_g:
+ *     col 0-3  the ungrouped form's dyn layout for lr_g / wd_g, so a row pointer is a valid dyn
+ *              for K12 and the SR forms:
+ *                SGD, RMSprop   (lr_g, -, -, t)
+ *                Adam           (-lr_g / (1 - beta1^t), sqrt(1 - beta2^t), -, t)
+ *                AdamW          (-lr_g / (1 - beta1^t), sqrt(1 - beta2^t), fp32(1 - lr_g*wd_g), t)
+ *                Lion           (lr_g, fp32(1 - lr_g*wd_g), -, t)
+ *              t: the 1-based update count as uint32 bits (read by the _sr forms only)
+ *     col 4    wd_g, the L2-coupled decay of SGD, Adam and RMSprop
+ *   n_groups       rows of group_dyn, >= 1
+ * Per element of a segment of group g, the ungrouped rule with lr = lr_g and wd = wd_g:
+ *   SGD      d = g^ + wd_g*w ; buf = first_step ? d : mu*buf + (1-dampening)*d ; w -= lr_g*buf
+ *   Adam     the frl_adam rule on g^ + wd_g*w, step size lr_g / bc1
+ *   AdamW    w *= fp32(1 - lr_g*wd_g), then frl_adam's rule with no decay term
+ *   RMSprop  the frl_rmsprop rule on g^ + wd_g*w, lr_g
+ *   Lion     w *= fp32(1 - lr_g*wd_g) ; w -= lr_g*sign(lerp(m, g^, 1-beta1)) ; m = lerp(m, g^, 1-beta2)
+ * with g^ = g * grad_scale (* *grad_scale_dev if the segment has FRL_LW_CLIPPED).  Bytes per
+ * parameter are the ungrouped form's: a tile reads its segment's row once.
+ * ---------------------------------------------------------------------------------------- */
+enum { FRL_GROUP_DYN_COLS = 8 };
+int frl_sgd_momentum_mt_grouped(float* p, float* buf, void* p_lp, const frl_grad_seg* segs_dev,
+                                const int64_t* tile_prefix_dev, const int32_t* tile_seg_dev, int64_t n_tiles,
+                                const int32_t* seg_group_dev, const int32_t* seg_flags_dev, const float* group_dyn,
+                                int n_groups, double mu, double dampening, double grad_scale,
+                                const float* grad_scale_dev, int first_step, void* stream);
+int frl_adam_mt_grouped(float* p, float* m, float* v, float* vmax, void* p_lp, const frl_grad_seg* segs_dev,
+                        const int64_t* tile_prefix_dev, const int32_t* tile_seg_dev, int64_t n_tiles,
+                        const int32_t* seg_group_dev, const int32_t* seg_flags_dev, const float* group_dyn,
+                        int n_groups, double beta1, double beta2, double eps, double grad_scale,
+                        const float* grad_scale_dev, void* stream);
+int frl_adamw_mt_grouped(float* p, float* m, float* v, float* vmax, void* p_lp, const frl_grad_seg* segs_dev,
+                         const int64_t* tile_prefix_dev, const int32_t* tile_seg_dev, int64_t n_tiles,
+                         const int32_t* seg_group_dev, const int32_t* seg_flags_dev, const float* group_dyn,
+                         int n_groups, double beta1, double beta2, double eps, double grad_scale,
+                         const float* grad_scale_dev, void* stream);
+int frl_lion_mt_grouped(float* p, float* m, void* p_lp, const frl_grad_seg* segs_dev,
+                        const int64_t* tile_prefix_dev, const int32_t* tile_seg_dev, int64_t n_tiles,
+                        const int32_t* seg_group_dev, const int32_t* seg_flags_dev, const float* group_dyn,
+                        int n_groups, double beta1, double beta2, double grad_scale, const float* grad_scale_dev,
+                        void* stream);
+int frl_rmsprop_mt_grouped(float* p, float* sq, float* buf, void* p_lp, const frl_grad_seg* segs_dev,
+                           const int64_t* tile_prefix_dev, const int32_t* tile_seg_dev, int64_t n_tiles,
+                           const int32_t* seg_group_dev, const int32_t* seg_flags_dev, const float* group_dyn,
+                           int n_groups, double alpha, double eps, double mu, double grad_scale,
+                           const float* grad_scale_dev, void* stream);
+int frl_sgd_momentum_mt_grouped_sr(void* p, float* buf, const frl_grad_seg* segs_dev, const int64_t* tile_prefix_dev,
+                                   const int32_t* tile_seg_dev, int64_t n_tiles, const int32_t* seg_group_dev,
+                                   const int32_t* seg_flags_dev, const float* group_dyn, int n_groups, uint64_t seed,
+                                   double mu, double dampening, double grad_scale, const float* grad_scale_dev,
+                                   int first_step, void* stream);
+int frl_adam_mt_grouped_sr(void* p, float* m, float* v, float* vmax, const frl_grad_seg* segs_dev,
+                           const int64_t* tile_prefix_dev, const int32_t* tile_seg_dev, int64_t n_tiles,
+                           const int32_t* seg_group_dev, const int32_t* seg_flags_dev, const float* group_dyn,
+                           int n_groups, uint64_t seed, double beta1, double beta2, double eps, double grad_scale,
+                           const float* grad_scale_dev, void* stream);
+int frl_adamw_mt_grouped_sr(void* p, float* m, float* v, float* vmax, const frl_grad_seg* segs_dev,
+                            const int64_t* tile_prefix_dev, const int32_t* tile_seg_dev, int64_t n_tiles,
+                            const int32_t* seg_group_dev, const int32_t* seg_flags_dev, const float* group_dyn,
+                            int n_groups, uint64_t seed, double beta1, double beta2, double eps, double grad_scale,
+                            const float* grad_scale_dev, void* stream);
+int frl_lion_mt_grouped_sr(void* p, float* m, const frl_grad_seg* segs_dev, const int64_t* tile_prefix_dev,
+                           const int32_t* tile_seg_dev, int64_t n_tiles, const int32_t* seg_group_dev,
+                           const int32_t* seg_flags_dev, const float* group_dyn, int n_groups, uint64_t seed,
+                           double beta1, double beta2, double grad_scale, const float* grad_scale_dev, void* stream);
+int frl_rmsprop_mt_grouped_sr(void* p, float* sq, float* buf, const frl_grad_seg* segs_dev,
+                              const int64_t* tile_prefix_dev, const int32_t* tile_seg_dev, int64_t n_tiles,
+                              const int32_t* seg_group_dev, const int32_t* seg_flags_dev, const float* group_dyn,
+                              int n_groups, uint64_t seed, double alpha, double eps, double mu, double grad_scale,
+                              const float* grad_scale_dev, void* stream);
+
+/* ------------------------------------------------------------------------------------------
  * K2-lw — layer-wise adaptive updates over a segment table (an extension: the reference offers
  * SGD, Adam and RMSprop only).  LARS (You et al. 2017) is layer adaptation on the SGD rule, LAMB
  * (You et al. 2019) on the Adam rule.  Segment table, p / state / p_lp and the other arguments

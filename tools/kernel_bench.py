@@ -1,7 +1,7 @@
 #!/usr/bin/env python
 """Micro-benchmark of every hand-written kernel at the BASELINE shapes (1 GPU).
 
-    python tools/kernel_bench.py [--only k2,k2lw,k2q8,k2af,k2w,k2lion,k3,k5a,k5nhwc,k13,k14,...] [--iters 20] [--json out.json]
+    python tools/kernel_bench.py [--only k2,k2lw,k2q8,k2af,k2w,k2lion,k2g,k3,k5a,k5nhwc,k13,k14,...] [--iters 20] [--json out.json]
 
 Each kernel is timed with CUDA events on the launching stream over ROTATING operand sets whose
 total size exceeds the 50 MB L2 (so every launch streams from HBM), after 3 warm-up launches.
@@ -938,11 +938,88 @@ def bench_k5nhwc(iters):
     return out
 
 
+def bench_k2g(iters):
+    """Grouped K2-mt (``frl_*_mt_grouped``) against ungrouped K2-mt on the headline MLP's arena (10
+    tensors, 54.7 M parameters) for SGD-momentum and AdamW: bf16 gradients in the arena, bf16 shadow,
+    fp32 state, each timed from a CUDA graph; the arena (1.1 / 1.5 GB of traffic per launch) is far
+    larger than L2, so every launch streams from HBM.  Three groups: the tensors with ndim <= 1 at
+    wd 0, the trunk at half the lr, the heads at the default.  Five rounds, ungrouped and grouped
+    alternating; the last record per rule is the medians (min-max) and grouped / ungrouped, against
+    the target of 1.02 at the same bytes per parameter."""
+    from frl_b200.multi_tensor import GradSegTable
+
+    class Slot:
+        def __init__(self, index, offset, shape):
+            self.index, self.offset, self.shape = index, offset, shape
+            self.numel = 1
+            for d in shape:
+                self.numel *= d
+            self.is_model = True
+
+    shapes = [(4096, 4096), (4096,)] * 3 + [(1000, 4096), (1000,), (64, 4096), (64,)]
+    slots, off = [], 0
+    for i, sh in enumerate(shapes):
+        slots.append(Slot(i, off, sh))
+        off = (off + slots[-1].numel + 7) // 8 * 8
+    n, n_real = off, sum(s.numel for s in slots)
+    grad = torch.randn(n, device=DEV).bfloat16()
+    table = GradSegTable(slots, DEV)
+    for s in slots:
+        table.point(s, grad.data_ptr() + 2 * s.offset, grad.dtype)
+    table.upload()
+    seg_group = [0 if len(s.shape) <= 1 else (1 if i < 6 else 2) for i, s in enumerate(slots)]
+    p = torch.randn(n, device=DEV) * 0.02
+    lp = torch.empty(n, device=DEV, dtype=torch.bfloat16)
+    m, v = torch.randn(n, device=DEV) * 1e-3, torch.rand(n, device=DEV) * 1e-6
+    lr, wd, step = 1e-3, 1e-2, 3
+    out = []
+    for rule, bpp in (("sgd", 20), ("adamw", 28)):
+        rows = torch.zeros(3, _native.GROUP_DYN_COLS)
+        for gi, (glr, gwd) in enumerate(((lr, 0.0), (0.5 * lr, wd), (lr, wd))):
+            if rule == "sgd":
+                rows[gi, 0] = glr
+            else:
+                rows[gi, 0] = -(glr / (1 - 0.9 ** step))
+                rows[gi, 1] = (1 - 0.999 ** step) ** 0.5
+                rows[gi, 2] = 1 - glr * gwd
+            rows[gi, 4] = gwd
+        rows.view(torch.int32)[:, 3] = step
+        groups = _native.SegGroups(seg_group, [_native.LW_CLIPPED] * len(slots), rows.to(DEV))
+        if rule == "sgd":
+            fns = {"ungrouped": lambda i: _native.sgd_momentum_mt(p, m, lp, table, lr=lr, mu=0.9, dampening=0.0,
+                                                                  wd=wd, first_step=False),
+                   "grouped": lambda i: _native.sgd_momentum_mt_grouped(p, m, lp, table, groups, mu=0.9,
+                                                                        dampening=0.0, first_step=False)}
+        else:
+            fns = {"ungrouped": lambda i: _native.adamw_mt(p, m, v, None, lp, table, lr=lr, beta1=0.9, beta2=0.999,
+                                                           eps=1e-8, wd=wd, step=step),
+                   "grouped": lambda i: _native.adamw_mt_grouped(p, m, v, None, lp, table, groups, beta1=0.9,
+                                                                 beta2=0.999, eps=1e-8)}
+        times = {"ungrouped": [], "grouped": []}
+        for r in range(5):
+            for form in ("ungrouped", "grouped"):
+                rec = timed("K2-mt %s %s mlp bf16-grad (%d tensors, %d params, 3 groups) round %d"
+                            % (rule, form, len(slots), n_real, r), fns[form], 1, bpp * n_real, iters,
+                            "%d B/param" % bpp, graph=True)
+                times[form].append(rec["us"])
+                out.append(rec)
+        med = {k: sorted(t)[len(t) // 2] for k, t in times.items()}
+        summary = {"kernel": "K2-mt %s grouped vs ungrouped, median of 5 (min-max)" % rule,
+                   "ungrouped_us": "%.1f (%.1f-%.1f)" % (med["ungrouped"], min(times["ungrouped"]),
+                                                        max(times["ungrouped"])),
+                   "grouped_us": "%.1f (%.1f-%.1f)" % (med["grouped"], min(times["grouped"]), max(times["grouped"])),
+                   "grouped_over_ungrouped": round(med["grouped"] / med["ungrouped"], 4),
+                   "within_2pct": med["grouped"] <= 1.02 * med["ungrouped"]}
+        print(json.dumps(summary), flush=True)
+        out.append(summary)
+    return out
+
+
 BENCHES = {"k2": bench_k2, "k2mt": bench_k2mt, "k2lw": bench_k2lw, "k3": bench_k3, "k4": bench_k4, "k5": bench_k5, "k5a": bench_k5a,
            "k5m": bench_k5m, "k4s": bench_k4s, "k6": bench_k6,
            "k8": bench_k8, "k8t": bench_k8t, "k9": bench_k9, "k10": bench_k10, "k11": bench_k11,
            "k2q8": bench_k2q8, "k2af": bench_k2af, "k13": bench_k13, "k14": bench_k14, "k2w": bench_k2w,
-           "k5nhwc": bench_k5nhwc, "k2lion": bench_k2lion}
+           "k5nhwc": bench_k5nhwc, "k2lion": bench_k2lion, "k2g": bench_k2g}
 
 
 def main():
