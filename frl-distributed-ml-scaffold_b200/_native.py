@@ -93,6 +93,23 @@ SIGNATURES = {
     "frl_rmsprop_mt_sr": (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _i64, _u64, _i64, _d, _d, _d, _d, _d, _d, _vp, _vp,
                                _vp]),
     "frl_weight_ema_bf16": (_i, [_vp, _vp, _i64, _d, _vp]),
+    "frl_sf_adamw": (_i, [_vp, _vp, _vp, _vp, _vp, _i64, _d, _d, _d, _d, _d, _d, _d, _vp, _vp, _i, _vp]),
+    "frl_sf_sgd": (_i, [_vp, _vp, _vp, _vp, _i64, _d, _d, _d, _d, _d, _vp, _vp, _i, _vp]),
+    "frl_sf_adamw_mt": (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _i64, _d, _d, _d, _d, _d, _d, _d, _vp, _vp, _vp]),
+    "frl_sf_sgd_mt": (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _i64, _d, _d, _d, _d, _d, _vp, _vp, _vp]),
+    "frl_sf_adamw_mt_grouped": (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _i64, _vp, _vp, _vp, _i, _d, _d, _d, _d, _vp,
+                                     _vp]),
+    "frl_sf_sgd_mt_grouped": (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _i64, _vp, _vp, _vp, _i, _d, _d, _vp, _vp]),
+    "frl_sf_adamw_sr": (_i, [_vp, _vp, _vp, _vp, _i64, _i64, _u64, _i64, _d, _d, _d, _d, _d, _d, _d, _vp, _vp, _i,
+                             _vp]),
+    "frl_sf_sgd_sr": (_i, [_vp, _vp, _vp, _i64, _i64, _u64, _i64, _d, _d, _d, _d, _d, _vp, _vp, _i, _vp]),
+    "frl_sf_adamw_mt_sr": (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _i64, _u64, _i64, _d, _d, _d, _d, _d, _d, _d, _vp, _vp,
+                                _vp]),
+    "frl_sf_sgd_mt_sr": (_i, [_vp, _vp, _vp, _vp, _vp, _i64, _u64, _i64, _d, _d, _d, _d, _d, _vp, _vp, _vp]),
+    "frl_sf_adamw_mt_grouped_sr": (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _i64, _vp, _vp, _vp, _i, _u64, _d, _d, _d, _d,
+                                        _vp, _vp]),
+    "frl_sf_sgd_mt_grouped_sr": (_i, [_vp, _vp, _vp, _vp, _vp, _i64, _vp, _vp, _vp, _i, _u64, _d, _d, _vp, _vp]),
+    "frl_sf_eval_weights": (_i, [_vp, _i, _vp, _vp, _i, _i64, _d, _vp]),
     "frl_sgd_momentum_mt_grouped": (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _i64, _vp, _vp, _vp, _i, _d, _d, _d, _vp, _i,
                                          _vp]),
     "frl_adam_mt_grouped": (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _i64, _vp, _vp, _vp, _i, _d, _d, _d, _d, _vp,
@@ -643,6 +660,103 @@ def rmsprop_mt_grouped_sr(p, sq, buf, table, groups, *, seed, alpha, eps, mu, gr
     _check(lib().frl_rmsprop_mt_grouped_sr(_ptr(p), _ptr(sq), _ptr(buf), *_grouped(table, groups), seed, alpha, eps,
                                            mu, grad_scale, _ptr(grad_scale_dev), _stream()),
            "frl_rmsprop_mt_grouped_sr")
+
+
+# ---- Schedule-Free AdamW / SGD (K2, K2-mt, K2-sr, grouped) and its evaluation weights (K2-sfx) --------
+# y is the weights the update moves (fp32 master, or the bf16 weights for the _sr forms), z the base
+# iterate, v AdamW's exp_avg_sq; lr / ckp1 the update's scalars (see frl_sf_* in include/frl_b200.h).
+
+def sf_adamw(y, g, z, v, p_lp, n, *, lr, ckp1, beta1, beta2, eps, wd, grad_scale=1.0, grad_scale_dev=None,
+             dyn=None) -> None:
+    _check(lib().frl_sf_adamw(_ptr(y), _ptr(g), _ptr(z), _ptr(v), _ptr(p_lp), n, lr, ckp1, beta1, beta2, eps, wd,
+                              grad_scale, _ptr(grad_scale_dev), _ptr(dyn), dtype_code(g.dtype), _stream()),
+           "frl_sf_adamw")
+
+
+def sf_sgd(y, g, z, p_lp, n, *, lr, ckp1, beta1, wd, grad_scale=1.0, grad_scale_dev=None, dyn=None) -> None:
+    _check(lib().frl_sf_sgd(_ptr(y), _ptr(g), _ptr(z), _ptr(p_lp), n, lr, ckp1, beta1, wd, grad_scale,
+                            _ptr(grad_scale_dev), _ptr(dyn), dtype_code(g.dtype), _stream()), "frl_sf_sgd")
+
+
+def _table(table):
+    return table.segs_dev_ptr, table.prefix_dev_ptr, table.tile_seg_dev_ptr, table.n_tiles
+
+
+def sf_adamw_mt(y, z, v, p_lp, table, *, lr, ckp1, beta1, beta2, eps, wd, grad_scale=1.0, grad_scale_dev=None,
+                dyn=None) -> None:
+    _check(lib().frl_sf_adamw_mt(_ptr(y), _ptr(z), _ptr(v), _ptr(p_lp), *_table(table), lr, ckp1, beta1, beta2, eps,
+                                 wd, grad_scale, _ptr(grad_scale_dev), _ptr(dyn), _stream()), "frl_sf_adamw_mt")
+
+
+def sf_sgd_mt(y, z, p_lp, table, *, lr, ckp1, beta1, wd, grad_scale=1.0, grad_scale_dev=None, dyn=None) -> None:
+    _check(lib().frl_sf_sgd_mt(_ptr(y), _ptr(z), _ptr(p_lp), *_table(table), lr, ckp1, beta1, wd, grad_scale,
+                               _ptr(grad_scale_dev), _ptr(dyn), _stream()), "frl_sf_sgd_mt")
+
+
+def sf_adamw_mt_grouped(y, z, v, p_lp, table, groups, *, beta1, beta2, eps, grad_scale=1.0,
+                        grad_scale_dev=None) -> None:
+    _check(lib().frl_sf_adamw_mt_grouped(_ptr(y), _ptr(z), _ptr(v), _ptr(p_lp), *_grouped(table, groups), beta1,
+                                         beta2, eps, grad_scale, _ptr(grad_scale_dev), _stream()),
+           "frl_sf_adamw_mt_grouped")
+
+
+def sf_sgd_mt_grouped(y, z, p_lp, table, groups, *, beta1, grad_scale=1.0, grad_scale_dev=None) -> None:
+    _check(lib().frl_sf_sgd_mt_grouped(_ptr(y), _ptr(z), _ptr(p_lp), *_grouped(table, groups), beta1, grad_scale,
+                                       _ptr(grad_scale_dev), _stream()), "frl_sf_sgd_mt_grouped")
+
+
+def sf_adamw_sr(y, g, z, v, n, *, arena_off, seed, t, lr, ckp1, beta1, beta2, eps, wd, grad_scale=1.0,
+                grad_scale_dev=None, dyn=None) -> None:
+    _check_sr(y, seed)
+    _check(lib().frl_sf_adamw_sr(_ptr(y), _ptr(g), _ptr(z), _ptr(v), n, arena_off, seed, t, lr, ckp1, beta1, beta2,
+                                 eps, wd, grad_scale, _ptr(grad_scale_dev), _ptr(dyn), dtype_code(g.dtype),
+                                 _stream()), "frl_sf_adamw_sr")
+
+
+def sf_sgd_sr(y, g, z, n, *, arena_off, seed, t, lr, ckp1, beta1, wd, grad_scale=1.0, grad_scale_dev=None,
+              dyn=None) -> None:
+    _check_sr(y, seed)
+    _check(lib().frl_sf_sgd_sr(_ptr(y), _ptr(g), _ptr(z), n, arena_off, seed, t, lr, ckp1, beta1, wd, grad_scale,
+                               _ptr(grad_scale_dev), _ptr(dyn), dtype_code(g.dtype), _stream()), "frl_sf_sgd_sr")
+
+
+def sf_adamw_mt_sr(y, z, v, table, *, seed, t, lr, ckp1, beta1, beta2, eps, wd, grad_scale=1.0,
+                   grad_scale_dev=None, dyn=None) -> None:
+    _check_sr(y, seed)
+    _check(lib().frl_sf_adamw_mt_sr(_ptr(y), _ptr(z), _ptr(v), *_table(table), seed, t, lr, ckp1, beta1, beta2, eps,
+                                    wd, grad_scale, _ptr(grad_scale_dev), _ptr(dyn), _stream()), "frl_sf_adamw_mt_sr")
+
+
+def sf_sgd_mt_sr(y, z, table, *, seed, t, lr, ckp1, beta1, wd, grad_scale=1.0, grad_scale_dev=None,
+                 dyn=None) -> None:
+    _check_sr(y, seed)
+    _check(lib().frl_sf_sgd_mt_sr(_ptr(y), _ptr(z), *_table(table), seed, t, lr, ckp1, beta1, wd, grad_scale,
+                                  _ptr(grad_scale_dev), _ptr(dyn), _stream()), "frl_sf_sgd_mt_sr")
+
+
+def sf_adamw_mt_grouped_sr(y, z, v, table, groups, *, seed, beta1, beta2, eps, grad_scale=1.0,
+                           grad_scale_dev=None) -> None:
+    _check_sr(y, seed)
+    _check(lib().frl_sf_adamw_mt_grouped_sr(_ptr(y), _ptr(z), _ptr(v), *_grouped(table, groups), seed, beta1, beta2,
+                                            eps, grad_scale, _ptr(grad_scale_dev), _stream()),
+           "frl_sf_adamw_mt_grouped_sr")
+
+
+def sf_sgd_mt_grouped_sr(y, z, table, groups, *, seed, beta1, grad_scale=1.0, grad_scale_dev=None) -> None:
+    _check_sr(y, seed)
+    _check(lib().frl_sf_sgd_mt_grouped_sr(_ptr(y), _ptr(z), *_grouped(table, groups), seed, beta1, grad_scale,
+                                          _ptr(grad_scale_dev), _stream()), "frl_sf_sgd_mt_grouped_sr")
+
+
+def sf_eval_weights(y, z, x, *, beta1) -> None:
+    """K2-sfx: x = lerp(y, z, 1 - 1/beta1) over ``y.numel()`` elements (see frl_sf_eval_weights); y / x fp32
+    or bf16, x may be y (in place)."""
+    n = y.numel()
+    if z.numel() != n or x.numel() != n or z.dtype != torch.float32:
+        raise NativeLibraryError("sf_eval_weights: y %s, z %s %s and x %s must be equally long, z fp32"
+                                 % (n, z.numel(), z.dtype, x.numel()))
+    _check(lib().frl_sf_eval_weights(_ptr(y), dtype_code(y.dtype), _ptr(z), _ptr(x), dtype_code(x.dtype), n, beta1,
+                                     _stream()), "frl_sf_eval_weights")
 
 
 # ---- K2-lw: layer-wise adaptive updates (LARS, LAMB) over a segment table -------------------------

@@ -629,3 +629,79 @@ extern "C" int frl_rmsprop_mt_grouped(float* p, float* sq, float* buf, void* p_l
                                                          tile_seg_dev, n_tiles, gs, grad_scale_dev, nullptr, st, name,
                                                          grp, n_groups);
 }
+
+// ---- Schedule-Free AdamW / SGD (K2, K2-mt, K2-mt grouped) --------------------------------------------
+// The AdamW / SGD sibling's arguments with (lr, ckp1, beta1) for the step count: lr the update's lr
+// (warm-up and, for AdamW, sqrt(1 - beta2^(k+1)) folded in), ckp1 the averaging weight; the kernel forms
+// y_lr = lr*(beta1*(1 - ckp1) - 1) in double.  z (state 0) and, for AdamW, exp_avg_sq (state 1); see
+// ScheduleFreeRule and include/frl_b200.h.
+
+extern "C" int frl_sf_adamw(float* y, const void* g, float* z, float* v, void* p_lp, int64_t n, double lr,
+                            double ckp1, double beta1, double beta2, double eps, double wd, double grad_scale,
+                            const float* grad_scale_dev, const float* dyn, int g_dtype, void* stream) {
+    FRL_CHECK_SF(true, beta1, z, v, "frl_sf_adamw");
+    return launch_update<ScheduleFreeRule<true>, 2>(make_sf_rule<true>(lr, ckp1, beta1, beta2, eps, wd), y, g, z, v,
+                                                    nullptr, p_lp, n, static_cast<float>(grad_scale), grad_scale_dev,
+                                                    dyn, g_dtype, static_cast<cudaStream_t>(stream), "frl_sf_adamw");
+}
+
+extern "C" int frl_sf_sgd(float* y, const void* g, float* z, void* p_lp, int64_t n, double lr, double ckp1,
+                          double beta1, double wd, double grad_scale, const float* grad_scale_dev, const float* dyn,
+                          int g_dtype, void* stream) {
+    FRL_CHECK_SF(false, beta1, z, z, "frl_sf_sgd");
+    return launch_update<ScheduleFreeRule<false>, 1>(make_sf_rule<false>(lr, ckp1, beta1, 0.0, 0.0, wd), y, g, z,
+                                                     nullptr, nullptr, p_lp, n, static_cast<float>(grad_scale),
+                                                     grad_scale_dev, dyn, g_dtype, static_cast<cudaStream_t>(stream),
+                                                     "frl_sf_sgd");
+}
+
+extern "C" int frl_sf_adamw_mt(float* y, float* z, float* v, void* p_lp, const frl_grad_seg* segs_dev,
+                               const int64_t* tile_prefix_dev, const int32_t* tile_seg_dev, int64_t n_tiles, double lr,
+                               double ckp1, double beta1, double beta2, double eps, double wd, double grad_scale,
+                               const float* grad_scale_dev, const float* dyn, void* stream) {
+    FRL_CHECK_SF(true, beta1, z, v, "frl_sf_adamw_mt");
+    return launch_update_mt<ScheduleFreeRule<true>, 2>(make_sf_rule<true>(lr, ckp1, beta1, beta2, eps, wd), y, z, v,
+                                                       nullptr, p_lp, segs_dev, tile_prefix_dev, tile_seg_dev,
+                                                       n_tiles, static_cast<float>(grad_scale), grad_scale_dev, dyn,
+                                                       static_cast<cudaStream_t>(stream), "frl_sf_adamw_mt");
+}
+
+extern "C" int frl_sf_sgd_mt(float* y, float* z, void* p_lp, const frl_grad_seg* segs_dev,
+                             const int64_t* tile_prefix_dev, const int32_t* tile_seg_dev, int64_t n_tiles, double lr,
+                             double ckp1, double beta1, double wd, double grad_scale, const float* grad_scale_dev,
+                             const float* dyn, void* stream) {
+    FRL_CHECK_SF(false, beta1, z, z, "frl_sf_sgd_mt");
+    return launch_update_mt<ScheduleFreeRule<false>, 1>(make_sf_rule<false>(lr, ckp1, beta1, 0.0, 0.0, wd), y, z,
+                                                        nullptr, nullptr, p_lp, segs_dev, tile_prefix_dev,
+                                                        tile_seg_dev, n_tiles, static_cast<float>(grad_scale),
+                                                        grad_scale_dev, dyn, static_cast<cudaStream_t>(stream),
+                                                        "frl_sf_sgd_mt");
+}
+
+// grouped: each segment's group row supplies lr, ckp1, y_lr (columns 0-2) and wd (column 4); beta1 is
+// only checked
+extern "C" int frl_sf_adamw_mt_grouped(float* y, float* z, float* v, void* p_lp, const frl_grad_seg* segs_dev,
+                                       const int64_t* tile_prefix_dev, const int32_t* tile_seg_dev, int64_t n_tiles,
+                                       const int32_t* seg_group_dev, const int32_t* seg_flags_dev,
+                                       const float* group_dyn, int n_groups, double beta1, double beta2, double eps,
+                                       double grad_scale, const float* grad_scale_dev, void* stream) {
+    FRL_CHECK_SF(true, beta1, z, v, "frl_sf_adamw_mt_grouped");
+    return launch_update_mt<ScheduleFreeRule<true>, 2, true>(
+        make_sf_rule<true>(0.0, 1.0, beta1, beta2, eps, 0.0), y, z, v, nullptr, p_lp, segs_dev, tile_prefix_dev,
+        tile_seg_dev, n_tiles, static_cast<float>(grad_scale), grad_scale_dev, nullptr,
+        static_cast<cudaStream_t>(stream), "frl_sf_adamw_mt_grouped",
+        GroupTable{seg_group_dev, seg_flags_dev, group_dyn}, n_groups);
+}
+
+extern "C" int frl_sf_sgd_mt_grouped(float* y, float* z, void* p_lp, const frl_grad_seg* segs_dev,
+                                     const int64_t* tile_prefix_dev, const int32_t* tile_seg_dev, int64_t n_tiles,
+                                     const int32_t* seg_group_dev, const int32_t* seg_flags_dev,
+                                     const float* group_dyn, int n_groups, double beta1, double grad_scale,
+                                     const float* grad_scale_dev, void* stream) {
+    FRL_CHECK_SF(false, beta1, z, z, "frl_sf_sgd_mt_grouped");
+    return launch_update_mt<ScheduleFreeRule<false>, 1, true>(
+        make_sf_rule<false>(0.0, 1.0, beta1, 0.0, 0.0, 0.0), y, z, nullptr, nullptr, p_lp, segs_dev, tile_prefix_dev,
+        tile_seg_dev, n_tiles, static_cast<float>(grad_scale), grad_scale_dev, nullptr,
+        static_cast<cudaStream_t>(stream), "frl_sf_sgd_mt_grouped",
+        GroupTable{seg_group_dev, seg_flags_dev, group_dyn}, n_groups);
+}

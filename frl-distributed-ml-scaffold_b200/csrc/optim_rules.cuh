@@ -111,6 +111,45 @@ struct LionRule {
     }
 };
 
+// torch's lerp in fp32, both branches as the single fmaf nvcc contracts torch's expression into
+__device__ __forceinline__ float lerp_torch_f32(float a, float b, float w) {
+    return fabsf(w) < 0.5f ? fmaf(w, b - a, a) : fmaf(-(b - a), 1.f - w, b);
+}
+
+// Schedule-Free (Defazio et al. 2024, The Road Less Scheduled), the schedulefree package's 1.x step
+// with Adam's bias correction folded into lr.  p is y (where gradients are taken); state 0 is z (the
+// base iterate), state 1 Adam's exp_avg_sq (ADAPTIVE only):
+//   ADAPTIVE: v = beta2*v + (1-beta2)*g^2 (Adam's fmaf form);  u = g / (sqrt(v) + eps)
+//   SGD:      u = g
+//   u = u + wd*y                       decay taken at y
+//   y = lerp(y, z, ckp1);  y = y + y_lr*u;  z = z - lr*u
+// dyn[0] lr, dyn[1] ckp1, dyn[2] y_lr = lr*(beta1*(1-ckp1) - 1), all formed on the host in double per
+// update, so a replayed graph follows the schedule-free weights and the scheduled lr.
+template <bool ADAPTIVE>
+struct ScheduleFreeRule {
+    float beta2, w2;        // beta2, 1 - beta2 (ADAPTIVE)
+    float eps, wd;
+    float lr, ckp1, y_lr;
+    static constexpr int kStates = ADAPTIVE ? 2 : 1;
+    __device__ __forceinline__ void patch(const float* dyn) {
+        lr = __ldg(dyn);
+        ckp1 = __ldg(dyn + 1);
+        y_lr = __ldg(dyn + 2);
+    }
+    __device__ __forceinline__ void patch_group(const float* row) { patch(row); wd = __ldg(row + 4); }
+    __device__ __forceinline__ void operator()(float& y, float g, float& z, float& v, float&) const {
+        float u = g;
+        if (ADAPTIVE) {
+            v = fmaf(w2 * g, g, v * beta2);
+            u = g / (sqrtf(v) + eps);
+        }
+        u = fmaf(wd, y, u);
+        y = lerp_torch_f32(y, z, ckp1);
+        y = fmaf(y_lr, u, y);
+        z = fmaf(-lr, u, z);
+    }
+};
+
 template <bool MOMENTUM>
 struct RmspropRule {
     float alpha, one_minus_alpha, eps, wd, mu, neg_lr;
@@ -183,6 +222,22 @@ static inline LionRule make_lion_rule(double lr, double beta1, double beta2, dou
     return LionRule{static_cast<float>(1.0 - beta1), static_cast<float>(1.0 - beta2), static_cast<float>(-lr),
                     static_cast<float>(1.0 - lr * wd)};
 }
+// the argument checks every Schedule-Free entry point makes before any launch (inside a function
+// returning int); v is checked only by the ADAPTIVE (AdamW) forms
+#define FRL_CHECK_SF(adaptive, beta1, z, v, name)                                                        \
+    do {                                                                                                 \
+        FRL_REQUIRE((z) != nullptr, FRL_E_ARG, "%s: null z", name);                                      \
+        FRL_REQUIRE(!(adaptive) || (v) != nullptr, FRL_E_ARG, "%s: null exp_avg_sq", name);              \
+        FRL_REQUIRE((beta1) > 0.0 && (beta1) < 1.0, FRL_E_ARG, "%s: beta1 %g outside (0, 1)", name, (beta1)); \
+    } while (0)
+template <bool A>
+static inline ScheduleFreeRule<A> make_sf_rule(double lr, double ckp1, double beta1, double beta2, double eps,
+                                               double wd) {
+    return ScheduleFreeRule<A>{static_cast<float>(beta2), static_cast<float>(1.0 - beta2), static_cast<float>(eps),
+                               static_cast<float>(wd), static_cast<float>(lr), static_cast<float>(ckp1),
+                               static_cast<float>(lr * (beta1 * (1.0 - ckp1) - 1.0))};
+}
+
 template <bool MOM>
 static inline RmspropRule<MOM> make_rmsprop_rule(double lr, double alpha, double eps, double wd, double mu) {
     return RmspropRule<MOM>{static_cast<float>(alpha), static_cast<float>(1.0 - alpha), static_cast<float>(eps),

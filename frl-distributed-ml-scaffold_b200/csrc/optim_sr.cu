@@ -569,3 +569,80 @@ extern "C" int frl_rmsprop_mt_grouped_sr(void* p, float* sq, float* buf, const f
                                                             n_tiles, seed, 1, gs, grad_scale_dev, nullptr, st, name,
                                                             grp, n_groups);
 }
+
+// ---- Schedule-Free AdamW / SGD on bf16 master weights (K2-sr, K2-mt-sr, K2-mt-sr grouped) -------------
+// The fp32-master forms' arguments (optim.cu) with the SR sibling's (arena_off, seed, t); y is the bf16
+// weights, z and exp_avg_sq stay fp32.
+
+extern "C" int frl_sf_adamw_sr(void* y, const void* g, float* z, float* v, int64_t n, int64_t arena_off,
+                               uint64_t seed, int64_t t, double lr, double ckp1, double beta1, double beta2,
+                               double eps, double wd, double grad_scale, const float* grad_scale_dev,
+                               const float* dyn, int g_dtype, void* stream) {
+    FRL_CHECK_SF(true, beta1, z, v, "frl_sf_adamw_sr");
+    return launch_update_sr<ScheduleFreeRule<true>, 2>(make_sf_rule<true>(lr, ckp1, beta1, beta2, eps, wd), y, g, z,
+                                                       v, nullptr, n, arena_off, seed, t,
+                                                       static_cast<float>(grad_scale), grad_scale_dev, dyn, g_dtype,
+                                                       static_cast<cudaStream_t>(stream), "frl_sf_adamw_sr");
+}
+
+extern "C" int frl_sf_sgd_sr(void* y, const void* g, float* z, int64_t n, int64_t arena_off, uint64_t seed,
+                             int64_t t, double lr, double ckp1, double beta1, double wd, double grad_scale,
+                             const float* grad_scale_dev, const float* dyn, int g_dtype, void* stream) {
+    FRL_CHECK_SF(false, beta1, z, z, "frl_sf_sgd_sr");
+    return launch_update_sr<ScheduleFreeRule<false>, 1>(make_sf_rule<false>(lr, ckp1, beta1, 0.0, 0.0, wd), y, g, z,
+                                                        nullptr, nullptr, n, arena_off, seed, t,
+                                                        static_cast<float>(grad_scale), grad_scale_dev, dyn, g_dtype,
+                                                        static_cast<cudaStream_t>(stream), "frl_sf_sgd_sr");
+}
+
+extern "C" int frl_sf_adamw_mt_sr(void* y, float* z, float* v, const frl_grad_seg* segs_dev,
+                                  const int64_t* tile_prefix_dev, const int32_t* tile_seg_dev, int64_t n_tiles,
+                                  uint64_t seed, int64_t t, double lr, double ckp1, double beta1, double beta2,
+                                  double eps, double wd, double grad_scale, const float* grad_scale_dev,
+                                  const float* dyn, void* stream) {
+    FRL_CHECK_SF(true, beta1, z, v, "frl_sf_adamw_mt_sr");
+    return launch_update_mt_sr<ScheduleFreeRule<true>, 2>(make_sf_rule<true>(lr, ckp1, beta1, beta2, eps, wd), y, z,
+                                                          v, nullptr, segs_dev, tile_prefix_dev, tile_seg_dev,
+                                                          n_tiles, seed, t, static_cast<float>(grad_scale),
+                                                          grad_scale_dev, dyn, static_cast<cudaStream_t>(stream),
+                                                          "frl_sf_adamw_mt_sr");
+}
+
+extern "C" int frl_sf_sgd_mt_sr(void* y, float* z, const frl_grad_seg* segs_dev, const int64_t* tile_prefix_dev,
+                                const int32_t* tile_seg_dev, int64_t n_tiles, uint64_t seed, int64_t t, double lr,
+                                double ckp1, double beta1, double wd, double grad_scale, const float* grad_scale_dev,
+                                const float* dyn, void* stream) {
+    FRL_CHECK_SF(false, beta1, z, z, "frl_sf_sgd_mt_sr");
+    return launch_update_mt_sr<ScheduleFreeRule<false>, 1>(make_sf_rule<false>(lr, ckp1, beta1, 0.0, 0.0, wd), y, z,
+                                                           nullptr, nullptr, segs_dev, tile_prefix_dev, tile_seg_dev,
+                                                           n_tiles, seed, t, static_cast<float>(grad_scale),
+                                                           grad_scale_dev, dyn, static_cast<cudaStream_t>(stream),
+                                                           "frl_sf_sgd_mt_sr");
+}
+
+extern "C" int frl_sf_adamw_mt_grouped_sr(void* y, float* z, float* v, const frl_grad_seg* segs_dev,
+                                          const int64_t* tile_prefix_dev, const int32_t* tile_seg_dev,
+                                          int64_t n_tiles, const int32_t* seg_group_dev, const int32_t* seg_flags_dev,
+                                          const float* group_dyn, int n_groups, uint64_t seed, double beta1,
+                                          double beta2, double eps, double grad_scale, const float* grad_scale_dev,
+                                          void* stream) {
+    FRL_CHECK_SF(true, beta1, z, v, "frl_sf_adamw_mt_grouped_sr");
+    return launch_update_mt_sr<ScheduleFreeRule<true>, 2, true>(
+        make_sf_rule<true>(0.0, 1.0, beta1, beta2, eps, 0.0), y, z, v, nullptr, segs_dev, tile_prefix_dev,
+        tile_seg_dev, n_tiles, seed, 1, static_cast<float>(grad_scale), grad_scale_dev, nullptr,
+        static_cast<cudaStream_t>(stream), "frl_sf_adamw_mt_grouped_sr",
+        GroupTable{seg_group_dev, seg_flags_dev, group_dyn}, n_groups);
+}
+
+extern "C" int frl_sf_sgd_mt_grouped_sr(void* y, float* z, const frl_grad_seg* segs_dev,
+                                        const int64_t* tile_prefix_dev, const int32_t* tile_seg_dev, int64_t n_tiles,
+                                        const int32_t* seg_group_dev, const int32_t* seg_flags_dev,
+                                        const float* group_dyn, int n_groups, uint64_t seed, double beta1,
+                                        double grad_scale, const float* grad_scale_dev, void* stream) {
+    FRL_CHECK_SF(false, beta1, z, z, "frl_sf_sgd_mt_grouped_sr");
+    return launch_update_mt_sr<ScheduleFreeRule<false>, 1, true>(
+        make_sf_rule<false>(0.0, 1.0, beta1, 0.0, 0.0, 0.0), y, z, nullptr, nullptr, segs_dev, tile_prefix_dev,
+        tile_seg_dev, n_tiles, seed, 1, static_cast<float>(grad_scale), grad_scale_dev, nullptr,
+        static_cast<cudaStream_t>(stream), "frl_sf_sgd_mt_grouped_sr",
+        GroupTable{seg_group_dev, seg_flags_dev, group_dyn}, n_groups);
+}

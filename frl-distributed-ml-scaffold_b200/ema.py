@@ -31,6 +31,23 @@ EMA_STATE_KEY = "weight_ema"
 SWAP_CHUNK = 4 << 20
 
 
+def module_state_dict(arena: ParamArena, module: nn.Module, weights=None) -> Dict[str, Any]:
+    """``module``'s fp32 CPU ``state_dict()`` keyed like the main checkpoint's (what ``<stem>.ema`` and
+    ``<stem>.sf`` hold, and ``initialModelPath`` loads), with the weights ``arena`` holds or, given
+    ``weights`` (an fp32 vector over the model range ``[0, model_end)``), each model parameter from it.
+    Buffers are the live ones."""
+    buffers = {name for name, _ in module.named_buffers()}
+    with arena.exported(cpu=True, module=module):
+        # parameters are private CPU copies inside exported(); buffers are the live tensors
+        sd = {k: v.detach().to("cpu", copy=k in buffers) for k, v in module.state_dict().items()}
+    if weights is not None:
+        names = {id(p): name for name, p in module.named_parameters()}
+        for s in arena.slots:
+            if s.is_model:
+                sd[names[id(s.param)]] = ParamArena.slot_view(weights, s).to("cpu", memory_format=torch.contiguous_format)
+    return sd
+
+
 class WeightEMA:
     """EMA of the model range of ``arena``'s master weights and of ``module``'s buffers.
 
@@ -137,18 +154,10 @@ class WeightEMA:
     def state_dict(self) -> Dict[str, Any]:
         """``{"decay", "updates", "state_dict"}``: ``state_dict`` is the module's fp32 CPU
         ``state_dict()`` with the averaged values in it, keyed like the main checkpoint's."""
-        buffers = {name for name, _, _ in self.buffers}
-        with self.swapped(), self.arena.exported(cpu=True, module=self.module):
-            # parameters are private CPU copies inside exported(); buffers are the live tensors
-            sd = {k: v.detach().to("cpu", copy=k in buffers) for k, v in self.module.state_dict().items()}
-        if self.bf16:
-            # the swap put the EMA rounded to bf16 in the weights: write the fp32 EMA itself, so a
-            # resumed EMA continues bit for bit
-            names = {id(p): name for name, p in self.module.named_parameters()}
-            for s in self.arena.slots:
-                if s.is_model:
-                    sd[names[id(s.param)]] = ParamArena.slot_view(self.ema, s).to(
-                        "cpu", memory_format=torch.contiguous_format)
+        with self.swapped():
+            # with bf16 master weights the swap put the EMA rounded to bf16 in the weights: write the
+            # fp32 EMA itself, so a resumed EMA continues bit for bit
+            sd = module_state_dict(self.arena, self.module, self.ema if self.bf16 else None)
         return {"decay": self.decay, "updates": self.updates, "state_dict": sd}
 
     @torch.no_grad()

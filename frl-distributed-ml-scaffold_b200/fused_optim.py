@@ -28,6 +28,7 @@ with the global count, ``state_dict()`` writes that count for every parameter an
 ``load_state_dict()`` takes the maximum over the loaded entries.  Models whose parameters all
 receive a gradient every step — every configuration of BASELINE.json — are unaffected.
 """
+from contextlib import contextmanager
 from typing import Any, Dict, List, Optional, Tuple
 
 import numpy as np
@@ -35,10 +36,15 @@ import torch
 
 from . import _native
 from .arena import ParamArena
-from .types import LayerAdaptation, MasterWeights, OptAlgorithm, OptimizerState, OptimOpts, Precision
+from .types import (LayerAdaptation, MasterWeights, OptAlgorithm, OptimizerState, OptimOpts, Precision,
+                    ScheduleFree)
 
 # Kernel entry points; tests exercising host logic on CPU swap this for an oracle-backed double.
 KERNELS = _native
+
+# the top-level key under which a Schedule-Free run's evaluation weights travel from a rank to the parent
+# inside the optimizer-state bytes; the parent takes them out and writes <stem>.sf
+SF_STATE_KEY = "schedule_free_x"
 
 # default key of the stochastic-rounding draws (param group ``sr_seed``, a uint64)
 SR_SEED = 0x5EED_B16F_0000_0001
@@ -819,6 +825,272 @@ class FusedLion(FusedArenaOptimizer):
         KERNELS.nvls_lion(self.arena.master[lo:hi], self._state("exp_avg")[lo:hi], mc_g, mc_out, hi - lo, self.nvls,
                           **self._hyper(), grad_scale=grad_scale, g_dtype=KERNELS.dtype_code(self.arena.grad.dtype),
                           dyn=self._dyn)
+
+
+# ---- Schedule-Free AdamW / SGD ----------------------------------------------------------------------
+
+def schedule_free_scalars(h: Dict[str, Any], adaptive: bool) -> Tuple[float, float, float, float, float]:
+    """The host half of a Schedule-Free update of param group ``h`` (the schedulefree package's 1.x
+    ``step()``, in double): ``(lr, ckp1, y_lr, lr_max, weight_sum)`` of the group's next update, from its
+    ``lr``, ``k`` (updates done), ``warmup_steps``, ``r``, ``weight_lr_power``, ``lr_max`` and ``weight_sum``.
+    AdamW folds Adam's bias correction sqrt(1 - beta2^(k+1)) into lr.  Pure: ``end_step`` commits the
+    last two and k + 1."""
+    k = int(h["k"])
+    warmup = int(h["warmup_steps"])
+    lr = float(h["lr"]) * ((k + 1) / warmup if k < warmup else 1.0)
+    if adaptive:
+        beta1, beta2 = float(h["betas"][0]), float(h["betas"][1])
+        lr *= (1.0 - beta2 ** (k + 1)) ** 0.5
+    else:
+        beta1 = float(h["momentum"])
+    lr_max = max(float(h["lr_max"]), lr)
+    weight = (k + 1) ** float(h["r"]) * lr_max ** float(h["weight_lr_power"])
+    weight_sum = float(h["weight_sum"]) + weight
+    ckp1 = weight / weight_sum if weight_sum != 0.0 else 0.0
+    return lr, ckp1, lr * (beta1 * (1.0 - ckp1) - 1.0), lr_max, weight_sum
+
+
+class FusedScheduleFree(FusedArenaOptimizer):
+    """Schedule-Free optimization (Defazio et al. 2024, *The Road Less Scheduled*) as the schedulefree
+    package's ``AdamWScheduleFree`` (``FusedScheduleFreeAdamW``) and ``SGDScheduleFree``
+    (``FusedScheduleFreeSGD``): the weights the model trains with are y, where gradients are taken; the
+    state ``z`` is the base AdamW / SGD iterate, a copy of y at the first update; the point to evaluate
+    at is x = lerp(y, z, 1 - 1/beta1), an online average of the z's that stands in for an lr schedule
+    and a weight EMA.  ``schedule_free_scalars`` is the host half of every update, feeding the by-value
+    arguments and the ``dyn`` rows alike; the ``frl_sf_*`` kernels (K2, K2-mt, K2-sr, grouped) the
+    element-wise half, on AdamW's / SGD-with-momentum's bytes.  ``swapped()`` puts x where the model
+    reads its weights for a block; ``eval_state_dict()`` exports x.  ``state_dict()`` is the package's
+    layout with the live y (``train_mode=True``): group ``lr``, ``betas`` / ``momentum``, ``eps`` (AdamW),
+    ``weight_decay``, ``warmup_steps``, ``r``, ``weight_lr_power``, ``k``, ``weight_sum``, ``lr_max``,
+    ``train_mode``; per parameter ``z`` (and ``exp_avg_sq``).  Every param group keeps its own ``k``,
+    ``lr_max`` and ``weight_sum``.  The model range only (criterion parameters keep y in ``swapped()``,
+    as they do under a weight EMA)."""
+
+    ADAPTIVE = False
+
+    def __init__(self, arena, defaults, param_groups=None, warmup_steps=0, r=0.0, weight_lr_power=2.0):
+        defaults.update(warmup_steps=int(warmup_steps), r=float(r), weight_lr_power=float(weight_lr_power), k=0,
+                        weight_sum=0.0, lr_max=-1.0, train_mode=True)
+        super().__init__(arena, defaults, param_groups)
+        self._swapped = False
+
+    @property
+    def beta1(self) -> float:
+        h = self.hyper
+        return float(h["betas"][0] if self.ADAPTIVE else h["momentum"])
+
+    def _kernel(self, name: str):
+        """``KERNELS.sf_adamw<name>`` or ``KERNELS.sf_sgd<name>``."""
+        return getattr(KERNELS, ("sf_adamw" if self.ADAPTIVE else "sf_sgd") + name)
+
+    def _states(self, lo: Optional[int] = None, hi: Optional[int] = None) -> Tuple[torch.Tensor, ...]:
+        names = ("z", "exp_avg_sq") if self.ADAPTIVE else ("z",)
+        return tuple(self._state(n) if lo is None else self._state(n)[lo:hi] for n in names)
+
+    def _rule(self) -> Dict[str, float]:
+        h = self.hyper
+        if self.ADAPTIVE:
+            return dict(beta1=self.beta1, beta2=float(h["betas"][1]), eps=float(h["eps"]))
+        return dict(beta1=self.beta1)
+
+    def _scalars(self) -> Dict[str, float]:
+        h = self.hyper
+        lr, ckp1 = schedule_free_scalars(h, self.ADAPTIVE)[:2]
+        return dict(lr=lr, ckp1=ckp1, wd=float(h["weight_decay"]), **self._rule())
+
+    def _dyn_row(self, h):
+        # dyn[0..2]: lr, ckp1, y_lr (the rows' column 4 is the group's weight decay)
+        return schedule_free_scalars(h, self.ADAPTIVE)[:3]
+
+    # -- stepping --------------------------------------------------------------------------------
+    @torch.no_grad()
+    def _init_z(self) -> None:
+        """z = y before the first update: the model range from the weights the model reads (the fp32
+        master, or the bf16 weights with bf16 master weights), the criterion range from the master."""
+        a = self.arena
+        z = self._state("z")
+        if a.master_base:
+            z[:a.master_base].copy_(a.lp[:a.master_base])
+        z[a.master_base:].copy_(a.master)
+
+    def begin_step(self) -> None:
+        if self._swapped:
+            raise RuntimeError("a Schedule-Free update inside swapped()")
+        if "z" not in self._vec:
+            self._init_z()
+        super().begin_step()
+
+    def end_step(self) -> None:
+        for h in self.param_groups:
+            _, _, _, h["lr_max"], h["weight_sum"] = schedule_free_scalars(h, self.ADAPTIVE)
+            h["k"] = int(h["k"]) + 1
+        super().end_step()
+
+    def _launch(self, lo, hi, grad_scale, coef):
+        p, g, lp = self._slices(lo, hi)
+        kw = dict(self._scalars(), grad_scale=grad_scale, grad_scale_dev=coef, dyn=self._dyn)
+        if self._use_sr(lo):
+            self._kernel("_sr")(p, g, *self._states(lo, hi), hi - lo, arena_off=lo, seed=self.sr_seed,
+                                t=self._steps + 1, **kw)
+            return
+        self._kernel("")(p, g, *self._states(lo, hi), lp, hi - lo, **kw)
+
+    def _launch_mt(self, table, grad_scale):
+        self._kernel("_mt")(self._master_base(), *self._states(), self._lp_mt(), table, **self._scalars(),
+                            grad_scale=grad_scale, dyn=self._dyn)
+
+    def _launch_mt_sr(self, table, grad_scale):
+        self._kernel("_mt_sr")(self.arena.lp, *self._states(), table, seed=self.sr_seed, t=self._steps + 1,
+                               **self._scalars(), grad_scale=grad_scale, dyn=self._dyn)
+
+    def _launch_mt_grouped(self, table, groups, grad_scale, coef):
+        self._kernel("_mt_grouped")(self._master_base(), *self._states(), self._lp_mt(), table, groups, **self._rule(),
+                                    grad_scale=grad_scale, grad_scale_dev=coef)
+
+    def _launch_mt_grouped_sr(self, table, groups, grad_scale, coef):
+        self._kernel("_mt_grouped_sr")(self.arena.lp, *self._states(), table, groups, seed=self.sr_seed,
+                                       **self._rule(), grad_scale=grad_scale, grad_scale_dev=coef)
+
+    def _launch_nvls(self, lo, hi, grad_scale):
+        raise RuntimeError("%s has no fused NVLS step (K7)" % type(self).__name__)
+
+    # -- the evaluation point x ------------------------------------------------------------------
+    def _y(self) -> torch.Tensor:
+        a = self.arena
+        return a.lp[:a.model_end] if a.bf16_master else a.master[:a.model_end]
+
+    @contextmanager
+    def swapped(self):
+        """The model computes with x = lerp(y, z, 1 - 1/beta1) in the model range inside the block (K2-sfx);
+        y is back, bit for bit, when it is left, also when it raises.  Fp32 master weights with a bf16
+        shadow: only the shadow is rewritten, and restored as the cast of the master every update writes.
+        Fp32 precision or bf16 master weights: x is written in place over y, which a transient copy
+        (freed on exit) keeps.  Before the first update x is y: nothing changes."""
+        if self._swapped:
+            raise RuntimeError("%s.swapped() is not reentrant" % type(self).__name__)
+        a = self.arena
+        n = a.model_end
+        if "z" not in self._vec or n == 0:
+            yield self
+            return
+        y, z = self._y(), self._state("z")[:n]
+        shadow = a.lp is not None and not a.bf16_master
+        kept = None if shadow else y.clone()
+        try:
+            KERNELS.sf_eval_weights(y, z, a.lp[:n] if shadow else y, beta1=self.beta1)
+            self._swapped = True
+            yield self
+        finally:
+            with torch.no_grad():
+                if shadow:
+                    a.lp[:n].copy_(a.master[:n])
+                else:
+                    y.copy_(kept)
+            kept = None
+            self._swapped = False
+
+    @torch.no_grad()
+    def eval_weights(self) -> torch.Tensor:
+        """x over the model range as a fresh fp32 vector (y before the first update)."""
+        y = self._y()
+        if "z" not in self._vec:
+            return y.float()
+        x = torch.empty(y.numel(), dtype=torch.float32, device=y.device)
+        KERNELS.sf_eval_weights(y, self._state("z")[:y.numel()], x, beta1=self.beta1)
+        return x
+
+    def eval_state_dict(self, module) -> Dict[str, Any]:
+        """``module``'s fp32 CPU ``state_dict()`` at x, keyed like the main checkpoint's (buffers: the live
+        ones, gathered at y): what ``<stem>.sf`` holds."""
+        from .ema import module_state_dict
+        return module_state_dict(self.arena, module, self.eval_weights())
+
+    # -- state dict ------------------------------------------------------------------------------
+    def state_dict(self) -> Dict[str, Any]:
+        if self._swapped:
+            raise RuntimeError("%s.state_dict() inside swapped()" % type(self).__name__)
+        return super().state_dict()
+
+    def load_state_dict(self, state_dict: Dict[str, Any]) -> None:
+        """A Schedule-Free state dict of the same rule only (unknown extra group keys are kept): one with
+        another optimizer's state keys, or a param group without ``k`` / ``weight_sum`` / ``lr_max`` or
+        with the other rule's ``betas`` / ``momentum``, is a ValueError naming the keys."""
+        own = {n for n, _ in self.STATE_NAMES}
+        rule = "betas" if self.ADAPTIVE else "momentum"
+        what = "AdamWScheduleFree" if self.ADAPTIVE else "SGDScheduleFree"
+        for entry in state_dict["state"].values():
+            foreign = sorted(k for k in entry if k not in own)
+            if foreign:
+                raise ValueError("a %s optimizer cannot load another optimizer's state dict (found %s; it keeps %s)"
+                                 % (what, foreign, sorted(own)))
+        for g in state_dict["param_groups"]:
+            if not {"k", "weight_sum", "lr_max", rule} <= set(g):
+                raise ValueError("a %s optimizer cannot load another optimizer's state dict (param group keys %s; "
+                                 "its group has k, weight_sum, lr_max and %s)"
+                                 % (what, sorted(k for k in g if k != "params"), rule))
+        super().load_state_dict(state_dict)
+        for g in self.param_groups:
+            g["k"] = int(g["k"])
+            g["train_mode"] = True
+            if self.ADAPTIVE:
+                g["betas"] = tuple(g["betas"])
+        self._steps = int(self.param_groups[0]["k"])
+
+
+class FusedScheduleFreeAdamW(FusedScheduleFree):
+    """``schedulefree.AdamWScheduleFree``: Adam's normalised step (no first moment: z and y carry the
+    momentum) with decoupled decay taken at y, on AdamW's state size (``z``, ``exp_avg_sq``)."""
+
+    ADAPTIVE = True
+    STATE_NAMES = (("z", "z"), ("exp_avg_sq", "exp_avg_sq"))
+
+    def __init__(self, arena, lr, betas=(0.9, 0.999), eps=1e-8, weight_decay=0.0, warmup_steps=0, r=0.0,
+                 weight_lr_power=2.0, param_groups=None):
+        super().__init__(arena, dict(lr=lr, betas=tuple(betas), eps=eps, weight_decay=weight_decay), param_groups,
+                         warmup_steps, r, weight_lr_power)
+
+
+class FusedScheduleFreeSGD(FusedScheduleFree):
+    """``schedulefree.SGDScheduleFree``: the gradient step on z, with ``momentum`` (in (0, 1)) as beta1, on
+    SGD-with-momentum's state size (``z``)."""
+
+    STATE_NAMES = (("z", "z"),)
+
+    def __init__(self, arena, lr, momentum=0.9, weight_decay=0.0, warmup_steps=0, r=0.0, weight_lr_power=2.0,
+                 param_groups=None):
+        super().__init__(arena, dict(lr=lr, momentum=momentum, weight_decay=weight_decay), param_groups,
+                         warmup_steps, r, weight_lr_power)
+
+
+def check_schedule_free(optim_opts: OptimOpts, layer_adaptation: LayerAdaptation, optimizer_state: OptimizerState,
+                        adafactor: bool, muon: bool, adamw: bool, lion: bool, ema: bool, schedule_free) -> None:
+    """Schedule-Free needs Adam without amsgrad (SF-AdamW) or SGD with momentum in (0, 1) (SF-SGD), no layer
+    adaptation, fp32 optimizer state, and none of Adafactor, Muon, ``adamw`` (SF-AdamW's decay is already
+    decoupled), Lion and a weight EMA (both want the held-out evaluation); anything else is a ValueError
+    naming the values."""
+    if not schedule_free:
+        return
+    algo = getattr(optim_opts.algo, "value", optim_opts.algo)
+    why = None
+    if optim_opts.algo not in (OptAlgorithm.ADAM, OptAlgorithm.SGD):
+        why = "optimizer %r (schedule_free needs adam or sgd)" % algo
+    elif optim_opts.algo == OptAlgorithm.ADAM and optim_opts.amsgrad:
+        why = "amsgrad"
+    elif optim_opts.algo == OptAlgorithm.SGD and not 0.0 < optim_opts.momentum < 1.0:
+        why = "sgd momentum %r (its beta1 must lie in (0, 1))" % (optim_opts.momentum,)
+    elif LayerAdaptation(layer_adaptation) is not LayerAdaptation.NONE:
+        why = "layer adaptation %r" % LayerAdaptation(layer_adaptation).value
+    elif OptimizerState(optimizer_state) is not OptimizerState.FP32:
+        why = "optimizer state %r" % OptimizerState(optimizer_state).value
+    else:
+        for flag, name in ((adafactor, "adafactor"), (muon, "muon"), (adamw, "adamw (its decay is already "
+                                                                             "decoupled)"),
+                           (lion, "lion"), (ema, "a weight EMA (both evaluate held-out splits at other weights)")):
+            if flag:
+                why = name
+                break
+    if why is not None:
+        raise ValueError("schedule_free cannot be combined with %s" % why)
 
 
 def is_adapted(slot) -> bool:
@@ -1632,8 +1904,8 @@ def create_fused_optimizer(arena: ParamArena, optim_opts: OptimOpts,
                            layer_adaptation: LayerAdaptation = LayerAdaptation.NONE,
                            optimizer_state: OptimizerState = OptimizerState.FP32,
                            adafactor: bool = False, muon: bool = False, adamw: bool = False,
-                           lion: bool = False, param_groups: Optional[List[Dict[str, Any]]] = None
-                           ) -> FusedArenaOptimizer:
+                           lion: bool = False, param_groups: Optional[List[Dict[str, Any]]] = None,
+                           schedule_free=None) -> FusedArenaOptimizer:
     """Same dispatch and argument mapping as the reference's ``_create_optimizer``; with a layer
     adaptation, its LARS / LAMB counterpart; with 8-bit optimizer state, ``FusedAdam8bit``; with
     ``adafactor``, ``FusedAdafactor`` (``lr`` caps the relative step, ``weightDecay`` is its
@@ -1642,7 +1914,10 @@ def create_fused_optimizer(arena: ParamArena, optim_opts: OptimOpts,
     ``adamw``, the Adam rule of whichever of ``FusedAdam``, ``FusedAdam8bit`` or ``FusedMuon`` is
     chosen takes decoupled weight decay (``torch.optim.AdamW``); with ``lion``, ``FusedLion`` (``momentum``
     is beta1, beta2 is 0.99, ``weightDecay`` its decoupled decay).  ``param_groups``: the canonical groups
-    of ``resolve_param_groups`` (SGD, Adam / AdamW, RMSprop and Lion only)."""
+    of ``resolve_param_groups`` (SGD, Adam / AdamW, RMSprop, Lion and Schedule-Free only).  ``schedule_free``:
+    a ``types.ScheduleFree`` (or True for its defaults) makes Adam ``FusedScheduleFreeAdamW`` (betas (0.9,
+    0.999), ``epsilon``) and SGD ``FusedScheduleFreeSGD`` (``momentum`` is beta1); ``weightDecay`` is the
+    decay taken at y."""
     check_layer_adaptation(optim_opts, layer_adaptation)
     check_optimizer_state(optim_opts, layer_adaptation, optimizer_state)
     check_adafactor(optim_opts, layer_adaptation, optimizer_state, adafactor)
@@ -1650,6 +1925,8 @@ def create_fused_optimizer(arena: ParamArena, optim_opts: OptimOpts,
     check_adamw(optim_opts, layer_adaptation, optimizer_state, adafactor, adamw)
     check_lion(optim_opts, layer_adaptation, lion)
     check_param_groups(layer_adaptation, optimizer_state, adafactor, muon, param_groups is not None)
+    check_schedule_free(optim_opts, layer_adaptation, optimizer_state, adafactor, muon, adamw, lion, False,
+                        schedule_free)
     check_master_weights(getattr(arena, "master_weights", MasterWeights.FP32), arena.precision, layer_adaptation,
                          optimizer_state, adafactor, muon)
     if muon:
@@ -1666,6 +1943,14 @@ def create_fused_optimizer(arena: ParamArena, optim_opts: OptimOpts,
     if layer_adaptation == LayerAdaptation.LAMB:
         return FusedLamb(arena, lr=optim_opts.lr, weight_decay=optim_opts.weightDecay, eps=optim_opts.epsilon)
     algo = optim_opts.algo
+    if schedule_free:
+        sf = ScheduleFree() if schedule_free is True else schedule_free
+        kw = dict(warmup_steps=sf.warmup_steps, r=sf.r, weight_lr_power=sf.weight_lr_power, param_groups=param_groups)
+        if algo == OptAlgorithm.ADAM:
+            return FusedScheduleFreeAdamW(arena, lr=optim_opts.lr, eps=optim_opts.epsilon,
+                                          weight_decay=optim_opts.weightDecay, **kw)
+        return FusedScheduleFreeSGD(arena, lr=optim_opts.lr, momentum=optim_opts.momentum,
+                                    weight_decay=optim_opts.weightDecay, **kw)
     if algo == OptAlgorithm.RMSPROP:
         return FusedRMSprop(arena, lr=optim_opts.lr, momentum=optim_opts.momentum,
                             weight_decay=optim_opts.weightDecay, param_groups=param_groups)

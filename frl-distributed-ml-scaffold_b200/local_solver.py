@@ -29,7 +29,8 @@ class LocalSolver:
               adamw: Optional[bool] = None,
               channels_last: Optional[bool] = None,
               master_weights: Optional[MasterWeights] = None,
-              lion: Optional[bool] = None, no_decay_1d: Optional[bool] = None) -> PerformanceSummary:
+              lion: Optional[bool] = None, no_decay_1d: Optional[bool] = None,
+              schedule_free=None) -> PerformanceSummary:
         if save_notebook:
             logger.warning("save_notebook is not supported by frl_b200 (visualisation only)")
         # a stale rendezvous file from a crashed run would poison the file:// store
@@ -45,6 +46,6 @@ class LocalSolver:
                                  grad_accumulation=grad_accumulation, ema_decay=ema_decay,
                                  optimizer_state=optimizer_state, adafactor=adafactor, muon=muon,
                                  adamw=adamw, channels_last=channels_last, master_weights=master_weights,
-                                 lion=lion, no_decay_1d=no_decay_1d):
+                                 lion=lion, no_decay_1d=no_decay_1d, schedule_free=schedule_free):
             pass
         return last

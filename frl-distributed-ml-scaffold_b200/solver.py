@@ -29,7 +29,8 @@ import torch.nn as nn
 from .arena import ParamArena
 from .criteria import BaseParallelCriterion
 from .ema import EMA_STATE_KEY
-from .fused_optim import (FusedAdafactor, FusedAdam8bit, FusedLion, FusedMuon, check_adafactor, check_adamw, check_lion, check_muon, check_layer_adaptation, check_master_weights, check_optimizer_state, check_param_groups,
+from .fused_optim import (FusedAdafactor, FusedAdam8bit, FusedLion, FusedMuon, FusedScheduleFree,
+                          FusedScheduleFreeAdamW, SF_STATE_KEY, check_schedule_free, check_adafactor, check_adamw, check_lion, check_muon, check_layer_adaptation, check_master_weights, check_optimizer_state, check_param_groups,
                           create_fused_optimizer, is_adapted, no_decay_1d_groups, resolve_param_groups)
 from .grad_sync import BufferBroadcaster, GradBucketPipeline
 from .lr_scheduler import DropEpochsScheduler, WarmupMultiStepLR
@@ -37,7 +38,7 @@ from .problem import Problem
 from .solver_worker import (FractionalPerformanceSummary, SerializableSampleSummary,
                             SolverWorker)
 from .types import (Device, LayerAdaptation, LRSchedulerAlgorithm, MasterWeights, Mode, OptimizerState, Precision, RunOpts,
-                    SampleSummary, Split)
+                    SampleSummary, ScheduleFree, Split)
 
 logging.basicConfig(level=logging.INFO, format="%(levelname)s (%(process)d) %(message)s")
 logger = logging.getLogger(__name__)
@@ -53,6 +54,9 @@ MUON_ENV = "FRL_B200_MUON"                         # "0" (default) | "1"
 ADAMW_ENV = "FRL_B200_ADAMW"                       # "0" (default) | "1"
 LION_ENV = "FRL_B200_LION"                         # "0" (default) | "1"
 NO_DECAY_1D_ENV = "FRL_B200_NO_DECAY_1D"           # "0" (default) | "1"
+SCHEDULE_FREE_ENV = "FRL_B200_SCHEDULE_FREE"       # "0" (default) | "1"
+SCHEDULE_FREE_WARMUP_ENV = "FRL_B200_SCHEDULE_FREE_WARMUP"   # integer >= 0 (default 0)
+SF_SUFFIX = ".sf"                                  # <stem>.sf: the Schedule-Free evaluation weights
 CHANNELS_LAST_ENV = "FRL_B200_CHANNELS_LAST"       # "0" (default) | "1"
 MASTER_WEIGHTS_ENV = "FRL_B200_MASTER_WEIGHTS"     # "fp32" (default) | "bf16"
 EMA_SUFFIX = ".ema"                        # <checkpoint>.ema: the weight EMA next to a checkpoint
@@ -108,6 +112,9 @@ class SolverWorkerArgs(NamedTuple):
     precision: Precision = Precision.FP32
     save_every: int = 1
     graph_step: Optional[bool] = None      # None: FRL_B200_CUDA_GRAPH (default off)
+    # Schedule-Free AdamW / SGD settings, None for off; placed before layer_adaptation, so every field from
+    # layer_adaptation to the end keeps its order and its position counted from the end of the tuple
+    schedule_free: Optional[ScheduleFree] = None
     layer_adaptation: LayerAdaptation = LayerAdaptation.NONE
     # no weight decay on parameters with ndim <= 1; None: FRL_B200_NO_DECAY_1D, read when the worker is
     # built.  Placed before lion, so every field from lion to the end keeps its order and its position
@@ -346,6 +353,36 @@ def resolve_no_decay_1d(explicit: Optional[bool] = None) -> bool:
     return raw == "1"
 
 
+def resolve_schedule_free(explicit=None) -> Optional[ScheduleFree]:
+    """The Schedule-Free settings of a run, or None for off: ``explicit`` (``True``, ``False`` or a
+    ``types.ScheduleFree``), else FRL_B200_SCHEDULE_FREE (``0``, the default, or ``1``) with
+    FRL_B200_SCHEDULE_FREE_WARMUP (an integer >= 0, default 0) as ``warmup_steps``.  Any other value is a
+    ValueError naming the variable or the argument."""
+    if explicit is None:
+        raw = os.environ.get(SCHEDULE_FREE_ENV, "0").strip()
+        if raw not in ("0", "1"):
+            raise ValueError("%s must be 0 or 1, got %r" % (SCHEDULE_FREE_ENV, raw))
+        if raw == "0":
+            return None
+        raw = os.environ.get(SCHEDULE_FREE_WARMUP_ENV, "0").strip()
+        if not raw.isdigit():
+            raise ValueError("%s must be an integer >= 0, got %r" % (SCHEDULE_FREE_WARMUP_ENV, raw))
+        return ScheduleFree(warmup_steps=int(raw))
+    if explicit is False:
+        return None
+    if explicit is True:
+        return ScheduleFree()
+    if not isinstance(explicit, ScheduleFree):
+        raise ValueError("schedule_free=%r: pass True, False or a types.ScheduleFree" % (explicit,))
+    w, r, p = explicit
+    if isinstance(w, bool) or not isinstance(w, (int, np.integer)) or w < 0:
+        raise ValueError("schedule_free: warmup_steps=%r must be an integer >= 0" % (w,))
+    for name, v in (("r", r), ("weight_lr_power", p)):
+        if isinstance(v, bool) or not isinstance(v, (int, float, np.integer, np.floating)) or not math.isfinite(v):
+            raise ValueError("schedule_free: %s=%r must be a finite real number" % (name, v))
+    return ScheduleFree(int(w), float(r), float(p))
+
+
 def has_param_group_hook(problem) -> bool:
     """True if ``problem`` defines ``get_param_groups`` other than the base class's (which returns None);
     a reference Problem subclass has none."""
@@ -395,6 +432,23 @@ def describe_param_groups(optimizer) -> str:
         return "none"
     return "%d: %s (grouped K2-mt)" % (len(optimizer.param_groups), ", ".join(
         "%d tensors, lr %r, wd %r" % (len(g["params"]), g["lr"], g["weight_decay"]) for g in optimizer.param_groups))
+
+
+def describe_schedule_free(optimizer, model: nn.Module) -> str:
+    """The INFO line's optimizer field under Schedule-Free: the rule, its settings and the kernels taken,
+    and a warning when the model has floating buffers (BatchNorm statistics are not recomputed at x)."""
+    h = optimizer.hyper
+    adaptive = isinstance(optimizer, FusedScheduleFreeAdamW)
+    name = "sf_adamw" if adaptive else "sf_sgd"
+    kernels = ("frl_%s_sr / frl_%s_mt_sr, K2-sr" % (name, name) if optimizer.sr else
+               "frl_%s / frl_%s_mt, K2 / K2-mt" % (name, name))
+    if optimizer.grouped:
+        kernels = "frl_%s_mt_grouped%s, grouped K2-mt" % (name, "_sr" if optimizer.sr else "")
+    text = "schedule-free %s, beta1 %r, warmup_steps %d, r %r, weight_lr_power %r (%s; held-out splits at x, K2-sfx)" % (
+        "adamw" if adaptive else "sgd", optimizer.beta1, h["warmup_steps"], h["r"], h["weight_lr_power"], kernels)
+    if any(b.is_floating_point() for b in model.buffers()):
+        text += "; WARNING: BatchNorm statistics are not recomputed at x, held-out splits use those gathered at y"
+    return text
 
 
 def resolve_channels_last(explicit: Optional[bool] = None) -> bool:
@@ -542,8 +596,9 @@ class Solver:
         # world > 1 without clipping: arena vectors other ranks reach go to symmetric/multicast
         # memory so all-reduce + update + broadcast can be one NVLS kernel per bucket
         ema_decay = args.ema_decay if run_opts.mode == Mode.TRAIN else 0.0
+        schedule_free = args.schedule_free if run_opts.mode == Mode.TRAIN else None
         symm_alloc = None
-        if (distributed and not run_opts.optim.gradientClip
+        if (distributed and not run_opts.optim.gradientClip and schedule_free is None
                 and args.layer_adaptation == LayerAdaptation.NONE and accum == 1 and ema_decay == 0.0
                 and args.optimizer_state is OptimizerState.FP32 and not args.adafactor and not args.muon
                 and not (MasterWeights(args.master_weights) is MasterWeights.BF16 and run_opts.mode == Mode.TRAIN)):
@@ -576,8 +631,10 @@ class Solver:
         param_groups = None
         if run_opts.mode == Mode.TRAIN:
             param_groups = problem_param_groups(problem, model, criterion, resolve_no_decay_1d(args.no_decay_1d))
+        check_schedule_free(run_opts.optim, args.layer_adaptation, opt_state, adafactor, muon, adamw, lion,
+                            ema_decay > 0.0, schedule_free)
         optimizer = create_fused_optimizer(arena, run_opts.optim, args.layer_adaptation, opt_state, adafactor,
-                                           muon, adamw, lion, param_groups)
+                                           muon, adamw, lion, param_groups, schedule_free)
         if checkpoint:
             optimizer.load_state_dict(checkpoint.optimizerState)
         ema = None
@@ -679,7 +736,9 @@ class Solver:
                         "frl_lion_sr / frl_lion_mt_sr, K2-sr" if optimizer.sr else "frl_lion / frl_lion_mt, K2 / K2-mt"))
                     if pipeline.fused_dw_update else
                     "frl_lion_sr / frl_lion_mt_sr, K2-sr" if optimizer.sr else "frl_lion / frl_lion_mt, K2 / K2-mt")
-                if isinstance(optimizer, FusedLion) else getattr(run_opts.optim.algo, "value", run_opts.optim.algo),
+                if isinstance(optimizer, FusedLion) else
+                describe_schedule_free(optimizer, model) if isinstance(optimizer, FusedScheduleFree) else
+                getattr(run_opts.optim.algo, "value", run_opts.optim.algo),
                 "8-bit block-wise (K2-q8), %.1f MiB instead of %.1f MiB" % (
                     optimizer.state_bytes / 2 ** 20, optimizer.fp32_state_bytes / 2 ** 20)
                 if isinstance(optimizer, FusedAdam8bit) else
@@ -833,6 +892,7 @@ class Solver:
         model = _torch_load(io.BytesIO(donor.modelBuffer), map_location="cpu")
         optimizer_state = _torch_load(io.BytesIO(donor.optimizerStateBuffer), map_location="cpu")
         ema = optimizer_state.pop(EMA_STATE_KEY, None)       # the main checkpoint keeps its format
+        sf_x = optimizer_state.pop(SF_STATE_KEY, None)
 
         logger.info("==> saving checkpoint to %s", str(save_dir))
         stem = os.path.join(save_dir, base_filename)
@@ -850,6 +910,9 @@ class Solver:
                 with open(stem + EMA_SUFFIX, "wb") as f_ema:
                     torch.save({"epoch": epoch, "decay": ema["decay"], "updates": ema["updates"],
                                 "state_dict": ema["state_dict"]}, f_ema)
+            if sf_x is not None:
+                with open(stem + SF_SUFFIX, "wb") as f_sf:
+                    torch.save({"epoch": epoch, "state_dict": sf_x}, f_sf)
 
     # ------------------------------------------------------------------------------------------
     # parent side: collecting per-epoch results from the ranks
@@ -917,7 +980,8 @@ class Solver:
               channels_last: Optional[bool] = None,
               master_weights: Optional[MasterWeights] = None,
               lion: Optional[bool] = None,
-              no_decay_1d: Optional[bool] = None
+              no_decay_1d: Optional[bool] = None,
+              schedule_free=None
               ) -> Iterator[PerformanceSummary]:
         """The reference's entry point (solver.py:728-739) plus two keyword-only extensions:
 
@@ -1084,6 +1148,26 @@ class Solver:
                        (host RNG state restored), and a ``get_model`` that touches CUDA there makes the
                        ranks spawn rather than fork.  None: FRL_B200_NO_DECAY_1D (``0`` by default, ``1`` to enable); any
                        other value raises ``ValueError``.  ``Mode.EVAL`` ignores groups.
+        ``schedule_free``  True or a ``types.ScheduleFree(warmup_steps=0, r=0.0, weight_lr_power=2.0)``:
+                       Schedule-Free optimization (Defazio et al. 2024, the schedulefree package's
+                       ``AdamWScheduleFree`` with ``OptAlgorithm.ADAM``, betas (0.9, 0.999) and ``epsilon``;
+                       ``SGDScheduleFree`` with ``OptAlgorithm.SGD``, whose ``momentum`` in (0, 1) is beta1).
+                       Training moves y, where gradients are taken, and z, the base AdamW / SGD iterate;
+                       every split other than ``Split.TRAIN`` of a TRAIN run is evaluated at x = lerp(y, z,
+                       1 - 1/beta1), the online average of the z's (K2-sfx; y comes back bit for bit).
+                       ``weightDecay`` is taken at y.  The per-epoch schedule still scales each group's lr,
+                       and the averaging follows it through lr_max.  Param groups, BF16 / FP8 / FP32, bf16
+                       master weights, clipping, accumulation, channels_last and graph replay work; the
+                       fused NVLS step (K7) and the dW-GEMM update (K12) are off.  Checkpoints hold the
+                       live y and the package's state dict (``z``, ``exp_avg_sq``, group ``k``, ``lr_max``,
+                       ``weight_sum``, ...), so a resume continues bit for bit; ``<stem>.sf`` next to every
+                       checkpoint holds ``{"epoch", "state_dict"}`` at x, so ``initialModelPath=<stem>.sf``
+                       with ``Mode.EVAL`` evaluates the Schedule-Free model.  BatchNorm statistics are the
+                       ones gathered at y.  RMSprop, amsgrad, LARS / LAMB, 8-bit state, Adafactor, Muon,
+                       ``adamw``, ``lion``, a weight EMA and SGD momentum outside (0, 1) raise ``ValueError``
+                       before a rank starts.  None: FRL_B200_SCHEDULE_FREE (``0`` by default, ``1`` to
+                       enable) with FRL_B200_SCHEDULE_FREE_WARMUP (an integer >= 0) as ``warmup_steps``;
+                       any other value raises ``ValueError``.  ``Mode.EVAL`` ignores it.
         """
         adapt = LayerAdaptation.NONE
         accum = 1
@@ -1094,6 +1178,7 @@ class Solver:
         use_adamw = False
         use_lion = False
         use_no_decay_1d = False
+        use_schedule_free = None
         if run_opts.mode == Mode.TRAIN:
             adapt = resolve_layer_adaptation(layer_adaptation)
             check_layer_adaptation(run_opts.optim, adapt)
@@ -1111,6 +1196,9 @@ class Solver:
             validate_param_groups(problem, use_no_decay_1d, adapt, opt_state, use_adafactor, use_muon)
             accum = resolve_grad_accumulation(grad_accumulation)
             decay = resolve_ema_decay(ema_decay)
+            use_schedule_free = resolve_schedule_free(schedule_free)
+            check_schedule_free(run_opts.optim, adapt, opt_state, use_adafactor, use_muon, use_adamw, use_lion,
+                                decay > 0.0, use_schedule_free)
         use_channels_last = resolve_channels_last(channels_last)
         check_channels_last(use_channels_last, use_adafactor)
         use_master = MasterWeights.FP32
@@ -1158,7 +1246,7 @@ class Solver:
                 layer_adaptation=adapt, grad_accumulation=accum, ema_decay=decay,
                 optimizer_state=opt_state, adafactor=use_adafactor, muon=use_muon, adamw=use_adamw,
                 channels_last=use_channels_last, master_weights=use_master, lion=use_lion,
-                no_decay_1d=use_no_decay_1d)
+                no_decay_1d=use_no_decay_1d, schedule_free=use_schedule_free)
             if not run_opts.singleThreaded:
                 parent_conn, child_conn = ctx.Pipe(duplex=False)
                 proc = ctx.Process(target=cls._solver_worker_process,

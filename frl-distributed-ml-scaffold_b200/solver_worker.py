@@ -36,7 +36,7 @@ from . import _native
 from .arena import ParamArena
 from .criteria import BaseParallelCriterion, GradNormWeightedCriterion
 from .ema import EMA_STATE_KEY
-from .fused_optim import FusedArenaOptimizer
+from .fused_optim import SF_STATE_KEY, FusedArenaOptimizer, FusedScheduleFree
 from .grad_sync import BufferBroadcaster, GradBucketPipeline, accumulation_plan
 from .model import MultiTaskModel
 from .problem import BatchMetrics, Ordering, Problem
@@ -680,9 +680,12 @@ class SolverWorker:
                 plan = accumulation_plan(n_batches, self.pipeline.accumulation, loader.batch_size,
                                          len(loader.sampler))
             log = LossLog(n_tasks, n_batches, self.device)
-            # with a weight EMA, the splits a TRAIN run only evaluates run on the averaged weights
-            weights = (self.ema.swapped() if self.ema is not None and mode == Mode.TRAIN
-                       and data_type != Split.TRAIN else nullcontext())
+            # with a weight EMA, the splits a TRAIN run only evaluates run on the averaged weights; under
+            # Schedule-Free, at its evaluation point x
+            held_out = mode == Mode.TRAIN and data_type != Split.TRAIN
+            weights = (self.ema.swapped() if self.ema is not None and held_out else
+                       self.optimizer.swapped() if isinstance(self.optimizer, FusedScheduleFree) and held_out
+                       else nullcontext())
             checked = 0
             batch_start = time.time()
             mark("setup done")
@@ -956,6 +959,9 @@ class SolverWorker:
                 if self.ema is not None:
                     # travels to the parent with the optimizer state, which writes it to <stem>.ema
                     state[EMA_STATE_KEY] = self.ema.state_dict()
+                if isinstance(self.optimizer, FusedScheduleFree):
+                    # travels to the parent with the optimizer state, which writes it to <stem>.sf
+                    state[SF_STATE_KEY] = self.optimizer.eval_state_dict(self.model)
                 torch.save(state, buf)
                 optim_bytes = buf.getvalue()
             self.model.train(was_training)

@@ -164,6 +164,20 @@ class MasterWeights(Enum):
     BF16 = "bf16"
 
 
+class ScheduleFree(NamedTuple):
+    """Extension (not in the reference): the settings of Schedule-Free optimization (Defazio et al.
+    2024, *The Road Less Scheduled*), chosen with ``Solver.solve(..., schedule_free=ScheduleFree(...))``
+    (``True`` for these defaults) or ``FRL_B200_SCHEDULE_FREE`` / ``FRL_B200_SCHEDULE_FREE_WARMUP``.
+
+    warmup_steps     - updates over which lr ramps linearly up, (k+1)/warmup_steps, then stays flat
+    r, weight_lr_power - the averaging weight of update k is (k+1)^r * lr_max^weight_lr_power (the
+                       schedulefree package's defaults 0 and 2)
+    """
+    warmup_steps: int = 0
+    r: float = 0.0
+    weight_lr_power: float = 2.0
+
+
 # --- records ---------------------------------------------------------------------------------
 
 class SampleSummary(NamedTuple):

@@ -363,6 +363,80 @@ int frl_rmsprop_mt_grouped_sr(void* p, float* sq, float* buf, const frl_grad_seg
                               int n_groups, uint64_t seed, double alpha, double eps, double mu, double grad_scale,
                               const float* grad_scale_dev, void* stream);
 
+/* Schedule-Free AdamW and SGD (Defazio et al. 2024, The Road Less Scheduled; the schedulefree
+ * package's 1.x step with Adam's bias correction folded into lr).  p is y, the point gradients are
+ * taken at; z (non-NULL, fp32) is the base iterate, a copy of y before the first update; AdamW also
+ * keeps v = exp_avg_sq (non-NULL).  Twelve update entry points, each with its AdamW (frl_sf_adamw*) or
+ * SGD (frl_sf_sgd*) sibling's arguments with (lr, ckp1, beta1) in place of the step count / momentum:
+ * frl_sf_{adamw,sgd} (K2), _mt (K2-mt), _mt_grouped, _sr and _mt_sr (K2-sr, bf16 y), _mt_grouped_sr.
+ * The caller forms per update, in double (k = updates done, 0-based):
+ *     lr   = group lr * warm-up factor (* sqrt(1 - beta2^(k+1)) for AdamW)
+ *     ckp1 = weight / weight_sum,  weight = (k+1)^r * lr_max^weight_lr_power,  lr_max = running max of lr
+ * and the kernel forms y_lr = lr*(beta1*(1 - ckp1) - 1) in double.  Per element, in fp32, g the scaled
+ * gradient:
+ *     AdamW: v = fmaf((1-beta2)*g, g, beta2*v) ; u = g / (sqrt(v) + eps)      SGD: u = g
+ *     u = fmaf(wd, y, u)                   decay taken at y
+ *     y = lerp(y, z, ckp1)                 torch's lerp formula, both branches
+ *     y = fmaf(y_lr, u, y) ; z = fmaf(-lr, u, z)
+ * Bytes moved per parameter are AdamW's (28 B) and SGD-with-momentum's (20 B).  dyn (may be NULL):
+ * dyn[0] = lr, dyn[1] = ckp1, dyn[2] = y_lr, and for the _sr forms dyn[3] = t; grouped rows carry the
+ * same columns 0-3 and wd in column 4 (the grouped forms take beta1 for the check only).  beta1 must lie
+ * in (0, 1) (FRL_E_ARG); every argument check is made before any launch; graph-capturable. */
+int frl_sf_adamw(float* y, const void* g, float* z, float* v, void* p_lp, int64_t n, double lr, double ckp1,
+                 double beta1, double beta2, double eps, double wd, double grad_scale, const float* grad_scale_dev,
+                 const float* dyn, int g_dtype, void* stream);
+int frl_sf_sgd(float* y, const void* g, float* z, void* p_lp, int64_t n, double lr, double ckp1, double beta1,
+               double wd, double grad_scale, const float* grad_scale_dev, const float* dyn, int g_dtype,
+               void* stream);
+int frl_sf_adamw_mt(float* y, float* z, float* v, void* p_lp, const frl_grad_seg* segs_dev,
+                    const int64_t* tile_prefix_dev, const int32_t* tile_seg_dev, int64_t n_tiles, double lr,
+                    double ckp1, double beta1, double beta2, double eps, double wd, double grad_scale,
+                    const float* grad_scale_dev, const float* dyn, void* stream);
+int frl_sf_sgd_mt(float* y, float* z, void* p_lp, const frl_grad_seg* segs_dev, const int64_t* tile_prefix_dev,
+                  const int32_t* tile_seg_dev, int64_t n_tiles, double lr, double ckp1, double beta1, double wd,
+                  double grad_scale, const float* grad_scale_dev, const float* dyn, void* stream);
+int frl_sf_adamw_mt_grouped(float* y, float* z, float* v, void* p_lp, const frl_grad_seg* segs_dev,
+                            const int64_t* tile_prefix_dev, const int32_t* tile_seg_dev, int64_t n_tiles,
+                            const int32_t* seg_group_dev, const int32_t* seg_flags_dev, const float* group_dyn,
+                            int n_groups, double beta1, double beta2, double eps, double grad_scale,
+                            const float* grad_scale_dev, void* stream);
+int frl_sf_sgd_mt_grouped(float* y, float* z, void* p_lp, const frl_grad_seg* segs_dev,
+                          const int64_t* tile_prefix_dev, const int32_t* tile_seg_dev, int64_t n_tiles,
+                          const int32_t* seg_group_dev, const int32_t* seg_flags_dev, const float* group_dyn,
+                          int n_groups, double beta1, double grad_scale, const float* grad_scale_dev, void* stream);
+int frl_sf_adamw_sr(void* y, const void* g, float* z, float* v, int64_t n, int64_t arena_off, uint64_t seed,
+                    int64_t t, double lr, double ckp1, double beta1, double beta2, double eps, double wd,
+                    double grad_scale, const float* grad_scale_dev, const float* dyn, int g_dtype, void* stream);
+int frl_sf_sgd_sr(void* y, const void* g, float* z, int64_t n, int64_t arena_off, uint64_t seed, int64_t t,
+                  double lr, double ckp1, double beta1, double wd, double grad_scale, const float* grad_scale_dev,
+                  const float* dyn, int g_dtype, void* stream);
+int frl_sf_adamw_mt_sr(void* y, float* z, float* v, const frl_grad_seg* segs_dev, const int64_t* tile_prefix_dev,
+                       const int32_t* tile_seg_dev, int64_t n_tiles, uint64_t seed, int64_t t, double lr,
+                       double ckp1, double beta1, double beta2, double eps, double wd, double grad_scale,
+                       const float* grad_scale_dev, const float* dyn, void* stream);
+int frl_sf_sgd_mt_sr(void* y, float* z, const frl_grad_seg* segs_dev, const int64_t* tile_prefix_dev,
+                     const int32_t* tile_seg_dev, int64_t n_tiles, uint64_t seed, int64_t t, double lr, double ckp1,
+                     double beta1, double wd, double grad_scale, const float* grad_scale_dev, const float* dyn,
+                     void* stream);
+int frl_sf_adamw_mt_grouped_sr(void* y, float* z, float* v, const frl_grad_seg* segs_dev,
+                               const int64_t* tile_prefix_dev, const int32_t* tile_seg_dev, int64_t n_tiles,
+                               const int32_t* seg_group_dev, const int32_t* seg_flags_dev, const float* group_dyn,
+                               int n_groups, uint64_t seed, double beta1, double beta2, double eps,
+                               double grad_scale, const float* grad_scale_dev, void* stream);
+int frl_sf_sgd_mt_grouped_sr(void* y, float* z, const frl_grad_seg* segs_dev, const int64_t* tile_prefix_dev,
+                             const int32_t* tile_seg_dev, int64_t n_tiles, const int32_t* seg_group_dev,
+                             const int32_t* seg_flags_dev, const float* group_dyn, int n_groups, uint64_t seed,
+                             double beta1, double grad_scale, const float* grad_scale_dev, void* stream);
+
+/* K2-sfx: the Schedule-Free evaluation weights x = lerp(y, z, c), c = fp32(1 - 1/beta1) formed in
+ * double, torch's lerp formula (the package's optimizer.eval()), over n elements.  y is fp32 or bf16
+ * (y_dtype), z fp32, x fp32 or bf16 rounded to nearest even (x_dtype); x may be y itself when the dtypes
+ * match (in place).  fp32 y -> bf16 x writes the shadow of an fp32-master run; the in-place forms need
+ * the caller to have stashed y.  beta1 in (0, 1); fp32 vectors and z 16-byte, bf16 vectors 8-byte
+ * aligned; every check before the launch; graph-capturable. */
+int frl_sf_eval_weights(const void* y, int y_dtype, const float* z, void* x, int x_dtype, int64_t n, double beta1,
+                        void* stream);
+
 /* ------------------------------------------------------------------------------------------
  * K2-lw — layer-wise adaptive updates over a segment table (an extension: the reference offers
  * SGD, Adam and RMSprop only).  LARS (You et al. 2017) is layer adaptation on the SGD rule, LAMB

@@ -1,7 +1,7 @@
 #!/usr/bin/env python
 """Micro-benchmark of every hand-written kernel at the BASELINE shapes (1 GPU).
 
-    python tools/kernel_bench.py [--only k2,k2lw,k2q8,k2af,k2w,k2lion,k2g,k3,k5a,k5nhwc,k13,k14,...] [--iters 20] [--json out.json]
+    python tools/kernel_bench.py [--only k2,k2lw,k2q8,k2af,k2w,k2lion,k2sf,k2g,k3,k5a,k5nhwc,k13,k14,...] [--iters 20] [--json out.json]
 
 Each kernel is timed with CUDA events on the launching stream over ROTATING operand sets whose
 total size exceeds the 50 MB L2 (so every launch streams from HBM), after 3 warm-up launches.
@@ -367,6 +367,80 @@ def bench_k2lion(iters):
                "within_3pct": med["lion"] <= 1.03 * med["sgd"],
                "lion_TBps": round(lion_tbs, 3), "lion_frac_of_3.35TBps": round(lion_tbs / 3.35, 3),
                "at_least_0.83": lion_tbs / 3.35 >= 0.83}
+    print(json.dumps(summary), flush=True)
+    out.append(summary)
+    return out
+
+
+def bench_k2sf(iters):
+    """Schedule-Free on the headline MLP's arena (``bench_k2lion``'s 10 tensors, 54.7 M parameters), bf16
+    gradients in the arena, bf16 shadow, each launch timed from a CUDA graph with the arena far larger than
+    L2: K2-mt SF-AdamW (``frl_sf_adamw_mt``) beside K2-mt AdamW (``frl_adamw_mt``), 28 B/param each, and
+    K2-mt SF-SGD (``frl_sf_sgd_mt``) beside K2-mt SGD with momentum, 20 B/param each; five rounds, the
+    arms alternating.  Then K2-sfx (``frl_sf_eval_weights``) from the fp32 master into the bf16 shadow,
+    10 B per model parameter.  The last record holds the medians (min-max), the ratios and the shares of
+    the data-sheet 3.35 TB/s."""
+    from frl_b200.multi_tensor import GradSegTable
+
+    class Slot:
+        def __init__(self, index, offset, shape):
+            self.index, self.offset, self.shape = index, offset, shape
+            self.numel = 1
+            for d in shape:
+                self.numel *= d
+            self.is_model = True
+
+    shapes = [(4096, 4096), (4096,)] * 3 + [(1000, 4096), (1000,), (64, 4096), (64,)]
+    slots, off = [], 0
+    for i, sh in enumerate(shapes):
+        slots.append(Slot(i, off, sh))
+        off = (off + slots[-1].numel + 7) // 8 * 8
+    n, n_real = off, sum(s.numel for s in slots)
+    grad = torch.randn(n, device=DEV).bfloat16()
+    table = GradSegTable(slots, DEV)
+    for s in slots:
+        table.point(s, grad.data_ptr() + 2 * s.offset, grad.dtype)
+    table.upload()
+    p = torch.randn(n, device=DEV) * 0.02
+    lp = torch.empty(n, device=DEV, dtype=torch.bfloat16)
+    s0 = p.clone()
+    s1 = torch.rand(n, device=DEV) * 1e-6
+    fns = {"adamw": lambda i: _native.adamw_mt(p, s0, s1, None, lp, table, lr=1e-3, beta1=0.9, beta2=0.999, eps=1e-8,
+                                               wd=1e-5, step=100),
+           "sf_adamw": lambda i: _native.sf_adamw_mt(p, s0, s1, lp, table, lr=1e-3, ckp1=0.01, beta1=0.9, beta2=0.999,
+                                                     eps=1e-8, wd=1e-5),
+           "sgd": lambda i: _native.sgd_momentum_mt(p, s0, lp, table, lr=1e-2, mu=0.9, dampening=0.0, wd=1e-5),
+           "sf_sgd": lambda i: _native.sf_sgd_mt(p, s0, lp, table, lr=1e-2, ckp1=0.01, beta1=0.9, wd=1e-5)}
+    nbytes = {"adamw": 28, "sf_adamw": 28, "sgd": 20, "sf_sgd": 20}
+    out, times = [], {k: [] for k in fns}
+    for r in range(5):
+        for rule in fns:
+            rec = timed("K2-mt %s mlp bf16-grad (%d tensors, %d params) round %d" % (rule, len(slots), n_real, r),
+                        fns[rule], 1, nbytes[rule] * n_real, iters, "%d B/param" % nbytes[rule], graph=True)
+            times[rule].append(rec["us"])
+            out.append(rec)
+    sfx_times = []
+    for r in range(5):
+        rec = timed("K2-sfx fp32 master + z -> bf16 shadow (%d elems) round %d" % (n, r),
+                    lambda i: _native.sf_eval_weights(p, s0, lp, beta1=0.9), 1, 10 * n, iters, "10 B/param",
+                    graph=True)
+        sfx_times.append(rec["us"])
+        out.append(rec)
+    med = {k: sorted(t)[len(t) // 2] for k, t in times.items()}
+    mm = lambda k: "%.1f (%.1f-%.1f)" % (med[k], min(times[k]), max(times[k]))   # noqa: E731
+    sf_adamw_tbs = 28 * n_real / med["sf_adamw"] / 1e6
+    sfx_med = sorted(sfx_times)[2]
+    sfx_tbs = 10 * n / sfx_med / 1e6
+    summary = {"kernel": "K2-mt schedule-free vs adamw / sgd momentum, K2-sfx; median of 5 (min-max)",
+               **{"%s_us" % k: mm(k) for k in fns},
+               "sf_adamw_over_adamw": round(med["sf_adamw"] / med["adamw"], 4),
+               "sf_adamw_within_3pct": med["sf_adamw"] <= 1.03 * med["adamw"],
+               "sf_adamw_frac_of_3.35TBps": round(sf_adamw_tbs / 3.35, 3),
+               "sf_adamw_at_least_0.83": sf_adamw_tbs / 3.35 >= 0.83,
+               "sf_sgd_over_sgd": round(med["sf_sgd"] / med["sgd"], 4),
+               "sf_sgd_within_3pct": med["sf_sgd"] <= 1.03 * med["sgd"],
+               "sfx_us": "%.1f (%.1f-%.1f)" % (sfx_med, min(sfx_times), max(sfx_times)),
+               "sfx_frac_of_3.35TBps": round(sfx_tbs / 3.35, 3), "sfx_at_least_0.8": sfx_tbs / 3.35 >= 0.8}
     print(json.dumps(summary), flush=True)
     out.append(summary)
     return out
@@ -1019,7 +1093,7 @@ BENCHES = {"k2": bench_k2, "k2mt": bench_k2mt, "k2lw": bench_k2lw, "k3": bench_k
            "k5m": bench_k5m, "k4s": bench_k4s, "k6": bench_k6,
            "k8": bench_k8, "k8t": bench_k8t, "k9": bench_k9, "k10": bench_k10, "k11": bench_k11,
            "k2q8": bench_k2q8, "k2af": bench_k2af, "k13": bench_k13, "k14": bench_k14, "k2w": bench_k2w,
-           "k5nhwc": bench_k5nhwc, "k2lion": bench_k2lion, "k2g": bench_k2g}
+           "k5nhwc": bench_k5nhwc, "k2lion": bench_k2lion, "k2g": bench_k2g, "k2sf": bench_k2sf}
 
 
 def main():
